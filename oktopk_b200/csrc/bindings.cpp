@@ -16,6 +16,7 @@
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "oktopk.cuh"
@@ -333,6 +334,35 @@ static void oktopk_run(uint64_t g, uint64_t res, uint64_t st, const std::vector<
     p.g_inc = (float)getf("g_inc", 1.008); p.g_dec = (float)getf("g_dec", 1.008);
     p.prefilter = (float)getf("prefilter", 0.8);
     p.timeout_ns = (unsigned long long)(getf("timeout_s", 0.0) * 1e9);
+    if (o.contains("srcs")) {
+        // the gradient is read from these (pointer, bucket offset, length) segments; the bucket is all-zero on entry
+        auto t = o["srcs"].cast<std::tuple<std::vector<uint64_t>, std::vector<long long>, std::vector<long long>>>();
+        const auto& ptr = std::get<0>(t);
+        const auto& off = std::get<1>(t);
+        const auto& len = std::get<2>(t);
+        if (off.size() != ptr.size() || len.size() != ptr.size()) throw std::runtime_error("oktopk_run: srcs table size mismatch");
+        if (ptr.size() > (size_t)kSrcSegMax) throw std::runtime_error("oktopk_run: more gradient sources than kSrcSegMax");
+        long long end = 0;
+        for (size_t i = 0; i < ptr.size(); ++i) {
+            if (off[i] < end || (off[i] & 3) || len[i] <= 0 || off[i] + len[i] > n || (ptr[i] & 15))
+                throw std::runtime_error("oktopk_run: gradient sources must be 16-byte aligned, in bucket order, "
+                                         "non-overlapping, at offsets that are multiples of 4 elements");
+            p.src[i] = P_<const float>(ptr[i]);
+            p.src_off[i] = (int)off[i];
+            p.src_len[i] = (int)len[i];
+            end = off[i] + len[i];
+        }
+        p.nsrc = (int)ptr.size();
+        p.zero_g = 0;
+    } else {
+        // the gradient was landed in the bucket: one segment, cleared by the pack pass for the reduce / final phases
+        if (g & 15) throw std::runtime_error("oktopk_run: the bucket must be 16-byte aligned");
+        p.src[0] = P_<const float>(g);
+        p.src_off[0] = 0;
+        p.src_len[0] = n;
+        p.nsrc = 1;
+        p.zero_g = 1;
+    }
     if (geti("split_phases", 0)) {
         // ablation / debugging: one launch per phase instead of the single persistent kernel
         for (int ph = p.phase_begin; ph < p.phase_end; ++ph) {
@@ -545,5 +575,6 @@ PYBIND11_MODULE(_C, m) {
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;
     m.attr("LAND_MAX") = kLandMax;
+    m.attr("SRC_SEG_MAX") = kSrcSegMax;
     m.attr("CHUNK") = kChunk;
 }

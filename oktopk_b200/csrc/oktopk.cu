@@ -16,7 +16,8 @@
 // destination region (lossless layout, oktopk.cuh) or, in the bounded layout, are protected by an
 // in-kernel overflow policy (raise the threshold, redo the pack pass: nothing selected is ever
 // lost), counts travel as release/acquire flags, and the over-selection guard is applied
-// receiver-side so that the common iteration is a single streaming pass (16 B/element).
+// receiver-side so that the common iteration is a single streaming pass (12 B/element when the gradient is read from
+// autograd's tensors, 16 B/element when it was landed in the bucket; see OktParams::src).
 // Grid-wide synchronisation: ONE grid barrier per call (reduce -> global selection); "everybody
 // finished packing / selecting" is a last-CTA ticket whose winner publishes the counts, and the
 // rank's own mailbox doubles as the local barrier of the next phase.
@@ -32,6 +33,38 @@ __device__ __forceinline__ int region_of(const int* s_edges, int P, int i) {
 #pragma unroll 1
     for (int r = 1; r < P; ++r) d += (i >= s_edges[r]) ? 1 : 0;
     return d;
+}
+
+// ---- gradient sources (OktParams::src*): a shared-memory copy of the segment table -----------------------------
+struct SrcSeg { const float* src; int off, len; };
+
+// last segment that starts at or before element e (-1: none)
+__device__ __forceinline__ int seg_find(const SrcSeg* s, int ns, int e) {
+    int lo = 0, hi = ns - 1, r = -1;
+    while (lo <= hi) {
+        const int mid = (lo + hi) >> 1;
+        if (s[mid].off <= e) { r = mid; lo = mid + 1; } else { hi = mid - 1; }
+    }
+    return r;
+}
+
+__device__ __forceinline__ float grad_at(const SrcSeg* s, int ns, int i) {
+    const int q = seg_find(s, ns, i);
+    return (q >= 0 && i - s[q].off < s[q].len) ? s[q].src[i - s[q].off] : 0.f;
+}
+
+// elements 4v .. 4v+3 of the gradient (plain loads: the exact-threshold pass runs once per recompute interval)
+__device__ __forceinline__ float4 grad4_at(const SrcSeg* s, int ns, int v) {
+    float4 out = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int q = seg_find(s, ns, 4 * v);
+    if (q < 0) return out;
+    const int r = 4 * v - s[q].off, len = s[q].len;
+    const float* src = s[q].src + r;
+    if (r + 4 <= len) return ld_stream_f4(reinterpret_cast<const float4*>(src));
+    if (r < len) out.x = src[0];
+    if (r + 1 < len) out.y = src[1];
+    if (r + 2 < len) out.z = src[2];
+    return out;
 }
 
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(const OktParams p) {
@@ -51,6 +84,9 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     __shared__ __align__(8) uint64_t s_pk_bar[kPackStages];
     __shared__ __align__(8) uint64_t s_pk_empty[kPackStages];
     __shared__ __align__(8) uint64_t s_sc_bar[kScanStages];
+    __shared__ SrcSeg s_src[kSrcSegMax];                    // gradient-source table
+    __shared__ int s_tail_v[kSrcSegMax], s_tail_q[kSrcSegMax];   // vectors where a segment ends mid-way (length % 4 != 0)
+    __shared__ int s_ntail;
     extern __shared__ __align__(128) float4 dyn_pk[];       // TMA ring of the streaming pass (kPackSmemBytes)
 
     OktState* st = p.st;
@@ -77,9 +113,24 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
         for (int q = 0; q < kScanStages; ++q) mbar_init(&s_sc_bar[q], 1);
         mbar_fence_init();
     }
-    __syncthreads();
-
     const int n4 = n >> 2;
+    const int nsrc = p.nsrc;
+    for (int q = tid; q < nsrc; q += kThreads) s_src[q] = SrcSeg{p.src[q], p.src_off[q], p.src_len[q]};
+    if (warp == 0) {                     // list the partial last vectors of the segments (the streaming pass patches them)
+        int cnt = 0;
+        for (int q0 = 0; q0 < nsrc; q0 += 32) {
+            const int q = q0 + lane;
+            const int end = q < nsrc ? p.src_off[q] + p.src_len[q] : 0;
+            const bool part = q < nsrc && (end & 3) != 0 && (end >> 2) < n4;
+            const unsigned m = __ballot_sync(0xffffffffu, part);
+            if (part) { const int t = cnt + __popc(m & ((1u << lane) - 1u)); s_tail_v[t] = end >> 2; s_tail_q[t] = q; }
+            cnt += __popc(m);
+        }
+        if (lane == 0) s_ntail = cnt;
+    }
+    __syncthreads();
+    const int ntail = s_ntail;
+
     float4* g4 = reinterpret_cast<float4*>(p.g);
     float4* r4 = reinterpret_cast<float4*>(p.res);
 
@@ -114,7 +165,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
             for (int u = 0; u < kLocTile; ++u) {
                 const int v = base + u * kThreads + tid;
                 in[u] = v < n4;
-                if (in[u]) { a[u] = ld_stream_f4(g4 + v); r[u] = ld_stream_f4(r4 + v); }
+                if (in[u]) { a[u] = grad4_at(s_src, nsrc, v); r[u] = ld_stream_f4(r4 + v); }
                 else { a[u] = make_float4(0.f, 0.f, 0.f, 0.f); r[u] = a[u]; }
             }
 #pragma unroll
@@ -153,7 +204,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
         }
         if (blockIdx.x == 0) {
             for (int i = n4 * 4 + tid; i < n; i += kThreads) {
-                float a = p.g[i] + p.res[i];
+                float a = grad_at(s_src, nsrc, i) + p.res[i];
                 p.res[i] = a;
                 if (prefilter) {
                     if (fabsf(a) > cut) { int pos = atomicAdd(&st->cand_cursor, 1); if (pos < p.ccap) p.cand[pos] = i; }
@@ -365,8 +416,13 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
             // the residual each) through a kPackStages-deep shared-memory ring.  One elected thread arms the stage's mbarrier
             // (expect_tx) and issues the two cp.async.bulk loads kPackStages-1 tiles ahead, so ~96 KB of reads per SM are in
             // flight independent of occupancy/register budget; consumers read the tile with conflict-free LDS.128, write the
-            // accumulator / the zeroed bucket back with streaming 128-bit stores (posted), and run the selection.
-            // 16 B/element of HBM traffic: the roofline floor of the whole call.
+            // accumulator (and, when the gradient was landed in the bucket, zeros over it) back with streaming 128-bit
+            // stores (posted), and run the selection.  HBM traffic: 12 B/element when the gradient is read from autograd's
+            // tensors (gradient + residual in, residual out), 16 B/element when it was landed (+ the bucket cleared).
+            // The gradient half of a tile is assembled from the source segments that overlap it, one bulk copy per piece;
+            // what no segment covers (padding, parameters without a gradient, the last 1-3 elements of a segment whose
+            // length is not a multiple of 4) is copied from the bucket, which is all-zero in that mode, and the partial
+            // last vector of a segment is patched by the consumer from global memory (never read past a source's end).
             // (The ring's mbarrier phases run on across redo passes: ring_it counts every tile ever pushed through.)
             auto arm = [&](int j) {                                         // thread 0 only; j = tile number of THIS pass
                 const int tile = blockIdx.x + j * G;
@@ -375,7 +431,31 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                 fence_proxy_async_all();
                 mbar_expect_tx(&s_pk_bar[stg], res_only ? bytes : 2u * bytes);
                 tma_load_1d(pk_r + stg * kTileV, r4 + (size_t)tile * kTileV, bytes, &s_pk_bar[stg]);
-                if (!res_only) tma_load_1d(pk_g + stg * kTileV, g4 + (size_t)tile * kTileV, bytes, &s_pk_bar[stg]);
+                if (res_only) return;
+                float4* dst = pk_g + stg * kTileV;
+                const int e0 = tile * kTileV * 4, e1 = e0 + (int)(bytes >> 2);
+                // first segment whose whole vectors reach past e0
+                int lo = 0, hi = nsrc;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (s_src[mid].off + (s_src[mid].len & ~3) <= e0) lo = mid + 1; else hi = mid;
+                }
+                int q = lo, e = e0;
+                while (e < e1) {
+                    if (q < nsrc && s_src[q].off <= e) {                    // inside segment q
+                        const int stop = min(e1, s_src[q].off + (s_src[q].len & ~3));
+                        if (stop > e) {
+                            tma_load_1d(dst + ((e - e0) >> 2), s_src[q].src + (e - s_src[q].off), (uint32_t)(stop - e) * 4u,
+                                        &s_pk_bar[stg]);
+                            e = stop;
+                        }
+                        ++q;
+                    } else {                                                // not covered: zeros from the bucket
+                        const int stop = q < nsrc ? min(e1, s_src[q].off) : e1;
+                        tma_load_1d(dst + ((e - e0) >> 2), p.g + e, (uint32_t)(stop - e) * 4u, &s_pk_bar[stg]);
+                        e = stop;
+                    }
+                }
             };
             if (tid == 0)
                 for (int j = 0; j < min(nmine, kPackStages - 1); ++j) {
@@ -407,11 +487,20 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                     if (in[u]) {
                         a[u] = pk_r[stg * kTileV + u * kThreads + tid];
                         if (!res_only) {
-                            const float4 gq = pk_g[stg * kTileV + u * kThreads + tid];
+                            float4 gq = pk_g[stg * kTileV + u * kThreads + tid];
+                            for (int t = 0; t < ntail; ++t)
+                                if (s_tail_v[t] == v) {                     // a segment ends inside this vector
+                                    const SrcSeg sg = s_src[s_tail_q[t]];
+                                    const float* src = sg.src + (sg.len & ~3);
+                                    const int c = sg.len & 3;
+                                    gq.x = src[0];
+                                    if (c > 1) gq.y = src[1];
+                                    if (c > 2) gq.z = src[2];
+                                }
                             a[u].x += gq.x; a[u].y += gq.y; a[u].z += gq.z; a[u].w += gq.w;
                             st_stream_f4(r4 + v, a[u]);
                         }
-                        if (attempt == 0) st_stream_f4(g4 + v, make_float4(0.f, 0.f, 0.f, 0.f));
+                        if (attempt == 0 && p.zero_g) st_stream_f4(g4 + v, make_float4(0.f, 0.f, 0.f, 0.f));
                     }
                 }
                 __syncwarp();                                               // the warp's part of the tile is in registers:
@@ -515,9 +604,9 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                 bool in = i < n;
                 float a = 0.f;
                 if (in) {
-                    a = res_only ? p.res[i] : (p.g[i] + p.res[i]);
+                    a = res_only ? p.res[i] : (grad_at(s_src, nsrc, i) + p.res[i]);
                     if (!res_only) p.res[i] = a;
-                    p.g[i] = 0.f;
+                    if (p.zero_g) p.g[i] = 0.f;
                 }
                 emit(i, a, in);
             }
@@ -590,7 +679,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
         const int len_me = s_edges[rank + 1] - off_me;
         float* greg = p.g + off_me;
         int pulled = 0;
-        // Scatter-add with first-touch detection: the pack pass zeroed the bucket, so the contribution that finds
+        // Scatter-add with first-touch detection: the bucket is all-zero here (cleared by the pack pass, or already zero
+        // when the gradient was read from its sources), so the contribution that finds
         // 0.0 is the first one of its index; that index goes on the candidate list the global selection walks, which
         // makes the selection O(#entries) instead of a scan of the whole region (4n/P bytes).  (A sum that passes
         // through exactly 0.0 can list an index twice; the selection claims each index with an exchange, so a

@@ -150,6 +150,15 @@ enum Phase : int {
 enum ResidualMode : int { RES_OKTOPK = 0, RES_LOCAL_GT = 1, RES_LOCAL_GE = 2 };
 enum GlobalMode : int { GLB_THRESHOLD = 0, GLB_EXACT_TOPK = 1, GLB_ALL_NONZERO = 2 };
 
+// Where the gradient that the call reduces comes from: an ordered table of (source, bucket element offset, length)
+// segments.  Either ONE segment that is the bucket itself (the gradient was landed there; the pack pass then clears
+// the bucket for the reduce / final phases), or the tensors autograd produced, read in place (the bucket must be
+// all-zero on entry and is not cleared).  Bucket elements that no segment covers read as zero.  Offsets are multiples
+// of 4 elements and sources 16-byte aligned; a length need not be.  Passed by value: a captured CUDA graph keeps the
+// addresses of its capture.  Sized for the largest bucket of the bench workloads (BERT-base: 132 tensors) with the
+// whole OktParams under the classic 4 KB kernel-parameter limit.
+constexpr int kSrcSegMax = 160;
+
 struct OktParams {
     float* g;            // gradient bucket (result written in place)
     float* res;          // residual / accumulator
@@ -185,7 +194,13 @@ struct OktParams {
     int dense_nnz_limit;                // GLB_ALL_NONZERO (TopkDSA): total gathered nnz >= this => dense allgather path (0 = never)
     int* host_fault;                    // mapped pinned int: fault code mirrored to the host without a sync (may be null)
     int trace;                          // 1: write a TraceRec per call
+    int zero_g;                         // 1: the pack pass clears the bucket (the gradient was landed in it)
+    int nsrc;                           // gradient-source segments (see kSrcSegMax)
+    int src_off[kSrcSegMax];
+    int src_len[kSrcSegMax];
+    const float* src[kSrcSegMax];
 };
+static_assert(sizeof(OktParams) <= 4096, "OktParams must fit the 4 KB kernel-parameter limit");
 
 // ---- gather-type schemes (TopkAopt / Gaussiank / TopkA): select -> own slot -> everyone adds all ---
 enum GatherSelect : int { GS_THRESHOLD_REUSE = 0, GS_GAUSSIAN = 1, GS_EXACT_TOPK = 2 };

@@ -83,6 +83,14 @@ class _BucketedComm:
             for p in b.params:
                 self._bucket_of[p] = b
                 self._hook_handles.append(p.register_post_accumulate_grad_hook(self._make_hook(p)))
+        # Ok-Topk with a fused update: the reduction reads the gradients straight from autograd's tensors, with no landing
+        # copy (see _source_table).  Its pack pass then leaves the bucket alone, so the bucket must be all-zero when such a
+        # call starts: the fused update clears the few entries the reduction wrote (zero_grad=1 after EVERY step, dense
+        # warm-up steps included), and CudaBucketEngine.reset_sparse_state / load_state_dict clear it after a fault or a
+        # checkpoint load.
+        fused_update = bool(getattr(self, "_okt_is_sgd", False)) or isinstance(self, BertAdam)
+        self._direct = (self._land and fused_update and allreducer.compressor.name == "oktopk"
+                        and all(b.flat_param is not None for b in self._buckets))
         if self._use_streams:
             # high priority: a bucket's (SM-partitioned) communication kernel should get its SMs as soon as backward
             # kernels retire CTAs, not after the whole backward queue
@@ -185,11 +193,39 @@ class _BucketedComm:
         if srcs:
             ext.require().land_grads(srcs, offs, numels, b.grad.data_ptr(), torch.cuda.current_stream().cuda_stream)
 
+    def _source_table(self, b: Bucket):
+        """(pointers, offsets, lengths) of the autograd-produced gradients of bucket ``b``, for a reduction that reads them
+        in place; ``p.grad`` is re-pointed at the bucket views (which receive the reduced gradient) and the source tensors
+        are held on the bucket until ``synchronize()`` has made the current stream wait for the reduction.  None if a
+        gradient cannot be read that way (already the bucket view, another dtype or layout, misaligned, too many
+        tensors): the step then lands the gradients as before."""
+        ptrs, offs, lens, held = [], [], [], []
+        for p, o, v in zip(b.params, b.offsets, b.grad_views):
+            g = p.grad
+            if g is None or g.numel() == 0:       # no gradient in this step: its slice of the all-zero bucket is read
+                continue
+            if (g.data_ptr() == v.data_ptr() or g.dtype != torch.float32 or not g.is_cuda or g.stride() != v.stride()
+                    or g.data_ptr() % 16):
+                return None
+            ptrs.append(g.data_ptr())
+            offs.append(o)
+            lens.append(g.numel())
+            held.append(g)
+        if len(ptrs) > ext.require().SRC_SEG_MAX:
+            return None
+        for p, v in zip(b.params, b.grad_views):
+            p.grad = v
+        b.held = held
+        return ptrs, offs, lens
+
     def _launch(self, b: Bucket) -> None:
         if b.launched:
             return
         b.launched = True
-        if self._land:
+        srcs = None
+        if self._direct and not self.momentum_correction and self._allreducer.reads_sources(b.name):
+            srcs = self._source_table(b)
+        if srcs is None and self._land:
             self._land_bucket(b)
         if self.momentum_correction:
             self._apply_momentum_correction(b)
@@ -198,10 +234,10 @@ class _BucketedComm:
             ev.record(torch.cuda.current_stream())
             self._comm_stream.wait_event(ev)
             with torch.cuda.stream(self._comm_stream):
-                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream)
+                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream, srcs=srcs)
                 b.event.record(self._comm_stream)
         else:
-            self._allreducer.reduce_bucket(b.name, b.grad)
+            self._allreducer.reduce_bucket(b.name, b.grad, srcs=srcs)
 
     def _apply_momentum_correction(self, b: Bucket) -> None:
         """``VGG/distributed_optimizer.py:81-88``: communicate the momentum-accumulated gradient."""
@@ -228,6 +264,8 @@ class _BucketedComm:
             cur = torch.cuda.current_stream()
             for b in self._buckets:
                 cur.wait_event(b.event)
+        for b in self._buckets:                   # the reductions' reads of the gradient tensors are ordered before
+            b.held = None                         # anything the current stream does next: their memory may be reused
         self._synced = True
 
     def _after_step(self) -> None:
@@ -237,6 +275,13 @@ class _BucketedComm:
         self._next_launch = 0
         self._synced = False
         self._allreducer.poll_faults()           # pinned host flag, no sync: a timed-out peer wait surfaces at once
+
+    def _clear_buckets(self) -> None:
+        """Re-establish the all-zero bucket that a reduction reading autograd's tensors expects."""
+        if self._direct:
+            with torch.no_grad():
+                for b in self._buckets:
+                    b.grad.zero_()
 
     def zero_grad(self, set_to_none: bool = False) -> None:  # noqa: ARG002 - views must survive
         if self._land:
@@ -293,7 +338,7 @@ class _BucketedComm:
             if use_kernel:
                 ext.require().fused_sgd(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
                                         mom.data_ptr() + 4 * s, e - s, lr, m, damp, wd, int(nest), int(first),
-                                        0 if self._land else 1, 1.0,
+                                        0 if self._land and not self._direct else 1, 1.0,
                                         torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
                                         self._allreducer.fault_ptr(b.name))
             else:
@@ -366,6 +411,7 @@ class _DistributedOptimizerMixin(_BucketedComm):
                         self.state[p]["momentum_buffer"] = v
         if okt is not None:
             self._allreducer.load_state_dict(okt)
+        self._clear_buckets()
 
 
 def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None, compression=NoneCompressor,
@@ -537,7 +583,7 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
             if use_kernel:
                 ext.require().fused_bert_adam(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
                                               m.data_ptr() + 4 * s, v.data_ptr() + 4 * s, e - s, lr, g["b1"], g["b2"],
-                                              g["e"], g["weight_decay"], 0 if self._land else 1,
+                                              g["e"], g["weight_decay"], 0 if self._land and not self._direct else 1,
                                               torch.cuda.current_stream().cuda_stream,
                                               self._lr_ptr(gi), self._allreducer.fault_ptr(b.name))
             else:
@@ -588,3 +634,4 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
                     self.state[p].setdefault("step", self.counter)
         if okt is not None:
             self._allreducer.load_state_dict(okt)
+        self._clear_buckets()

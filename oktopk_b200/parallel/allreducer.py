@@ -86,7 +86,18 @@ class AllReducer:
         self._dist_states[name] = SparseState(numel, self.world.size)
         return torch.zeros(numel, dtype=torch.float32, device=device)
 
-    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None) -> torch.Tensor:
+    def reads_sources(self, name: str) -> bool:
+        """True if the next reduction of bucket ``name`` can read the gradient straight from autograd's tensors
+        (``reduce_bucket(srcs=...)``) instead of from the bucket.  Not in the diagnostic modes, which read the bucket."""
+        from ..utils import settings
+        eng = self._engines.get(name)
+        if eng is None or settings.PROFILING_GRAD or settings.PROFILING_NORM:
+            return False
+        return eng.reads_sources(self.compressor.name, self.get_current_density())
+
+    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None, srcs=None) -> torch.Tensor:
+        """Reduce bucket ``name`` in place.  ``srcs = (pointers, offsets, lengths)``: the gradient is in these fp32
+        tensors rather than in ``flat``, which must then be all-zero (only where ``reads_sources(name)``)."""
         density = self.get_current_density()
         from ..utils import settings
         if settings.PROFILING_GRAD and self.cfg.sparse:
@@ -94,7 +105,7 @@ class AllReducer:
         if settings.PROFILING_NORM and self.cfg.sparse:
             return self._reduce_profiled(name, flat, stream, density)
         if name in self._engines:
-            out = self._engines[name].reduce(self.compressor.name, density, stream=stream, g=flat)
+            out = self._engines[name].reduce(self.compressor.name, density, stream=stream, g=flat, srcs=srcs)
             if settings.PROFILING:
                 self._profile_iteration(name)
             return out

@@ -37,6 +37,7 @@ class Bucket:
     launched: bool = False
     dirty: bool = True
     event: Optional["torch.cuda.Event"] = None
+    held: Optional[List[torch.Tensor]] = None      # gradient tensors a running reduction reads (until synchronize())
 
     def views(self, flat: torch.Tensor) -> List[torch.Tensor]:
         """Per-parameter aliases of a flat buffer with the PARAMETER'S OWN memory layout: a channels_last conv weight

@@ -131,9 +131,24 @@ class CudaBucketEngine:
         return max(int(self.n * d), 1)
 
     # ------------------------------------------------------------------ the step
+    def reads_sources(self, compressor: str, density: Optional[float] = None) -> bool:
+        """True if the next ``reduce`` call can read the gradient from its source tensors (``reduce(srcs=...)``) instead of
+        the bucket: an Ok-Topk call of the fused kernel, whose pack pass then reads every source once and leaves the bucket
+        alone.  The bucket must be all-zero when such a call starts."""
+        cfg = self.cfg
+        return (compressor == "oktopk" and cfg.sparse and self.host.counter >= cfg.warmup_iters
+                and not self._dense_switch(compressor, density))
+
     def reduce(self, compressor: str, density: Optional[float] = None,
-               stream: Optional[torch.cuda.Stream] = None, g: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Allreduce this bucket in place (``self.grad`` unless an external ``g`` is given)."""
+               stream: Optional[torch.cuda.Stream] = None, g: Optional[torch.Tensor] = None,
+               srcs: Optional[tuple] = None) -> torch.Tensor:
+        """Allreduce this bucket in place (``self.grad`` unless an external ``g`` is given).
+
+        ``srcs = (pointers, offsets, lengths)``: the gradient is not in the bucket but in these fp32 tensors, at these
+        element offsets of the bucket (Ok-Topk only, see ``reads_sources``); the result is written into the bucket."""
+        if srcs is not None and (g is not None and g.data_ptr() != self.grad.data_ptr()
+                                 or not self.reads_sources(compressor, density)):
+            raise ValueError("gradient sources are only read by an Ok-Topk call on the engine's own bucket")
         cfg = self.cfg
         st = self.host
         ext_g = g is not None and g.data_ptr() != self.grad.data_ptr()
@@ -161,7 +176,7 @@ class CudaBucketEngine:
             self.last_mode = "dense(auto)"
         elif compressor in _FUSED:
             self._res_clean = False
-            self._fused(compressor, density, s, g if ext_g else self.grad)
+            self._fused(compressor, density, s, g if ext_g else self.grad, srcs)
         elif compressor in _GATHER:
             self._res_clean = False
             self._gather(compressor, density, s, g if ext_g else self.grad)
@@ -188,7 +203,8 @@ class CudaBucketEngine:
                          self.dense_grid, s, self.state_ptr, float(self.cfg.peer_timeout_s), self.mc_grad,
                          self.host_flag_dev)
 
-    def _fused(self, compressor: str, density: Optional[float], s: int, g: torch.Tensor) -> None:
+    def _fused(self, compressor: str, density: Optional[float], s: int, g: torch.Tensor,
+               srcs: Optional[tuple] = None) -> None:
         cfg = self.cfg
         k = self.k_now(density)
         it = self.host.counter - cfg.warmup_iters
@@ -225,6 +241,8 @@ class CudaBucketEngine:
                     and cfg.dsa_dense_fallback_frac > 0:
                 o["dense_nnz_limit"] = max(int(self.n * cfg.dsa_dense_fallback_frac), 1)
                 o["peer_g"] = self.peer_grad
+        if srcs is not None:
+            o["srcs"] = srcs
         self.C.oktopk_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                           self.rank, k, self.cap, self.gcap, o, self.grid, s)
         self.last_mode = compressor
@@ -325,8 +343,11 @@ class CudaBucketEngine:
 
     def reset_sparse_state(self) -> None:
         """After a fault: drop the (possibly half-consumed) residual and thresholds, restore uniform regions, so that
-        all replicas restart the sparse scheme from the same state (the next call recomputes exact thresholds)."""
+        all replicas restart the sparse scheme from the same state (the next call recomputes exact thresholds).  The
+        bucket is cleared too: the update that would have cleared it was skipped, and a call that reads the gradient from
+        its sources expects an all-zero bucket."""
         self.residual.zero_()
+        self.grad.zero_()
         self.host.counter = self.cfg.warmup_iters if self.host.counter >= self.cfg.warmup_iters else self.host.counter
         self._write_edges(offsets_of(uniform_boundaries(self.n, self.P)) + [self.n], 0.0, 0.0)
 
