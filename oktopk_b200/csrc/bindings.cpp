@@ -482,6 +482,13 @@ static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int 
                               S_(stream)),
        "fused_bert_adam");
 }
+static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double beta1, double beta2, double eps,
+                       double wd, int decoupled, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("fused_adam: scal_ptr must point at the group's device scalars");
+    ck(launch_fused_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, beta1, beta2, (float)eps, (float)wd,
+                         decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
+       "fused_adam");
+}
 static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, uint64_t gamma, uint64_t beta, uint64_t cbias,
                        uint64_t save_mean, uint64_t save_invstd, uint64_t rmean, uint64_t rvar, uint64_t nbt, double momentum,
                        double eps, int relu, int M, int C, int W, int slot, int max_ctas, uint64_t stream) {
@@ -565,6 +572,9 @@ PYBIND11_MODULE(_C, m) {
     m.def("fused_bert_adam", &fused_bert_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"),
           py::arg("stream"), py::arg("lr_ptr") = 0, py::arg("fault_ptr") = 0);
+    m.def("fused_adam", &fused_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
+          py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("decoupled"), py::arg("zero_grad"),
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
     m.def("momentum_correct", &momentum_correct);
     m.def("maxpool2_fwd", &maxpool2_fwd);
     m.def("maxpool2_bwd", &maxpool2_bwd);

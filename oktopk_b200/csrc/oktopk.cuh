@@ -276,6 +276,10 @@ cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float lr, fl
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float lr, float b1, float b2,
                                    float eps, float weight_decay, int zero_grad, const float* lr_ptr,
                                    const int* fault, cudaStream_t stream);
+// torch.optim.Adam / AdamW update; scal -> {1 - lr*wd, -lr / (1 - beta1^t), sqrt(1 - beta2^t)} of this step
+cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
+                              float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
+                              cudaStream_t stream);
 // multi-tensor gradient landing: copy up to kLandMax autograd-produced gradient tensors into the flat bucket in ONE launch
 constexpr int kLandMax = 96;
 struct LandParams {

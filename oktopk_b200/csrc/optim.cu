@@ -92,6 +92,53 @@ __global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __r
         }
 }
 
+// torch.optim.Adam / AdamW (foreach, non-capturable branch), one rounding per op.  The per-step scalars (decay = 1 - lr*wd,
+// step_size = -lr / (1 - beta1^t), bc2_sqrt = sqrt(1 - beta2^t)) are computed on the host in double and read from device
+// memory, so that a captured CUDA graph picks up the schedule and the bias correction of every replay.
+// decoupled: AdamW (p *= 1 - lr*wd) instead of L2 (g += wd*p).  w = 1 - beta1 is the weight of torch's lerp, whose
+// formula depends on whether the weight is below 0.5.  (47 registers, 5 CTAs per SM: capping at 32 for 8 CTAs spills
+// around the IEEE division's slow path.)
+__global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                                  float* __restrict__ m, float* __restrict__ v, int n,
+                                                                  float w, float b2, float omb2, float eps, float wd,
+                                                                  int decoupled, int zero_grad,
+                                                                  const float* __restrict__ scal,
+                                                                  const int* __restrict__ fault) {
+    if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
+    const float decay = scal[0], step_size = scal[1], bc2_sqrt = scal[2];
+    const bool small_w = fabsf(w) < 0.5f;
+    const float lw = small_w ? w : 1.f - w;
+    const int n4 = n >> 2;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    float4* g4 = reinterpret_cast<float4*>(g);
+    float4* m4 = reinterpret_cast<float4*>(m);
+    float4* v4 = reinterpret_cast<float4*>(v);
+    auto upd = [&](float& pw, float gw, float& mw, float& vw) {
+        if (decoupled) pw = pw * decay;                  // decay == 1 exactly when wd == 0
+        else if (wd != 0.f) gw = gw + wd * pw;
+        mw = small_w ? mw + lw * (gw - mw) : gw - (gw - mw) * lw;
+        vw = vw * b2;
+        vw = vw + omb2 * gw * gw;
+        const float d = sqrtf(vw) / bc2_sqrt + eps;
+        pw = pw + (step_size * mw) / d;
+    };
+    for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
+        float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = m4[i], vw = v4[i];
+        upd(pw.x, gw.x, mw.x, vw.x); upd(pw.y, gw.y, mw.y, vw.y);
+        upd(pw.z, gw.z, mw.z, vw.z); upd(pw.w, gw.w, mw.w, vw.w);
+        p4[i] = pw; m4[i] = mw; v4[i] = vw;
+        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f))
+            g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if (blockIdx.x == 0)
+        for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
+            float pw = p[i], gw = g[i], mw = m[i], vw = v[i];
+            upd(pw, gw, mw, vw);
+            p[i] = pw; m[i] = mw; v[i] = vw;
+            if (zero_grad) g[i] = 0.f;
+        }
+}
+
 // momentum correction (VGG/distributed_optimizer.py:81-88): buf = m*buf + g ; g = buf
 __global__ void __launch_bounds__(kOptThreads) momentum_correct_kernel(float* __restrict__ g, float* __restrict__ buf,
                                                                         int n, float momentum) {
@@ -148,6 +195,16 @@ cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n
                                    const int* fault, cudaStream_t stream) {
     fused_bert_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, lr, b1, b2, eps, weight_decay,
                                                                    zero_grad, lr_ptr, fault);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
+                              float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
+                              cudaStream_t stream) {
+    // 1 - beta in double, rounded once: torch passes these factors as Python floats
+    fused_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, (float)(1.0 - beta1), (float)beta2,
+                                                              (float)(1.0 - beta2), eps, weight_decay, decoupled,
+                                                              zero_grad, scal, fault);
     return cudaGetLastError();
 }
 

@@ -13,7 +13,7 @@ _ERR: Optional[BaseException] = None
 # kernels launched by this package since import (the bench reports the delta over its timed region)
 LAUNCH_COUNT = {"total": 0}
 _LAUNCHERS = {"oktopk_run": 1, "gather_run": 1, "gtopk_run": 1, "dense_run": 1, "kth_abs": 1, "fused_sgd": 1,
-              "fused_bert_adam": 1, "momentum_correct": 1, "clip_by_norm": 2, "land_grads": 1, "bn_forward": 1, "bn_backward": 1,
+              "fused_bert_adam": 1, "fused_adam": 1, "momentum_correct": 1, "clip_by_norm": 2, "land_grads": 1, "bn_forward": 1, "bn_backward": 1,
               "maxpool2_fwd": 1, "maxpool2_bwd": 1}
 
 

@@ -14,13 +14,16 @@ What is different by design (GPU-first):
     last gradient, in a fixed bucket order on every rank, and ``synchronize()`` is a stream wait;
   * gradients / parameters / momentum are views into flat buffers, the update is one fused kernel
     per (bucket, param group) that also zeroes the gradient bucket (``zero_grad()`` is then free);
-  * any torch optimizer can be wrapped (the reference re-implements SGD only, A.4-7): SGD and
-    BertAdam take the fused kernels, everything else falls through to its own ``step()``;
+  * any torch optimizer can be wrapped (the reference re-implements SGD only, A.4-7): SGD, BertAdam and
+    ``torch.optim.Adam`` / ``AdamW`` built with ``fused=True`` take the fused kernels (Adam: fp32 CUDA parameters,
+    no amsgrad / maximize / differentiable, Python-number lr and betas); everything else falls through to its own
+    ``step()``;
   * ``state_dict()`` carries residuals, thresholds, region boundaries and counters (SURVEY 5.4).
 """
 from __future__ import annotations
 
 import math
+import warnings
 from typing import Dict, Iterable, List, Optional
 
 import torch
@@ -88,7 +91,10 @@ class _BucketedComm:
         # call starts: the fused update clears the few entries the reduction wrote (zero_grad=1 after EVERY step, dense
         # warm-up steps included), and CudaBucketEngine.reset_sparse_state / load_state_dict clear it after a fault or a
         # checkpoint load.
-        fused_update = bool(getattr(self, "_okt_is_sgd", False)) or isinstance(self, BertAdam)
+        if getattr(self, "_okt_adam", False):     # the fused Adam kernel works on flat fp32 CUDA buckets only
+            self._okt_adam = ext.available() and all(b.flat_param is not None and b.grad.is_cuda for b in self._buckets)
+        fused_update = (bool(getattr(self, "_okt_is_sgd", False)) or isinstance(self, BertAdam)
+                        or bool(getattr(self, "_okt_adam", False)))
         self._direct = (self._land and fused_update and allreducer.compressor.name == "oktopk"
                         and all(b.flat_param is not None for b in self._buckets))
         if self._use_streams:
@@ -96,15 +102,17 @@ class _BucketedComm:
             # kernels retire CTAs, not after the whole backward queue
             self._comm_stream = torch.cuda.Stream(priority=-1)
         allreducer.add_resync_hook(self._resync_replicas)
-        # device-resident learning rates (one float per param group): the fused update kernels read lr from
-        # memory so that a captured CUDA graph of the whole step stays valid when the schedule moves
+        # device-resident per-group scalars (the learning rate; for wrapped Adam the step's decay, step size and bias
+        # correction): the fused update kernels read them from memory so that a captured CUDA graph of the whole step
+        # stays valid when the schedule moves
         self._lr_dev = None
         self._lr_pin, self._lr_ev, self._lr_ring, self._lr_last = [], [], 0, None
+        self._scal_n = 3 if getattr(self, "_okt_adam", False) else 1       # device scalars per param group
         dev0 = self._buckets[0].params[0].device if self._buckets else torch.device("cpu")
         if dev0.type == "cuda" and ext.available():
-            G = len(self.param_groups)
-            self._lr_dev = torch.zeros(max(G, 1), dtype=torch.float32, device=dev0)
-            self._lr_pin = [torch.zeros(max(G, 1), dtype=torch.float32).pin_memory() for _ in range(8)]
+            n = max(len(self.param_groups), 1) * self._scal_n
+            self._lr_dev = torch.zeros(n, dtype=torch.float32, device=dev0)
+            self._lr_pin = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(8)]
             self._lr_ev = [None] * len(self._lr_pin)
 
     def _resync_replicas(self) -> None:
@@ -125,20 +133,25 @@ class _BucketedComm:
     def _group_lr(self, gi: int) -> float:
         return float(self.param_groups[gi]["lr"])
 
+    def _group_scalars(self, gi: int):
+        """The device scalars of param group ``gi`` for the coming step (``_scal_n`` of them)."""
+        return (self._group_lr(gi),)
+
     def refresh_lr(self) -> None:
-        """Push the current per-group learning rates to the device (one tiny async H2D, only when changed).
+        """Push the current per-group device scalars to the device (one tiny async H2D, only when changed).
         Never called while a stream is capturing: graph replays call it right before ``replay()``."""
         if self._lr_dev is None:
             return
-        vals = [self._group_lr(gi) for gi in range(len(self.param_groups))]
+        vals = [self._group_scalars(gi) for gi in range(len(self.param_groups))]
         if vals == self._lr_last:
             return
         self._lr_ring = (self._lr_ring + 1) % len(self._lr_pin)
         pin = self._lr_pin[self._lr_ring]
         if self._lr_ev[self._lr_ring] is not None:          # the host may run many (graph-replayed) steps ahead:
             self._lr_ev[self._lr_ring].synchronize()        # never overwrite a staging slot whose copy is pending
-        for i, v in enumerate(vals):
-            pin[i] = v
+        for gi, sc in enumerate(vals):
+            for j, v in enumerate(sc):
+                pin[gi * self._scal_n + j] = v
         self._lr_dev.copy_(pin, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
@@ -146,7 +159,7 @@ class _BucketedComm:
         self._lr_last = vals
 
     def _lr_ptr(self, gi: int) -> int:
-        return 0 if self._lr_dev is None else self._lr_dev.data_ptr() + 4 * gi
+        return 0 if self._lr_dev is None else self._lr_dev.data_ptr() + 4 * self._scal_n * gi
 
     def _maybe_refresh_lr(self) -> None:
         if self._lr_dev is not None and not torch.cuda.is_current_stream_capturing():
@@ -380,6 +393,12 @@ class _DistributedOptimizerMixin(_BucketedComm):
             with torch.no_grad():
                 for b in self._buckets:
                     self._fused_sgd(b)
+        elif self._okt_adam:
+            self._maybe_refresh_lr()
+            with torch.no_grad():
+                for b in self._buckets:
+                    self._fused_torch_adam(b)
+            self.counter += 1
         else:
             super().step()
             for b in self._buckets:
@@ -387,8 +406,77 @@ class _DistributedOptimizerMixin(_BucketedComm):
         self._after_step()
         return loss
 
+    # ------------------------------------------------------------------ wrapped torch.optim.Adam / AdamW (fused=True)
+    def _group_scalars(self, gi: int):
+        if not self._okt_adam:
+            return super()._group_scalars(gi)
+        # torch's non-capturable Adam, in double: t = the step about to run
+        g = self.param_groups[gi]
+        lr, (b1, b2), t = float(g["lr"]), g["betas"], float(self.counter + 1)
+        return (1 - lr * g["weight_decay"], (lr / (1 - b1 ** t)) * -1, (1 - b2 ** t) ** 0.5)
+
+    def _adam_flat_state(self, b: Bucket):
+        """The bucket's flat ``exp_avg`` / ``exp_avg_sq`` buffers; ``self.state[p]`` holds views of them."""
+        fs = self._flat_state.setdefault(b.index, {})
+        if "exp_avg" not in fs:
+            fs["exp_avg"], fs["exp_avg_sq"] = torch.zeros_like(b.grad), torch.zeros_like(b.grad)
+            for p, vm, vv in zip(b.params, b.views(fs["exp_avg"]), b.views(fs["exp_avg_sq"])):
+                self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"] = vm, vv
+        return fs["exp_avg"], fs["exp_avg_sq"]
+
+    def _fused_torch_adam(self, b: Bucket) -> None:
+        m, v = self._adam_flat_state(b)
+        for gi, s, e in b.group_slices:
+            g = self.param_groups[gi]
+            ext.require().fused_adam(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s, m.data_ptr() + 4 * s,
+                                     v.data_ptr() + 4 * s, e - s, g["betas"][0], g["betas"][1], g["eps"],
+                                     g["weight_decay"], int(bool(g["decoupled_weight_decay"])),
+                                     0 if self._land and not self._direct else 1,
+                                     torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
+                                     self._allreducer.fault_ptr(b.name))
+        b.dirty = False
+
+    def _adopt_adam_state(self) -> None:
+        """Move per-parameter Adam state (from ``load_state_dict`` or the wrapped optimizer) into the flat buffers and
+        take the common step count as ``counter``.  Unequal step counts cannot share one bias correction: the optimizer
+        then keeps the per-parameter state and uses torch's own ``step()`` from here on."""
+        have = [p for b in self._buckets for p in b.params if "exp_avg" in self.state.get(p, {})]
+        steps = {float(self.state[p]["step"]) for p in have}
+        if len(steps) > 1:
+            warnings.warn("DistributedOptimizer: the loaded Adam state has unequal step counts per parameter %s; "
+                          "using torch's Adam step from now on" % sorted(steps))
+            self._okt_adam = False
+            self._clear_buckets()
+            self._direct = False                  # torch's step reads the gradients from the landed bucket
+            for b in self._buckets:
+                fs = self._flat_state.get(b.index, {})
+                fs.pop("exp_avg", None)
+                fs.pop("exp_avg_sq", None)
+            return
+        self.counter = int(steps.pop()) if steps else 0
+        loaded = {p: (self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"]) for p in have}
+        with torch.no_grad():
+            for b in self._buckets:
+                m, v = self._adam_flat_state(b)      # (re-points state[p] at the views when it creates the buffers)
+                for p, vm, vv in zip(b.params, b.views(m), b.views(v)):
+                    src = loaded.get(p)
+                    if src is None:                  # no state for p: fresh moments, as torch would start them
+                        vm.zero_()
+                        vv.zero_()
+                    else:
+                        vm.copy_(src[0])
+                        vv.copy_(src[1])
+                    st = self.state[p]
+                    st.pop("step", None)          # the step count is ``counter``
+                    st["exp_avg"], st["exp_avg_sq"] = vm, vv
+
     def state_dict(self):
         sd = super().state_dict()
+        if self._okt_adam:                        # torch's fused Adam format: a float32 0-dim step on the param's device
+            params = [p for g in self.param_groups for p in g["params"]]
+            for i, st in list(sd["state"].items()):
+                sd["state"][i] = dict(st, step=torch.tensor(float(self.counter), dtype=torch.float32,
+                                                            device=params[i].device))
         sd["oktopk"] = self._allreducer.state_dict()
         return sd
 
@@ -396,6 +484,8 @@ class _DistributedOptimizerMixin(_BucketedComm):
         state_dict = dict(state_dict)
         okt = state_dict.pop("oktopk", None)
         super().load_state_dict(state_dict)
+        if self._okt_adam:
+            self._adopt_adam_state()
         if self._okt_is_sgd:                      # re-alias momentum into the flat buffers
             for b in self._buckets:
                 fs = self._flat_state.setdefault(b.index, {})
@@ -434,8 +524,28 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
                     backend=backend, err_callback=err_handler, layerwise_times=layerwise_times,
                     sigma_scale=sigma_scale, norm_clip=norm_clip, writer=writer)
     obj._okt_is_sgd = isinstance(optimizer, torch.optim.SGD)
+    obj._okt_adam = _fused_adam_applies(optimizer)
+    if obj._okt_adam:
+        obj.counter = 0                           # steps taken: Adam's bias correction (GraphedTrainStep keeps it too)
     obj._okt_setup(named_parameters, ar, flatten_params=flatten_params)
+    if obj._okt_adam and obj.state:
+        obj._adopt_adam_state()
     return obj
+
+
+def _fused_adam_applies(opt: torch.optim.Optimizer) -> bool:
+    """A torch Adam / AdamW that asked for a fused kernel (``fused=True``) and whose options the flat-bucket kernel
+    implements: it then runs ``fused_adam`` instead of torch's update.  Flat fp32 CUDA buckets are checked at setup."""
+    if not isinstance(opt, torch.optim.Adam):
+        return False
+    for g in opt.param_groups:
+        if g.get("fused") is not True or g.get("amsgrad") or g.get("maximize") or g.get("differentiable"):
+            return False
+        if torch.is_tensor(g["lr"]) or any(torch.is_tensor(b) for b in g["betas"]):
+            return False
+        if any(not p.is_cuda or p.dtype != torch.float32 for p in g["params"]):
+            return False
+    return True
 
 
 def rank() -> int:
