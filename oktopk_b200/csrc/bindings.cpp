@@ -489,23 +489,29 @@ static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, do
                          decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
        "fused_adam");
 }
+// dtype of x, y, dy, dx: 0 = fp32, 1 = bf16 (parameters, statistics and dgamma / dbeta are fp32 either way)
+static BnDtype bn_dtype(int dtype, const char* what) {
+    if (dtype != 0 && dtype != 1) throw std::runtime_error(std::string(what) + ": dtype must be 0 (fp32) or 1 (bf16)");
+    return static_cast<BnDtype>(dtype);
+}
 static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, uint64_t gamma, uint64_t beta, uint64_t cbias,
                        uint64_t save_mean, uint64_t save_invstd, uint64_t rmean, uint64_t rvar, uint64_t nbt, double momentum,
-                       double eps, int relu, int M, int C, int W, int slot, int max_ctas, uint64_t stream) {
+                       double eps, int relu, int M, int C, int W, int slot, int max_ctas, uint64_t stream, int dtype) {
     if (C % 4 != 0) throw std::runtime_error("bn_forward: channel count must be a multiple of 4");
     if (slot < 0) throw std::runtime_error("bn_forward: negative slot");
-    ck(launch_bn_forward(P_<const float>(x), P_<float>(y), P_<unsigned char>(arg), P_<float>(partial), P_<const float>(gamma),
+    ck(launch_bn_forward(P_<const void>(x), P_<void>(y), P_<unsigned char>(arg), P_<float>(partial), P_<const float>(gamma),
                          P_<const float>(beta), P_<const float>(cbias), P_<float>(save_mean), P_<float>(save_invstd),
                          P_<float>(rmean), P_<float>(rvar), P_<long long>(nbt), (float)momentum, (float)eps, relu, M, C, W, slot,
-                         max_ctas, S_(stream)), "bn_forward");
+                         max_ctas, bn_dtype(dtype, "bn_forward"), S_(stream)), "bn_forward");
 }
 static void bn_backward(uint64_t x, uint64_t dy, uint64_t arg, uint64_t dx, uint64_t partial, uint64_t gamma, uint64_t beta,
                         uint64_t save_mean, uint64_t save_invstd, uint64_t dgamma, uint64_t dbeta, int relu, int M, int C, int W,
-                        int slot, int max_ctas, uint64_t stream) {
+                        int slot, int max_ctas, uint64_t stream, int dtype) {
     if (slot < 0) throw std::runtime_error("bn_backward: negative slot");
-    ck(launch_bn_backward(P_<const float>(x), P_<const float>(dy), P_<const unsigned char>(arg), P_<float>(dx), P_<float>(partial),
+    ck(launch_bn_backward(P_<const void>(x), P_<const void>(dy), P_<const unsigned char>(arg), P_<void>(dx), P_<float>(partial),
                           P_<const float>(gamma), P_<const float>(beta), P_<const float>(save_mean), P_<const float>(save_invstd),
-                          P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, S_(stream)), "bn_backward");
+                          P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, bn_dtype(dtype, "bn_backward"),
+                          S_(stream)), "bn_backward");
 }
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
     if ((C % 4) || (H % 2) || (W % 2)) throw std::runtime_error("maxpool2_fwd: needs C % 4 == 0 and even H, W");

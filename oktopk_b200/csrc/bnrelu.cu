@@ -1,5 +1,5 @@
-// Fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool] for channels_last fp32 activations, training mode, forward and
-// backward: one cooperative kernel per pass.
+// Fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool] for channels_last fp32 or bf16 activations, training mode,
+// forward and backward: one cooperative kernel per pass.
 //
 // The CNN zoo of the reference (VGG/models/vgg.py:28-36 and the ResNets) is stacks of  Conv2d -> BatchNorm2d -> ReLU
 // [-> MaxPool2d].  Run through stock framework ops, a VGG-16 step at 16 images per GPU spends a quarter of its time in the
@@ -31,6 +31,15 @@
 // Layout: x is [M, C] row-major (NHWC with M = N*H*W), C a multiple of 4; each thread owns 4 consecutive channels
 // (128-bit accesses) and strides over rows; tiles are contiguous row ranges.  With a pool, a tile is a whole number of
 // image row pairs (rows_per_block % 2W == 0), so no 2x2 window straddles two tiles.
+//
+// Activation type (BnAct): x, y, dy and dx are fp32 (one float4 per access) or bf16 (four bf16 in one 8-byte access).
+// A bf16 load is widened to a float4, which is exact, and from there the arithmetic is the fp32 kernel's, operation for
+// operation: same tiles, partials, combine, running-statistic fma, ReLU mask, pool arg-max and dx formula.  Only the
+// stores of y and dx round to bf16 (to nearest, ties to even).  The bf16 kernel is therefore, bit for bit, the fp32
+// kernel run on x.float() (and dy.float()) with y and dx rounded.  gamma, beta, the conv bias, the running and saved
+// statistics, the partials and dgamma / dbeta stay fp32 either way, as in torch's batch-norm under bf16 autocast.
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 #include "oktopk.cuh"
 
@@ -76,6 +85,25 @@ __host__ __device__ inline BnGeom bn_geom(int M, int C) {
 __device__ __forceinline__ float4 f4_fma(const float4& x, const float4& a, const float4& b) {
     return make_float4(fmaf(x.x, a.x, b.x), fmaf(x.y, a.y, b.y), fmaf(x.z, a.z, b.z), fmaf(x.w, a.w, b.w));
 }
+
+// Four consecutive channels of an activation in storage (V), widened to fp32 for arithmetic and narrowed for a store.
+template <typename T> struct BnAct;
+template <> struct BnAct<float> {
+    using V = float4;
+    static __device__ __forceinline__ float4 wide(const float4& v) { return v; }
+    static __device__ __forceinline__ float4 narrow(const float4& v) { return v; }
+};
+template <> struct BnAct<__nv_bfloat16> {
+    using V = uint2;                          // channels 0, 1 in x (low half first), 2, 3 in y
+    static __device__ __forceinline__ float4 wide(const uint2& v) {   // a bf16 is the high half of its fp32: exact
+        return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u), __uint_as_float(v.y << 16),
+                           __uint_as_float(v.y & 0xffff0000u));
+    }
+    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // round to nearest, ties to even
+        const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
+    }
+};
 
 // one step of a 2x2 max-pool window: first maximum in row-major window order wins, NaN propagates (as at::max_pool2d)
 __device__ __forceinline__ void pool_step(float4& m, uchar4& a, const float4& v, unsigned char k) {
@@ -172,9 +200,10 @@ __device__ __forceinline__ void bn_release(unsigned int* sync, bool last, unsign
 }
 
 // ---------------------------------------------------------------------------------------------- forward
+template <typename T>
 struct BnFwdArgs {
-    const float* x;
-    float* y;                   // [M, C], or with a pool [M/4, C]
+    const T* x;
+    T* y;                       // [M, C], or with a pool [M/4, C]
     unsigned char* arg;         // pool only: arg-max (0..3) per pooled element
     float* partial;             // [nblk][2][C]  (sum, sum of squares)
     const float* gamma; const float* beta; const float* cbias;
@@ -185,15 +214,18 @@ struct BnFwdArgs {
     BnGeom g;
 };
 
-template <bool kPool>
-__global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
+template <bool kPool, typename T>
+__global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p) {
+    using A = BnAct<T>;
+    using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals, then a = gamma/std, b = beta - mean a | pool: held y
     __shared__ float4 s_red[2 * kBnThreads];
     const BnGeom& g = p.g;
     const int tx = threadIdx.x % g.tpr, ty = threadIdx.x / g.tpr;
-    const float4* x4 = reinterpret_cast<const float4*>(p.x);
+    const V* x4 = reinterpret_cast<const V*>(p.x);
+    auto ldx = [&](size_t o) { return A::wide(__ldg(x4 + o)); };
     const size_t st1 = (size_t)g.rpi * g.cv;
-    float4 h[kBnHold];                        // the CTA's first tile (grid <= tiles: every CTA has one)
+    V h[kBnHold];                             // the CTA's first tile (grid <= tiles: every CTA has one), as stored
 
     // (1) partial sums, four or more independent 128-bit loads in flight per thread
     for (int t = blockIdx.x; t < g.nblk; t += gridDim.x) {
@@ -211,17 +243,17 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
                 if (held) {
 #pragma unroll
                     for (int k = 0; k < kBnHold; ++k)
-                        h[k] = r + k * g.rpi < row1 ? __ldg(x4 + (size_t)(r + k * g.rpi) * g.cv + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        h[k] = r + k * g.rpi < row1 ? __ldg(x4 + (size_t)(r + k * g.rpi) * g.cv + col) : V{};
 #pragma unroll
                     for (int k = 0; k < kBnHold; ++k)
-                        if (r + k * g.rpi < row1) acc(h[k]);
+                        if (r + k * g.rpi < row1) acc(A::wide(h[k]));
                 } else {
                     for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
-                        const float4* q0 = x4 + (size_t)r * g.cv + col;
-                        const float4 v0 = __ldg(q0), v1 = __ldg(q0 + st1), v2 = __ldg(q0 + 2 * st1), v3 = __ldg(q0 + 3 * st1);
+                        const size_t o = (size_t)r * g.cv + col;
+                        const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
                         acc(v0); acc(v1); acc(v2); acc(v3);
                     }
-                    for (; r < row1; r += g.rpi) acc(__ldg(x4 + (size_t)r * g.cv + col));
+                    for (; r < row1; r += g.rpi) acc(ldx((size_t)r * g.cv + col));
                 }
             }
             bn_tile_partial(s, q, tx, ty, col, g, s_red, p.partial, t);
@@ -267,7 +299,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
         if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
         return v;
     };
-    float4* y4 = reinterpret_cast<float4*>(p.y);
+    V* y4 = reinterpret_cast<V*>(p.y);
     for (int t = blockIdx.x; t < g.nblk; t += gridDim.x) {
         const bool held = g.hold && t == (int)blockIdx.x;
         const int row0 = t * g.rows_per_block, row1 = min(g.M, row0 + g.rows_per_block);
@@ -279,15 +311,16 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
                 if (held) {
 #pragma unroll
                     for (int k = 0; k < kBnHold; ++k)
-                        if (r + k * g.rpi < row1) y4[(size_t)(r + k * g.rpi) * g.cv + col] = yval(h[k], col);
+                        if (r + k * g.rpi < row1) y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(yval(A::wide(h[k]), col));
                     continue;
                 }
                 for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                     const size_t o = (size_t)r * g.cv + col;
-                    const float4 v0 = __ldg(x4 + o), v1 = __ldg(x4 + o + st1), v2 = __ldg(x4 + o + 2 * st1), v3 = __ldg(x4 + o + 3 * st1);
-                    y4[o] = yval(v0, col); y4[o + st1] = yval(v1, col); y4[o + 2 * st1] = yval(v2, col); y4[o + 3 * st1] = yval(v3, col);
+                    const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
+                    y4[o] = A::narrow(yval(v0, col)); y4[o + st1] = A::narrow(yval(v1, col));
+                    y4[o + 2 * st1] = A::narrow(yval(v2, col)); y4[o + 3 * st1] = A::narrow(yval(v3, col));
                 }
-                for (; r < row1; r += g.rpi) { const size_t o = (size_t)r * g.cv + col; y4[o] = yval(__ldg(x4 + o), col); }
+                for (; r < row1; r += g.rpi) { const size_t o = (size_t)r * g.cv + col; y4[o] = A::narrow(yval(ldx(o), col)); }
             }
         } else {
             // a held tile is staged in shared memory (its windows span threads); the window of pooled pixel pp is the
@@ -297,11 +330,11 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
                 if (ty < g.rpi) {
 #pragma unroll
                     for (int k = 0; k < kBnHold; ++k)
-                        if (row0 + ty + k * g.rpi < row1) sy[(ty + k * g.rpi) * g.cv + tx] = yval(h[k], tx);
+                        if (row0 + ty + k * g.rpi < row1) sy[(ty + k * g.rpi) * g.cv + tx] = yval(A::wide(h[k]), tx);
                 }
                 __syncthreads();
             }
-            auto at = [&](int lr, int c) { return held ? sy[lr * g.cv + c] : yval(__ldg(x4 + (size_t)(row0 + lr) * g.cv + c), c); };
+            auto at = [&](int lr, int c) { return held ? sy[lr * g.cv + c] : yval(ldx((size_t)(row0 + lr) * g.cv + c), c); };
             const int W = g.W, Wo = W >> 1, npool = (row1 - row0) / 4 * g.cv;
             uchar4* a4 = reinterpret_cast<uchar4*>(p.arg);
             for (int i = threadIdx.x; i < npool; i += kBnThreads) {
@@ -314,7 +347,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
                 pool_step(m, a, v2, 2);
                 pool_step(m, a, v3, 3);
                 const size_t o = (size_t)(row0 / 4 + pp) * g.cv + c;
-                y4[o] = m;
+                y4[o] = A::narrow(m);
                 a4[o] = a;
             }
         }
@@ -322,11 +355,12 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs p) {
 }
 
 // ---------------------------------------------------------------------------------------------- backward
+template <typename T>
 struct BnBwdArgs {
-    const float* x;
-    const float* dy;            // [M, C], or with a pool the pooled gradient [M/4, C]
+    const T* x;
+    const T* dy;                // [M, C], or with a pool the pooled gradient [M/4, C]
     const unsigned char* arg;   // pool only: the forward's arg-max
-    float* dx;
+    T* dx;
     float* partial;             // [nblk][2][C]  (dbeta, dgamma)
     const float* gamma; const float* beta; const float* save_mean; const float* save_invstd;
     float* dgamma; float* dbeta;
@@ -335,23 +369,26 @@ struct BnBwdArgs {
     BnGeom g;
 };
 
-template <bool kPool>
-__global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs p) {
+template <bool kPool, typename T>
+__global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p) {
+    using A = BnAct<T>;
+    using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals
     __shared__ float4 s_red[2 * kBnThreads];
     const BnGeom& g = p.g;
     const int tx = threadIdx.x % g.tpr, ty = threadIdx.x / g.tpr;
-    const float4* x4 = reinterpret_cast<const float4*>(p.x);
-    const float4* d4 = reinterpret_cast<const float4*>(p.dy);
+    const V* x4 = reinterpret_cast<const V*>(p.x);
+    const V* d4 = reinterpret_cast<const V*>(p.dy);
     const uchar4* a4 = reinterpret_cast<const uchar4*>(p.arg);
+    auto ldx = [&](size_t o) { return A::wide(__ldg(x4 + o)); };
     const size_t st1 = (size_t)g.rpi * g.cv;
     // the gradient reaching the batch-norm output at row r: dy, or the pooled dy at the window's arg-max and 0 elsewhere
     auto grad = [&](int row0, int r, int col) -> float4 {
-        if (!kPool) return __ldg(d4 + (size_t)r * g.cv + col);
+        if (!kPool) return A::wide(__ldg(d4 + (size_t)r * g.cv + col));
         const int lr = r - row0, hl = lr / g.W, w = lr - hl * g.W;
         const size_t o = (size_t)(row0 / 4 + (hl >> 1) * (g.W >> 1) + (w >> 1)) * g.cv + col;
         const int k = (hl & 1) * 2 + (w & 1);
-        const float4 d = __ldg(d4 + o);
+        const float4 d = A::wide(__ldg(d4 + o));
         const uchar4 a = __ldg(a4 + o);
         return make_float4(a.x == k ? d.x : 0.f, a.y == k ? d.y : 0.f, a.z == k ? d.z : 0.f, a.w == k ? d.w : 0.f);
     };
@@ -380,7 +417,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs p) {
         return make_float4((v.x - k.mean.x) * k.istd.x, (v.y - k.mean.y) * k.istd.y, (v.z - k.mean.z) * k.istd.z,
                            (v.w - k.mean.w) * k.istd.w);
     };
-    float4 hx[kBnHold], hd[kBnHold];          // the CTA's first tile: x and the incoming gradient
+    V hx[kBnHold];                            // the CTA's first tile: x as stored
+    float4 hd[kBnHold];                       // and the incoming gradient (with a pool: expanded at the arg-max)
 
     // (1) partials, eight or more independent 128-bit loads in flight per thread
     for (int t = blockIdx.x; t < g.nblk; t += gridDim.x) {
@@ -402,21 +440,21 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs p) {
 #pragma unroll
                     for (int j = 0; j < kBnHold; ++j) {
                         const int rr = r + j * g.rpi;
-                        hx[j] = rr < row1 ? __ldg(x4 + (size_t)rr * g.cv + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        hx[j] = rr < row1 ? __ldg(x4 + (size_t)rr * g.cv + col) : V{};
                         hd[j] = rr < row1 ? grad(row0, rr, col) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
 #pragma unroll
                     for (int j = 0; j < kBnHold; ++j)
-                        if (r + j * g.rpi < row1) acc(hx[j], hd[j]);
+                        if (r + j * g.rpi < row1) acc(A::wide(hx[j]), hd[j]);
                 } else {
                     for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                         const size_t o = (size_t)r * g.cv + col;
-                        const float4 v0 = __ldg(x4 + o), v1 = __ldg(x4 + o + st1), v2 = __ldg(x4 + o + 2 * st1), v3 = __ldg(x4 + o + 3 * st1);
+                        const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
                         const float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
                                      e3 = grad(row0, r + 3 * g.rpi, col);
                         acc(v0, e0); acc(v1, e1); acc(v2, e2); acc(v3, e3);
                     }
-                    for (; r < row1; r += g.rpi) acc(__ldg(x4 + (size_t)r * g.cv + col), grad(row0, r, col));
+                    for (; r < row1; r += g.rpi) acc(ldx((size_t)r * g.cv + col), grad(row0, r, col));
                 }
             }
             bn_tile_partial(sb, sg, tx, ty, col, g, s_red, p.partial, t);
@@ -446,28 +484,28 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs p) {
             const double M = (double)g.M;
             const float4 mb = make_float4((float)(db.x / M), (float)(db.y / M), (float)(db.z / M), (float)(db.w / M));
             const float4 mg = make_float4((float)(dg.x / M), (float)(dg.y / M), (float)(dg.z / M), (float)(dg.w / M));
-            float4* o4 = reinterpret_cast<float4*>(p.dx);
+            V* o4 = reinterpret_cast<V*>(p.dx);
             auto out = [&](size_t off, const float4& v, float4 d) {
                 const float4 xh = xhat(k, v);
                 mask(k, v, d);
-                o4[off] = make_float4(k.a.x * (d.x - mb.x - xh.x * mg.x), k.a.y * (d.y - mb.y - xh.y * mg.y),
-                                      k.a.z * (d.z - mb.z - xh.z * mg.z), k.a.w * (d.w - mb.w - xh.w * mg.w));
+                o4[off] = A::narrow(make_float4(k.a.x * (d.x - mb.x - xh.x * mg.x), k.a.y * (d.y - mb.y - xh.y * mg.y),
+                                                k.a.z * (d.z - mb.z - xh.z * mg.z), k.a.w * (d.w - mb.w - xh.w * mg.w)));
             };
             int r = row0 + ty;
             if (held) {
 #pragma unroll
                 for (int j = 0; j < kBnHold; ++j)
-                    if (r + j * g.rpi < row1) out((size_t)(r + j * g.rpi) * g.cv + col, hx[j], hd[j]);
+                    if (r + j * g.rpi < row1) out((size_t)(r + j * g.rpi) * g.cv + col, A::wide(hx[j]), hd[j]);
                 continue;
             }
             for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                 const size_t o = (size_t)r * g.cv + col;
-                const float4 v0 = __ldg(x4 + o), v1 = __ldg(x4 + o + st1), v2 = __ldg(x4 + o + 2 * st1), v3 = __ldg(x4 + o + 3 * st1);
+                const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
                 const float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
                              e3 = grad(row0, r + 3 * g.rpi, col);
                 out(o, v0, e0); out(o + st1, v1, e1); out(o + 2 * st1, v2, e2); out(o + 3 * st1, v3, e3);
             }
-            for (; r < row1; r += g.rpi) out((size_t)r * g.cv + col, __ldg(x4 + (size_t)r * g.cv + col), grad(row0, r, col));
+            for (; r < row1; r += g.rpi) out((size_t)r * g.cv + col, ldx((size_t)r * g.cv + col), grad(row0, r, col));
         }
     }
 }
@@ -515,27 +553,63 @@ static cudaError_t bn_prepare(BnGeom& g, unsigned int*& sync, int M, int C, int 
     return sync == nullptr ? cudaErrorInvalidDevice : cudaSuccess;
 }
 
-cudaError_t launch_bn_forward(const float* x, float* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
-                              const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
-                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas,
-                              cudaStream_t stream) {
-    BnFwdArgs p{x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt, momentum, eps, relu, nullptr, {}};
+template <typename T>
+static cudaError_t bn_forward_t(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma,
+                                const float* beta, const float* cbias, float* save_mean, float* save_invstd, float* rmean,
+                                float* rvar, long long* nbt, float momentum, float eps, int relu, int M, int C, int W, int slot,
+                                int max_ctas, cudaStream_t stream) {
+    BnFwdArgs<T> p{static_cast<const T*>(x), static_cast<T*>(y), arg, partial, gamma, beta, cbias, save_mean, save_invstd,
+                   rmean, rvar, nbt, momentum, eps, relu, nullptr, {}};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
     size_t smem = sizeof(float) * 2 * C;
     if (W > 0 && p.g.hold) smem += sizeof(float4) * p.g.rows_per_block * p.g.cv;
-    return W > 0 ? bn_launch(bn_fwd_kernel<true>, p, smem, max_ctas, stream) : bn_launch(bn_fwd_kernel<false>, p, smem, max_ctas, stream);
+    return W > 0 ? bn_launch(bn_fwd_kernel<true, T>, p, smem, max_ctas, stream)
+                 : bn_launch(bn_fwd_kernel<false, T>, p, smem, max_ctas, stream);
 }
 
-cudaError_t launch_bn_backward(const float* x, const float* dy, const unsigned char* arg, float* dx, float* partial,
-                               const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
-                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas,
-                               cudaStream_t stream) {
-    BnBwdArgs p{x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu, nullptr, {}};
+template <typename T>
+static cudaError_t bn_backward_t(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
+                                 const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                                 float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas,
+                                 cudaStream_t stream) {
+    BnBwdArgs<T> p{static_cast<const T*>(x), static_cast<const T*>(dy), arg, static_cast<T*>(dx), partial, gamma, beta,
+                   save_mean, save_invstd, dgamma, dbeta, relu, nullptr, {}};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
     const size_t smem = sizeof(float) * 2 * C;
-    return W > 0 ? bn_launch(bn_bwd_kernel<true>, p, smem, max_ctas, stream) : bn_launch(bn_bwd_kernel<false>, p, smem, max_ctas, stream);
+    return W > 0 ? bn_launch(bn_bwd_kernel<true, T>, p, smem, max_ctas, stream)
+                 : bn_launch(bn_bwd_kernel<false, T>, p, smem, max_ctas, stream);
+}
+
+cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
+                              const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
+                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                              cudaStream_t stream) {
+    switch (dtype) {
+        case BnDtype::kF32:
+            return bn_forward_t<float>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
+                                       momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+        case BnDtype::kBF16:
+            return bn_forward_t<__nv_bfloat16>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar,
+                                               nbt, momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
+                               const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
+                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                               cudaStream_t stream) {
+    switch (dtype) {
+        case BnDtype::kF32:
+            return bn_backward_t<float>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
+                                        M, C, W, slot, max_ctas, stream);
+        case BnDtype::kBF16:
+            return bn_backward_t<__nv_bfloat16>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta,
+                                                relu, M, C, W, slot, max_ctas, stream);
+    }
+    return cudaErrorInvalidValue;
 }
 
 }  // namespace okt

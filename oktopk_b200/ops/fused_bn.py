@@ -1,4 +1,4 @@
-"""Fused (conv-bias +) BatchNorm2d + ReLU [+ 2x2 max-pool] for channels_last fp32 activations (``csrc/bnrelu.cu``).
+"""Fused (conv-bias +) BatchNorm2d + ReLU [+ 2x2 max-pool] for channels_last fp32 or bf16 activations (``csrc/bnrelu.cu``).
 
 ``bias_bn_relu(x, bn, conv_bias, relu=True, pool=None)`` replaces ``pool(relu(bn(x + conv_bias)))`` in training mode on
 CUDA with one kernel forward and one backward instead of the seven stock ones (bias add, batch-norm, clamp, counter
@@ -9,8 +9,14 @@ never stored.  The convolution is then called WITHOUT its bias: a bias in front 
 identically zero (returned as ``None``; autograd's own reduction over ``dy`` returns rounding noise for it).
 Parameters, buffers and ``state_dict`` keys are the stock modules' ones.
 
-Falls back to the stock ops whenever the fast path does not apply (CPU, eval mode, non-fp32, not channels_last,
-channels not a multiple of 4, cumulative-average momentum).  A pool that cannot be folded in (not 2x2 / stride 2, odd
+bf16: under ``torch.autocast("cuda", torch.bfloat16)`` (or with bf16 activations and autocast off) the convolution
+returns bf16 and the kernels' bf16 instantiation runs.  As torch's batch-norm does under autocast, it takes bf16
+activations with fp32 parameters and statistics: ``y`` and ``dx`` are bf16; ``dgamma``, ``dbeta`` and the running
+statistics fp32.  Its results are bit for bit those of the fp32 kernels run on ``x.float()`` (and ``dy.float()``), with
+``y`` and ``dx`` rounded to bf16.  fp16 autocast keeps the stock ops.
+
+Falls back to the stock ops whenever the fast path does not apply (CPU, eval mode, activations neither fp32 nor bf16,
+fp16 autocast, parameters not fp32, not channels_last, channels not a multiple of 4, cumulative-average momentum).  A pool that cannot be folded in (not 2x2 / stride 2, odd
 height or width, or batch-norm tiles that are not whole pairs of image rows) runs after the fused kernel on its own.
 """
 from __future__ import annotations
@@ -29,6 +35,9 @@ MAX_CTAS = 0
 
 _SLOTS = itertools.count()
 
+# the kernels' activation type argument (csrc/bindings.cpp bn_forward / bn_backward)
+_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1}
+
 
 def _sync_slot(bn: torch.nn.BatchNorm2d) -> int:
     """The grid hand-off counters of ``bn``'s kernels (csrc/bnrelu.cu ``g_bn_sync``): one slot per module, so that the
@@ -39,11 +48,20 @@ def _sync_slot(bn: torch.nn.BatchNorm2d) -> int:
     return s
 
 
+def _dtype_ok(x: torch.Tensor) -> bool:
+    """fp32 or bf16 activations, with autocast off or in bf16 (fp16 autocast keeps the stock ops)."""
+    return (x.dtype in (torch.float32, torch.bfloat16)
+            and (not torch.is_autocast_enabled() or torch.get_autocast_dtype("cuda") == torch.bfloat16))
+
+
+def _bn_params_fp32(bn: torch.nn.BatchNorm2d) -> bool:
+    return all(t is None or t.dtype == torch.float32 for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+
+
 def _fast_path_ok(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
-    return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and bn.training and bn.affine
-            and bn.momentum is not None and x.size(1) % 4 == 0
-            and x.is_contiguous(memory_format=torch.channels_last) and ext.available()
-            and not torch.is_autocast_enabled())
+    return (x.is_cuda and _dtype_ok(x) and x.dim() == 4 and bn.training and bn.affine
+            and bn.momentum is not None and x.size(1) % 4 == 0 and _bn_params_fp32(bn)
+            and x.is_contiguous(memory_format=torch.channels_last) and ext.available())
 
 
 def _is_2x2(pool: torch.nn.MaxPool2d) -> bool:
@@ -66,6 +84,7 @@ class _BiasBNReLUPool(torch.autograd.Function):
         C = ext.require()
         N, Ch, H, W = x.shape
         M = N * H * W
+        dtype = _DTYPE_FLAG[x.dtype]
         if pool:
             y = torch.empty((N, Ch, H // 2, W // 2), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
             arg = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)
@@ -80,9 +99,9 @@ class _BiasBNReLUPool(torch.autograd.Function):
                      beta.data_ptr(), 0 if cbias is None else cbias.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch,
                      0 if rmean is None else rmean.data_ptr(), 0 if rvar is None else rvar.data_ptr(),
                      0 if nbt is None else nbt.data_ptr(), float(momentum), float(eps), int(relu), M, Ch,
-                     W if pool else 0, slot, MAX_CTAS, s)
+                     W if pool else 0, slot, MAX_CTAS, s, dtype)
         ctx.save_for_backward(x, gamma, beta, stats, arg)
-        ctx.relu, ctx.pool, ctx.slot = bool(relu), bool(pool), slot
+        ctx.relu, ctx.pool, ctx.slot, ctx.dtype = bool(relu), bool(pool), slot, dtype
         return y
 
     @staticmethod
@@ -91,6 +110,7 @@ class _BiasBNReLUPool(torch.autograd.Function):
         x, gamma, beta, stats, arg = ctx.saved_tensors
         N, Ch, H, W = x.shape
         M = N * H * W
+        assert dy.dtype == x.dtype, (dy.dtype, x.dtype)          # y was allocated in x.dtype
         if not dy.is_contiguous(memory_format=torch.channels_last):
             dy = dy.contiguous(memory_format=torch.channels_last)
         dx = torch.empty_like(x)
@@ -100,7 +120,8 @@ class _BiasBNReLUPool(torch.autograd.Function):
         s = torch.cuda.current_stream().cuda_stream
         C.bn_backward(x.data_ptr(), dy.data_ptr(), 0 if arg is None else arg.data_ptr(), dx.data_ptr(), partial.data_ptr(),
                       gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch, dgb.data_ptr(),
-                      dgb.data_ptr() + 4 * Ch, int(ctx.relu), M, Ch, W if ctx.pool else 0, ctx.slot, MAX_CTAS, s)
+                      dgb.data_ptr() + 4 * Ch, int(ctx.relu), M, Ch, W if ctx.pool else 0, ctx.slot, MAX_CTAS, s,
+                      ctx.dtype)
         # conv bias: the loss does not depend on it (see module docstring) -> no gradient
         return dx, dgb[:Ch], dgb[Ch:], None, None, None, None, None, None, None, None, None
 
@@ -108,7 +129,7 @@ class _BiasBNReLUPool(torch.autograd.Function):
 def bias_bn_relu(x: torch.Tensor, bn: torch.nn.BatchNorm2d, conv_bias: Optional[torch.Tensor] = None,
                  relu: bool = True, pool: Optional[torch.nn.MaxPool2d] = None) -> torch.Tensor:
     """``pool(relu(bn(x + conv_bias)))`` (``relu=False``: without the ReLU; ``pool=None``: without the pool)."""
-    if _fast_path_ok(x, bn):
+    if _fast_path_ok(x, bn) and (conv_bias is None or conv_bias.dtype == torch.float32):
         track = bn.track_running_stats and bn.running_mean is not None
         fuse = pool is not None and _pool_fusable(x, pool)
         y = _BiasBNReLUPool.apply(x, bn.weight, bn.bias, conv_bias, bn.running_mean if track else None,
@@ -140,10 +161,10 @@ def conv_bn_relu(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2
 
 
 def _fast_path_ok_pre(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d) -> bool:
-    return (x.is_cuda and x.dtype == torch.float32 and bn.training and bn.affine and bn.momentum is not None
+    return (x.is_cuda and _dtype_ok(x) and bn.training and bn.affine and bn.momentum is not None
             and conv.out_channels % 4 == 0 and conv.padding_mode == "zeros" and ext.available()
-            and x.is_contiguous(memory_format=torch.channels_last) and not torch.is_autocast_enabled()
-            and not isinstance(conv.padding, str))
+            and (conv.bias is None or conv.bias.dtype == torch.float32) and _bn_params_fp32(bn)
+            and x.is_contiguous(memory_format=torch.channels_last) and not isinstance(conv.padding, str))
 
 
 class _MaxPool2x2(torch.autograd.Function):
