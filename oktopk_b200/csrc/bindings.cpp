@@ -467,19 +467,18 @@ static void kth_abs(uint64_t x, int n, int k, uint64_t st, uint64_t out, int gri
     ck(launch_kth_abs(P_<float>(x), n, k, P_<OktState>(st), P_<float>(out), grid, S_(stream)), "kth_abs launch");
 }
 
-static void fused_sgd(uint64_t p, uint64_t g, uint64_t mom, int n, double lr, double momentum, double dampening,
-                      double wd, int nesterov, int first, int zero_grad, double grad_scale, uint64_t stream,
-                      uint64_t lr_ptr, uint64_t fault_ptr) {
-    ck(launch_fused_sgd(P_<float>(p), P_<float>(g), P_<float>(mom), n, (float)lr, (float)momentum, (float)dampening,
-                        (float)wd, nesterov, first, zero_grad, (float)grad_scale, P_<float>(lr_ptr), P_<int>(fault_ptr),
-                        S_(stream)),
+static void fused_sgd(uint64_t p, uint64_t g, uint64_t mom, int n, double momentum, double dampening, double wd,
+                      int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("fused_sgd: scal_ptr must point at the group's device scalars");
+    ck(launch_fused_sgd(P_<float>(p), P_<float>(g), P_<float>(mom), n, (float)momentum, (float)dampening, (float)wd,
+                        nesterov, first, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
        "fused_sgd");
 }
-static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double lr, double b1, double b2,
-                            double eps, double wd, int zero_grad, uint64_t stream, uint64_t lr_ptr, uint64_t fault_ptr) {
-    ck(launch_fused_bert_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, (float)lr, (float)b1,
-                              (float)b2, (float)eps, (float)wd, zero_grad, P_<float>(lr_ptr), P_<int>(fault_ptr),
-                              S_(stream)),
+static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double b1, double b2, double eps,
+                            double wd, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("fused_bert_adam: scal_ptr must point at the group's device scalars");
+    ck(launch_fused_bert_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, (float)b1, (float)b2,
+                              (float)eps, (float)wd, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
        "fused_bert_adam");
 }
 static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double beta1, double beta2, double eps,
@@ -572,12 +571,12 @@ PYBIND11_MODULE(_C, m) {
         ck(cudaMemsetAsync(&P_<OktState>(st)->fault, 0, sizeof(int), S_(stream)), "clear_fault");
     });
     m.def("kth_abs", &kth_abs);
-    m.def("fused_sgd", &fused_sgd, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("n"), py::arg("lr"),
-          py::arg("momentum"), py::arg("dampening"), py::arg("wd"), py::arg("nesterov"), py::arg("first"),
-          py::arg("zero_grad"), py::arg("grad_scale"), py::arg("stream"), py::arg("lr_ptr") = 0, py::arg("fault_ptr") = 0);
+    m.def("fused_sgd", &fused_sgd, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("n"), py::arg("momentum"),
+          py::arg("dampening"), py::arg("wd"), py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"),
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
     m.def("fused_bert_adam", &fused_bert_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
-          py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"),
-          py::arg("stream"), py::arg("lr_ptr") = 0, py::arg("fault_ptr") = 0);
+          py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"), py::arg("stream"),
+          py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
     m.def("fused_adam", &fused_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("decoupled"), py::arg("zero_grad"),
           py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0);

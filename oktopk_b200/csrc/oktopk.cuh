@@ -270,12 +270,13 @@ int gtopk_max_coop_grid(int device);
 int gather_max_coop_grid(int device);
 cudaError_t launch_dense_allreduce(const DenseParams& p, int grid, cudaStream_t stream);
 cudaError_t launch_kth_abs(const float* x, int n, int k, OktState* st, float* out_thr, int grid, cudaStream_t stream);
-cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float lr, float momentum, float dampening,
-                             float weight_decay, int nesterov, int first_step, int zero_grad, float grad_scale,
-                             const float* lr_ptr, const int* fault, cudaStream_t stream);
-cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float lr, float b1, float b2,
-                                   float eps, float weight_decay, int zero_grad, const float* lr_ptr,
-                                   const int* fault, cudaStream_t stream);
+// fused optimizer updates: scal -> the step's scalars in device memory ({lr} for SGD and BertAdam)
+cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
+                             int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
+                             cudaStream_t stream);
+cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
+                                   float weight_decay, int zero_grad, const float* scal, const int* fault,
+                                   cudaStream_t stream);
 // torch.optim.Adam / AdamW update; scal -> {1 - lr*wd, -lr / (1 - beta1^t), sqrt(1 - beta2^t)} of this step
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,

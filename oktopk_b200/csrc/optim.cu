@@ -11,92 +11,98 @@ namespace okt {
 
 constexpr int kOptThreads = 256;
 
-__global__ void __launch_bounds__(kOptThreads) fused_sgd_kernel(float* __restrict__ p, float* __restrict__ g,
-                                                                 float* __restrict__ mom, int n, float lr,
-                                                                 float momentum, float dampening, float wd,
-                                                                 int nesterov, int first, int zero_grad,
-                                                                 float grad_scale, const float* __restrict__ lr_ptr,
-                                                                 const int* __restrict__ fault) {
-    // a bounded cross-GPU wait timed out inside the reduction of this bucket: the gradient is partial, do NOT apply it
-    // (the host sees the mirrored fault flag at its next step() and re-synchronises the replicas)
+// The pass all three update kernels share.  A bounded cross-GPU wait timed out inside the reduction of this bucket: the
+// gradient is partial, do NOT apply it (the host sees the mirrored fault flag at its next step() and re-synchronises the
+// replicas).  Otherwise the kScal per-step scalars are read from device memory (the launch is CUDA-graph replayable)
+// and upd(s, p, g, m, v) updates every element; m and v are its first and, with kState == 2, second state element,
+// loaded when `load` (else 0) and written back when `store`.  Only the non-zero gradient lines are zeroed: the
+// reduced gradient is sparse, ~k/n of the lines are dirty.
+template <int kScal, int kState, typename Upd>
+__device__ __forceinline__ void update_pass(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
+                                            float* __restrict__ v, int n, bool load, bool store, int zero_grad,
+                                            const float* __restrict__ scal, const int* __restrict__ fault, Upd upd) {
     if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
-    if (lr_ptr) lr = *lr_ptr;            // device-resident learning rate: the launch is CUDA-graph replayable
-    const int n4 = n >> 2;
-    float4* p4 = reinterpret_cast<float4*>(p);
-    float4* g4 = reinterpret_cast<float4*>(g);
-    float4* m4 = reinterpret_cast<float4*>(mom);
-    const float damp = first ? 0.f : dampening;       // torch: the first step copies d_p into the buffer
-    auto upd = [&](float& pw, float gw, float& mw) {
-        float d = gw * grad_scale + wd * pw;
-        if (momentum != 0.f) {
-            mw = first ? d : (momentum * mw + (1.f - damp) * d);
-            d = nesterov ? (d + momentum * mw) : mw;
-        }
-        pw -= lr * d;
-    };
-    for (int v = blockIdx.x * kOptThreads + threadIdx.x; v < n4; v += gridDim.x * kOptThreads) {
-        float4 pw = p4[v];
-        float4 gw = ld_stream_f4(g4 + v);
-        float4 mw = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (momentum != 0.f && !first) mw = m4[v];
-        upd(pw.x, gw.x, mw.x); upd(pw.y, gw.y, mw.y); upd(pw.z, gw.z, mw.z); upd(pw.w, gw.w, mw.w);
-        p4[v] = pw;
-        if (momentum != 0.f) m4[v] = mw;
-        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f))
-            g4[v] = make_float4(0.f, 0.f, 0.f, 0.f);    // sparse result: only ~k/n of the lines are dirty
-    }
-    if (blockIdx.x == 0)
-        for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
-            float pw = p[i], gw = g[i], mw = (momentum != 0.f && !first) ? mom[i] : 0.f;
-            upd(pw, gw, mw);
-            p[i] = pw;
-            if (momentum != 0.f) mom[i] = mw;
-            if (zero_grad) g[i] = 0.f;
-        }
-}
-
-__global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __restrict__ p, float* __restrict__ g,
-                                                                       float* __restrict__ m, float* __restrict__ v,
-                                                                       int n, float lr, float b1, float b2, float eps,
-                                                                       float wd, int zero_grad,
-                                                                       const float* __restrict__ lr_ptr,
-                                                                       const int* __restrict__ fault) {
-    if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
-    if (lr_ptr) lr = *lr_ptr;
+    float s[kScal];
+#pragma unroll
+    for (int j = 0; j < kScal; ++j) s[j] = scal[j];
     const int n4 = n >> 2;
     float4* p4 = reinterpret_cast<float4*>(p);
     float4* g4 = reinterpret_cast<float4*>(g);
     float4* m4 = reinterpret_cast<float4*>(m);
     float4* v4 = reinterpret_cast<float4*>(v);
-    auto upd = [&](float& pw, float gw, float& mw, float& vw) {
-        mw = b1 * mw + (1.f - b1) * gw;
-        vw = b2 * vw + (1.f - b2) * gw * gw;
-        float u = mw / (sqrtf(vw) + eps);
-        if (wd > 0.f) u += wd * pw;
-        pw -= lr * u;
-    };
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
-        float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = m4[i], vw = v4[i];
-        upd(pw.x, gw.x, mw.x, vw.x); upd(pw.y, gw.y, mw.y, vw.y);
-        upd(pw.z, gw.z, mw.z, vw.z); upd(pw.w, gw.w, mw.w, vw.w);
-        p4[i] = pw; m4[i] = mw; v4[i] = vw;
-        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f))
-            g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = zero, vw = zero;
+        if (load) {
+            mw = m4[i];
+            if (kState == 2) vw = v4[i];
+        }
+        upd(s, pw.x, gw.x, mw.x, vw.x); upd(s, pw.y, gw.y, mw.y, vw.y);
+        upd(s, pw.z, gw.z, mw.z, vw.z); upd(s, pw.w, gw.w, mw.w, vw.w);
+        p4[i] = pw;
+        if (store) {
+            m4[i] = mw;
+            if (kState == 2) v4[i] = vw;
+        }
+        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
     }
     if (blockIdx.x == 0)
         for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
-            float pw = p[i], gw = g[i], mw = m[i], vw = v[i];
-            upd(pw, gw, mw, vw);
-            p[i] = pw; m[i] = mw; v[i] = vw;
+            float pw = p[i], gw = g[i], mw = 0.f, vw = 0.f;
+            if (load) {
+                mw = m[i];
+                if (kState == 2) vw = v[i];
+            }
+            upd(s, pw, gw, mw, vw);
+            p[i] = pw;
+            if (store) {
+                m[i] = mw;
+                if (kState == 2) v[i] = vw;
+            }
             if (zero_grad) g[i] = 0.f;
         }
 }
 
+// scal -> {lr}
+__global__ void __launch_bounds__(kOptThreads) fused_sgd_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                                 float* __restrict__ mom, int n, float momentum,
+                                                                 float dampening, float wd, int nesterov, int first,
+                                                                 int zero_grad, const float* __restrict__ scal,
+                                                                 const int* __restrict__ fault) {
+    const float damp = first ? 0.f : dampening;       // torch: the first step copies d_p into the buffer
+    // every rounding spelled out, so that where nvcc contracts into an fma cannot change the result
+    update_pass<1, 1>(p, g, mom, nullptr, n, momentum != 0.f && !first, momentum != 0.f, zero_grad, scal, fault,
+                      [=](const float* s, float& pw, float gw, float& mw, float&) {
+                          float d = __fmaf_rn(wd, pw, gw);
+                          if (momentum != 0.f) {
+                              mw = first ? d : __fmaf_rn(1.f - damp, d, __fmul_rn(momentum, mw));
+                              d = nesterov ? __fmaf_rn(momentum, mw, d) : mw;
+                          }
+                          pw = __fmaf_rn(-s[0], d, pw);
+                      });
+}
+
+// scal -> {scheduled lr}
+__global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                                       float* __restrict__ m, float* __restrict__ v,
+                                                                       int n, float b1, float b2, float eps, float wd,
+                                                                       int zero_grad, const float* __restrict__ scal,
+                                                                       const int* __restrict__ fault) {
+    update_pass<1, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault,
+                      [=](const float* s, float& pw, float gw, float& mw, float& vw) {
+                          mw = b1 * mw + (1.f - b1) * gw;
+                          vw = b2 * vw + (1.f - b2) * gw * gw;
+                          float u = mw / (sqrtf(vw) + eps);
+                          if (wd > 0.f) u += wd * pw;
+                          pw -= s[0] * u;
+                      });
+}
+
 // torch.optim.Adam / AdamW (foreach, non-capturable branch), one rounding per op.  The per-step scalars (decay = 1 - lr*wd,
-// step_size = -lr / (1 - beta1^t), bc2_sqrt = sqrt(1 - beta2^t)) are computed on the host in double and read from device
-// memory, so that a captured CUDA graph picks up the schedule and the bias correction of every replay.
+// step_size = -lr / (1 - beta1^t), bc2_sqrt = sqrt(1 - beta2^t)) are computed on the host in double, so that a captured
+// CUDA graph picks up the schedule and the bias correction of every replay.
 // decoupled: AdamW (p *= 1 - lr*wd) instead of L2 (g += wd*p).  w = 1 - beta1 is the weight of torch's lerp, whose
-// formula depends on whether the weight is below 0.5.  (47 registers, 5 CTAs per SM: capping at 32 for 8 CTAs spills
+// formula depends on whether the weight is below 0.5.  (48 registers, 5 CTAs per SM: capping at 32 for 8 CTAs spills
 // around the IEEE division's slow path.)
 __global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restrict__ p, float* __restrict__ g,
                                                                   float* __restrict__ m, float* __restrict__ v, int n,
@@ -104,39 +110,19 @@ __global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restri
                                                                   int decoupled, int zero_grad,
                                                                   const float* __restrict__ scal,
                                                                   const int* __restrict__ fault) {
-    if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
-    const float decay = scal[0], step_size = scal[1], bc2_sqrt = scal[2];
     const bool small_w = fabsf(w) < 0.5f;
     const float lw = small_w ? w : 1.f - w;
-    const int n4 = n >> 2;
-    float4* p4 = reinterpret_cast<float4*>(p);
-    float4* g4 = reinterpret_cast<float4*>(g);
-    float4* m4 = reinterpret_cast<float4*>(m);
-    float4* v4 = reinterpret_cast<float4*>(v);
-    auto upd = [&](float& pw, float gw, float& mw, float& vw) {
-        if (decoupled) pw = pw * decay;                  // decay == 1 exactly when wd == 0
-        else if (wd != 0.f) gw = gw + wd * pw;
-        mw = small_w ? mw + lw * (gw - mw) : gw - (gw - mw) * lw;
-        vw = vw * b2;
-        vw = vw + omb2 * gw * gw;
-        const float d = sqrtf(vw) / bc2_sqrt + eps;
-        pw = pw + (step_size * mw) / d;
-    };
-    for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
-        float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = m4[i], vw = v4[i];
-        upd(pw.x, gw.x, mw.x, vw.x); upd(pw.y, gw.y, mw.y, vw.y);
-        upd(pw.z, gw.z, mw.z, vw.z); upd(pw.w, gw.w, mw.w, vw.w);
-        p4[i] = pw; m4[i] = mw; v4[i] = vw;
-        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f))
-            g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (blockIdx.x == 0)
-        for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
-            float pw = p[i], gw = g[i], mw = m[i], vw = v[i];
-            upd(pw, gw, mw, vw);
-            p[i] = pw; m[i] = mw; v[i] = vw;
-            if (zero_grad) g[i] = 0.f;
-        }
+    update_pass<3, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault,
+                      [=](const float* s, float& pw, float gw, float& mw, float& vw) {
+                          const float decay = s[0], step_size = s[1], bc2_sqrt = s[2];
+                          if (decoupled) pw = pw * decay;                  // decay == 1 exactly when wd == 0
+                          else if (wd != 0.f) gw = gw + wd * pw;
+                          mw = small_w ? mw + lw * (gw - mw) : gw - (gw - mw) * lw;
+                          vw = vw * b2;
+                          vw = vw + omb2 * gw * gw;
+                          const float d = sqrtf(vw) / bc2_sqrt + eps;
+                          pw = pw + (step_size * mw) / d;
+                      });
 }
 
 // momentum correction (VGG/distributed_optimizer.py:81-88): buf = m*buf + g ; g = buf
@@ -182,19 +168,19 @@ static inline int opt_grid(int n) {
     return g;
 }
 
-cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float lr, float momentum, float dampening,
-                             float weight_decay, int nesterov, int first_step, int zero_grad, float grad_scale,
-                             const float* lr_ptr, const int* fault, cudaStream_t stream) {
-    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, lr, momentum, dampening, weight_decay,
-                                                             nesterov, first_step, zero_grad, grad_scale, lr_ptr, fault);
+cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
+                             int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
+                             cudaStream_t stream) {
+    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, momentum, dampening, weight_decay, nesterov,
+                                                             first_step, zero_grad, scal, fault);
     return cudaGetLastError();
 }
 
-cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float lr, float b1, float b2,
-                                   float eps, float weight_decay, int zero_grad, const float* lr_ptr,
-                                   const int* fault, cudaStream_t stream) {
-    fused_bert_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, lr, b1, b2, eps, weight_decay,
-                                                                   zero_grad, lr_ptr, fault);
+cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
+                                   float weight_decay, int zero_grad, const float* scal, const int* fault,
+                                   cudaStream_t stream) {
+    fused_bert_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, b1, b2, eps, weight_decay, zero_grad,
+                                                                   scal, fault);
     return cudaGetLastError();
 }
 

@@ -91,11 +91,10 @@ class _BucketedComm:
         # call starts: the fused update clears the few entries the reduction wrote (zero_grad=1 after EVERY step, dense
         # warm-up steps included), and CudaBucketEngine.reset_sparse_state / load_state_dict clear it after a fault or a
         # checkpoint load.
-        if getattr(self, "_okt_adam", False):     # the fused Adam kernel works on flat fp32 CUDA buckets only
-            self._okt_adam = ext.available() and all(b.flat_param is not None and b.grad.is_cuda for b in self._buckets)
-        fused_update = (bool(getattr(self, "_okt_is_sgd", False)) or isinstance(self, BertAdam)
-                        or bool(getattr(self, "_okt_adam", False)))
-        self._direct = (self._land and fused_update and allreducer.compressor.name == "oktopk"
+        if self._update is _AdamUpdate:           # the fused Adam kernel works on flat fp32 CUDA buckets only
+            if not (ext.available() and all(b.flat_param is not None and b.grad.is_cuda for b in self._buckets)):
+                self._update = None
+        self._direct = (self._land and self._update is not None and allreducer.compressor.name == "oktopk"
                         and all(b.flat_param is not None for b in self._buckets))
         if self._use_streams:
             # high priority: a bucket's (SM-partitioned) communication kernel should get its SMs as soon as backward
@@ -107,10 +106,9 @@ class _BucketedComm:
         # stays valid when the schedule moves
         self._lr_dev = None
         self._lr_pin, self._lr_ev, self._lr_ring, self._lr_last = [], [], 0, None
-        self._scal_n = 3 if getattr(self, "_okt_adam", False) else 1       # device scalars per param group
         dev0 = self._buckets[0].params[0].device if self._buckets else torch.device("cpu")
-        if dev0.type == "cuda" and ext.available():
-            n = max(len(self.param_groups), 1) * self._scal_n
+        if dev0.type == "cuda" and ext.available() and self._update is not None:
+            n = max(len(self.param_groups), 1) * self._update.n_scalars
             self._lr_dev = torch.zeros(n, dtype=torch.float32, device=dev0)
             self._lr_pin = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(8)]
             self._lr_ev = [None] * len(self._lr_pin)
@@ -130,28 +128,27 @@ class _BucketedComm:
                 if torch.is_tensor(t):
                     w.broadcast(t, 0)
 
-    def _group_lr(self, gi: int) -> float:
-        return float(self.param_groups[gi]["lr"])
-
-    def _group_scalars(self, gi: int):
-        """The device scalars of param group ``gi`` for the coming step (``_scal_n`` of them)."""
-        return (self._group_lr(gi),)
+    @property
+    def _okt_adam(self) -> bool:
+        """True while the step runs the flat-bucket ``fused_adam`` kernel (derived from ``_update``, never set)."""
+        return self._update is _AdamUpdate
 
     def refresh_lr(self) -> None:
         """Push the current per-group device scalars to the device (one tiny async H2D, only when changed).
         Never called while a stream is capturing: graph replays call it right before ``replay()``."""
-        if self._lr_dev is None:
+        if self._lr_dev is None or self._update is None:
             return
-        vals = [self._group_scalars(gi) for gi in range(len(self.param_groups))]
+        vals = [self._update.scalars(self, g) for g in self.param_groups]
         if vals == self._lr_last:
             return
         self._lr_ring = (self._lr_ring + 1) % len(self._lr_pin)
         pin = self._lr_pin[self._lr_ring]
         if self._lr_ev[self._lr_ring] is not None:          # the host may run many (graph-replayed) steps ahead:
             self._lr_ev[self._lr_ring].synchronize()        # never overwrite a staging slot whose copy is pending
+        n = self._update.n_scalars
         for gi, sc in enumerate(vals):
             for j, v in enumerate(sc):
-                pin[gi * self._scal_n + j] = v
+                pin[gi * n + j] = v
         self._lr_dev.copy_(pin, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
@@ -159,7 +156,7 @@ class _BucketedComm:
         self._lr_last = vals
 
     def _lr_ptr(self, gi: int) -> int:
-        return 0 if self._lr_dev is None else self._lr_dev.data_ptr() + 4 * self._scal_n * gi
+        return self._lr_dev.data_ptr() + 4 * self._update.n_scalars * gi
 
     def _maybe_refresh_lr(self) -> None:
         if self._lr_dev is not None and not torch.cuda.is_current_stream_capturing():
@@ -333,41 +330,129 @@ class _BucketedComm:
         self._allreducer.close()
 
     # ------------------------------------------------------------------ fused updates
-    def _fused_sgd(self, b: Bucket) -> None:
+    def step(self, closure=None):
+        """``synchronize()`` + parameter update (``VGG/distributed_optimizer.py:185-190``)."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        if not self.local:
+            self.synchronize()
+        if self._update is None:
+            super().step()
+            for b in self._buckets:
+                b.dirty = True
+        else:
+            self._maybe_refresh_lr()
+            with torch.no_grad():
+                for b in self._buckets:
+                    self._fused_update(b)
+            self.counter += 1
+        self._after_step()
+        return loss
+
+    def _flat_buffers(self, b: Bucket) -> Dict[str, torch.Tensor]:
+        """The bucket's flat state buffers, one per state key of the update, allocated zeroed on first use;
+        ``self.state[p]`` holds views of them."""
         fs = self._flat_state.setdefault(b.index, {})
-        first = "momentum" not in fs
-        mom = fs.get("momentum")
-        if mom is None:
-            mom = fs["momentum"] = torch.zeros_like(b.grad)
-            for p, v in zip(b.params, b.views(mom)):
-                self.state[p]["momentum_buffer"] = v
-        use_kernel = b.grad.is_cuda and b.flat_param is not None and ext.available()
+        for k in self._update.keys:
+            if k not in fs:
+                fs[k] = torch.zeros_like(b.grad)
+                for p, v in zip(b.params, b.views(fs[k])):
+                    self.state[p][k] = v
+        return fs
+
+    def _fused_update(self, b: Bucket) -> None:
+        first = self._update.keys[0] not in self._flat_state.get(b.index, {})
+        fs = self._flat_buffers(b)
+        on_gpu = b.grad.is_cuda and b.flat_param is not None and ext.available()
+        # after a landing step the next landing copy overwrites the whole bucket: it need not be cleared
+        zero_grad = 0 if self._land and not self._direct else 1
         for gi, s, e in b.group_slices:
-            g = self.param_groups[gi]
-            lr, m, damp, wd, nest = g["lr"], g.get("momentum", 0.0), g.get("dampening", 0.0), \
-                g.get("weight_decay", 0.0), bool(g.get("nesterov", False))
-            if self.momentum_correction:
-                m = 0.0                            # momentum already applied before communication
-            if use_kernel:
-                ext.require().fused_sgd(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
-                                        mom.data_ptr() + 4 * s, e - s, lr, m, damp, wd, int(nest), int(first),
-                                        0 if self._land and not self._direct else 1, 1.0,
-                                        torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
-                                        self._allreducer.fault_ptr(b.name))
-            else:
-                gs, ms = b.grad[s:e], mom[s:e]
-                if b.flat_param is not None:
-                    self._sgd_math(b.flat_param[s:e], gs, ms, lr, m, damp, wd, nest, first)
-                else:
-                    for p, o in zip(b.params, b.offsets):
-                        if s <= o < e:
-                            self._sgd_math(p.data.view(-1), gs[o - s:o - s + p.numel()], ms[o - s:o - s + p.numel()],
-                                           lr, m, damp, wd, nest, first)
-                gs.zero_()
+            def launch(fn, *hyper):
+                fn(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
+                   *(fs[k].data_ptr() + 4 * s for k in self._update.keys), e - s, *hyper, zero_grad,
+                   torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi), self._allreducer.fault_ptr(b.name))
+            self._update.update(self, b, self.param_groups[gi], s, e, fs, first, launch if on_gpu else None)
+            if not on_gpu:
+                b.grad[s:e].zero_()
         b.dirty = False
 
+    def _adopt_state(self, counter: Optional[int] = None) -> None:
+        """Move per-parameter state (from ``load_state_dict`` or the wrapped optimizer) into the flat buffers.  A bucket
+        gets buffers iff one of its parameters has state (zeros for those without): SGD's first step copies the update
+        into a fresh momentum buffer.  The step count is ``counter``: given, or the per-parameter ``step`` of torch's
+        format, which must then be equal.  Unequal step counts cannot share one bias correction: the optimizer then keeps
+        the per-parameter state and uses torch's own ``step()`` from here on."""
+        keys = self._update.keys
+        have = {p for b in self._buckets for p in b.params if self.state.get(p, {}).get(keys[0]) is not None}
+        if counter is None:
+            steps = {float(self.state[p]["step"]) for p in have if "step" in self.state[p]}
+            if len(steps) > 1:
+                warnings.warn("DistributedOptimizer: the loaded Adam state has unequal step counts per parameter %s; "
+                              "using torch's Adam step from now on" % sorted(steps))
+                self._update = None
+                self._clear_buckets()
+                self._direct = False              # torch's step reads the gradients from the landed bucket
+                for b in self._buckets:
+                    for k in keys:
+                        self._flat_state.get(b.index, {}).pop(k, None)
+                return
+            counter = int(steps.pop()) if steps else 0
+        self.counter = counter
+        loaded = {(p, k): self.state[p][k] for p in have for k in keys}
+        with torch.no_grad():
+            for b in self._buckets:
+                for p in b.params:
+                    self.state.get(p, {}).pop("step", None)      # the step count is ``counter``
+                if not any(p in have for p in b.params):
+                    for k in keys:
+                        self._flat_state.get(b.index, {}).pop(k, None)
+                    continue
+                fs = self._flat_buffers(b)          # (points state[p] at the views when it allocates them)
+                for k in keys:
+                    for p, v in zip(b.params, b.views(fs[k])):
+                        if p in have:
+                            v.copy_(loaded[p, k])
+                        else:
+                            v.zero_()
+                        self.state[p][k] = v
+
+
+# ====================================================================================== fused update families
+# What a fused flat-bucket update needs to know about one optimizer: the per-parameter state it keeps in flat buffers
+# (``keys``), its device scalars per param group (``scalars``, ``n_scalars`` of them) and its update of one (bucket,
+# param group) slice: the kernel through ``launch``, or, with ``launch`` None (no flat CUDA bucket or no extension, as on
+# the CPU; SGD and BertAdam only), the same math in torch.
+class _SGDUpdate:
+    """``torch.optim.SGD``: weight decay, momentum, dampening, nesterov."""
+    keys = ("momentum_buffer",)
+    n_scalars = 1
+
     @staticmethod
-    def _sgd_math(p, g, mom, lr, m, damp, wd, nest, first) -> None:
+    def scalars(opt, g):
+        return (float(g["lr"]),)
+
+    @staticmethod
+    def update(opt, b, g, s, e, fs, first, launch):
+        lr, m, damp, wd, nest = g["lr"], g.get("momentum", 0.0), g.get("dampening", 0.0), \
+            g.get("weight_decay", 0.0), bool(g.get("nesterov", False))
+        if opt.momentum_correction:
+            m = 0.0                                # momentum already applied before communication
+        if launch is not None:
+            launch(ext.require().fused_sgd, m, damp, wd, int(nest), int(first))
+            return
+        gs, ms = b.grad[s:e], fs["momentum_buffer"][s:e]
+        if b.flat_param is not None:
+            _SGDUpdate.math(b.flat_param[s:e], gs, ms, lr, m, damp, wd, nest, first)
+        else:
+            for p, o in zip(b.params, b.offsets):
+                if s <= o < e:
+                    _SGDUpdate.math(p.data.view(-1), gs[o - s:o - s + p.numel()], ms[o - s:o - s + p.numel()],
+                                    lr, m, damp, wd, nest, first)
+
+    @staticmethod
+    def math(p, g, mom, lr, m, damp, wd, nest, first) -> None:
         d = g.add(p, alpha=wd) if wd != 0 else g.clone()
         if m != 0:
             if first:
@@ -378,101 +463,68 @@ class _BucketedComm:
         p.add_(d, alpha=-lr)
 
 
-# ====================================================================================== DistributedOptimizer
-class _DistributedOptimizerMixin(_BucketedComm):
-    def step(self, closure=None):
-        """``synchronize()`` + parameter update (``VGG/distributed_optimizer.py:185-190``)."""
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        if not self.local:
-            self.synchronize()
-        if self._okt_is_sgd:
-            self._maybe_refresh_lr()
-            with torch.no_grad():
-                for b in self._buckets:
-                    self._fused_sgd(b)
-        elif self._okt_adam:
-            self._maybe_refresh_lr()
-            with torch.no_grad():
-                for b in self._buckets:
-                    self._fused_torch_adam(b)
-            self.counter += 1
-        else:
-            super().step()
-            for b in self._buckets:
-                b.dirty = True
-        self._after_step()
-        return loss
+class _AdamUpdate:
+    """``torch.optim.Adam`` / ``AdamW`` built with ``fused=True`` (see ``_fused_adam_applies``): kernel only."""
+    keys = ("exp_avg", "exp_avg_sq")
+    n_scalars = 3
 
-    # ------------------------------------------------------------------ wrapped torch.optim.Adam / AdamW (fused=True)
-    def _group_scalars(self, gi: int):
-        if not self._okt_adam:
-            return super()._group_scalars(gi)
+    @staticmethod
+    def scalars(opt, g):
         # torch's non-capturable Adam, in double: t = the step about to run
-        g = self.param_groups[gi]
-        lr, (b1, b2), t = float(g["lr"]), g["betas"], float(self.counter + 1)
+        lr, (b1, b2), t = float(g["lr"]), g["betas"], float(opt.counter + 1)
         return (1 - lr * g["weight_decay"], (lr / (1 - b1 ** t)) * -1, (1 - b2 ** t) ** 0.5)
 
-    def _adam_flat_state(self, b: Bucket):
-        """The bucket's flat ``exp_avg`` / ``exp_avg_sq`` buffers; ``self.state[p]`` holds views of them."""
-        fs = self._flat_state.setdefault(b.index, {})
-        if "exp_avg" not in fs:
-            fs["exp_avg"], fs["exp_avg_sq"] = torch.zeros_like(b.grad), torch.zeros_like(b.grad)
-            for p, vm, vv in zip(b.params, b.views(fs["exp_avg"]), b.views(fs["exp_avg_sq"])):
-                self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"] = vm, vv
-        return fs["exp_avg"], fs["exp_avg_sq"]
+    @staticmethod
+    def update(opt, b, g, s, e, fs, first, launch):
+        launch(ext.require().fused_adam, g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"],
+               int(bool(g["decoupled_weight_decay"])))
 
-    def _fused_torch_adam(self, b: Bucket) -> None:
-        m, v = self._adam_flat_state(b)
-        for gi, s, e in b.group_slices:
-            g = self.param_groups[gi]
-            ext.require().fused_adam(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s, m.data_ptr() + 4 * s,
-                                     v.data_ptr() + 4 * s, e - s, g["betas"][0], g["betas"][1], g["eps"],
-                                     g["weight_decay"], int(bool(g["decoupled_weight_decay"])),
-                                     0 if self._land and not self._direct else 1,
-                                     torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
-                                     self._allreducer.fault_ptr(b.name))
-        b.dirty = False
 
-    def _adopt_adam_state(self) -> None:
-        """Move per-parameter Adam state (from ``load_state_dict`` or the wrapped optimizer) into the flat buffers and
-        take the common step count as ``counter``.  Unequal step counts cannot share one bias correction: the optimizer
-        then keeps the per-parameter state and uses torch's own ``step()`` from here on."""
-        have = [p for b in self._buckets for p in b.params if "exp_avg" in self.state.get(p, {})]
-        steps = {float(self.state[p]["step"]) for p in have}
-        if len(steps) > 1:
-            warnings.warn("DistributedOptimizer: the loaded Adam state has unequal step counts per parameter %s; "
-                          "using torch's Adam step from now on" % sorted(steps))
-            self._okt_adam = False
-            self._clear_buckets()
-            self._direct = False                  # torch's step reads the gradients from the landed bucket
-            for b in self._buckets:
-                fs = self._flat_state.get(b.index, {})
-                fs.pop("exp_avg", None)
-                fs.pop("exp_avg_sq", None)
+class _BertAdamUpdate:
+    """``BertAdam``: no bias correction, decoupled weight decay, the learning rate of its schedule."""
+    keys = ("next_m", "next_v")
+    n_scalars = 1
+
+    @staticmethod
+    def scalars(opt, g):
+        return (float(opt._scheduled_lr(g, opt.counter)),)
+
+    @staticmethod
+    def update(opt, b, g, s, e, fs, first, launch):
+        if opt.clip_reduced and g["max_grad_norm"] > 0:
+            for p, o in zip(b.params, b.offsets):
+                if s <= o < e:
+                    gv = b.grad[o:o + p.numel()]
+                    nrm = float(gv.norm())
+                    if nrm > g["max_grad_norm"]:
+                        gv.mul_(g["max_grad_norm"] / (nrm + 1e-6))
+        if launch is not None:
+            launch(ext.require().fused_bert_adam, g["b1"], g["b2"], g["e"], g["weight_decay"])
             return
-        self.counter = int(steps.pop()) if steps else 0
-        loaded = {p: (self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"]) for p in have}
-        with torch.no_grad():
-            for b in self._buckets:
-                m, v = self._adam_flat_state(b)      # (re-points state[p] at the views when it creates the buffers)
-                for p, vm, vv in zip(b.params, b.views(m), b.views(v)):
-                    src = loaded.get(p)
-                    if src is None:                  # no state for p: fresh moments, as torch would start them
-                        vm.zero_()
-                        vv.zero_()
-                    else:
-                        vm.copy_(src[0])
-                        vv.copy_(src[1])
-                    st = self.state[p]
-                    st.pop("step", None)          # the step count is ``counter``
-                    st["exp_avg"], st["exp_avg_sq"] = vm, vv
+        lr = opt._scheduled_lr(g, opt.counter)
+        gs, ms, vs = b.grad[s:e], fs["next_m"][s:e], fs["next_v"][s:e]
+        ms.mul_(g["b1"]).add_(gs, alpha=1 - g["b1"])
+        vs.mul_(g["b2"]).addcmul_(gs, gs, value=1 - g["b2"])
+        upd = ms / (vs.sqrt() + g["e"])
+        if b.flat_param is not None:
+            ps = b.flat_param[s:e]
+            if g["weight_decay"] > 0.0:
+                upd += g["weight_decay"] * ps
+            ps.add_(upd, alpha=-lr)
+        else:
+            for p, o in zip(b.params, b.offsets):
+                if s <= o < e:
+                    u = upd[o - s:o - s + p.numel()].view_as(p)
+                    if g["weight_decay"] > 0.0:
+                        u = u + g["weight_decay"] * p.data
+                    p.data.add_(u, alpha=-lr)
 
+
+# ====================================================================================== DistributedOptimizer
+class _DistributedOptimizerMixin(_BucketedComm):
     def state_dict(self):
         sd = super().state_dict()
-        if self._okt_adam:                        # torch's fused Adam format: a float32 0-dim step on the param's device
+        if self._update is _AdamUpdate:           # torch's fused Adam format: a float32 0-dim step on the param's device
             params = [p for g in self.param_groups for p in g["params"]]
             for i, st in list(sd["state"].items()):
                 sd["state"][i] = dict(st, step=torch.tensor(float(self.counter), dtype=torch.float32,
@@ -484,21 +536,8 @@ class _DistributedOptimizerMixin(_BucketedComm):
         state_dict = dict(state_dict)
         okt = state_dict.pop("oktopk", None)
         super().load_state_dict(state_dict)
-        if self._okt_adam:
-            self._adopt_adam_state()
-        if self._okt_is_sgd:                      # re-alias momentum into the flat buffers
-            for b in self._buckets:
-                fs = self._flat_state.setdefault(b.index, {})
-                have = [("momentum_buffer" in self.state.get(p, {})) and self.state[p]["momentum_buffer"] is not None
-                        for p in b.params]
-                if any(have):
-                    mom = fs.get("momentum")
-                    if mom is None:
-                        mom = fs["momentum"] = torch.zeros_like(b.grad)
-                    for p, v, h in zip(b.params, b.views(mom), have):
-                        if h:
-                            v.copy_(self.state[p]["momentum_buffer"])
-                        self.state[p]["momentum_buffer"] = v
+        if self._update is not None:
+            self._adopt_state()
         if okt is not None:
             self._allreducer.load_state_dict(okt)
         self._clear_buckets()
@@ -523,13 +562,17 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
     ar = AllReducer(compression=compression, sparse=is_sparse, density=density, cfg=cfg, world=world,
                     backend=backend, err_callback=err_handler, layerwise_times=layerwise_times,
                     sigma_scale=sigma_scale, norm_clip=norm_clip, writer=writer)
-    obj._okt_is_sgd = isinstance(optimizer, torch.optim.SGD)
-    obj._okt_adam = _fused_adam_applies(optimizer)
-    if obj._okt_adam:
+    if isinstance(optimizer, torch.optim.SGD):
+        obj._update = _SGDUpdate
+    elif _fused_adam_applies(optimizer):
+        obj._update = _AdamUpdate
+    else:
+        obj._update = None                        # torch's own step()
+    if obj._update is not None:
         obj.counter = 0                           # steps taken: Adam's bias correction (GraphedTrainStep keeps it too)
     obj._okt_setup(named_parameters, ar, flatten_params=flatten_params)
-    if obj._okt_adam and obj.state:
-        obj._adopt_adam_state()
+    if obj._update is not None and obj.state:
+        obj._adopt_state()
     return obj
 
 
@@ -631,8 +674,9 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
                         weight_decay=weight_decay, max_grad_norm=max_grad_norm)
         torch.optim.Optimizer.__init__(self, params, defaults)
         self.rank = rank
-        self.counter = 0
+        self.counter = 0                          # steps taken: the schedule's position and every parameter's step
         self.clip_reduced = clip_reduced
+        self._update = _BertAdamUpdate
         base = cfg if cfg is not None else OkTopkConfig(
             warmup_iters=0, local_recompute_interval=128, global_recompute_interval=128, overselect_guard_loops=0,
             local_adapt_low=4 / 5, local_adapt_high=5 / 4, local_adapt_factor=1.025, global_adapt_low=4 / 5,
@@ -640,9 +684,6 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
         ar = AllReducer(compression=compressor, sparse=(compressor != "none"), density=density,
                         cfg=base.replace(density=density), world=world, backend=backend)
         self._okt_setup(named_parameters, ar, flatten_params=flatten_params)
-
-    def _group_lr(self, gi: int) -> float:
-        return float(self._scheduled_lr(self.param_groups[gi], self.counter))
 
     def get_lr(self) -> List[float]:
         out = []
@@ -656,70 +697,10 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
             return g["lr"] * SCHEDULES[g["schedule"]](step / g["t_total"], g["warmup"])
         return g["lr"]
 
-    def step(self, closure=None):
-        loss = None
-        if closure is not None:
-            with torch.enable_grad():
-                loss = closure()
-        if not self.local:
-            self.synchronize()
-        self._maybe_refresh_lr()
-        with torch.no_grad():
-            for b in self._buckets:
-                self._fused_adam(b)
-        self.counter += 1
-        self._after_step()
-        return loss
-
-    def _fused_adam(self, b: Bucket) -> None:
-        fs = self._flat_state.setdefault(b.index, {})
-        if "next_m" not in fs:
-            fs["next_m"] = torch.zeros_like(b.grad)
-            fs["next_v"] = torch.zeros_like(b.grad)
-            for p, vm, vv in zip(b.params, b.views(fs["next_m"]), b.views(fs["next_v"])):
-                self.state[p]["next_m"], self.state[p]["next_v"], self.state[p]["step"] = vm, vv, 0
-        m, v = fs["next_m"], fs["next_v"]
-        use_kernel = b.grad.is_cuda and b.flat_param is not None and ext.available()
-        for gi, s, e in b.group_slices:
-            g = self.param_groups[gi]
-            lr = self._scheduled_lr(g, self.counter)
-            if self.clip_reduced and g["max_grad_norm"] > 0:
-                for p, o in zip(b.params, b.offsets):
-                    if s <= o < e:
-                        gv = b.grad[o:o + p.numel()]
-                        nrm = float(gv.norm())
-                        if nrm > g["max_grad_norm"]:
-                            gv.mul_(g["max_grad_norm"] / (nrm + 1e-6))
-            if use_kernel:
-                ext.require().fused_bert_adam(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
-                                              m.data_ptr() + 4 * s, v.data_ptr() + 4 * s, e - s, lr, g["b1"], g["b2"],
-                                              g["e"], g["weight_decay"], 0 if self._land and not self._direct else 1,
-                                              torch.cuda.current_stream().cuda_stream,
-                                              self._lr_ptr(gi), self._allreducer.fault_ptr(b.name))
-            else:
-                gs, ms, vs = b.grad[s:e], m[s:e], v[s:e]
-                ms.mul_(g["b1"]).add_(gs, alpha=1 - g["b1"])
-                vs.mul_(g["b2"]).addcmul_(gs, gs, value=1 - g["b2"])
-                upd = ms / (vs.sqrt() + g["e"])
-                if b.flat_param is not None:
-                    ps = b.flat_param[s:e]
-                    if g["weight_decay"] > 0.0:
-                        upd += g["weight_decay"] * ps
-                    ps.add_(upd, alpha=-lr)
-                else:
-                    for p, o in zip(b.params, b.offsets):
-                        if s <= o < e:
-                            u = upd[o - s:o - s + p.numel()].view_as(p)
-                            if g["weight_decay"] > 0.0:
-                                u = u + g["weight_decay"] * p.data
-                            p.data.add_(u, alpha=-lr)
-                gs.zero_()
-        for p in b.params:
-            self.state[p]["step"] += 1
-        b.dirty = False
-
     def state_dict(self):
         sd = torch.optim.Optimizer.state_dict(self)
+        for i, st in list(sd["state"].items()):
+            sd["state"][i] = dict(st, step=self.counter)
         sd["oktopk"] = self._allreducer.state_dict()
         sd["counter"] = self.counter
         return sd
@@ -727,21 +708,9 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
     def load_state_dict(self, state_dict):
         state_dict = dict(state_dict)
         okt = state_dict.pop("oktopk", None)
-        self.counter = state_dict.pop("counter", 0)
+        counter = state_dict.pop("counter", 0)
         torch.optim.Optimizer.load_state_dict(self, state_dict)
-        for b in self._buckets:
-            fs = self._flat_state.setdefault(b.index, {})
-            if any("next_m" in self.state.get(p, {}) for p in b.params):
-                if "next_m" not in fs:
-                    fs["next_m"] = torch.zeros_like(b.grad)
-                    fs["next_v"] = torch.zeros_like(b.grad)
-                for p, vm, vv in zip(b.params, b.views(fs["next_m"]), b.views(fs["next_v"])):
-                    stp = self.state.get(p, {})
-                    if "next_m" in stp:
-                        vm.copy_(stp["next_m"])
-                        vv.copy_(stp["next_v"])
-                    self.state[p]["next_m"], self.state[p]["next_v"] = vm, vv
-                    self.state[p].setdefault("step", self.counter)
+        self._adopt_state(counter)
         if okt is not None:
             self._allreducer.load_state_dict(okt)
         self._clear_buckets()

@@ -256,6 +256,40 @@ def test_graphed_adamw_steps_match_eager_steps_bitwise():
         o.close()
 
 
+def test_graphed_bert_adam_checkpoints_the_steps_taken():
+    """BertAdam under whole-step CUDA graphs: the checkpointed per-parameter step is the number of steps taken (a replay
+    runs no Python), and the parameters match eager steps bit for bit."""
+    import oktopk_b200 as okt
+    from oktopk_b200.train.graph_step import GraphedTrainStep
+    torch.backends.cudnn.deterministic = True
+    base = _vgg()
+    nets, opts = [], []
+    for _ in range(2):
+        net = copy.deepcopy(base)
+        cfg = okt.preset("vgg16", density=0.01, warmup_iters=4)
+        nets.append(net)
+        opts.append(okt.BertAdam(_groups(net), lr=1e-3, warmup=0.1, t_total=100, compressor="oktopk", density=0.01,
+                                 named_parameters=list(net.named_parameters()), cfg=cfg))
+    gs = GraphedTrainStep(_Shim(nets[0], opts[0]), warmup_eager=2)
+    n_steps = 8
+    for batch in _batches(n_steps):
+        gs.step(batch)
+        opts[1].zero_grad()
+        torch.nn.functional.cross_entropy(nets[1](batch[0]), batch[1]).backward()
+        opts[1].step()
+    torch.cuda.synchronize()
+    assert gs.enabled, gs.why_disabled
+    assert len(gs.graphs) >= 2
+    for o in opts:
+        sd = o.state_dict()
+        assert o.counter == sd["counter"] == n_steps
+        assert sd["state"] and all(st["step"] == n_steps for st in sd["state"].values())
+    for (name, a), b in zip(nets[0].named_parameters(), nets[1].parameters()):
+        assert torch.equal(a, b), name
+    for o in opts:
+        o.close()
+
+
 # ---------------------------------------------------------------------------------------------------- 5. checkpoints
 def test_wrapper_state_dict_loads_into_torch_adamw():
     a = _vgg()

@@ -45,11 +45,13 @@ def test_fused_sgd_matches_torch():
     pr = p.clone().requires_grad_(True)
     opt = torch.optim.SGD([pr], lr=0.1, momentum=0.9, weight_decay=1e-4, nesterov=True)
     mom = torch.zeros(n, device="cuda")
+    lr = torch.tensor([0.1], device="cuda")
     for it in range(3):
         pr.grad = g.clone()
         opt.step()
         gg = g.clone()
-        C.fused_sgd(p.data_ptr(), gg.data_ptr(), mom.data_ptr(), n, 0.1, 0.9, 0.0, 1e-4, 1, int(it == 0), 1, 1.0, _stream())
+        C.fused_sgd(p.data_ptr(), gg.data_ptr(), mom.data_ptr(), n, 0.9, 0.0, 1e-4, 1, int(it == 0), 1, _stream(),
+                    lr.data_ptr())
         assert float(gg.abs().max()) == 0.0          # gradient bucket zeroed in the same pass
     torch.testing.assert_close(p, pr.detach(), rtol=1e-5, atol=1e-6)
 
@@ -60,13 +62,15 @@ def test_fused_bert_adam_matches_reference_math():
     n = 65537
     p = torch.randn(n, device="cuda"); m = torch.zeros(n, device="cuda"); v = torch.zeros(n, device="cuda")
     pr, mr, vr = p.clone(), m.clone(), v.clone()
+    lr = torch.tensor([2e-4], device="cuda")
     for it in range(3):
         g = torch.randn(n, device="cuda")
         mr.mul_(0.9).add_(g, alpha=0.1)
         vr.mul_(0.999).addcmul_(g, g, value=0.001)
         upd = mr / (vr.sqrt() + 1e-6) + 0.01 * pr
         pr.add_(upd, alpha=-2e-4)
-        C.fused_bert_adam(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), n, 2e-4, 0.9, 0.999, 1e-6, 0.01, 1, _stream())
+        C.fused_bert_adam(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), n, 0.9, 0.999, 1e-6, 0.01, 1, _stream(),
+                          lr.data_ptr())
     torch.testing.assert_close(p, pr, rtol=1e-5, atol=1e-6)
 
 
@@ -362,11 +366,12 @@ def test_fused_update_is_skipped_when_the_bucket_faulted():
     n = 10_000
     p = torch.ones(n, device="cuda"); g = torch.ones(n, device="cuda"); mom = torch.zeros(n, device="cuda")
     flag = torch.zeros(1, dtype=torch.int32, device="cuda")
-    C.fused_sgd(p.data_ptr(), g.data_ptr(), mom.data_ptr(), n, 0.1, 0.0, 0.0, 0.0, 0, 1, 0, 1.0, _stream(), 0, flag.data_ptr())
+    lr = torch.tensor([0.1], device="cuda")
+    C.fused_sgd(p.data_ptr(), g.data_ptr(), mom.data_ptr(), n, 0.0, 0.0, 0.0, 0, 1, 0, _stream(), lr.data_ptr(), flag.data_ptr())
     torch.cuda.synchronize()
     assert float(p[0]) == pytest.approx(0.9)
     flag.fill_(1)
-    C.fused_sgd(p.data_ptr(), g.data_ptr(), mom.data_ptr(), n, 0.1, 0.0, 0.0, 0.0, 0, 0, 0, 1.0, _stream(), 0, flag.data_ptr())
+    C.fused_sgd(p.data_ptr(), g.data_ptr(), mom.data_ptr(), n, 0.0, 0.0, 0.0, 0, 0, 0, _stream(), lr.data_ptr(), flag.data_ptr())
     torch.cuda.synchronize()
     assert float(p[0]) == pytest.approx(0.9)          # partial gradient not applied
 

@@ -1,4 +1,5 @@
 """Single-process CPU tests: optimizer wrappers, model parameter counts, trainer/CLI/checkpoint plumbing."""
+import copy
 import math
 import os
 
@@ -166,6 +167,88 @@ def test_optimizer_state_dict_carries_sparse_state_and_resumes_bitwise():
     for p, q in zip(a.parameters(), b.parameters()):
         assert torch.equal(p, q)
     oa.close(); ob.close()
+
+
+def _bert_adam(net):
+    named = list(net.named_parameters())
+    groups = [{"params": [p for n, p in named if "bias" not in n], "weight_decay": 0.01},
+              {"params": [p for n, p in named if "bias" in n], "weight_decay": 0.0}]
+    return BertAdam(groups, lr=1e-2, warmup=0.1, t_total=100, named_parameters=named, compressor="none", density=1.0)
+
+
+def _train(net, opt, its, device="cpu"):
+    for it in its:
+        x, y = _batch(it)
+        opt.zero_grad()
+        torch.nn.functional.cross_entropy(net(x.to(device)), y.to(device)).backward()
+        opt.step()
+
+
+@pytest.mark.parametrize("device", ["cpu", pytest.param("cuda", marks=pytest.mark.gpu)])
+def test_bert_adam_state_dict_resumes_bitwise(device):
+    """Every parameter's checkpointed step is the optimizer's step count; a fresh BertAdam resumes from the checkpoint
+    bit for bit (moments, schedule position, flat-buffer aliasing)."""
+    a = _mlp().to(device)
+    oa = _bert_adam(a)
+    _train(a, oa, range(4), device)
+    sd = copy.deepcopy(oa.state_dict())
+    assert sd["counter"] == 4 and sd["state"] and all(st["step"] == 4 for st in sd["state"].values())
+    b = _mlp(seed=1).to(device)
+    b.load_state_dict(a.state_dict())
+    ob = _bert_adam(b)
+    ob.load_state_dict(sd)
+    assert ob.counter == 4 and all("step" not in ob.state[p] for p in b.parameters())
+    _train(a, oa, range(4, 8), device)
+    _train(b, ob, range(4, 8), device)
+    for p, q in zip(a.parameters(), b.parameters()):
+        assert torch.equal(p, q)
+        assert torch.equal(oa.state[p]["next_m"], ob.state[q]["next_m"])
+        assert torch.equal(oa.state[p]["next_v"], ob.state[q]["next_v"])
+    assert all(st["step"] == 8 for st in ob.state_dict()["state"].values())
+    oa.close(); ob.close()
+
+
+def test_wrapped_sgd_state_dict_moves_to_and_from_torch_sgd():
+    kw = dict(lr=0.1, momentum=0.9, weight_decay=1e-4)
+
+    def wrap(net):
+        return okt.DistributedOptimizer(torch.optim.SGD(net.parameters(), **kw), named_parameters=net.named_parameters(),
+                                        compression=okt.compressors["none"], is_sparse=False)
+
+    def close(net_a, net_b):
+        for p, q in zip(net_a.parameters(), net_b.parameters()):
+            torch.testing.assert_close(p, q, rtol=1e-5, atol=1e-6)
+
+    # wrapper -> torch
+    a = _mlp()
+    opt = wrap(a)
+    _train(a, opt, range(3))
+    b = _mlp(seed=1)
+    b.load_state_dict(a.state_dict())
+    ref = torch.optim.SGD(b.parameters(), **kw)
+    ref.load_state_dict(copy.deepcopy(opt.state_dict()))
+    _train(a, opt, range(3, 6))
+    _train(b, ref, range(3, 6))
+    close(a, b)
+    opt.close()
+    # torch -> wrapper: the momentum lands in the flat buffer, and the next step is not a first step
+    b = _mlp()
+    ref = torch.optim.SGD(b.parameters(), **kw)
+    _train(b, ref, range(3))
+    a = _mlp(seed=1)
+    a.load_state_dict(b.state_dict())
+    opt = wrap(a)
+    opt.load_state_dict(copy.deepcopy(ref.state_dict()))
+    (bk,) = opt._buckets
+    flat = opt._flat_state[bk.index]["momentum_buffer"]
+    for p, q in zip(a.parameters(), b.parameters()):
+        buf = opt.state[p]["momentum_buffer"]
+        assert buf.untyped_storage().data_ptr() == flat.untyped_storage().data_ptr()
+        assert torch.equal(buf, ref.state[q]["momentum_buffer"])
+    _train(a, opt, range(3, 6))
+    _train(b, ref, range(3, 6))
+    close(a, b)
+    opt.close()
 
 
 def test_momentum_correction_mode_runs():
