@@ -10,7 +10,7 @@ Public API (parity with the reference's ``distributed_optimizer`` / ``compressio
                                    compression=okt.compressors['oktopk'], is_sparse=True, density=0.001)
     opt.zero_grad(); loss.backward(); opt.step()
 """
-from .config import OkTopkConfig, preset  # noqa: F401
+from .config import LossScale, OkTopkConfig, preset  # noqa: F401
 from .compression import compressors, NoneCompressor, TopKCompressor, GaussianCompressor  # noqa: F401
 from .parallel.world import init, world, rank, size, shutdown  # noqa: F401
 from .parallel.state import SparseState  # noqa: F401

@@ -107,6 +107,49 @@ class OkTopkConfig:
         return dataclasses.asdict(self)
 
 
+@dataclass(frozen=True)
+class LossScale:
+    """Dynamic loss scaling for fp16 training (``DistributedOptimizer(..., loss_scale=LossScale())``).
+
+    The defaults are ``torch.amp.GradScaler``'s; ``growth_factor=1, backoff_factor=1`` is a fixed scale.  Use
+    ``opt.scale_loss(loss).backward()`` and ``opt.step()`` as usual; ``torch.amp.GradScaler`` itself cannot be combined
+    with the optimizer (it would read the gradients while their reduction is still running).
+
+    Semantics, per step:
+      1. Every bucket's gradient is multiplied by ``inv_scale`` (the fp32 reciprocal of the scale computed in double)
+         before it reaches a residual, a threshold or a momentum: these stay in unscaled units across scale changes.
+      2. Per bucket: if any rank sees a non-finite value in the bucket, every rank skips the bucket's reduction.  Its
+         residual, thresholds, region edges and device trace stay bitwise unchanged.
+      3. Per step: if any bucket was skipped, no parameter and no optimizer state is updated (the gradient bucket is
+         still cleared) and the scale backs off; otherwise the growth tracker advances and the scale grows every
+         ``growth_interval`` clean steps, exactly as ``torch._amp_update_scale_``.  Buckets that were clean and already
+         reduced in a skipped step keep their residual update (a single-bucket model skips completely).
+      4. A skipped step does not advance the wrapped fused Adam's bias-correction step.  BertAdam's schedule and the
+         engines' iteration counters do advance: a skipped exact-threshold or re-partition iteration leaves the previous
+         threshold and region edges in force.  SGD with ``dampening != 0`` whose very first step is skipped starts its
+         momentum from a zero buffer rather than from a copy of the first gradient.
+    """
+    init_scale: float = 2.0 ** 16
+    growth_factor: float = 2.0
+    backoff_factor: float = 0.5
+    growth_interval: int = 2000
+
+    def __post_init__(self):
+        if not (self.init_scale > 0 and self.growth_factor >= 1 and 0 < self.backoff_factor <= 1
+                and self.growth_interval >= 1):
+            raise ValueError("LossScale: need init_scale > 0, growth_factor >= 1, 0 < backoff_factor <= 1, "
+                             "growth_interval >= 1")
+
+    @staticmethod
+    def parse(spec) -> Optional["LossScale"]:
+        """``None`` / ``LossScale`` pass through; ``"dynamic"`` is the default dynamic scale; a number is a fixed scale."""
+        if spec is None or isinstance(spec, LossScale):
+            return spec
+        if isinstance(spec, str) and spec.strip().lower() == "dynamic":
+            return LossScale()
+        return LossScale(init_scale=float(spec), growth_factor=1.0, backoff_factor=1.0)
+
+
 def _vgg() -> OkTopkConfig:
     # VGG/allreducer.py:573-579,209-211,696-699,1054-1057; VGG/compression.py:393-404
     return OkTopkConfig(

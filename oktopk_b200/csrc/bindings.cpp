@@ -200,7 +200,7 @@ static py::dict layout_info(int P, int n, int cap, int gcap) {
     d["total"] = L.total; d["rs_mbox"] = L.rs_mbox; d["rs_thr"] = L.rs_thr; d["ag_mbox"] = L.ag_mbox;
     d["cut_mbox"] = L.cut_mbox; d["cut_data"] = L.cut_data; d["send_idx"] = L.send_idx; d["send_val"] = L.send_val;
     d["gat_idx"] = L.gat_idx; d["gat_val"] = L.gat_val; d["cap"] = L.cap; d["gcap"] = L.gcap; d["scap"] = L.scap;
-    d["done_mbox"] = L.done_mbox; d["tree_mbox"] = L.tree_mbox;
+    d["done_mbox"] = L.done_mbox; d["tree_mbox"] = L.tree_mbox; d["scale_mbox"] = L.scale_mbox;
     d["chunk"] = kChunk; d["maxp"] = OKT_MAXP; d["threads"] = kThreads;
     return d;
 }
@@ -311,6 +311,7 @@ static void oktopk_run(uint64_t g, uint64_t res, uint64_t st, const std::vector<
     p.redo_factor = (float)getf("redo_factor", 1.5);
     p.dense_nnz_limit = geti("dense_nnz_limit", 0);
     p.host_fault = o.contains("host_fault") ? P_<int>(o["host_fault"].cast<uint64_t>()) : nullptr;
+    p.skip = o.contains("skip") ? P_<const int>(o["skip"].cast<uint64_t>()) : nullptr;
     p.trace = geti("trace", 0);
     p.exact_local = geti("exact_local", 0);
     p.repartition = geti("repartition", 0);
@@ -389,6 +390,7 @@ static void gather_run(uint64_t g, uint64_t res, uint64_t st, const std::vector<
     p.cand = o.contains("cand") ? P_<int>(o["cand"].cast<uint64_t>()) : nullptr;
     p.ccap = o.contains("ccap") ? o["ccap"].cast<int>() : 0;
     p.host_fault = o.contains("host_fault") ? P_<int>(o["host_fault"].cast<uint64_t>()) : nullptr;
+    p.skip = o.contains("skip") ? P_<const int>(o["skip"].cast<uint64_t>()) : nullptr;
     if (p.reselect && (p.bitmap == nullptr || p.cand == nullptr || p.ccap <= 0))
         throw std::runtime_error("gather_run: TopkA2 needs the bitmap and candidate scratch");
     p.select_mode = o["select_mode"].cast<int>();
@@ -421,6 +423,7 @@ static void gtopk_run(uint64_t g, uint64_t res, uint64_t st, const std::vector<u
     p.sel_val = P_<float>(o["sel_val"].cast<uint64_t>());
     p.selcap = o["selcap"].cast<int>();
     p.host_fault = o.contains("host_fault") ? P_<int>(o["host_fault"].cast<uint64_t>()) : nullptr;
+    p.skip = o.contains("skip") ? P_<const int>(o["skip"].cast<uint64_t>()) : nullptr;
     ck(launch_gtopk(p, grid, S_(stream)), "gtopk launch");
 }
 
@@ -449,7 +452,7 @@ static void land_grads(const std::vector<uint64_t>& srcs, const std::vector<long
 
 static void dense_run(const std::vector<uint64_t>& bufs, const std::vector<uint64_t>& flags, uint64_t epoch, int n,
                       int rank, int grid, uint64_t stream, uint64_t st, double timeout_s, uint64_t mc,
-                      uint64_t host_fault) {
+                      uint64_t host_fault, uint64_t skip) {
     DenseParams p;
     std::memset(&p, 0, sizeof(p));
     if (bufs.size() > OKT_MAXP || bufs.size() != flags.size()) throw std::runtime_error("bad peer tables");
@@ -460,6 +463,7 @@ static void dense_run(const std::vector<uint64_t>& bufs, const std::vector<uint6
     p.timeout_ns = (unsigned long long)(timeout_s * 1e9);
     p.mc = P_<float>(mc);
     p.host_fault = P_<int>(host_fault);
+    p.skip = P_<const int>(skip);
     ck(launch_dense_allreduce(p, grid, S_(stream)), "dense allreduce launch");
 }
 
@@ -468,24 +472,29 @@ static void kth_abs(uint64_t x, int n, int k, uint64_t st, uint64_t out, int gri
 }
 
 static void fused_sgd(uint64_t p, uint64_t g, uint64_t mom, int n, double momentum, double dampening, double wd,
-                      int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+                      int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
+                      uint64_t skip_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_sgd: scal_ptr must point at the group's device scalars");
     ck(launch_fused_sgd(P_<float>(p), P_<float>(g), P_<float>(mom), n, (float)momentum, (float)dampening, (float)wd,
-                        nesterov, first, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
+                        nesterov, first, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
+                        S_(stream)),
        "fused_sgd");
 }
 static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double b1, double b2, double eps,
-                            double wd, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+                            double wd, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
+                            uint64_t skip_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_bert_adam: scal_ptr must point at the group's device scalars");
     ck(launch_fused_bert_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, (float)b1, (float)b2,
-                              (float)eps, (float)wd, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
+                              (float)eps, (float)wd, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
+                              S_(stream)),
        "fused_bert_adam");
 }
 static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double beta1, double beta2, double eps,
-                       double wd, int decoupled, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr) {
+                       double wd, int decoupled, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
+                       uint64_t skip_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_adam: scal_ptr must point at the group's device scalars");
     ck(launch_fused_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, beta1, beta2, (float)eps, (float)wd,
-                         decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), S_(stream)),
+                         decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
        "fused_adam");
 }
 // dtype of x, y, dy, dx: 0 = fp32, 1 = bf16 (parameters, statistics and dgamma / dbeta are fp32 either way)
@@ -527,6 +536,38 @@ static void clip_by_norm(uint64_t x, int n, uint64_t scratch, double max_norm, u
     ck(launch_scale(P_<float>(x), n, P_<float>(scratch), (float)max_norm, S_(stream)), "clip scale");
 }
 
+// ------------------------------------------------------------------------------------------- loss scaling
+// srcs = (pointers, lengths): the gradient tensors of the direct Ok-Topk path, or the landed bucket as one segment.
+static void unscale_check(const std::vector<uint64_t>& srcs, const std::vector<long long>& lens, uint64_t ls, uint64_t sync,
+                          uint64_t st, uint64_t host_fault, const std::vector<uint64_t>& peers, size_t mbox_off, int rank,
+                          double timeout_s, uint64_t stream) {
+    ScaleParams p;
+    std::memset(&p, 0, sizeof(p));
+    if (srcs.empty() || srcs.size() != lens.size()) throw std::runtime_error("unscale_check: bad source table");
+    if (srcs.size() > (size_t)kSrcSegMax) throw std::runtime_error("unscale_check: more gradient sources than kSrcSegMax");
+    if (peers.size() > OKT_MAXP) throw std::runtime_error("world larger than OKT_MAXP");
+    int blk = 0;
+    for (size_t i = 0; i < srcs.size(); ++i) {
+        if ((srcs[i] & 15) || lens[i] <= 0 || lens[i] > (1LL << 31) - 1)
+            throw std::runtime_error("unscale_check: sources must be 16-byte aligned and non-empty");
+        p.src[i] = P_<float>(srcs[i]);
+        p.len[i] = (int)lens[i];
+        p.blk_begin[i] = blk;
+        blk += (int)((lens[i] + kScalePerCta - 1) / kScalePerCta);
+    }
+    p.blk_begin[srcs.size()] = blk;
+    p.nseg = (int)srcs.size();
+    p.ls = P_<LossScaleDev>(ls);
+    p.sync = P_<ScaleSync>(sync);
+    p.fault = &P_<OktState>(st)->fault;
+    p.host_fault = P_<int>(host_fault);
+    for (size_t i = 0; i < peers.size(); ++i) p.peers[i] = P_<char>(peers[i]);
+    p.mbox_off = mbox_off;
+    p.P = (int)peers.size(); p.rank = rank;
+    p.timeout_ns = (unsigned long long)(timeout_s * 1e9);
+    ck(launch_unscale_check(p, S_(stream)), "unscale_check");
+}
+
 PYBIND11_MODULE(_C, m) {
     m.doc() = "oktopk_b200 native extension (sm_90a kernels + symmetric peer memory)";
     m.def("symm_alloc", &symm_alloc);
@@ -546,7 +587,7 @@ PYBIND11_MODULE(_C, m) {
     m.def("gather_run", &gather_run);
     m.def("dense_run", &dense_run, py::arg("bufs"), py::arg("flags"), py::arg("epoch"), py::arg("n"), py::arg("rank"),
           py::arg("grid"), py::arg("stream"), py::arg("st") = 0, py::arg("timeout_s") = 0.0, py::arg("mc") = 0,
-          py::arg("host_fault") = 0);
+          py::arg("host_fault") = 0, py::arg("skip") = 0);
     m.def("gtopk_run", &gtopk_run);
     m.def("land_grads", &land_grads);
     m.def("read_trace", &read_trace);
@@ -573,14 +614,28 @@ PYBIND11_MODULE(_C, m) {
     m.def("kth_abs", &kth_abs);
     m.def("fused_sgd", &fused_sgd, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("n"), py::arg("momentum"),
           py::arg("dampening"), py::arg("wd"), py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"),
-          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
     m.def("fused_bert_adam", &fused_bert_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"), py::arg("stream"),
-          py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
+          py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
     m.def("fused_adam", &fused_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("decoupled"), py::arg("zero_grad"),
-          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0);
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
     m.def("momentum_correct", &momentum_correct);
+    m.def("unscale_check", &unscale_check);
+    m.def("scale_update", [](uint64_t ls, double growth, double backoff, int interval, uint64_t stream) {
+        ck(launch_scale_update(P_<LossScaleDev>(ls), growth, backoff, interval, S_(stream)), "scale_update");
+    });
+    m.def("adam_scalars", [](uint64_t ls, uint64_t hyper, uint64_t scal, int groups, uint64_t stream) {
+        ck(launch_adam_scalars(P_<const LossScaleDev>(ls), P_<const double>(hyper), P_<float>(scal), groups, S_(stream)),
+           "adam_scalars");
+    });
+    m.def("carry_residual", [](uint64_t g, uint64_t res, int n, uint64_t skip, uint64_t stream) {
+        ck(launch_carry_residual(P_<float>(g), P_<float>(res), n, P_<const int>(skip), S_(stream)), "carry_residual");
+    });
+    m.attr("LOSS_SCALE_BYTES") = sizeof(LossScaleDev);
+    m.attr("SCALE_SYNC_BYTES") = sizeof(ScaleSync);
+    m.attr("VERDICT_OFFSET") = offsetof(ScaleSync, verdict);
     m.def("maxpool2_fwd", &maxpool2_fwd);
     m.def("maxpool2_bwd", &maxpool2_bwd);
     m.def("bn_forward", &bn_forward);

@@ -85,7 +85,7 @@ __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_re
 // so a dead or wedged peer turns into a reported error instead of a hung GPU.  Once a fault is recorded every
 // later wait of the same bucket returns immediately.
 enum FaultCode : int { FAULT_NONE = 0, FAULT_RS_TIMEOUT = 1, FAULT_AG_TIMEOUT = 2, FAULT_CUT_TIMEOUT = 3, FAULT_DENSE_TIMEOUT = 4,
-                       FAULT_TREE_TIMEOUT = 5, FAULT_DONE_TIMEOUT = 6 };
+                       FAULT_TREE_TIMEOUT = 5, FAULT_DONE_TIMEOUT = 6, FAULT_SCALE_TIMEOUT = 7 };
 
 struct SpinGuard {
     int* fault;
@@ -101,6 +101,12 @@ __device__ __forceinline__ void raise_fault(const SpinGuard& sg) {
         *reinterpret_cast<volatile int*>(sg.host_fault) = sg.code;
         __threadfence_system();
     }
+}
+
+// Loss scaling: the bucket's (or step's) verdict, written by an earlier kernel of the stream; null when scaling is off.
+// A reduction kernel returns at entry when it is set -- every rank holds the same verdict, so no peer waits for it.
+__device__ __forceinline__ bool verdict_set(const int* skip) {
+    return skip != nullptr && *reinterpret_cast<const volatile int*>(skip) != 0;
 }
 
 // Spin until the mailbox word carries `epoch` in its high half; returns the low half (payload), 0 on fault.

@@ -52,6 +52,7 @@ __device__ __forceinline__ void cta_peer_barrier(const DenseParams& p, int phase
 }
 
 __global__ void __launch_bounds__(kDenseThreads, 1) dense_allreduce_kernel(const DenseParams p) {
+    if (verdict_set(p.skip)) return;
     const int P = p.P, rank = p.rank;
     // one monotonically increasing ticket per CTA, device resident (CUDA-graph friendly)
     __shared__ unsigned long long s_ticket;

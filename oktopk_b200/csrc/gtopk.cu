@@ -27,6 +27,7 @@ __global__ void __launch_bounds__(kThreads, 2) gtopk_kernel(const TreeParams p) 
     __shared__ int s_cnt;
     __shared__ __align__(128) PullSmem s_pull;
 
+    if (verdict_set(p.skip)) return;
     OktState* st = p.st;
     const int tid = threadIdx.x, lane = tid & 31;
     const int gtid = blockIdx.x * kThreads + tid;

@@ -89,6 +89,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     __shared__ int s_ntail;
     extern __shared__ __align__(128) float4 dyn_pk[];       // TMA ring of the streaming pass (kPackSmemBytes)
 
+    if (verdict_set(p.skip)) return;
     OktState* st = p.st;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int gtid = blockIdx.x * kThreads + tid;

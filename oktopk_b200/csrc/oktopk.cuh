@@ -101,7 +101,8 @@ struct SymmLayout {
     size_t cut_data;     // int32  [2][MAXP][MAXP]
     size_t done_mbox;    // uint64 [2][MAXP]       "finished reading your memory" flags (dense fallback, tree schemes)
     size_t tree_mbox;    // uint64 [2][MAXP]       gTopk: per-round list-ready flags (((epoch<<5)|round) << 32 | count)
-    size_t send_idx;     // int32  [scap]          my selections, bucketed by destination region
+    size_t scale_mbox;   // uint64 [2][MAXP]       loss scaling: src's non-finite flag of the bucket (epoch<<32 | flag)
+    size_t send_idx;    // int32  [scap]          my selections, bucketed by destination region
     size_t send_val;     // float  [scap]
     size_t gat_idx;      // int32  [2][gcap]       my region's globally selected entries
     size_t gat_val;      // float  [2][gcap]
@@ -123,6 +124,7 @@ inline SymmLayout make_layout(int P, int n, int cap, int gcap) {
     L.cut_data = o; o += sizeof(int) * 2 * OKT_MAXP * OKT_MAXP;
     L.done_mbox = o; o += sizeof(uint64_t) * 2 * OKT_MAXP;
     L.tree_mbox = o; o += sizeof(uint64_t) * 2 * OKT_MAXP;
+    L.scale_mbox = o; o += sizeof(uint64_t) * 2 * OKT_MAXP;
     o = align_up(o, 1024);
     const size_t scap = cap > 0 ? (size_t)P * cap : align_up((size_t)n, 4) + 4 * (size_t)OKT_MAXP + 1024;
     L.send_idx = o; o += sizeof(int) * scap;   o = align_up(o, 1024);
@@ -193,6 +195,7 @@ struct OktParams {
     float redo_factor;                  // first raise; squared after every further attempt
     int dense_nnz_limit;                // GLB_ALL_NONZERO (TopkDSA): total gathered nnz >= this => dense allgather path (0 = never)
     int* host_fault;                    // mapped pinned int: fault code mirrored to the host without a sync (may be null)
+    const int* skip;                    // loss scaling: the bucket verdict of unscale_check (null = scaling off); set = return
     int trace;                          // 1: write a TraceRec per call
     int zero_g;                         // 1: the pack pass clears the bucket (the gradient was landed in it)
     int nsrc;                           // gradient-source segments (see kSrcSegMax)
@@ -226,6 +229,7 @@ struct GatherParams {
     int* cand;                // union candidate list (capacity ccap)
     int ccap;
     int* host_fault;
+    const int* skip;          // loss scaling: bucket verdict (null = scaling off)
 };
 
 // ---- gTopk: log2(P) rounds of pairwise list merges toward rank 0, then a broadcast ------------------
@@ -246,6 +250,7 @@ struct TreeParams {
     float* sel_val;
     int selcap;
     int* host_fault;
+    const int* skip;          // loss scaling: bucket verdict (null = scaling off)
 };
 
 // ---- dense allreduce over peer memory -------------------------------------------------------------
@@ -259,6 +264,7 @@ struct DenseParams {
     unsigned long long timeout_ns;
     float* mc;                // multicast (NVLS) mapping of the bucket, or null: switch-side reduction with multimem.*
     int* host_fault;
+    const int* skip;          // loss scaling: bucket verdict (null = scaling off)
 };
 
 // ---- host-callable launchers (implemented in the .cu files) ----------------------------------------
@@ -270,17 +276,62 @@ int gtopk_max_coop_grid(int device);
 int gather_max_coop_grid(int device);
 cudaError_t launch_dense_allreduce(const DenseParams& p, int grid, cudaStream_t stream);
 cudaError_t launch_kth_abs(const float* x, int n, int k, OktState* st, float* out_thr, int grid, cudaStream_t stream);
-// fused optimizer updates: scal -> the step's scalars in device memory ({lr} for SGD and BertAdam)
+// fused optimizer updates: scal -> the step's scalars in device memory ({lr} for SGD and BertAdam); skip -> the step
+// verdict of loss scaling (null = off): when set, p / m / v are left alone and only the gradient is cleared
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
-                             cudaStream_t stream);
+                             const int* skip, cudaStream_t stream);
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
                                    float weight_decay, int zero_grad, const float* scal, const int* fault,
-                                   cudaStream_t stream);
+                                   const int* skip, cudaStream_t stream);
 // torch.optim.Adam / AdamW update; scal -> {1 - lr*wd, -lr / (1 - beta1^t), sqrt(1 - beta2^t)} of this step
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
-                              cudaStream_t stream);
+                              const int* skip, cudaStream_t stream);
+
+// ---- dynamic loss scaling (csrc/scale.cu) ------------------------------------------------------------
+// One per optimizer, in device memory.  found_inf is the step verdict: the OR of the bucket verdicts of the step.
+struct LossScaleDev {
+    float scale;
+    float inv_scale;                  // fp32 of 1 / (double)scale, as torch.amp.GradScaler computes it
+    int growth_tracker;
+    int found_inf;
+    long long skipped;                // steps skipped so far
+    long long adam_step;              // steps applied so far: the bias-correction step of the wrapped Adam
+};
+// One per bucket, device-local: the last-CTA ticket and epoch of unscale_check and the agreed bucket verdict.
+struct ScaleSync {
+    int flag;                         // OR of the CTAs' local non-finite flags (reset by the last CTA)
+    unsigned int ticket;
+    unsigned int epoch;               // completed checks; the mailbox words carry epoch + 1
+    int verdict;                      // 1: some rank saw a non-finite value, every rank skips the bucket's reduction
+};
+constexpr int kScaleThreads = 256;
+constexpr int kScalePerCta = 8192;    // floats per CTA
+struct ScaleParams {
+    LossScaleDev* ls;
+    ScaleSync* sync;
+    int* fault;                       // bucket fault word (OktState::fault)
+    int* host_fault;
+    char* peers[OKT_MAXP];            // every rank's symmetric comm block (the scale mailboxes are at L.scale_mbox)
+    size_t mbox_off;
+    int P, rank;
+    unsigned long long timeout_ns;
+    int nseg;                         // the source table of the direct Ok-Topk path, or one segment = the landed bucket
+    int len[kSrcSegMax];
+    int blk_begin[kSrcSegMax + 1];    // first CTA of segment t (CTAs dealt proportionally to length)
+    float* src[kSrcSegMax];
+};
+static_assert(sizeof(ScaleParams) <= 4096, "ScaleParams must fit the 4 KB kernel-parameter limit");
+cudaError_t launch_unscale_check(const ScaleParams& p, cudaStream_t stream);
+// end of step: growth / backoff of torch._amp_update_scale_, new inv_scale, skipped-step and Adam step counts, verdict
+// cleared.  adam_scalars (start of step): the wrapped Adam's per-group scalars for step adam_step + 1, in double, from
+// hyper = {lr, weight_decay, beta1, beta2} per group into scal (3 floats per group).
+cudaError_t launch_scale_update(LossScaleDev* ls, double growth_factor, double backoff_factor, int growth_interval,
+                                cudaStream_t stream);
+cudaError_t launch_adam_scalars(const LossScaleDev* ls, const double* hyper, float* scal, int groups, cudaStream_t stream);
+// dense switch carry-over under loss scaling: g += res; res = 0 -- unless the bucket verdict is set
+cudaError_t launch_carry_residual(float* g, float* res, int n, const int* skip, cudaStream_t stream);
 // multi-tensor gradient landing: copy up to kLandMax autograd-produced gradient tensors into the flat bucket in ONE launch
 constexpr int kLandMax = 96;
 struct LandParams {

@@ -20,17 +20,28 @@ constexpr int kOptThreads = 256;
 template <int kScal, int kState, typename Upd>
 __device__ __forceinline__ void update_pass(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                                             float* __restrict__ v, int n, bool load, bool store, int zero_grad,
-                                            const float* __restrict__ scal, const int* __restrict__ fault, Upd upd) {
+                                            const float* __restrict__ scal, const int* __restrict__ fault,
+                                            const int* __restrict__ skip, Upd upd) {
     if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
-    float s[kScal];
-#pragma unroll
-    for (int j = 0; j < kScal; ++j) s[j] = scal[j];
     const int n4 = n >> 2;
     float4* p4 = reinterpret_cast<float4*>(p);
     float4* g4 = reinterpret_cast<float4*>(g);
     float4* m4 = reinterpret_cast<float4*>(m);
     float4* v4 = reinterpret_cast<float4*>(v);
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (verdict_set(skip)) {              // loss scaling skips this step: parameters and state stay, the gradient is cleared
+        if (!zero_grad) return;
+        for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
+            const float4 gw = ld_stream_f4(g4 + i);
+            if (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f) g4[i] = zero;
+        }
+        if (blockIdx.x == 0)
+            for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) g[i] = 0.f;
+        return;
+    }
+    float s[kScal];
+#pragma unroll
+    for (int j = 0; j < kScal; ++j) s[j] = scal[j];
     for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
         float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = zero, vw = zero;
         if (load) {
@@ -68,10 +79,11 @@ __global__ void __launch_bounds__(kOptThreads) fused_sgd_kernel(float* __restric
                                                                  float* __restrict__ mom, int n, float momentum,
                                                                  float dampening, float wd, int nesterov, int first,
                                                                  int zero_grad, const float* __restrict__ scal,
-                                                                 const int* __restrict__ fault) {
+                                                                 const int* __restrict__ fault,
+                                                                 const int* __restrict__ skip) {
     const float damp = first ? 0.f : dampening;       // torch: the first step copies d_p into the buffer
     // every rounding spelled out, so that where nvcc contracts into an fma cannot change the result
-    update_pass<1, 1>(p, g, mom, nullptr, n, momentum != 0.f && !first, momentum != 0.f, zero_grad, scal, fault,
+    update_pass<1, 1>(p, g, mom, nullptr, n, momentum != 0.f && !first, momentum != 0.f, zero_grad, scal, fault, skip,
                       [=](const float* s, float& pw, float gw, float& mw, float&) {
                           float d = __fmaf_rn(wd, pw, gw);
                           if (momentum != 0.f) {
@@ -87,8 +99,9 @@ __global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __r
                                                                        float* __restrict__ m, float* __restrict__ v,
                                                                        int n, float b1, float b2, float eps, float wd,
                                                                        int zero_grad, const float* __restrict__ scal,
-                                                                       const int* __restrict__ fault) {
-    update_pass<1, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault,
+                                                                       const int* __restrict__ fault,
+                                                                       const int* __restrict__ skip) {
+    update_pass<1, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip,
                       [=](const float* s, float& pw, float gw, float& mw, float& vw) {
                           mw = b1 * mw + (1.f - b1) * gw;
                           vw = b2 * vw + (1.f - b2) * gw * gw;
@@ -109,10 +122,11 @@ __global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restri
                                                                   float w, float b2, float omb2, float eps, float wd,
                                                                   int decoupled, int zero_grad,
                                                                   const float* __restrict__ scal,
-                                                                  const int* __restrict__ fault) {
+                                                                  const int* __restrict__ fault,
+                                                                  const int* __restrict__ skip) {
     const bool small_w = fabsf(w) < 0.5f;
     const float lw = small_w ? w : 1.f - w;
-    update_pass<3, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault,
+    update_pass<3, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip,
                       [=](const float* s, float& pw, float gw, float& mw, float& vw) {
                           const float decay = s[0], step_size = s[1], bc2_sqrt = s[2];
                           if (decoupled) pw = pw * decay;                  // decay == 1 exactly when wd == 0
@@ -170,27 +184,27 @@ static inline int opt_grid(int n) {
 
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
-                             cudaStream_t stream) {
+                             const int* skip, cudaStream_t stream) {
     fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, momentum, dampening, weight_decay, nesterov,
-                                                             first_step, zero_grad, scal, fault);
+                                                             first_step, zero_grad, scal, fault, skip);
     return cudaGetLastError();
 }
 
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
                                    float weight_decay, int zero_grad, const float* scal, const int* fault,
-                                   cudaStream_t stream) {
+                                   const int* skip, cudaStream_t stream) {
     fused_bert_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, b1, b2, eps, weight_decay, zero_grad,
-                                                                   scal, fault);
+                                                                   scal, fault, skip);
     return cudaGetLastError();
 }
 
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
-                              cudaStream_t stream) {
+                              const int* skip, cudaStream_t stream) {
     // 1 - beta in double, rounded once: torch passes these factors as Python floats
     fused_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, (float)(1.0 - beta1), (float)beta2,
                                                               (float)(1.0 - beta2), eps, weight_decay, decoupled,
-                                                              zero_grad, scal, fault);
+                                                              zero_grad, scal, fault, skip);
     return cudaGetLastError();
 }
 

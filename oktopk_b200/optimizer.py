@@ -29,18 +29,91 @@ from typing import Dict, Iterable, List, Optional
 import torch
 
 from .compression import NoneCompressor, compressors, resolve_compressor
-from .config import OkTopkConfig
+from .config import LossScale, OkTopkConfig
 from .ops import ext
 from .parallel.allreducer import AllReducer
 from .parallel.buckets import Bucket, attach, build_buckets
 from .parallel.world import World, world as _world
 
 
+# ====================================================================================== loss scaling
+class _ScaleState:
+    """The optimizer's loss-scale state, laid out as the kernels' ``LossScaleDev`` (csrc/oktopk.cuh) in one small
+    tensor on the parameters' device: scale, inv_scale (fp32), growth tracker, step verdict (int32), skipped steps and
+    the wrapped Adam's applied-step count (int64).  On the CUDA engine the check and the update run on the device
+    (csrc/scale.cu); elsewhere the same rules run in torch ops with a host read of the verdict."""
+
+    def __init__(self, ls: LossScale, device: torch.device):
+        self.cfg = ls
+        self.buf = torch.zeros(32, dtype=torch.uint8, device=device)
+        self.f32 = self.buf[0:8].view(torch.float32)          # scale, inv_scale
+        self.i32 = self.buf[8:16].view(torch.int32)           # growth_tracker, found_inf
+        self.i64 = self.buf[16:32].view(torch.int64)          # skipped, adam_step
+        self.native = device.type == "cuda" and ext.available()
+        self.reset()
+
+    @property
+    def ptr(self) -> int:
+        return self.buf.data_ptr()
+
+    @property
+    def found_ptr(self) -> int:
+        return self.buf.data_ptr() + 12
+
+    def reset(self, scale: Optional[float] = None, growth_tracker: int = 0, skipped: int = 0, adam_step: int = 0) -> None:
+        from .parallel.oracle import inv_scale_of
+        scale = self.cfg.init_scale if scale is None else scale
+        vals = torch.zeros(32, dtype=torch.uint8)
+        vals[0:8].view(torch.float32).copy_(torch.tensor([scale, inv_scale_of(scale)], dtype=torch.float32))
+        vals[8:16].view(torch.int32).copy_(torch.tensor([growth_tracker, 0], dtype=torch.int32))
+        vals[16:32].view(torch.int64).copy_(torch.tensor([skipped, adam_step], dtype=torch.int64))
+        self.buf.copy_(vals)
+
+    def scale(self) -> torch.Tensor:
+        return self.f32[0]
+
+    def state(self) -> Dict:
+        """Synchronous read."""
+        h = self.buf.cpu()
+        f, i, q = h[0:8].view(torch.float32), h[8:16].view(torch.int32), h[16:32].view(torch.int64)
+        return {"scale": float(f[0]), "growth_tracker": int(i[0]), "skipped_steps": int(q[0]), "adam_step": int(q[1]),
+                "found_inf": int(i[1])}
+
+    def found_host(self) -> bool:
+        return bool(self.i32[1].item())
+
+    def check_host(self, flat: torch.Tensor, world: World) -> bool:
+        """The torch-ops form of unscale_check (``backend='dist'``): unscale ``flat`` in place, agree across ranks on
+        whether any of them saw a non-finite value (a host read), and fold the verdict into the step's."""
+        with torch.no_grad():
+            bad = (~torch.isfinite(flat)).any().to(torch.int32).reshape(1)
+            flat.mul_(self.f32[1])
+            world.all_reduce_sum(bad)
+            skip = bool(bad.item())
+            if skip:
+                self.i32[1].fill_(1)
+        return skip
+
+    def update(self) -> None:
+        """End of step: growth / backoff, counters, verdict cleared (on the current stream)."""
+        c = self.cfg
+        if self.native:
+            ext.require().scale_update(self.ptr, float(c.growth_factor), float(c.backoff_factor), int(c.growth_interval),
+                                       torch.cuda.current_stream().cuda_stream)
+            return
+        from .parallel.oracle import update_scale
+        st = self.state()
+        found = bool(st["found_inf"])
+        scale, tracker = update_scale(st["scale"], st["growth_tracker"], found, c)
+        self.reset(scale, tracker, st["skipped_steps"] + int(found), st["adam_step"] + int(not found))
+
+
 # ====================================================================================== comm mixin
 class _BucketedComm:
     """Bucket bookkeeping, autograd hooks, stream choreography.  Mixed into optimizer classes."""
 
-    def _okt_setup(self, named_parameters, allreducer: AllReducer, flatten_params: bool = True) -> None:
+    def _okt_setup(self, named_parameters, allreducer: AllReducer, flatten_params: bool = True,
+                   loss_scale: Optional[LossScale] = None) -> None:
         if named_parameters is not None:
             named_parameters = list(named_parameters)
             if any(not isinstance(p, tuple) for p in named_parameters):
@@ -60,6 +133,7 @@ class _BucketedComm:
         self._cfg: OkTopkConfig = allreducer.cfg
         self.local = False
         self._synced = False
+        self._ls: Optional[_ScaleState] = None
         self.momentum_correction = False
         self._buckets: List[Bucket] = build_buckets(self.param_groups, names, self._cfg.bucket_elems)
         self._bucket_of: Dict[torch.nn.Parameter, Bucket] = {}
@@ -101,16 +175,24 @@ class _BucketedComm:
             # kernels retire CTAs, not after the whole backward queue
             self._comm_stream = torch.cuda.Stream(priority=-1)
         allreducer.add_resync_hook(self._resync_replicas)
+        if loss_scale is not None:
+            allreducer.enable_loss_scaling()
+            self._ls = _ScaleState(loss_scale, self._buckets[0].params[0].device if self._buckets else torch.device("cpu"))
         # device-resident per-group scalars (the learning rate; for wrapped Adam the step's decay, step size and bias
         # correction): the fused update kernels read them from memory so that a captured CUDA graph of the whole step
         # stays valid when the schedule moves
-        self._lr_dev = None
+        # With loss scaling the wrapped Adam's step count is on the device (a skipped step does not advance it): the host
+        # stages {lr, weight_decay, beta1, beta2} per group in double (_hyper_dev) and a kernel derives the scalars.
+        self._lr_dev = self._hyper_dev = None
         self._lr_pin, self._lr_ev, self._lr_ring, self._lr_last = [], [], 0, None
         dev0 = self._buckets[0].params[0].device if self._buckets else torch.device("cpu")
         if dev0.type == "cuda" and ext.available() and self._update is not None:
-            n = max(len(self.param_groups), 1) * self._update.n_scalars
-            self._lr_dev = torch.zeros(n, dtype=torch.float32, device=dev0)
-            self._lr_pin = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(8)]
+            groups = max(len(self.param_groups), 1)
+            self._lr_dev = torch.zeros(groups * self._update.n_scalars, dtype=torch.float32, device=dev0)
+            stage = self._lr_dev
+            if self._ls is not None and self._update is _AdamUpdate:
+                stage = self._hyper_dev = torch.zeros(groups * 4, dtype=torch.float64, device=dev0)
+            self._lr_pin = [torch.zeros_like(stage, device="cpu").pin_memory() for _ in range(8)]
             self._lr_ev = [None] * len(self._lr_pin)
 
     def _resync_replicas(self) -> None:
@@ -145,11 +227,11 @@ class _BucketedComm:
         pin = self._lr_pin[self._lr_ring]
         if self._lr_ev[self._lr_ring] is not None:          # the host may run many (graph-replayed) steps ahead:
             self._lr_ev[self._lr_ring].synchronize()        # never overwrite a staging slot whose copy is pending
-        n = self._update.n_scalars
+        n = len(vals[0]) if vals else 0
         for gi, sc in enumerate(vals):
             for j, v in enumerate(sc):
                 pin[gi * n + j] = v
-        self._lr_dev.copy_(pin, non_blocking=True)
+        (self._hyper_dev if self._hyper_dev is not None else self._lr_dev).copy_(pin, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
         self._lr_ev[self._lr_ring] = ev
@@ -244,10 +326,10 @@ class _BucketedComm:
             ev.record(torch.cuda.current_stream())
             self._comm_stream.wait_event(ev)
             with torch.cuda.stream(self._comm_stream):
-                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream, srcs=srcs)
+                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream, srcs=srcs, scale=self._ls)
                 b.event.record(self._comm_stream)
         else:
-            self._allreducer.reduce_bucket(b.name, b.grad, srcs=srcs)
+            self._allreducer.reduce_bucket(b.name, b.grad, srcs=srcs, scale=self._ls)
 
     def _apply_momentum_correction(self, b: Bucket) -> None:
         """``VGG/distributed_optimizer.py:81-88``: communicate the momentum-accumulated gradient."""
@@ -261,6 +343,48 @@ class _BucketedComm:
         else:
             buf.mul_(0.9).add_(b.grad)
             b.grad.copy_(buf)
+
+    # ------------------------------------------------------------------ loss scaling
+    @property
+    def momentum_correction(self) -> bool:
+        return self._momentum_correction
+
+    @momentum_correction.setter
+    def momentum_correction(self, on: bool) -> None:
+        if on and getattr(self, "_ls", None) is not None:
+            raise ValueError("loss_scale cannot be combined with momentum_correction: the momentum buffer would absorb "
+                             "the gradient of a skipped step")
+        self._momentum_correction = bool(on)
+
+    def scale_loss(self, loss: torch.Tensor) -> torch.Tensor:
+        """``loss * scale`` with the scale read from device memory (no synchronisation, capturable).  Without a
+        ``loss_scale`` the loss is returned as is."""
+        if self._ls is None:
+            return loss
+        return loss * self._ls.scale()
+
+    def loss_scale_state(self) -> Optional[Dict]:
+        """``{scale, growth_tracker, skipped_steps}`` (a synchronous read: logging and tests), None without scaling."""
+        if self._ls is None:
+            return None
+        st = self._ls.state()
+        return {k: st[k] for k in ("scale", "growth_tracker", "skipped_steps")}
+
+    def _scale_state_dict(self) -> Optional[Dict]:
+        if self._ls is None:
+            return None
+        st = self._ls.state()
+        st.pop("found_inf")
+        return st
+
+    def _load_scale_state(self, sd: Optional[Dict], adam_step: int) -> None:
+        """A checkpoint without scale state starts from ``init_scale``."""
+        if self._ls is None:
+            return
+        if sd is None:
+            self._ls.reset(adam_step=adam_step)
+        else:
+            self._ls.reset(sd["scale"], sd["growth_tracker"], sd["skipped_steps"], sd.get("adam_step", adam_step))
 
     # ------------------------------------------------------------------ public API
     def synchronize(self) -> None:
@@ -338,18 +462,31 @@ class _BucketedComm:
                 loss = closure()
         if not self.local:
             self.synchronize()
+        # the fused kernels read the step verdict themselves; the torch update paths need it on the host
+        host_skip = self._ls is not None and not self._device_update() and self._ls.found_host()
         if self._update is None:
-            super().step()
+            if not host_skip:
+                super().step()
             for b in self._buckets:
                 b.dirty = True
         else:
             self._maybe_refresh_lr()
+            if self._hyper_dev is not None and self._update is _AdamUpdate:
+                ext.require().adam_scalars(self._ls.ptr, self._hyper_dev.data_ptr(), self._lr_dev.data_ptr(),
+                                           len(self.param_groups), torch.cuda.current_stream().cuda_stream)
             with torch.no_grad():
                 for b in self._buckets:
-                    self._fused_update(b)
+                    self._fused_update(b, host_skip)
             self.counter += 1
+        if self._ls is not None:
+            self._ls.update()
         self._after_step()
         return loss
+
+    def _device_update(self) -> bool:
+        """Every bucket is updated by a fused kernel (which reads the step verdict of loss scaling on the device)."""
+        return self._update is not None and self._lr_dev is not None and all(
+            b.grad.is_cuda and b.flat_param is not None for b in self._buckets)
 
     def _flat_buffers(self, b: Bucket) -> Dict[str, torch.Tensor]:
         """The bucket's flat state buffers, one per state key of the update, allocated zeroed on first use;
@@ -362,18 +499,21 @@ class _BucketedComm:
                     self.state[p][k] = v
         return fs
 
-    def _fused_update(self, b: Bucket) -> None:
+    def _fused_update(self, b: Bucket, host_skip: bool = False) -> None:
         first = self._update.keys[0] not in self._flat_state.get(b.index, {})
         fs = self._flat_buffers(b)
         on_gpu = b.grad.is_cuda and b.flat_param is not None and ext.available()
         # after a landing step the next landing copy overwrites the whole bucket: it need not be cleared
         zero_grad = 0 if self._land and not self._direct else 1
+        skip_ptr = self._ls.found_ptr if self._ls is not None else 0
         for gi, s, e in b.group_slices:
             def launch(fn, *hyper):
                 fn(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
                    *(fs[k].data_ptr() + 4 * s for k in self._update.keys), e - s, *hyper, zero_grad,
-                   torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi), self._allreducer.fault_ptr(b.name))
-            self._update.update(self, b, self.param_groups[gi], s, e, fs, first, launch if on_gpu else None)
+                   torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi), self._allreducer.fault_ptr(b.name),
+                   skip_ptr)
+            if on_gpu or not host_skip:
+                self._update.update(self, b, self.param_groups[gi], s, e, fs, first, launch if on_gpu else None)
             if not on_gpu:
                 b.grad[s:e].zero_()
         b.dirty = False
@@ -470,6 +610,8 @@ class _AdamUpdate:
 
     @staticmethod
     def scalars(opt, g):
+        if opt._hyper_dev is not None:            # loss scaling: the device knows t (csrc/scale.cu adam_scalars)
+            return (float(g["lr"]), float(g["weight_decay"]), float(g["betas"][0]), float(g["betas"][1]))
         # torch's non-capturable Adam, in double: t = the step about to run
         lr, (b1, b2), t = float(g["lr"]), g["betas"], float(opt.counter + 1)
         return (1 - lr * g["weight_decay"], (lr / (1 - b1 ** t)) * -1, (1 - b2 ** t) ** 0.5)
@@ -524,20 +666,25 @@ class _BertAdamUpdate:
 class _DistributedOptimizerMixin(_BucketedComm):
     def state_dict(self):
         sd = super().state_dict()
+        scale = self._scale_state_dict()
         if self._update is _AdamUpdate:           # torch's fused Adam format: a float32 0-dim step on the param's device
             params = [p for g in self.param_groups for p in g["params"]]
+            steps = scale["adam_step"] if scale is not None else self.counter     # skipped steps do not count
             for i, st in list(sd["state"].items()):
-                sd["state"][i] = dict(st, step=torch.tensor(float(self.counter), dtype=torch.float32,
-                                                            device=params[i].device))
+                sd["state"][i] = dict(st, step=torch.tensor(float(steps), dtype=torch.float32, device=params[i].device))
         sd["oktopk"] = self._allreducer.state_dict()
+        if scale is not None:
+            sd["loss_scale"] = scale
         return sd
 
     def load_state_dict(self, state_dict):
         state_dict = dict(state_dict)
         okt = state_dict.pop("oktopk", None)
+        scale = state_dict.pop("loss_scale", None)
         super().load_state_dict(state_dict)
         if self._update is not None:
             self._adopt_state()
+        self._load_scale_state(scale, getattr(self, "counter", 0))
         if okt is not None:
             self._allreducer.load_state_dict(okt)
         self._clear_buckets()
@@ -547,12 +694,15 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
                          is_sparse: bool = False, err_handler=None, layerwise_times=None, sigma_scale: float = 2.5,
                          density: float = 0.1, norm_clip: Optional[float] = None, writer=None,
                          cfg: Optional[OkTopkConfig] = None, world: Optional[World] = None,
-                         backend: Optional[str] = None, flatten_params: bool = True):
+                         backend: Optional[str] = None, flatten_params: bool = True,
+                         loss_scale: Optional[LossScale] = None):
     """Wrap ``optimizer`` so that ``step()`` first allreduces the gradients with the chosen scheme.
 
     Horovod-style dynamic subclass of the user's optimizer class, as in the reference
     (``VGG/distributed_optimizer.py:203-207``).  ``compression`` may be a registry key, a compressor
     class (``compressors['oktopk']``) or an instance; ``cfg`` overrides the scalar arguments.
+    ``loss_scale``: dynamic loss scaling for fp16 training (see ``LossScale``); back-propagate
+    ``opt.scale_loss(loss)``.
     """
     base_cls = optimizer.__class__
     cls = type(base_cls.__name__, (_DistributedOptimizerMixin, base_cls), {})
@@ -570,9 +720,10 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
         obj._update = None                        # torch's own step()
     if obj._update is not None:
         obj.counter = 0                           # steps taken: Adam's bias correction (GraphedTrainStep keeps it too)
-    obj._okt_setup(named_parameters, ar, flatten_params=flatten_params)
+    obj._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale)
     if obj._update is not None and obj.state:
         obj._adopt_state()
+        obj._load_scale_state(None, obj.counter)
     return obj
 
 
@@ -661,7 +812,8 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, warmup=-1, t_total=-1, schedule="warmup_linear", b1=0.9, b2=0.999, e=1e-6,
                  weight_decay=0.01, max_grad_norm=1.0, density=1.0, compressor="none", rank=-1, named_parameters=None,
                  cfg: Optional[OkTopkConfig] = None, world: Optional[World] = None, backend: Optional[str] = None,
-                 clip_reduced: bool = False, flatten_params: bool = True, **_ignored):
+                 clip_reduced: bool = False, flatten_params: bool = True, loss_scale: Optional[LossScale] = None,
+                 **_ignored):
         if lr < 0.0:
             raise ValueError("Invalid learning rate: {} - should be >= 0.0".format(lr))
         if schedule not in SCHEDULES:
@@ -683,7 +835,7 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
             global_adapt_high=5 / 4, global_adapt_inc=1.036, global_adapt_dec=1.025, balanced_allgather=True)
         ar = AllReducer(compression=compressor, sparse=(compressor != "none"), density=density,
                         cfg=base.replace(density=density), world=world, backend=backend)
-        self._okt_setup(named_parameters, ar, flatten_params=flatten_params)
+        self._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale)
 
     def get_lr(self) -> List[float]:
         out = []
@@ -703,14 +855,19 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
             sd["state"][i] = dict(st, step=self.counter)
         sd["oktopk"] = self._allreducer.state_dict()
         sd["counter"] = self.counter
+        scale = self._scale_state_dict()
+        if scale is not None:
+            sd["loss_scale"] = scale
         return sd
 
     def load_state_dict(self, state_dict):
         state_dict = dict(state_dict)
         okt = state_dict.pop("oktopk", None)
         counter = state_dict.pop("counter", 0)
+        scale = state_dict.pop("loss_scale", None)
         torch.optim.Optimizer.load_state_dict(self, state_dict)
         self._adopt_state(counter)
+        self._load_scale_state(scale, counter)
         if okt is not None:
             self._allreducer.load_state_dict(okt)
         self._clear_buckets()

@@ -95,17 +95,33 @@ class AllReducer:
             return False
         return eng.reads_sources(self.compressor.name, self.get_current_density())
 
-    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None, srcs=None) -> torch.Tensor:
+    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None, srcs=None, scale=None) -> torch.Tensor:
         """Reduce bucket ``name`` in place.  ``srcs = (pointers, offsets, lengths)``: the gradient is in these fp32
-        tensors rather than in ``flat``, which must then be all-zero (only where ``reads_sources(name)``)."""
+        tensors rather than in ``flat``, which must then be all-zero (only where ``reads_sources(name)``).
+
+        ``scale``: the optimizer's loss-scale state (``optimizer._ScaleState``).  The gradient is unscaled first, and the
+        reduction is skipped on every rank when any rank's bucket holds a non-finite value (``config.LossScale``)."""
+        skip = 0
+        if scale is not None:
+            eng = self._engines.get(name)
+            if eng is not None:                   # on the device: no host synchronisation, graph-replayable
+                eng.unscale_check(scale.ptr, stream, srcs)
+                skip = eng.verdict_ptr
+            elif scale.check_host(flat, self.world):
+                st = self._dist_states.get(name)
+                if st is None:
+                    st = self._dist_states[name] = SparseState(flat.numel(), self.world.size)
+                st.counter += 1
+                return flat
         density = self.get_current_density()
         from ..utils import settings
         if settings.PROFILING_GRAD and self.cfg.sparse:
             self._dump_grad(name, flat, density)
         if settings.PROFILING_NORM and self.cfg.sparse:
-            return self._reduce_profiled(name, flat, stream, density)
+            return self._reduce_profiled(name, flat, stream, density, skip)
         if name in self._engines:
-            out = self._engines[name].reduce(self.compressor.name, density, stream=stream, g=flat, srcs=srcs)
+            out = self._engines[name].reduce(self.compressor.name, density, stream=stream, g=flat, srcs=srcs,
+                                             skip=skip)
             if settings.PROFILING:
                 self._profile_iteration(name)
             return out
@@ -202,7 +218,7 @@ class AllReducer:
             np.save(os.path.join(directory, "%s-rank%d-epoch%d.npy" % (nm, self.world.rank, epoch)), np.asarray(col))
         self._profiling_norms = []
 
-    def _reduce_profiled(self, name: str, flat: torch.Tensor, stream, density: float) -> torch.Tensor:
+    def _reduce_profiled(self, name: str, flat: torch.Tensor, stream, density: float, skip: int = 0) -> torch.Tensor:
         """``settings.PROFILING_NORM`` (``VGG/allreducer.py:584-606,1072-1080``): one extra dense allreduce of the
         error-compensated gradient per step gives the true global top-k, against which the sparse result's relative
         error (the paper's xi) and the selected counts are recorded.  Diagnostic mode: synchronous and slow."""
@@ -218,7 +234,7 @@ class AllReducer:
                 self.world.all_reduce_sum(acc)
             acc /= self.world.size
         if eng is not None:
-            out = eng.reduce(self.compressor.name, density, stream=stream, g=flat)
+            out = eng.reduce(self.compressor.name, density, stream=stream, g=flat, skip=skip)
             if flat.is_cuda:
                 torch.cuda.synchronize()
         else:
@@ -273,6 +289,10 @@ class AllReducer:
                        "volume_elems": st.last_volume_elems, "mode": st.last_mode,
                        "edges": st.region_offsets + [st.numel]}
         return out if name is None else out[name]
+
+    def enable_loss_scaling(self) -> None:
+        for eng in self._engines.values():
+            eng.enable_loss_scaling()
 
     def fault_ptr(self, name: str) -> int:
         """Device address of the bucket's fault word (the fused optimizer kernels skip the update when it is set)."""

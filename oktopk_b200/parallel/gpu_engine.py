@@ -102,6 +102,7 @@ class CudaBucketEngine:
         self.fault_ptr = C.fault_ptr(self.state_ptr)
         self.host_flag, self.host_flag_dev = C.host_flag_alloc()      # fault code mirrored to pinned host memory
         self.dense_epoch_ptr = C.dev_alloc_zero(8 * self.dense_grid)
+        self.scale_sync_ptr = 0                  # loss scaling: check ticket, epoch, bucket verdict (enable_loss_scaling)
         self.residual = torch.zeros(self.n, dtype=torch.float32, device=self.device)
         # first-touch candidate list of the reduce phase: at most one entry per distinct index of my region
         # (also: pre-filtered candidates of the exact-threshold radix select, union lists of TopkA2 / gTopk)
@@ -117,6 +118,7 @@ class CudaBucketEngine:
         self._dist_state: Optional[SparseState] = None
         self.last_mode = ""
         self._res_clean = False                  # True while the residual is known to be all-zero (dense-switch calls)
+        self._skip = 0                           # bucket verdict address of the running call (loss scaling), 0 = off
 
     # ------------------------------------------------------------------ helpers
     def _stream(self, stream: Optional[torch.cuda.Stream]) -> int:
@@ -139,13 +141,39 @@ class CudaBucketEngine:
         return (compressor == "oktopk" and cfg.sparse and self.host.counter >= cfg.warmup_iters
                 and not self._dense_switch(compressor, density))
 
+    def enable_loss_scaling(self) -> None:
+        """Allocate the device words of ``unscale_check`` (before any graph capture; a no-op when already done)."""
+        if not self.scale_sync_ptr:
+            self.scale_sync_ptr = self.C.dev_alloc_zero(self.C.SCALE_SYNC_BYTES)
+
+    @property
+    def verdict_ptr(self) -> int:
+        """Device address of the bucket verdict that ``unscale_check`` writes and ``reduce(skip=...)`` reads."""
+        self.enable_loss_scaling()
+        return self.scale_sync_ptr + self.C.VERDICT_OFFSET
+
+    def unscale_check(self, loss_scale_ptr: int, stream: Optional[torch.cuda.Stream] = None,
+                      srcs: Optional[tuple] = None) -> None:
+        """Loss scaling, before ``reduce(skip=self.verdict_ptr)``: multiply the gradient (the ``srcs`` tensors, else the
+        bucket) by the optimizer's inv_scale in place and agree with every peer on the bucket verdict (set if any rank
+        saw a non-finite value; ORed into the step verdict)."""
+        self.enable_loss_scaling()
+        if srcs is not None and len(srcs[0]):
+            ptrs, lens = list(srcs[0]), list(srcs[2])
+        else:                                      # the landed bucket (or, with no gradient at all, the all-zero one)
+            ptrs, lens = [self.grad.data_ptr()], [self.n]
+        self.C.unscale_check(ptrs, lens, loss_scale_ptr, self.scale_sync_ptr, self.state_ptr, self.host_flag_dev,
+                             self.peer_comm, self.layout["scale_mbox"], self.rank, float(self.cfg.peer_timeout_s),
+                             self._stream(stream))
+
     def reduce(self, compressor: str, density: Optional[float] = None,
                stream: Optional[torch.cuda.Stream] = None, g: Optional[torch.Tensor] = None,
-               srcs: Optional[tuple] = None) -> torch.Tensor:
+               srcs: Optional[tuple] = None, skip: int = 0) -> torch.Tensor:
         """Allreduce this bucket in place (``self.grad`` unless an external ``g`` is given).
 
         ``srcs = (pointers, offsets, lengths)``: the gradient is not in the bucket but in these fp32 tensors, at these
-        element offsets of the bucket (Ok-Topk only, see ``reads_sources``); the result is written into the bucket."""
+        element offsets of the bucket (Ok-Topk only, see ``reads_sources``); the result is written into the bucket.
+        ``skip``: device address of the bucket verdict of loss scaling (0 = off); when set the kernels return at entry."""
         if srcs is not None and (g is not None and g.data_ptr() != self.grad.data_ptr()
                                  or not self.reads_sources(compressor, density)):
             raise ValueError("gradient sources are only read by an Ok-Topk call on the engine's own bucket")
@@ -154,6 +182,7 @@ class CudaBucketEngine:
         ext_g = g is not None and g.data_ptr() != self.grad.data_ptr()
         dense = (not cfg.sparse) or compressor in ("none", None) or st.counter < cfg.warmup_iters
         s = self._stream(stream)
+        self._skip = int(skip)
         if dense:
             if ext_g:
                 self.grad.copy_(g)
@@ -166,7 +195,9 @@ class CudaBucketEngine:
             # (nothing is left behind, so the residual is cleared) -- OkTopkConfig.dense_switch_density
             if ext_g:
                 self.grad.copy_(g)
-            if not self._res_clean:                # a dense call leaves nothing behind: after the first switched call
+            if self._skip:                         # under loss scaling a skipped call keeps its residual: always carry
+                self.C.carry_residual(self.grad.data_ptr(), self.residual.data_ptr(), self.n, self._skip, s)
+            elif not self._res_clean:              # a dense call leaves nothing behind: after the first switched call
                 self.grad.add_(self.residual)      # the residual is known to be all-zero and the carry-over is skipped
                 self.residual.zero_()
                 self._res_clean = True
@@ -201,7 +232,7 @@ class CudaBucketEngine:
             return
         self.C.dense_run(self.peer_grad, self.peer_flags, self.dense_epoch_ptr, self.n, self.rank,
                          self.dense_grid, s, self.state_ptr, float(self.cfg.peer_timeout_s), self.mc_grad,
-                         self.host_flag_dev)
+                         self.host_flag_dev, self._skip)
 
     def _fused(self, compressor: str, density: Optional[float], s: int, g: torch.Tensor,
                srcs: Optional[tuple] = None) -> None:
@@ -243,6 +274,8 @@ class CudaBucketEngine:
                 o["peer_g"] = self.peer_grad
         if srcs is not None:
             o["srcs"] = srcs
+        if self._skip:
+            o["skip"] = self._skip
         self.C.oktopk_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                           self.rank, k, self.cap, self.gcap, o, self.grid, s)
         self.last_mode = compressor
@@ -268,6 +301,8 @@ class CudaBucketEngine:
             o["gauss_mode"] = {"vgg": 0, "lstm": 1, "bert": 2}[cfg.gaussian_mode]
             o["gauss_loops"] = cfg.gaussian_loops
             o["gauss_factor"] = cfg.gaussian_factor
+        if self._skip:
+            o["skip"] = self._skip
         self.C.gather_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                           self.rank, k, self.cap, self.gcap, o, self.gather_grid, s)
         self.last_mode = compressor
@@ -291,6 +326,8 @@ class CudaBucketEngine:
                    "selcap": self._sel[2]}
         if cfg.norm_clip is not None:
             o["clip_max_norm"] = float((1.0 / self.P) ** 0.5 * cfg.norm_clip)
+        if self._skip:
+            o["skip"] = self._skip
         self.C.gtopk_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                          self.rank, k, self.cap, self.gcap, o, self.tree_grid, s)
         self.last_mode = compressor
@@ -333,7 +370,8 @@ class CudaBucketEngine:
         code = int(self.stats().get("fault", 0))
         if code:
             names = {1: "reduce-scatter mailbox", 2: "allgather mailbox", 3: "region-cut mailbox", 4: "dense barrier",
-                     5: "gTopk tree mailbox", 6: "dense-fallback done flags"}
+                     5: "gTopk tree mailbox", 6: "dense-fallback done flags",
+                     7: "loss-scale verdict mailbox"}
             raise PeerTimeoutError("bucket %s: peer wait timed out in the %s (fault %d, timeout %.1fs)"
                                    % (self.name, names.get(code, "?"), code, self.cfg.peer_timeout_s))
 
@@ -380,7 +418,7 @@ class CudaBucketEngine:
         except Exception:  # noqa: BLE001
             pass
         self.host_flag = 0
-        for attr in ("state_ptr", "dense_epoch_ptr"):
+        for attr in ("state_ptr", "dense_epoch_ptr", "scale_sync_ptr"):
             ptr = getattr(self, attr, 0)
             if ptr:
                 try:

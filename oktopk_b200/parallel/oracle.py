@@ -462,3 +462,42 @@ def run_oracle(name: str, grads, states, cfg: OkTopkConfig, density=None):
     for st in states:
         st.counter += 1
     return out
+
+
+# --------------------------------------------------------------------------- dynamic loss scaling (config.LossScale)
+def inv_scale_of(scale: float) -> float:
+    """``torch.amp.GradScaler``'s inverse scale: the fp32 reciprocal of the scale computed in double."""
+    return float(_np.float32(1.0 / float(_np.float32(scale))))
+
+
+def update_scale(scale: float, growth_tracker: int, found_inf: bool, ls) -> Tuple[float, int]:
+    """``torch._amp_update_scale_``: back off on a skipped step, grow after ``growth_interval`` clean steps (fp32 scale,
+    products in double)."""
+    if found_inf:
+        return float(_np.float32(float(scale) * ls.backoff_factor)), 0
+    successful = growth_tracker + 1
+    if successful == ls.growth_interval:
+        with _np.errstate(over="ignore"):
+            grown = _np.float32(float(scale) * ls.growth_factor)
+        return (float(grown) if _np.isfinite(grown) else scale), 0
+    return scale, successful
+
+
+def unscale_check_oracle(grads: List[torch.Tensor], inv_scale: float) -> bool:
+    """Every rank's bucket is multiplied by ``inv_scale`` in place; returns the verdict all ranks agree on: True if any
+    rank's bucket held a non-finite value (checked on the incoming values)."""
+    bad = False
+    for g in grads:
+        bad |= bool((~torch.isfinite(g)).any())
+        g.mul_(torch.tensor(inv_scale, dtype=torch.float32))
+    return bad
+
+
+def run_oracle_scaled(name: str, grads, states, cfg: OkTopkConfig, inv_scale: float, density=None):
+    """One reduction under loss scaling: unscale, agree, and either skip -- residuals, thresholds and region edges
+    untouched, counters advanced -- or reduce the unscaled gradients.  Returns (results or None, skipped)."""
+    if unscale_check_oracle(grads, inv_scale):
+        for st in states:
+            st.counter += 1
+        return None, True
+    return run_oracle(name, grads, states, cfg, density), False

@@ -64,6 +64,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--cuda-graph", action="store_true", help="capture forward+backward+allreduce+update into CUDA graphs")
     p.add_argument("--fp16", action="store_true", help="fp16 autocast (reference: apex amp O3, main_bert.py:1009-1023)")
     p.add_argument("--bf16", action="store_true", help="bf16 autocast")
+    p.add_argument("--loss-scale", type=str, default=None,
+                   help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
     p.add_argument("--dataparallel", action="store_true", help="accepted for parity: data parallelism is the only mode")
     p.add_argument("--do_train", action="store_true", help="accepted for parity")
@@ -121,7 +123,7 @@ def main(argv=None) -> int:
                      density=args.density, max_iters=args.max_iters, checkpoint_dir=args.checkpoint_dir, cfg=cfg,
                      log_dir=args.log_dir, seq_len=args.max_seq_length, seed=args.seed, backend=args.backend,
                      cuda_graph=args.cuda_graph, model_kwargs=model_kwargs or None, norm_clip=args.norm_clip,
-                     autocast="bf16" if args.bf16 else ("fp16" if args.fp16 else None))
+                     autocast="bf16" if args.bf16 else ("fp16" if args.fp16 else None), loss_scale=args.loss_scale)
     if args.trace:
         import json
         os.makedirs(args.trace, exist_ok=True)

@@ -126,9 +126,13 @@ class GraphedTrainStep:
         tr = self.tr
         self.opt.zero_grad()
         loss, _ = tr._forward_loss(batch)
-        loss.backward()
+        self._backward(loss)
         tr.update_model()
         return loss.detach()
+
+    def _backward(self, loss: torch.Tensor) -> None:
+        # with loss scaling the scale is read from device memory: the captured graph stays valid when it moves
+        (self.opt.scale_loss(loss) if getattr(self.opt, "_ls", None) is not None else loss).backward()
 
     def step(self, batch) -> torch.Tensor:
         """Run one optimizer step on ``batch`` (device tensors); returns the (device) loss."""
@@ -180,7 +184,7 @@ class GraphedTrainStep:
             with torch.cuda.graph(g, pool=self.pool):
                 self.opt.zero_grad()
                 loss, _ = tr._forward_loss(self.static_in)
-                loss.backward()
+                self._backward(loss)
                 tr.update_model()
                 out = loss.detach()
             if self.static_loss is None:

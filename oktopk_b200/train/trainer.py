@@ -20,7 +20,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import compression as _comp
-from ..config import OkTopkConfig, preset as _preset
+from ..config import LossScale, OkTopkConfig, preset as _preset
 from ..models import create_net
 from ..optimizer import BertAdam, DistributedOptimizer, broadcast_parameters
 from ..parallel.world import World, world as _world
@@ -49,7 +49,7 @@ class Trainer:
                  seed: int = 0, prefix: str = "run", log_dir: Optional[str] = None, num_workers: int = 0,
                  seq_len: int = 128, t_total: int = -1, warmup: float = -1, pretrain: Optional[str] = None,
                  norm_clip: Optional[float] = None, backend: Optional[str] = None, cuda_graph: bool = False,
-                 model_kwargs: Optional[dict] = None, autocast: Optional[str] = None):
+                 model_kwargs: Optional[dict] = None, autocast: Optional[str] = None, loss_scale=None):
         self.world = world or _world()
         self.rank, self.nworkers = self.world.rank, self.world.size
         # The host side of a step is tiny tensor ops (collate 16 images, one pinned copy): on a many-core box an
@@ -77,6 +77,8 @@ class Trainer:
         net, self.ext = create_net(self.num_classes, dnn, **(model_kwargs or {}))
         # optional mixed precision (the reference's --fp16 is apex O3, off in every script; bf16 autocast here)
         self.autocast = {"bf16": torch.bfloat16, "fp16": torch.float16}.get(autocast or "", None)
+        # dynamic (or fixed) loss scaling, off by default: "dynamic", a number (fixed scale) or a LossScale
+        self.loss_scale = LossScale.parse(loss_scale)
         self.net = net.to(self.device)
         self.is_bert = dnn.startswith("bert")
         # CNN zoo on the GPU: channels_last weights and activations.  cuDNN's TF32/fp32 convolution kernels are NHWC: with
@@ -111,7 +113,7 @@ class Trainer:
                       {"params": [p for n, p in named if any(nd in n for nd in no_decay)], "weight_decay": 0.0}]
             self.optimizer = BertAdam(groups, lr=lr, warmup=warmup, t_total=t_total, density=self.cfg.density,
                                       compressor=self.cfg.compressor, rank=self.rank, named_parameters=named,
-                                      cfg=self.cfg, world=self.world)
+                                      cfg=self.cfg, world=self.world, loss_scale=self.loss_scale)
         else:
             if self.dataset == "ptb":
                 base = torch.optim.SGD(self.net.parameters(), lr=lr, momentum=0.0, weight_decay=0.0)
@@ -122,7 +124,7 @@ class Trainer:
             self.optimizer = DistributedOptimizer(base, named_parameters=self.net.named_parameters(),
                                                   compression=_comp.compressors[self.cfg.compressor],
                                                   is_sparse=self.cfg.sparse, cfg=self.cfg, world=self.world,
-                                                  err_handler=self._err_handler)
+                                                  err_handler=self._err_handler, loss_scale=self.loss_scale)
         # ---- data -----------------------------------------------------------------------------
         self.trainset = D.build_dataset(self.dataset, data_dir, train=True, seed=seed, seq=seq_len, batch_size=batch_size)
         self.loader, self.sampler = D.build_loader(self.trainset, self.dataset, batch_size, self.rank, self.nworkers,
@@ -208,6 +210,13 @@ class Trainer:
         out = self.net(x)
         return self.criterion(out, y), (out, y)
 
+    def backward(self, loss: torch.Tensor) -> None:
+        """Back-propagate ``loss``, multiplied by the optimizer's loss scale when loss scaling is on (the recorded loss
+        stays unscaled)."""
+        if self.loss_scale is not None:
+            loss = self.optimizer.scale_loss(loss)
+        loss.backward()
+
     def train(self, num_of_iters: int = 1) -> float:
         """``DLTrainer.train`` (``VGG/dl_trainer.py:597-707``): forward+backward micro-steps; the
         communication happens inside backward (bucket hooks), the update in ``update_model``."""
@@ -219,7 +228,7 @@ class Trainer:
             batch = self.prefetch.next(defer=True)
             self.timers.add("io", time.perf_counter() - t0)
             loss, aux = self._forward_loss(batch)
-            loss.backward()
+            self.backward(loss)
             self.prefetch.advance()              # stage the next batch while the GPU works through this one
             self._last_loss = loss.detach()
             self.loss_n += 1
