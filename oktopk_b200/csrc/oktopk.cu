@@ -98,7 +98,13 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     char* me = p.peers[rank];
     const uint32_t epoch = st->epoch + 1u;     // every CTA reads it before anybody can bump it (see PH_FINAL)
     const int par = epoch & 1u;
-    const bool two_pass = p.exact_local || p.repartition;
+    // Carried threshold: every CTA reads it before the pack publisher can rewrite it.  A threshold-reuse call that finds
+    // it at 0 (the last exact call saw fewer than k non-zeros) recomputes the exact threshold: at 0 every non-zero would
+    // be selected and no ladder rung (0 * f = 0) could cap the volume.  Decided here, not on the host, so that a
+    // captured graph stays valid whatever the threshold.
+    const float thr_in = st->local_thr;
+    const bool exact_local = p.exact_local || thr_in == 0.f;
+    const bool two_pass = exact_local || p.repartition;
     uint32_t pipe_it = 0;
 
     for (int b = tid; b < kHistBins; b += kThreads) s_hist[b] = 0;
@@ -139,12 +145,12 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     if (p.phase_begin <= PH_LOCAL && PH_LOCAL < p.phase_end && two_pass) {
         // (1) acc = g + residual -> residual; exact iterations histogram the top digit on the fly,
         //     threshold-reuse iterations count the guard ladder.
-        const float thr0 = st->local_thr;
-        const LadderCfg lcl = ladder_cfg(p, !p.exact_local);
+        const float thr0 = thr_in;
+        const LadderCfg lcl = ladder_cfg(p, !exact_local);
         ladder_build(s_lthr, s_lcnt, lcl, thr0);
 
         auto visit = [&](float x) {
-            if (p.exact_local) {
+            if (exact_local) {
                 hist_add(s_hist, x, 0, 0u);
             } else {
                 float ax = fabsf(x);
@@ -156,7 +162,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
         // radix select -- a few k of them.  The k-th largest of the candidates IS the k-th largest overall as long as
         // at least k elements pass the cut; otherwise (first call, or the gradient scale collapsed) fall back to the
         // full three-pass select.
-        const float cut = (p.exact_local && thr0 > 0.f) ? thr0 * p.prefilter : -1.f;
+        const float cut = (exact_local && thr0 > 0.f) ? thr0 * p.prefilter : -1.f;
         const bool prefilter = cut > 0.f;
         constexpr int kLocTile = 4;
         for (int base = blockIdx.x * kThreads * kLocTile; base < n4; base += gridDim.x * kThreads * kLocTile) {
@@ -214,7 +220,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                 }
             }
         }
-        if (p.exact_local) {
+        if (exact_local) {
             float thr;
             bool done = false;
             if (prefilter) {
@@ -353,7 +359,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
 
     // ======================================================================== PH_PACK (+ publish to the region owners)
     if (p.phase_begin <= PH_PACK && PH_PACK < p.phase_end) {
-        float thr_sel = two_pass ? st->local_thr_used : st->local_thr;
+        float thr_sel = two_pass ? st->local_thr_used : thr_in;
         const bool bounded = p.L.cap > 0;
         // Overflow policy of the bounded layout (Ok-Topk residual rule): if a destination's slot is full, raise the threshold
         // and redo the pack pass from the accumulator (already in the residual buffer).  Everything above the final
@@ -520,8 +526,11 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                     for (int c = 0; c < 4; ++c) {
                         const bool pred = in[u] && fabsf(xs[c]) > thr_sel;
                         // TopkDSA zeroes the residual at the exact top-k INCLUDING the k-th element itself, which the
-                        // strict '>' select does not send (reference quirk, SURVEY B.4-3): a rare, direct store
-                        if (p.residual_mode == RES_LOCAL_GE && in[u] && xs[c] != 0.f && fabsf(xs[c]) == thr_sel)
+                        // strict '>' select does not send (reference quirk, SURVEY B.4-3).  On a tie at the k-th
+                        // magnitude the top-k holds only k - #(|x| > thr) of the tied elements -- the radix select's
+                        // remaining rank, sel_krem -- so a ticket bounds the clears to that many (which ones is unspecified)
+                        if (p.residual_mode == RES_LOCAL_GE && in[u] && xs[c] != 0.f && fabsf(xs[c]) == thr_sel &&
+                            atomicAdd(&st->tie_cursor, 1) < (int)__ldcg(&st->sel_krem))
                             p.res[4 * (base + u * kThreads + tid) + c] = 0.f;
                         const unsigned m = __ballot_sync(0xffffffffu, pred);
                         msk[u * 4 + c] = m;
@@ -614,7 +623,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
             if (p.residual_mode == RES_LOCAL_GE && blockIdx.x == 0 && (n & 3)) {      // scalar tail of the same rule
                 for (int i = n4 * 4 + tid; i < n; i += kThreads) {
                     float x = p.res[i];
-                    if (x != 0.f && fabsf(x) == thr_sel) p.res[i] = 0.f;
+                    if (x != 0.f && fabsf(x) == thr_sel && atomicAdd(&st->tie_cursor, 1) < (int)__ldcg(&st->sel_krem))
+                        p.res[i] = 0.f;
                 }
             }
             ladder_flush(st, s_lcnt);
@@ -648,6 +658,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                 st->local_thr_used = t;
                 st->pack_thr = thr_sel;
                 st->stat_local_count = cnt;
+                st->tie_cursor = 0;
                 float nt = t;
                 if ((double)cnt < p.l_low_cnt) nt = t / p.l_factor;
                 else if ((double)cnt > p.l_high_cnt) nt = t * p.l_factor;

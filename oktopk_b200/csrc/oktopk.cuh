@@ -53,6 +53,7 @@ struct OktState {
     int guard_counts[kGuardMax];          // selected elements whose HIGHEST passed ladder rung is j (suffix sums = #(|acc| > T_j))
     uint32_t sel_prefix;                  // radix-select running prefix / remaining rank
     uint32_t sel_krem;
+    int tie_cursor;                       // TopkDSA: elements at |x| == threshold seen by the pack pass (reset by its publisher)
     int cuts[OKT_MAXP];
     // statistics of the last call (read lazily by the host; never on the hot path)
     int stat_local_count;

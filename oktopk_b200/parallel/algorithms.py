@@ -19,8 +19,8 @@ import torch
 
 from ..compression import gaussian_correct_threshold, gen_threshold_from_normal_distribution
 from ..config import OkTopkConfig
-from .oracle import (adapt_global, adapt_local, boundaries_from_cuts, guard_threshold,
-                     kth_largest_abs, quantile_cuts)
+from .oracle import (adapt_global, adapt_local, boundaries_from_cuts, ftz, guard_threshold,
+                     kth_largest_abs, quantile_cuts, topk_tie_inclusive)
 from .state import SparseState, offsets_of, uniform_boundaries
 from .world import World
 
@@ -63,8 +63,10 @@ def _sparse_reduce_scatter(send, world: World, cfg: OkTopkConfig, region_len: in
     def reduce_chunk(chunk):
         for _src, (idx, val) in chunk:
             if idx.numel():
-                # indices are unique within one source -> plain indexed add is exact
-                reduced[idx.long()] += val
+                # indices are unique within one source -> plain indexed add is exact; subnormals flushed as the
+                # device's atomics do (oracle.ftz)
+                i = idx.long()
+                reduced[i] = ftz(reduced[i] + ftz(val))
 
     world.exchange_pairwise(send, rsizes, throttle=min(cfg.throttle, P), on_chunk=reduce_chunk)
     st.last_volume_elems += 2 * (sum(ssizes) - ssizes[world.rank]) + 2 * (sum(rsizes) - rsizes[world.rank])
@@ -143,7 +145,7 @@ def oktopk_allreduce(g: torch.Tensor, st: SparseState, cfg: OkTopkConfig, world:
         res = st.ensure_residual(g)
         g.add_(res)
         res.copy_(g)
-        if it % cfg.local_recompute_interval == 0:
+        if it % cfg.local_recompute_interval == 0 or st.local_thr == 0.0:    # a carried 0 cannot be capped: recompute
             thr = kth_largest_abs(g, k)
         else:
             thr = guard_threshold(g.abs(), st.local_thr, k, cfg)
@@ -214,27 +216,29 @@ def topka_allreduce(g, st: SparseState, cfg: OkTopkConfig, world: World, density
                 g.mul_(mx / nrm)
         res = st.ensure_residual(g)
         g.add_(res)
-        idx = torch.topk(g.abs(), k=k).indices
+        st.local_thr = kth_largest_abs(g, k)
+        idx = topk_tie_inclusive(g, k)                              # ties at the k-th magnitude: more than k entries
         vals = g[idx].clone()
         res.copy_(g)
         res[idx] = 0.0
-        all_i = world.all_gather_fixed(idx.to(torch.int32))      # B10: fixed k per rank
-        all_v = world.all_gather_fixed(vals)
+        (all_i, all_v), counts = world.all_gatherv([idx.to(torch.int32), vals])
         g.zero_()
-        for r in range(P):
-            g[all_i[r].long()] += all_v[r]
+        for ri, rv in zip(all_i.split(counts), all_v.split(counts)):     # rank order, as the oracle adds them
+            g[ri.long()] += rv
         if reselect:
-            J = torch.topk(g.abs(), k=k).indices
+            U = torch.unique(all_i.long())
             keep = torch.zeros(n, dtype=torch.bool, device=g.device)
-            keep[J] = True
+            if U.numel() > k:
+                keep[U] = g[U].abs() >= float(torch.topk(g[U].abs(), k=k).values[-1])
+            else:
+                keep[U] = True
             g.mul_(keep)
             lost = ~keep[idx]
             res[idx[lost]] += vals[lost]
         g.div_(P)
-        st.local_thr = float(vals.abs().min())
-        st.last_local_count = k
+        st.last_local_count = int(idx.numel())
         st.last_global_count = int((g != 0).sum())
-        st.last_volume_elems = 4 * k * (P - 1)
+        st.last_volume_elems = 2 * (sum(counts) - counts[world.rank]) * 2
         st.last_mode = "topkA2" if reselect else "topkA"
     return g
 
@@ -285,7 +289,7 @@ def gtopk_allreduce(g, st: SparseState, cfg: OkTopkConfig, world: World, density
                 g.mul_(mx / nrm)
         res = st.ensure_residual(g)
         g.add_(res)
-        idx0 = torch.topk(g.abs(), k=k).indices.sort().values
+        idx0 = topk_tie_inclusive(g, k)
         val0 = g[idx0].clone()
         res.copy_(g)
         res[idx0] = 0.0
@@ -328,7 +332,7 @@ def gtopk_allreduce(g, st: SparseState, cfg: OkTopkConfig, world: World, density
         keep[bi.long()] = True
         lost = ~keep[idx0]
         res[idx0[lost]] += val0[lost]
-        st.last_local_count = k
+        st.last_local_count = int(idx0.numel())
         st.last_global_count = m
         st.last_volume_elems = vol
         st.last_mode = "gtopk"

@@ -40,6 +40,22 @@ def kth_largest_abs(x: torch.Tensor, k: int) -> float:
     return float(torch.topk(x.abs().view(-1), k=k).values[-1])
 
 
+def ftz(x: torch.Tensor) -> torch.Tensor:
+    """Subnormals flushed to zero.  The reduce phase of the fused kernel sums with fp32 global atomics, which flush
+    subnormal inputs and results to zero (PTX ``atom/red.add.f32``): a selected entry whose value or sum is subnormal
+    reaches the owner as 0, is not gathered, and stays in the sender's residual."""
+    return torch.where(x.abs() < torch.finfo(x.dtype).tiny, torch.zeros_like(x), x)
+
+
+def topk_tie_inclusive(x: torch.Tensor, k: int) -> torch.Tensor:
+    """Ascending indices of the exact top-k by magnitude, every element tied at the k-th magnitude included and zeros
+    excluded (``|x| >= kth && |x| > 0``): more than k indices on a tie, fewer when x has fewer than k non-zeros.  The
+    local picks of TopkA / TopkA2 / gTopk and their merge rounds select this way on the device; ``torch.topk`` returns
+    exactly k but leaves unspecified which tied elements, so it cannot be the reference on tied data."""
+    ax = x.abs()
+    return ((ax >= kth_largest_abs(x, k)) & (ax > 0)).nonzero().view(-1)
+
+
 def guard_threshold(absx: torch.Tensor, thr: float, k: int, cfg: OkTopkConfig) -> float:
     """``add2residual`` over-selection guard (``VGG/compression.py:392-404``) + the optional hard cap
     (``OkTopkConfig.overselect_cap``): one geometric ladder ``T_0 = thr, T_j = T_{j-1} * f`` (``f`` = guard factor on the
@@ -131,13 +147,14 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
     repart = it % cfg.repartition_interval == 0
 
     accs, thrs = [], []
-    # (1) error feedback + local threshold
+    # (1) error feedback + local threshold; a carried threshold of 0 (the last exact call saw fewer than k non-zeros) is
+    #     recomputed exactly: at 0 every non-zero would be selected and no ladder rung (0 * f) could cap the volume
     for r in range(P):
         st = states[r]
         res = st.ensure_residual(grads[r])
         acc = grads[r] + res
         res.copy_(acc)
-        if exact_local:
+        if exact_local or st.local_thr == 0.0:
             thr = kth_largest_abs(acc, k)
         else:
             thr = guard_threshold(acc.abs(), st.local_thr, k, cfg)
@@ -168,7 +185,8 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
         local_masks.append(mask)
         cnt = int(mask.sum())
         states[r].last_local_count = cnt
-        reduced += torch.where(mask, accs[r], torch.zeros_like(accs[r]))
+        states[r].last_thr_used = thrs[r]
+        reduced = ftz(reduced + ftz(torch.where(mask, accs[r], torch.zeros_like(accs[r]))))
         for d in range(P):
             if d != r:
                 c = int(mask[edges[d]:edges[d + 1]].sum())
@@ -218,12 +236,15 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
 
 # --------------------------------------------------------------------------- TopkA / TopkA2
 def topka_oracle(grads, states, cfg: OkTopkConfig, density=None, reselect: bool = False):
-    """Appendix B.1.  ``reselect=True`` is TopkA2 (global top-k of the sum + put-back)."""
+    """Appendix B.1.  ``reselect=True`` is TopkA2 (global top-k of the sum + put-back).  Both selections are
+    tie-inclusive (``topk_tie_inclusive``; the re-selection keeps every union entry at or above the k-th magnitude of
+    the union, and the whole union when it has at most k entries)."""
     P = len(grads)
     n = grads[0].numel()
     density = cfg.density if density is None else density
     k = _k(n, density)
     total = torch.zeros_like(grads[0])
+    picked = torch.zeros(n, dtype=torch.bool, device=total.device)
     picks = []
     for r in range(P):
         st = states[r]
@@ -232,20 +253,24 @@ def topka_oracle(grads, states, cfg: OkTopkConfig, density=None, reselect: bool 
         if cfg.norm_clip is not None:
             _clip(g, (1.0 / P) ** 0.5 * cfg.norm_clip)
         acc = g + res
-        idx = torch.topk(acc.abs(), k=k).indices
+        idx = topk_tie_inclusive(acc, k)
         vals = acc[idx]
         res.copy_(acc)
         res[idx] = 0.0
         total[idx] += vals
+        picked[idx] = True
         picks.append((idx, vals))
-        st.local_thr = float(vals.abs().min())
-        st.last_local_count = k
-        st.last_volume_elems = 2 * k * (P - 1) * 2 if P > 1 else 0
+        st.local_thr = kth_largest_abs(acc, k)
+        st.last_local_count = int(idx.numel())
+        st.last_volume_elems = 2 * int(idx.numel()) * (P - 1) * 2 if P > 1 else 0
         st.last_mode = "topkA2" if reselect else "topkA"
     if reselect:
-        J = torch.topk(total.abs(), k=k).indices
+        U = picked.nonzero().view(-1)
         keep = torch.zeros(n, dtype=torch.bool, device=total.device)
-        keep[J] = True
+        if U.numel() > k:
+            keep[U] = total[U].abs() >= float(torch.topk(total[U].abs(), k=k).values[-1])
+        else:
+            keep[U] = True
         total = torch.where(keep, total, torch.zeros_like(total))
         for r in range(P):
             idx, vals = picks[r]
@@ -307,14 +332,13 @@ def gtopk_oracle(grads, states, cfg: OkTopkConfig, density=None):
         if cfg.norm_clip is not None:
             _clip(g, (1.0 / P) ** 0.5 * cfg.norm_clip)
         acc = g + res
-        idx = torch.topk(acc.abs(), k=k).indices
-        idx = idx.sort().values
+        idx = topk_tie_inclusive(acc, k)
         vals = acc[idx]
         res.copy_(acc)
         res[idx] = 0.0
         lists.append((idx, vals))
         picks.append((idx, vals))
-        st.last_local_count = k
+        st.last_local_count = int(idx.numel())
         st.last_mode = "gtopk"
     step = 1
     while step < P:
@@ -336,7 +360,8 @@ def gtopk_oracle(grads, states, cfg: OkTopkConfig, density=None):
 
 
 def merge_topk(a, b, k: int, n: int):
-    """Sum coincident indices, keep the top-k of the union by magnitude (``VGG/allreducer.py:129-138``)."""
+    """Sum coincident indices, keep the top-k of the union by magnitude (``VGG/allreducer.py:129-138``): tie-inclusive,
+    and a sum that cancelled to exactly 0 is dropped (its picks go back to their residuals), as on the device."""
     ia, va = a
     ib, vb = b
     idx = torch.cat([ia, ib])
@@ -344,10 +369,10 @@ def merge_topk(a, b, k: int, n: int):
     uniq, inv = torch.unique(idx, return_inverse=True)   # sorted
     summed = torch.zeros(uniq.numel(), dtype=val.dtype, device=val.device)
     summed.index_add_(0, inv, val)
+    keep = summed != 0
     if uniq.numel() > k:
-        top = torch.topk(summed.abs(), k=k).indices.sort().values
-        uniq, summed = uniq[top], summed[top]
-    return uniq, summed
+        keep &= summed.abs() >= float(torch.topk(summed.abs(), k=k).values[-1])
+    return uniq[keep], summed[keep]
 
 
 # --------------------------------------------------------------------------- Gaussiank
@@ -386,7 +411,9 @@ def topkdsa_oracle(grads, states, cfg: OkTopkConfig, density=None, gaussian_sa: 
     Exact local threshold every iteration, uniform regions, sparse reduce-scatter, allgather
     of all non-zeros of the reduced regions, dense fallback when the result is not sparse.
     Error feedback is the classic local one (residual zeroed at the exact local top-k for
-    TopkDSA; at the strict ``>thr`` selection for gaussiankSA).
+    TopkDSA; at the strict ``>thr`` selection for gaussiankSA).  TopkDSA's top-k holds exactly
+    ``k - #(|acc| > thr)`` of the elements tied at the k-th magnitude; which of them ``torch.topk``
+    (or the device) picks is unspecified, so only that count is part of the specification.
     """
     P = len(grads)
     n = grads[0].numel()
@@ -405,7 +432,7 @@ def topkdsa_oracle(grads, states, cfg: OkTopkConfig, density=None, gaussian_sa: 
             res[mask] = 0.0
         else:
             res[top.indices] = 0.0
-        reduced += torch.where(mask, acc, torch.zeros_like(acc))
+        reduced = ftz(reduced + ftz(torch.where(mask, acc, torch.zeros_like(acc))))
         st.local_thr = thr
         st.last_local_count = int(mask.sum())
         st.last_mode = "gaussiankSA" if gaussian_sa else "topkSA"

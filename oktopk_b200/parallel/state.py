@@ -44,6 +44,7 @@ class SparseState:
     residual: Optional[torch.Tensor] = None
     # bookkeeping for observability (SURVEY 5.1/5.5)
     last_local_count: int = 0
+    last_thr_used: float = 0.0             # Ok-Topk: threshold the last call selected with (after the guard), before adaptation
     last_global_count: int = 0
     last_volume_elems: int = 0             # scalars sent + received by this rank in the last call
     last_mode: str = ""
