@@ -21,7 +21,7 @@ from ..compression import gaussian_correct_threshold, gen_threshold_from_normal_
 from ..config import OkTopkConfig
 from .oracle import (adapt_global, adapt_local, boundaries_from_cuts, ftz, guard_threshold,
                      kth_largest_abs, quantile_cuts, topk_tie_inclusive)
-from .state import SparseState, offsets_of, uniform_boundaries
+from .state import SparseState, offsets_of, plan_call, uniform_boundaries
 from .world import World
 
 
@@ -138,25 +138,24 @@ def oktopk_allreduce(g: torch.Tensor, st: SparseState, cfg: OkTopkConfig, world:
     n = g.numel()
     density = cfg.density if density is None else density
     k = _k(n, density)
-    it = st.counter - cfg.warmup_iters
+    plan = plan_call(cfg, "oktopk", st.counter, density, P)
     st.last_volume_elems = 0
     with torch.no_grad():
         # (1) error feedback + local threshold
         res = st.ensure_residual(g)
         g.add_(res)
         res.copy_(g)
-        if it % cfg.local_recompute_interval == 0 or st.local_thr == 0.0:    # a carried 0 cannot be capped: recompute
+        if plan.exact_local or st.local_thr == 0.0:    # a carried 0 cannot be capped: recompute
             thr = kth_largest_abs(g, k)
         else:
             thr = guard_threshold(g.abs(), st.local_thr, k, cfg)
         st.local_thr = thr
 
         # (2) region re-partition: average the local quantile cut points (B4)
-        if it % cfg.repartition_interval == 0:
+        if plan.repartition:
             sel = (g.abs() > thr).nonzero(as_tuple=False).view(-1)
             cuts = torch.tensor(quantile_cuts(sel, P, n), dtype=torch.int64, device=g.device)
-            if P > 1:
-                world.all_reduce_sum(cuts)
+            world.all_reduce_sum(cuts)
             st.boundaries, st.region_offsets = boundaries_from_cuts((cuts // P).tolist(), n)
         edges = st.region_offsets + [n]
 
@@ -171,7 +170,7 @@ def oktopk_allreduce(g: torch.Tensor, st: SparseState, cfg: OkTopkConfig, world:
 
         # (5) global selection on my region + sparse allgather
         off = st.region_offsets[rank]
-        if it % cfg.global_recompute_interval == 0:
+        if plan.exact_global:
             ridx = reduced.nonzero(as_tuple=False).view(-1)
             all_i, all_v, total = _allgather_sparse((ridx + off).to(torch.int32), reduced[ridx], world,
                                                     cfg.replace(balanced_allgather=False), st)
@@ -250,12 +249,12 @@ def topkaopt_allreduce(g, st: SparseState, cfg: OkTopkConfig, world: World, dens
     n = g.numel()
     density = cfg.density if density is None else density
     k = _k(n, density)
-    it = st.counter - cfg.warmup_iters
+    exact = plan_call(cfg, "topkAopt", st.counter, density, P).exact_local
     with torch.no_grad():
         res = st.ensure_residual(g)
         g.add_(res)
         res.copy_(g)
-        if it % cfg.topkaopt_recompute_interval == 0:
+        if exact:
             st.local_thr = kth_largest_abs(g, k)
         idx = (g.abs() > st.local_thr).nonzero(as_tuple=False).view(-1)
         vals = g[idx]
@@ -438,20 +437,17 @@ ALGORITHMS = {
 def sparse_allreduce(name: str, g: torch.Tensor, st: SparseState, cfg: OkTopkConfig, world: World,
                      density: Optional[float] = None) -> torch.Tensor:
     """Dispatch on the compressor name exactly like ``AllReducer.run`` (``VGG/allreducer.py:573-1622``):
-    dense during warm-up / for ``none``, else the named scheme.  Advances the bucket counter."""
-    from .oracle import dense_switch_applies
-    d = cfg.density if density is None else density
-    if (not cfg.sparse) or name in ("none", None) or st.counter < cfg.warmup_iters:
+    dense as ``plan_call`` says (warm-up, ``none``, the dense switch), else the named scheme.  Advances the bucket
+    counter."""
+    kind = plan_call(cfg, name, st.counter, density, world.size).kind
+    if kind in ("dense", "dense_switch"):
+        if kind == "dense_switch":
+            with torch.no_grad():
+                res = st.ensure_residual(g)
+                g.add_(res)
+                res.zero_()
         dense_allreduce(g, world)
-        st.last_mode = "dense"
-        st.last_volume_elems = 2 * g.numel() * (world.size - 1) // max(world.size, 1)
-    elif dense_switch_applies(name, d, cfg, world.size):
-        with torch.no_grad():                     # same rule as the CUDA engine (gpu_engine._dense_switch)
-            res = st.ensure_residual(g)
-            g.add_(res)
-            res.zero_()
-        dense_allreduce(g, world)
-        st.last_mode = "dense(auto)"
+        st.last_mode = "dense" if kind == "dense" else "dense(auto)"
         st.last_volume_elems = 2 * g.numel() * (world.size - 1) // max(world.size, 1)
     else:
         ALGORITHMS[name](g, st, cfg, world, density)

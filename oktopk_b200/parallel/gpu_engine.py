@@ -18,7 +18,7 @@ import torch
 
 from ..config import OkTopkConfig
 from ..ops import ext
-from .state import SparseState, uniform_boundaries, offsets_of
+from .state import CallPlan, SparseState, plan_call, uniform_boundaries, offsets_of
 from .symm import SymmBlock, make_symm_block
 from .world import World
 
@@ -26,10 +26,6 @@ RES_OKTOPK, RES_LOCAL_GT, RES_LOCAL_GE = 0, 1, 2
 GLB_THRESHOLD, GLB_EXACT_TOPK, GLB_ALL_NONZERO = 0, 1, 2
 GS_THRESHOLD_REUSE, GS_GAUSSIAN, GS_EXACT_TOPK = 0, 1, 2
 
-_FUSED = {"oktopk", "topkSA", "topkDSA", "gaussiankSA"}
-_GATHER = {"topkA", "topkA2", "topkAopt", "gaussiank", "gaussiankconcat"}
-_TREE = {"gtopk"}
-_DIST_ONLY: set = set()                 # every scheme has a native kernel; 'backend=dist' selects the NCCL + torch-ops path
 _CLASSIC_RESIDUAL = {"topkSA", "topkDSA", "gaussiankSA"}   # residual zeroed at selection: the gather must be lossless
 
 
@@ -115,7 +111,6 @@ class CudaBucketEngine:
         self._sel: Optional[tuple] = None                    # gTopk: private copy of my picks for the put-back
         self.host = SparseState(self.n, self.P)          # counter + (lazily refreshed) mirrors
         self._write_edges(self.host.region_offsets + [self.n])
-        self._dist_state: Optional[SparseState] = None
         self.last_mode = ""
         self._res_clean = False                  # True while the residual is known to be all-zero (dense-switch calls)
         self._skip = 0                           # bucket verdict address of the running call (loss scaling), 0 = off
@@ -133,13 +128,14 @@ class CudaBucketEngine:
         return max(int(self.n * d), 1)
 
     # ------------------------------------------------------------------ the step
+    def _plan(self, compressor: str, density: Optional[float]) -> CallPlan:
+        return plan_call(self.cfg, compressor, self.host.counter, density, self.P)
+
     def reads_sources(self, compressor: str, density: Optional[float] = None) -> bool:
         """True if the next ``reduce`` call can read the gradient from its source tensors (``reduce(srcs=...)``) instead of
         the bucket: an Ok-Topk call of the fused kernel, whose pack pass then reads every source once and leaves the bucket
         alone.  The bucket must be all-zero when such a call starts."""
-        cfg = self.cfg
-        return (compressor == "oktopk" and cfg.sparse and self.host.counter >= cfg.warmup_iters
-                and not self._dense_switch(compressor, density))
+        return compressor == "oktopk" and self._plan(compressor, density).kind == "fused"
 
     def enable_loss_scaling(self) -> None:
         """Allocate the device words of ``unscale_check`` (before any graph capture; a no-op when already done)."""
@@ -174,58 +170,38 @@ class CudaBucketEngine:
         ``srcs = (pointers, offsets, lengths)``: the gradient is not in the bucket but in these fp32 tensors, at these
         element offsets of the bucket (Ok-Topk only, see ``reads_sources``); the result is written into the bucket.
         ``skip``: device address of the bucket verdict of loss scaling (0 = off); when set the kernels return at entry."""
-        if srcs is not None and (g is not None and g.data_ptr() != self.grad.data_ptr()
-                                 or not self.reads_sources(compressor, density)):
-            raise ValueError("gradient sources are only read by an Ok-Topk call on the engine's own bucket")
-        cfg = self.cfg
-        st = self.host
         ext_g = g is not None and g.data_ptr() != self.grad.data_ptr()
-        dense = (not cfg.sparse) or compressor in ("none", None) or st.counter < cfg.warmup_iters
+        plan = self._plan(compressor, density)
+        if srcs is not None and (ext_g or compressor != "oktopk" or plan.kind != "fused"):
+            raise ValueError("gradient sources are only read by an Ok-Topk call on the engine's own bucket")
         s = self._stream(stream)
         self._skip = int(skip)
-        if dense:
+        out = g if ext_g else self.grad
+        if plan.kind in ("dense", "dense_switch"):
             if ext_g:
                 self.grad.copy_(g)
+            if plan.kind == "dense_switch":
+                # reduce the error-compensated gradient densely (nothing is left behind, so the residual is cleared)
+                if self._skip:                     # under loss scaling a skipped call keeps its residual: always carry
+                    self.C.carry_residual(self.grad.data_ptr(), self.residual.data_ptr(), self.n, self._skip, s)
+                elif not self._res_clean:          # a dense call leaves nothing behind: after the first switched call
+                    self.grad.add_(self.residual)  # the residual is known to be all-zero and the carry-over is skipped
+                    self.residual.zero_()
+                    self._res_clean = True
             self._dense(s)
             if ext_g:
                 g.copy_(self.grad)
-            self.last_mode = "dense"
-        elif self._dense_switch(compressor, density):
-            # predicted slower than the dense kernel at this density: reduce the error-compensated gradient densely
-            # (nothing is left behind, so the residual is cleared) -- OkTopkConfig.dense_switch_density
-            if ext_g:
-                self.grad.copy_(g)
-            if self._skip:                         # under loss scaling a skipped call keeps its residual: always carry
-                self.C.carry_residual(self.grad.data_ptr(), self.residual.data_ptr(), self.n, self._skip, s)
-            elif not self._res_clean:              # a dense call leaves nothing behind: after the first switched call
-                self.grad.add_(self.residual)      # the residual is known to be all-zero and the carry-over is skipped
-                self.residual.zero_()
-                self._res_clean = True
-            self._dense(s)
-            if ext_g:
-                g.copy_(self.grad)
-            self.last_mode = "dense(auto)"
-        elif compressor in _FUSED:
-            self._res_clean = False
-            self._fused(compressor, density, s, g if ext_g else self.grad, srcs)
-        elif compressor in _GATHER:
-            self._res_clean = False
-            self._gather(compressor, density, s, g if ext_g else self.grad)
-        elif compressor in _TREE:
-            self._res_clean = False
-            self._tree(compressor, density, s, g if ext_g else self.grad)
-        elif compressor in _DIST_ONLY:
-            self._res_clean = False
-            self._dist(compressor, density, g if ext_g else self.grad)
+            self.last_mode = "dense" if plan.kind == "dense" else "dense(auto)"
         else:
-            raise KeyError("unknown compressor %r" % (compressor,))
-        st.counter += 1
-        return g if ext_g else self.grad
-
-    def _dense_switch(self, compressor: str, density: Optional[float]) -> bool:
-        from .oracle import dense_switch_applies
-        d = self.cfg.density if density is None else density
-        return dense_switch_applies(compressor, d, self.cfg, self.P)
+            self._res_clean = False
+            if plan.kind == "fused":
+                self._fused(compressor, plan, density, s, out, srcs)
+            elif plan.kind == "gather":
+                self._gather(compressor, plan, density, s, out)
+            else:
+                self._tree(compressor, density, s, out)
+        self.host.counter += 1
+        return out
 
     def _dense(self, s: int) -> None:
         if self.P == 1:
@@ -234,11 +210,10 @@ class CudaBucketEngine:
                          self.dense_grid, s, self.state_ptr, float(self.cfg.peer_timeout_s), self.mc_grad,
                          self.host_flag_dev, self._skip)
 
-    def _fused(self, compressor: str, density: Optional[float], s: int, g: torch.Tensor,
+    def _fused(self, compressor: str, plan: CallPlan, density: Optional[float], s: int, g: torch.Tensor,
                srcs: Optional[tuple] = None) -> None:
         cfg = self.cfg
         k = self.k_now(density)
-        it = self.host.counter - cfg.warmup_iters
         o: Dict = {"pull_tma": 1 if cfg.pull_mode == "tma" else 0, "deterministic": int(cfg.deterministic),
                    "split_phases": 0 if cfg.fused else 1, "timeout_s": float(cfg.peer_timeout_s),
                    "cand": self.cand.data_ptr(), "ccap": self.ccap, "host_fault": self.host_flag_dev,
@@ -248,10 +223,10 @@ class CudaBucketEngine:
                    "cand_mode": int(cfg.gselect_mode == "list" or (cfg.gselect_mode == "auto" and k * 200 <= self.n))}
         if compressor == "oktopk":
             o.update(
-                exact_local=int(it % cfg.local_recompute_interval == 0),
-                repartition=int(it % cfg.repartition_interval == 0 and self.P > 1),
+                exact_local=int(plan.exact_local),
+                repartition=int(plan.repartition),
                 residual_mode=RES_OKTOPK,
-                global_mode=GLB_EXACT_TOPK if it % cfg.global_recompute_interval == 0 else GLB_THRESHOLD,
+                global_mode=GLB_EXACT_TOPK if plan.exact_global else GLB_THRESHOLD,
                 guard_loops=cfg.overselect_guard_loops,
                 guard_limit=cfg.overselect_guard_num * k // cfg.overselect_guard_den,
                 guard_factor=cfg.overselect_guard_factor,
@@ -280,11 +255,10 @@ class CudaBucketEngine:
                           self.rank, k, self.cap, self.gcap, o, self.grid, s)
         self.last_mode = compressor
 
-    def _gather(self, compressor: str, density: Optional[float], s: int, g: torch.Tensor) -> None:
+    def _gather(self, compressor: str, plan: CallPlan, density: Optional[float], s: int, g: torch.Tensor) -> None:
         cfg = self.cfg
         d = cfg.density if density is None else density
         k = self.k_now(density)
-        it = self.host.counter - cfg.warmup_iters
         o: Dict = {"density": d, "pull_tma": 1 if cfg.pull_mode == "tma" else 0, "timeout_s": float(cfg.peer_timeout_s),
                    "host_fault": self.host_flag_dev}
         if cfg.norm_clip is not None and compressor in ("topkA", "topkA2"):       # VGG/allreducer.py:1372-1379
@@ -295,7 +269,7 @@ class CudaBucketEngine:
                 o.update(reselect=1, bitmap=self._bitmap_ptr(), cand=self.cand.data_ptr(), ccap=self.ccap)
         elif compressor == "topkAopt":
             o["select_mode"] = GS_THRESHOLD_REUSE
-            o["exact_now"] = int(it % cfg.topkaopt_recompute_interval == 0)
+            o["exact_now"] = int(plan.exact_local)
         else:
             o["select_mode"] = GS_GAUSSIAN
             o["gauss_mode"] = {"vgg": 0, "lstm": 1, "bert": 2}[cfg.gaussian_mode]
@@ -330,15 +304,6 @@ class CudaBucketEngine:
             o["skip"] = self._skip
         self.C.gtopk_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                          self.rank, k, self.cap, self.gcap, o, self.tree_grid, s)
-        self.last_mode = compressor
-
-    def _dist(self, compressor: str, density: Optional[float], g: torch.Tensor) -> None:
-        from .algorithms import ALGORITHMS
-        if self._dist_state is None:
-            self._dist_state = SparseState(self.n, self.P)
-            self._dist_state.residual = self.residual
-        self._dist_state.counter = self.host.counter
-        ALGORITHMS[compressor](g, self._dist_state, self.cfg, self.world, density)
         self.last_mode = compressor
 
     # ------------------------------------------------------------------ observability / checkpoint

@@ -19,7 +19,7 @@ import torch
 
 from ..compression import gaussian_correct_threshold, gen_threshold_from_normal_distribution
 from ..config import OkTopkConfig
-from .state import SparseState, offsets_of, uniform_boundaries
+from .state import SparseState, offsets_of, plan_call, uniform_boundaries
 
 
 # --------------------------------------------------------------------------- helpers
@@ -136,15 +136,12 @@ def dense_oracle(grads: List[torch.Tensor], states=None, cfg=None) -> List[torch
 # --------------------------------------------------------------------------- Ok-Topk
 def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkTopkConfig,
                   density: float = None) -> List[torch.Tensor]:
-    """SURVEY 3.3 steps (1)-(7).  ``it`` below is the sparse-iteration index (counter - warm-up)."""
+    """SURVEY 3.3 steps (1)-(7), with the exact-threshold and re-partition iterations of ``plan_call``."""
     P = len(grads)
     n = grads[0].numel()
     density = cfg.density if density is None else density
     k = _k(n, density)
-    it = states[0].counter - cfg.warmup_iters
-    exact_local = it % cfg.local_recompute_interval == 0
-    exact_global = it % cfg.global_recompute_interval == 0
-    repart = it % cfg.repartition_interval == 0
+    plan = plan_call(cfg, "oktopk", states[0].counter, density, P)
 
     accs, thrs = [], []
     # (1) error feedback + local threshold; a carried threshold of 0 (the last exact call saw fewer than k non-zeros) is
@@ -154,7 +151,7 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
         res = st.ensure_residual(grads[r])
         acc = grads[r] + res
         res.copy_(acc)
-        if exact_local or st.local_thr == 0.0:
+        if plan.exact_local or st.local_thr == 0.0:
             thr = kth_largest_abs(acc, k)
         else:
             thr = guard_threshold(acc.abs(), st.local_thr, k, cfg)
@@ -163,12 +160,11 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
         thrs.append(thr)
 
     # (2) balanced region re-partition
-    if repart:
+    if plan.repartition:
         cuts = torch.zeros(P - 1, dtype=torch.int64)
         for r in range(P):
             sel = (accs[r].abs() > thrs[r]).nonzero().view(-1)
-            c = quantile_cuts(sel, P, n)
-            cuts += torch.tensor(c, dtype=torch.int64) if P > 1 else cuts
+            cuts += torch.tensor(quantile_cuts(sel, P, n), dtype=torch.int64)
         avg = (cuts // P).tolist()
         b, off = boundaries_from_cuts(avg, n)
         for st in states:
@@ -195,7 +191,7 @@ def oktopk_oracle(grads: List[torch.Tensor], states: List[SparseState], cfg: OkT
         states[r].local_thr = adapt_local(thrs[r], cnt, k, cfg)
 
     # (5) global selection
-    if exact_global:
+    if plan.exact_global:
         nz = reduced.nonzero().view(-1)
         vals = reduced[nz]
         kk = min(nz.numel(), k)
@@ -296,14 +292,14 @@ def topkaopt_oracle(grads, states, cfg: OkTopkConfig, density=None):
     n = grads[0].numel()
     density = cfg.density if density is None else density
     k = _k(n, density)
-    it = states[0].counter - cfg.warmup_iters
+    exact = plan_call(cfg, "topkAopt", states[0].counter, density, P).exact_local
     total = torch.zeros_like(grads[0])
     for r in range(P):
         st = states[r]
         res = st.ensure_residual(grads[r])
         acc = grads[r] + res
         res.copy_(acc)
-        if it % cfg.topkaopt_recompute_interval == 0:
+        if exact:
             st.local_thr = kth_largest_abs(acc, k)
         mask = acc.abs() > st.local_thr
         res[mask] = 0.0
@@ -462,27 +458,17 @@ ORACLES = {
 }
 
 
-def dense_switch_applies(name: str, density: float, cfg: OkTopkConfig, world: int) -> bool:
-    """The rule shared by the oracle, the torch.distributed path and the CUDA engine."""
-    return (cfg.dense_switch_density > 0 and density >= cfg.dense_switch_density and world > 1
-            and name in ("oktopk", "topkSA", "topkDSA", "gaussiankSA"))
-
-
 def run_oracle(name: str, grads, states, cfg: OkTopkConfig, density=None):
-    """One reduction of every rank's bucket, warm-up handled, counters advanced."""
-    d = cfg.density if density is None else density
-    if (not cfg.sparse) or name in ("none", None) or states[0].counter < cfg.warmup_iters:
-        out = dense_oracle(grads)
-        for st in states:
-            st.last_mode = "dense"
-    elif dense_switch_applies(name, d, cfg, len(grads)):
-        # automatic dense switch (OkTopkConfig.dense_switch_density): the error-compensated gradient is reduced densely,
-        # nothing is left behind
+    """One reduction of every rank's bucket, dense as ``plan_call`` says (warm-up, ``none``, the dense switch),
+    counters advanced."""
+    kind = plan_call(cfg, name, states[0].counter, density, len(grads)).kind
+    if kind in ("dense", "dense_switch"):
         for g, st in zip(grads, states):
-            res = st.ensure_residual(g)
-            g.add_(res)
-            res.zero_()
-            st.last_mode = "dense(auto)"
+            if kind == "dense_switch":            # the error-compensated gradient is reduced densely, nothing left behind
+                res = st.ensure_residual(g)
+                g.add_(res)
+                res.zero_()
+            st.last_mode = "dense" if kind == "dense" else "dense(auto)"
         out = dense_oracle(grads)
     else:
         out = ORACLES[name](grads, states, cfg, density)

@@ -5,13 +5,66 @@ The reference keeps this in dicts keyed by the joined parameter names
 ``_global_threshold``, ``_boundaries``, ``_region_offsets``) plus the compressor's class-level
 ``residuals`` dict (``VGG/compression.py:170``).  Here it is one object per bucket, and it is
 checkpointable (the reference never saves any of it, SURVEY 5.4).
+
+``plan_call`` decides from the bucket counter what one reduction runs; the CUDA engine, the dist backend, the oracle
+and the whole-step CUDA graphs all follow it.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
 import torch
+
+# the kernel family that runs each scheme; the automatic dense switch applies exactly to the "fused" family
+FAMILY = {
+    "oktopk": "fused", "topkSA": "fused", "topkDSA": "fused", "gaussiankSA": "fused",
+    "topkA": "gather", "topkA2": "gather", "topkAopt": "gather", "gaussiank": "gather", "gaussiankconcat": "gather",
+    "gtopk": "tree",
+}
+
+
+@dataclass(frozen=True)
+class CallPlan:
+    """What one bucket reduction runs.  ``kind``: ``"dense"`` (warm-up, ``compressor none``, ``sparse=False``),
+    ``"dense_switch"`` or the scheme's ``FAMILY``.  The flags are set only where the launch differs: Ok-Topk's exact
+    local threshold, exact global top-k and region re-partition (only at P > 1), and TopkAopt's exact-threshold
+    iteration in ``exact_local``.  Equal plans launch the same kernels, so a plan keys a captured CUDA graph."""
+
+    kind: str
+    exact_local: bool = False
+    exact_global: bool = False
+    repartition: bool = False
+
+
+def plan_call(cfg, compressor: Optional[str], counter: int, density: Optional[float], world_size: int) -> CallPlan:
+    """The plan of the reduction a bucket runs at ``counter`` (its completed reductions, warm-up included).  ``density``
+    None means ``cfg.density``.  An unknown compressor raises ``KeyError``."""
+    if not cfg.sparse or compressor in ("none", None) or counter < cfg.warmup_iters:
+        return CallPlan("dense")
+    family = FAMILY[compressor]
+    d = cfg.density if density is None else density
+    if family == "fused" and world_size > 1 and cfg.dense_switch_density > 0 and d >= cfg.dense_switch_density:
+        # predicted slower than the dense kernel at this density: the error-compensated gradient is reduced densely
+        return CallPlan("dense_switch")
+    it = counter - cfg.warmup_iters
+    if compressor == "oktopk":
+        return CallPlan(family, exact_local=it % cfg.local_recompute_interval == 0,
+                        exact_global=it % cfg.global_recompute_interval == 0,
+                        repartition=world_size > 1 and it % cfg.repartition_interval == 0)
+    if compressor == "topkAopt":
+        return CallPlan(family, exact_local=it % cfg.topkaopt_recompute_interval == 0)
+    return CallPlan(family)
+
+
+def schedule_period(cfg, compressor: Optional[str]) -> int:
+    """Sparse iterations after which ``plan_call`` repeats itself."""
+    if compressor == "oktopk":
+        return math.lcm(cfg.local_recompute_interval, cfg.global_recompute_interval, cfg.repartition_interval)
+    if compressor == "topkAopt":
+        return cfg.topkaopt_recompute_interval
+    return 1
 
 
 def uniform_boundaries(n: int, P: int) -> List[int]:

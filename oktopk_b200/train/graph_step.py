@@ -6,17 +6,17 @@ step is several hundred kernels of a few microseconds each.  Everything on our p
 because nothing depends on host-visible values: thresholds, region edges, slot cursors, flag epochs
 and the learning rate live in device memory, and the persistent cooperative kernel is a normal graph
 node.  The only host-side variation is *which* flavour of the kernel a step needs (exact threshold
-re-computation / region re-partition iterations, SURVEY 3.3), so one graph is captured per flavour
-the first time it occurs and the host picks the graph from the iteration counter.
+re-computation / region re-partition iterations, SURVEY 3.3): each engine's ``plan_call``.  One graph
+is captured per flavour the first time it occurs and the host picks the graph from the iteration counter.
 """
 from __future__ import annotations
 
-import math
 from typing import Dict, Optional, Tuple
 
 import torch
 
 from ..ops import ext
+from ..parallel.state import plan_call, schedule_period
 
 
 class GraphedTrainStep:
@@ -40,48 +40,25 @@ class GraphedTrainStep:
         return [self.opt._allreducer._engines.get(b.name) for b in self.opt._buckets]
 
     def _key(self, counters=None) -> Tuple:
-        """The flavour of the step the engines are about to run (or would run at the given iteration counters)."""
-        cfg = self.opt._cfg
-        key = [("density", self.opt.get_current_density())]     # k and the guard limits are baked into the launch
+        """The flavour of the step the engines are about to run (or would run at the given iteration counters): the
+        density (k and the guard limits are baked into the launch) followed by every engine's ``CallPlan``."""
         engines = self._engines()
+        if any(e is None for e in engines):
+            return ("nograph",)
         if counters is None:
-            counters = [None if e is None else e.host.counter for e in engines]
-        for eng, c in zip(engines, counters):
-            if eng is None:
-                return ("nograph",)
-            if (not cfg.sparse) or c < cfg.warmup_iters:
-                key.append(("dense",))
-                continue
-            it = c - cfg.warmup_iters
-            name = self.opt._allreducer.compressor.name
-            if name == "oktopk":
-                key.append((it % cfg.local_recompute_interval == 0, it % cfg.global_recompute_interval == 0,
-                            it % cfg.repartition_interval == 0))
-            elif name == "topkAopt":
-                key.append((it % cfg.topkaopt_recompute_interval == 0,))
-            else:
-                key.append(("every",))
-        return tuple(key)
+            counters = [e.host.counter for e in engines]
+        cfg, density = self.opt._cfg, self.opt.get_current_density()
+        name = self.opt._allreducer.compressor.name
+        return (density,) + tuple(plan_call(cfg, name, c, density, e.P) for e, c in zip(engines, counters))
 
     def _sparse_flavours(self):
         """Every (key, representative sparse-iteration index) the schedule can produce -- a handful: for Ok-Topk the
-        common threshold-reuse step, the exact-threshold step (1 in tau) and the exact + re-partition step."""
+        common threshold-reuse step, the exact-threshold step (1 in tau) and, at P > 1, the exact + re-partition step."""
         cfg = self.opt._cfg
-        name = self.opt._allreducer.compressor.name
-        if name == "oktopk":
-            period = 1
-            for v in (cfg.local_recompute_interval, cfg.global_recompute_interval, cfg.repartition_interval):
-                period = period * v // math.gcd(period, v)
-        elif name == "topkAopt":
-            period = cfg.topkaopt_recompute_interval
-        else:
-            period = 1
         seen = {}
         n_eng = len(self._engines())
-        for it in range(min(period, 1 << 16)):
-            k = self._key([cfg.warmup_iters + it] * n_eng)
-            if k not in seen:
-                seen[k] = it
+        for it in range(min(schedule_period(cfg, self.opt._allreducer.compressor.name), 1 << 16)):
+            seen.setdefault(self._key([cfg.warmup_iters + it] * n_eng), it)
         return seen
 
     def precapture_sparse(self) -> int:
@@ -151,7 +128,7 @@ class GraphedTrainStep:
                     return self._eager(batch)
                 s.copy_(t, non_blocking=True)
         self.opt.refresh_lr()
-        if not self._precaptured and all(k != ("dense",) for k in key[1:]):
+        if not self._precaptured and all(plan.kind != "dense" for plan in key[1:]):
             self.precapture_sparse()             # first sparse step: capture every flavour of the schedule at once
         g = self.graphs.get(key)
         if g is None:

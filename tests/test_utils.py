@@ -138,28 +138,79 @@ def test_lr_schedule_boundaries_follow_the_reference():
     tr.close()
 
 
-def test_graph_step_enumerates_every_flavour_of_the_schedule():
-    """GraphedTrainStep._sparse_flavours: Ok-Topk's schedule has exactly three step flavours (threshold reuse, exact
-    thresholds, exact + re-partition); they are what precapture_sparse() captures up front."""
+def test_graph_step_enumerates_every_call_plan_of_the_schedule():
+    """GraphedTrainStep._sparse_flavours, keyed by the density and each engine's CallPlan: at P = 2 Ok-Topk's schedule
+    has exactly three step flavours (threshold reuse, exact thresholds, exact + re-partition), at P = 1 two (a
+    re-partition changes nothing there), and under the dense switch one; they are what precapture_sparse() captures up
+    front."""
     from types import SimpleNamespace
     from oktopk_b200.config import OkTopkConfig
+    from oktopk_b200.parallel.state import CallPlan
     from oktopk_b200.train.graph_step import GraphedTrainStep
     cfg = OkTopkConfig(density=0.001, warmup_iters=512, local_recompute_interval=32, global_recompute_interval=32,
                        repartition_interval=64)
-    eng = SimpleNamespace(host=SimpleNamespace(counter=600))
+    eng = SimpleNamespace(host=SimpleNamespace(counter=600), P=2)
     opt = SimpleNamespace(_cfg=cfg, _buckets=[SimpleNamespace(name="b0")],
                           _allreducer=SimpleNamespace(_engines={"b0": eng}, compressor=SimpleNamespace(name="oktopk")),
                           get_current_density=lambda: 0.001)
     gs = GraphedTrainStep(SimpleNamespace(optimizer=opt))
+
+    def flags(fl):
+        assert all(k[0] == 0.001 and k[1].kind == "fused" for k in fl)
+        return sorted((k[1].exact_local, k[1].exact_global, k[1].repartition) for k in fl)
     fl = gs._sparse_flavours()
-    kinds = sorted(k[1] for k in fl)
-    assert kinds == [(False, False, False), (True, True, False), (True, True, True)]
-    assert fl[[k for k in fl if k[1] == (True, True, True)][0]] == 0
-    assert gs._key([512 + 32])[1] == (True, True, False) and gs._key([100])[1] == ("dense",)
+    assert flags(fl) == [(False, False, False), (True, True, False), (True, True, True)]
+    assert fl[(0.001, CallPlan("fused", True, True, True))] == 0
+    assert gs._key([512 + 32])[1] == CallPlan("fused", True, True, False) and gs._key([100])[1] == CallPlan("dense")
+    eng.P = 1
+    fl = gs._sparse_flavours()
+    assert flags(fl) == [(False, False, False), (True, True, False)]
+    assert fl[(0.001, CallPlan("fused", True, True, False))] == 0
+    eng.P = 2
+    opt.get_current_density = lambda: 0.1                 # at or above dense_switch_density (0.05): every step is dense
+    assert gs._sparse_flavours() == {(0.1, CallPlan("dense_switch")): 0}
+    opt.get_current_density = lambda: 0.001
     opt._allreducer.compressor.name = "topkAopt"
     assert len(gs._sparse_flavours()) == 2
     opt._allreducer.compressor.name = "gtopk"
     assert len(gs._sparse_flavours()) == 1               # native tree kernel: one flavour, capturable
+
+
+@pytest.mark.parametrize("P", [1, 2])
+def test_plan_call_follows_the_schedule_of_every_scheme(P):
+    """plan_call against the schedule written out here: dense warm-up, then Ok-Topk's exact local / exact global /
+    re-partition iterations (re-partition only at P > 1), TopkAopt's exact-threshold iterations, and no flags for the
+    other schemes; the dense switch takes the fused family only, at P > 1."""
+    from oktopk_b200.config import OkTopkConfig
+    from oktopk_b200.parallel.state import CallPlan, plan_call, schedule_period
+    cfg = OkTopkConfig(density=0.01, warmup_iters=5, local_recompute_interval=4, global_recompute_interval=6,
+                       repartition_interval=8, topkaopt_recompute_interval=3, dense_switch_density=0.05)
+    family = {"oktopk": "fused", "topkSA": "fused", "topkDSA": "fused", "gaussiankSA": "fused", "topkA": "gather",
+              "topkA2": "gather", "topkAopt": "gather", "gaussiank": "gather", "gaussiankconcat": "gather",
+              "gtopk": "tree"}
+    for name, fam in family.items():
+        period = {"oktopk": 24, "topkAopt": 3}.get(name, 1)
+        assert schedule_period(cfg, name) == period
+        for c in range(5 + 2 * 24):                      # two periods of the longest schedule
+            it = c - 5
+            if c < 5:
+                want = CallPlan("dense")
+            elif name == "oktopk":
+                want = CallPlan("fused", it % 4 == 0, it % 6 == 0, P > 1 and it % 8 == 0)
+            elif name == "topkAopt":
+                want = CallPlan("gather", exact_local=it % 3 == 0)
+            else:
+                want = CallPlan(fam)
+            assert plan_call(cfg, name, c, None, P) == want, (name, c)
+            if c >= 5:
+                assert plan_call(cfg, name, c + period, None, P) == want, (name, c)
+        switched = plan_call(cfg, name, 5, 0.05, P)
+        assert switched == (CallPlan("dense_switch") if fam == "fused" and P > 1 else plan_call(cfg, name, 5, None, P))
+        assert plan_call(cfg.replace(dense_switch_density=0.0), name, 5, 0.5, P).kind == fam
+        assert plan_call(cfg.replace(sparse=False), name, 5, None, P) == CallPlan("dense")
+    assert plan_call(cfg, "none", 5, None, P) == plan_call(cfg, None, 5, None, P) == CallPlan("dense")
+    with pytest.raises(KeyError):
+        plan_call(cfg, "nosuchscheme", 5, None, P)
 
 
 def test_bench_output_dump_is_seeded_and_bounded(tmp_path):
