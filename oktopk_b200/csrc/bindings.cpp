@@ -497,9 +497,9 @@ static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, do
                          decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
        "fused_adam");
 }
-// dtype of x, y, dy, dx: 0 = fp32, 1 = bf16 (parameters, statistics and dgamma / dbeta are fp32 either way)
+// dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case)
 static BnDtype bn_dtype(int dtype, const char* what) {
-    if (dtype != 0 && dtype != 1) throw std::runtime_error(std::string(what) + ": dtype must be 0 (fp32) or 1 (bf16)");
+    if (dtype < 0 || dtype > 2) throw std::runtime_error(std::string(what) + ": dtype must be 0 (fp32), 1 (bf16) or 2 (fp16)");
     return static_cast<BnDtype>(dtype);
 }
 static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, uint64_t gamma, uint64_t beta, uint64_t cbias,

@@ -1,4 +1,4 @@
-// Fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool] for channels_last fp32 or bf16 activations, training mode,
+// Fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations, training mode,
 // forward and backward: one cooperative kernel per pass.
 //
 // The CNN zoo of the reference (VGG/models/vgg.py:28-36 and the ResNets) is stacks of  Conv2d -> BatchNorm2d -> ReLU
@@ -32,13 +32,24 @@
 // (128-bit accesses) and strides over rows; tiles are contiguous row ranges.  With a pool, a tile is a whole number of
 // image row pairs (rows_per_block % 2W == 0), so no 2x2 window straddles two tiles.
 //
-// Activation type (BnAct): x, y, dy and dx are fp32 (one float4 per access) or bf16 (four bf16 in one 8-byte access).
-// A bf16 load is widened to a float4, which is exact, and from there the arithmetic is the fp32 kernel's, operation for
-// operation: same tiles, partials, combine, running-statistic fma, ReLU mask, pool arg-max and dx formula.  Only the
-// stores of y and dx round to bf16 (to nearest, ties to even).  The bf16 kernel is therefore, bit for bit, the fp32
-// kernel run on x.float() (and dy.float()) with y and dx rounded.  gamma, beta, the conv bias, the running and saved
-// statistics, the partials and dgamma / dbeta stay fp32 either way, as in torch's batch-norm under bf16 autocast.
+// Activation type (BnAct): x, y, dy and dx are fp32 (one float4 per access), bf16 or fp16 (four 16-bit values in one
+// 8-byte access).  A bf16 or fp16 load is widened to a float4, which is exact, and from there the arithmetic is the fp32
+// kernel's, operation for operation: same tiles, partials, combine, running-statistic fma, ReLU mask, pool arg-max and
+// dx formula.  Only the stores of y and dx round to the 16-bit type (to nearest, ties to even).  The bf16 and fp16
+// kernels are therefore, bit for bit, the fp32 kernel run on x.float() (and dy.float()) with y and dx rounded.  gamma,
+// beta, the conv bias, the running and saved statistics, the partials and dgamma / dbeta stay fp32 in every case, as in
+// torch's batch-norm under autocast.
+//
+// fp16 has three more significand bits than bf16 but a far narrower range, so its range rules are part of the spec:
+//   - overflow: a y or dx whose magnitude rounds past 65504 is stored as +-inf, as torch's .half() does.  Under loss
+//     scaling a too-large scaled gradient overflowing in dx is the normal way an fp16 step overflows; the inf must reach
+//     the optimizer's non-finite check, so nothing is saturated or clamped;
+//   - subnormals: results below 2^-14 in magnitude are rounded to fp16 subnormals, not flushed to zero (cvt.rn.f16x2.f32
+//     without .ftz; the build does not pass -ftz or --use_fast_math), and subnormal inputs widen exactly;
+//   - non-finite inputs: an inf or NaN in x or dy propagates exactly as in the fp32 kernel on the widened input, into
+//     the statistics and the running statistics too (as stock batch-norm does).  There is no extra finite check.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "oktopk.cuh"
@@ -101,6 +112,18 @@ template <> struct BnAct<__nv_bfloat16> {
     }
     static __device__ __forceinline__ uint2 narrow(const float4& v) {  // round to nearest, ties to even
         const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
+    }
+};
+template <> struct BnAct<__half> {
+    using V = uint2;                          // channels 0, 1 in x (low half first), 2, 3 in y
+    static __device__ __forceinline__ float4 wide(const uint2& v) {   // every fp16, subnormals included, is an fp32: exact
+        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+        return make_float4(lo.x, lo.y, hi.x, hi.y);
+    }
+    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // nearest even; past 65504 -> inf; no flush to zero
+        const __half2 lo = __floats2half2_rn(v.x, v.y), hi = __floats2half2_rn(v.z, v.w);
         return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
     }
 };
@@ -593,6 +616,9 @@ cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float*
         case BnDtype::kBF16:
             return bn_forward_t<__nv_bfloat16>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar,
                                                nbt, momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+        case BnDtype::kF16:
+            return bn_forward_t<__half>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
+                                        momentum, eps, relu, M, C, W, slot, max_ctas, stream);
     }
     return cudaErrorInvalidValue;
 }
@@ -608,6 +634,9 @@ cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned cha
         case BnDtype::kBF16:
             return bn_backward_t<__nv_bfloat16>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta,
                                                 relu, M, C, W, slot, max_ctas, stream);
+        case BnDtype::kF16:
+            return bn_backward_t<__half>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
+                                         M, C, W, slot, max_ctas, stream);
     }
     return cudaErrorInvalidValue;
 }

@@ -346,7 +346,7 @@ cudaError_t launch_land(const LandParams& lp, float* bucket, cudaStream_t stream
 // fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool when W > 0], channels_last, training mode (csrc/bnrelu.cu):
 // one cooperative kernel per pass.  `slot` names the call site's grid hand-off counters; max_ctas > 0 caps the grid.
 // x, y, dy and dx are of type `dtype`; parameters, statistics, partials and dgamma / dbeta are fp32.
-enum class BnDtype : int { kF32 = 0, kBF16 = 1 };
+enum class BnDtype : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 int bn_tile_rows(int M, int C);
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,

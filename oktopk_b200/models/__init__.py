@@ -20,7 +20,7 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
-        net = VGG(d, num_classes)
+        net = VGG(d, num_classes, fuse_fp16=bool(kwargs.get("fuse_fp16", False)))
     elif d in ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110"):
         net = zoo.CifarResNet(int(d[6:]), num_classes)
     elif d.startswith("preresnet"):

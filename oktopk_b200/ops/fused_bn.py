@@ -1,4 +1,5 @@
-"""Fused (conv-bias +) BatchNorm2d + ReLU [+ 2x2 max-pool] for channels_last fp32 or bf16 activations (``csrc/bnrelu.cu``).
+"""Fused (conv-bias +) BatchNorm2d + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations
+(``csrc/bnrelu.cu``).
 
 ``bias_bn_relu(x, bn, conv_bias, relu=True, pool=None)`` replaces ``pool(relu(bn(x + conv_bias)))`` in training mode on
 CUDA with one kernel forward and one backward instead of the seven stock ones (bias add, batch-norm, clamp, counter
@@ -13,11 +14,21 @@ bf16: under ``torch.autocast("cuda", torch.bfloat16)`` (or with bf16 activations
 returns bf16 and the kernels' bf16 instantiation runs.  As torch's batch-norm does under autocast, it takes bf16
 activations with fp32 parameters and statistics: ``y`` and ``dx`` are bf16; ``dgamma``, ``dbeta`` and the running
 statistics fp32.  Its results are bit for bit those of the fp32 kernels run on ``x.float()`` (and ``dy.float()``), with
-``y`` and ``dx`` rounded to bf16.  fp16 autocast keeps the stock ops.
+``y`` and ``dx`` rounded to bf16.
 
-Falls back to the stock ops whenever the fast path does not apply (CPU, eval mode, activations neither fp32 nor bf16,
-fp16 autocast, parameters not fp32, not channels_last, channels not a multiple of 4, cumulative-average momentum).  A pool that cannot be folded in (not 2x2 / stride 2, odd
-height or width, or batch-norm tiles that are not whole pairs of image rows) runs after the fused kernel on its own.
+fp16 is opt-in: every entry point takes ``fp16=False``, and only with ``fp16=True`` do fp16 activations (autocast off
+or ``torch.autocast("cuda", torch.float16)``) take the kernels' fp16 instantiation; the fp32 input of a convolution
+under fp16 autocast then qualifies too, since the convolution hands the batch-norm fp16.  The kernel is the bf16 one's
+spec in fp16: bit for bit the fp32 kernels on the widened input with ``y`` and ``dx`` rounded to fp16.  fp16's narrow
+range is kept as torch's ``.half()`` keeps it: a value that rounds past 65504 is stored as inf (under loss scaling that
+inf is what the optimizer's overflow check sees), subnormals are not flushed, and an inf or NaN input propagates as in
+the fp32 kernel.  Without ``fp16=True`` fp16 activations and fp16 autocast keep the stock ops.
+
+Falls back to the stock ops whenever the fast path does not apply (CPU, eval mode, activations neither fp32 nor bf16
+nor opted-in fp16, fp16 autocast without ``fp16=True``, parameters not fp32, not channels_last, channels not a multiple
+of 4, cumulative-average momentum).  A pool that cannot be folded in (not 2x2 / stride 2, odd height or width, or
+batch-norm tiles that are not whole pairs of image rows) runs after the fused kernel on its own, on stock ``MaxPool2d``
+for 16-bit activations (the standalone pool kernels are fp32 only).
 """
 from __future__ import annotations
 
@@ -36,7 +47,7 @@ MAX_CTAS = 0
 _SLOTS = itertools.count()
 
 # the kernels' activation type argument (csrc/bindings.cpp bn_forward / bn_backward)
-_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1}
+_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 
 def _sync_slot(bn: torch.nn.BatchNorm2d) -> int:
@@ -48,18 +59,23 @@ def _sync_slot(bn: torch.nn.BatchNorm2d) -> int:
     return s
 
 
-def _dtype_ok(x: torch.Tensor) -> bool:
-    """fp32 or bf16 activations, with autocast off or in bf16 (fp16 autocast keeps the stock ops)."""
-    return (x.dtype in (torch.float32, torch.bfloat16)
-            and (not torch.is_autocast_enabled() or torch.get_autocast_dtype("cuda") == torch.bfloat16))
+def _dtype_ok(x: torch.Tensor, fp16: bool = False) -> bool:
+    """fp32 or bf16 activations, with autocast off or in bf16.  With ``fp16``, also fp16 activations with autocast off,
+    and fp16 or fp32 ones under fp16 autocast (a convolution there turns fp32 input into fp16, and stock batch-norm runs
+    an fp32 activation in fp32).  Without ``fp16``, fp16 activations and fp16 autocast keep the stock ops."""
+    if not torch.is_autocast_enabled():
+        return x.dtype in (torch.float32, torch.bfloat16) or (fp16 and x.dtype == torch.float16)
+    if torch.get_autocast_dtype("cuda") == torch.float16:
+        return fp16 and x.dtype in (torch.float32, torch.float16)
+    return x.dtype in (torch.float32, torch.bfloat16) and torch.get_autocast_dtype("cuda") == torch.bfloat16
 
 
 def _bn_params_fp32(bn: torch.nn.BatchNorm2d) -> bool:
     return all(t is None or t.dtype == torch.float32 for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
 
 
-def _fast_path_ok(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
-    return (x.is_cuda and _dtype_ok(x) and x.dim() == 4 and bn.training and bn.affine
+def _fast_path_ok(x: torch.Tensor, bn: torch.nn.BatchNorm2d, fp16: bool = False) -> bool:
+    return (x.is_cuda and _dtype_ok(x, fp16) and x.dim() == 4 and bn.training and bn.affine
             and bn.momentum is not None and x.size(1) % 4 == 0 and _bn_params_fp32(bn)
             and x.is_contiguous(memory_format=torch.channels_last) and ext.available())
 
@@ -127,9 +143,10 @@ class _BiasBNReLUPool(torch.autograd.Function):
 
 
 def bias_bn_relu(x: torch.Tensor, bn: torch.nn.BatchNorm2d, conv_bias: Optional[torch.Tensor] = None,
-                 relu: bool = True, pool: Optional[torch.nn.MaxPool2d] = None) -> torch.Tensor:
-    """``pool(relu(bn(x + conv_bias)))`` (``relu=False``: without the ReLU; ``pool=None``: without the pool)."""
-    if _fast_path_ok(x, bn) and (conv_bias is None or conv_bias.dtype == torch.float32):
+                 relu: bool = True, pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False) -> torch.Tensor:
+    """``pool(relu(bn(x + conv_bias)))`` (``relu=False``: without the ReLU; ``pool=None``: without the pool;
+    ``fp16``: fp16 activations and fp16 autocast take the fused kernels too)."""
+    if _fast_path_ok(x, bn, fp16) and (conv_bias is None or conv_bias.dtype == torch.float32):
         track = bn.track_running_stats and bn.running_mean is not None
         fuse = pool is not None and _pool_fusable(x, pool)
         y = _BiasBNReLUPool.apply(x, bn.weight, bn.bias, conv_bias, bn.running_mean if track else None,
@@ -144,13 +161,13 @@ def bias_bn_relu(x: torch.Tensor, bn: torch.nn.BatchNorm2d, conv_bias: Optional[
 
 
 def conv_bn_relu(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, relu: bool = True,
-                 pool: Optional[torch.nn.MaxPool2d] = None) -> torch.Tensor:
+                 pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False) -> torch.Tensor:
     """``pool(relu(bn(conv(x))))`` with the convolution's bias folded into the fused batch-norm when the fast path
-    applies."""
-    if _fast_path_ok_pre(x, conv, bn):
+    applies (``fp16``: see ``bias_bn_relu``)."""
+    if _fast_path_ok_pre(x, conv, bn, fp16):
         z = F.conv2d(x, conv.weight, None, conv.stride, conv.padding, conv.dilation, conv.groups)
-        if _fast_path_ok(z, bn):
-            return bias_bn_relu(z, bn, conv.bias, relu, pool)
+        if _fast_path_ok(z, bn, fp16):
+            return bias_bn_relu(z, bn, conv.bias, relu, pool, fp16)
         if conv.bias is not None:
             z = z + conv.bias.view(1, -1, 1, 1)
         y = bn(z)
@@ -160,8 +177,8 @@ def conv_bn_relu(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2
     return y if pool is None else max_pool_2x2(y, pool)
 
 
-def _fast_path_ok_pre(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d) -> bool:
-    return (x.is_cuda and _dtype_ok(x) and bn.training and bn.affine and bn.momentum is not None
+def _fast_path_ok_pre(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, fp16: bool = False) -> bool:
+    return (x.is_cuda and _dtype_ok(x, fp16) and bn.training and bn.affine and bn.momentum is not None
             and conv.out_channels % 4 == 0 and conv.padding_mode == "zeros" and ext.available()
             and (conv.bias is None or conv.bias.dtype == torch.float32) and _bn_params_fp32(bn)
             and x.is_contiguous(memory_format=torch.channels_last) and not isinstance(conv.padding, str))
@@ -203,8 +220,9 @@ def max_pool_2x2(x: torch.Tensor, pool: torch.nn.MaxPool2d) -> torch.Tensor:
     return pool(x)
 
 
-def run_fused_sequential(seq: torch.nn.Sequential, x: torch.Tensor) -> torch.Tensor:
-    """Run an ``nn.Sequential`` fusing every ``Conv2d -> BatchNorm2d [-> ReLU] [-> MaxPool2d]`` run it contains."""
+def run_fused_sequential(seq: torch.nn.Sequential, x: torch.Tensor, fp16: bool = False) -> torch.Tensor:
+    """Run an ``nn.Sequential`` fusing every ``Conv2d -> BatchNorm2d [-> ReLU] [-> MaxPool2d]`` run it contains
+    (``fp16``: see ``bias_bn_relu``)."""
     mods = list(seq.children())
     i = 0
     while i < len(mods):
@@ -213,7 +231,7 @@ def run_fused_sequential(seq: torch.nn.Sequential, x: torch.Tensor) -> torch.Ten
             relu = i + 2 < len(mods) and isinstance(mods[i + 2], torch.nn.ReLU)
             j = i + (3 if relu else 2)
             pool = mods[j] if j < len(mods) and isinstance(mods[j], torch.nn.MaxPool2d) else None
-            x = conv_bn_relu(x, m, mods[i + 1], relu, pool)
+            x = conv_bn_relu(x, m, mods[i + 1], relu, pool, fp16)
             i = j + (1 if pool is not None else 0)
         elif isinstance(m, torch.nn.MaxPool2d):
             x = max_pool_2x2(x, m)

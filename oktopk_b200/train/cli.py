@@ -64,6 +64,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--cuda-graph", action="store_true", help="capture forward+backward+allreduce+update into CUDA graphs")
     p.add_argument("--fp16", action="store_true", help="fp16 autocast (reference: apex amp O3, main_bert.py:1009-1023)")
     p.add_argument("--bf16", action="store_true", help="bf16 autocast")
+    p.add_argument("--fused-bn-fp16", action="store_true",
+                   help="with --fp16: VGG's Conv -> BN -> ReLU [-> pool] blocks take the fused fp16 batch-norm kernels "
+                        "(default: stock modules under fp16)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -76,11 +79,8 @@ def build_parser() -> argparse.ArgumentParser:
     return p
 
 
-def main(argv=None) -> int:
-    args = build_parser().parse_args(argv)
-    import oktopk_b200 as okt
-    from .trainer import preset_for, robust_ssgd
-    okt.init()
+def model_args(args: argparse.Namespace):
+    """``(dnn, model_kwargs)`` for ``create_net`` from the parsed flags."""
     dnn = args.dnn
     model_kwargs = {}
     if args.module:                       # 'models.bert12.depth=4' => 12 layers run as 4 stage modules
@@ -94,6 +94,20 @@ def main(argv=None) -> int:
         model_kwargs["config"] = cfg_path
     if args.recompute_step:
         model_kwargs["recompute"] = True
+    if args.fused_bn_fp16:
+        model_kwargs["fuse_fp16"] = True
+    return dnn, model_kwargs
+
+
+def main(argv=None) -> int:
+    parser = build_parser()
+    args = parser.parse_args(argv)
+    if args.fused_bn_fp16 and not args.fp16:
+        parser.error("--fused-bn-fp16 needs --fp16")
+    import oktopk_b200 as okt
+    from .trainer import preset_for, robust_ssgd
+    okt.init()
+    dnn, model_kwargs = model_args(args)
     if args.train_path and not args.data_dir:
         args.data_dir = os.path.dirname(os.path.abspath(args.train_path))
     cfg = okt.preset(args.preset or preset_for(dnn), density=args.density, sigma_scale=args.sigma_scale)

@@ -100,7 +100,8 @@ def _kernel_pair_us(C, shape, pooled, dtype, iters):
     nbt = torch.zeros((), dtype=torch.long, device="cuda")
     stats, dgb = torch.empty(2 * Ch, device="cuda"), torch.empty(2 * Ch, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
-    flag = 1 if dtype == torch.bfloat16 else 0
+    from oktopk_b200.ops.fused_bn import _DTYPE_FLAG
+    flag = _DTYPE_FLAG[dtype]
     Wp = W if pooled else 0
 
     def pair():
