@@ -497,29 +497,35 @@ static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, do
                          decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
        "fused_adam");
 }
-// dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case)
+// dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case).
+// res (forward and backward) and dres (backward), 0 = absent: y = relu(bn(x) + res) and dres = the residual's gradient,
+// [M, C] in x's dtype, with relu = 1 and W = 0.
 static BnDtype bn_dtype(int dtype, const char* what) {
     if (dtype < 0 || dtype > 2) throw std::runtime_error(std::string(what) + ": dtype must be 0 (fp32), 1 (bf16) or 2 (fp16)");
     return static_cast<BnDtype>(dtype);
 }
 static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, uint64_t gamma, uint64_t beta, uint64_t cbias,
                        uint64_t save_mean, uint64_t save_invstd, uint64_t rmean, uint64_t rvar, uint64_t nbt, double momentum,
-                       double eps, int relu, int M, int C, int W, int slot, int max_ctas, uint64_t stream, int dtype) {
+                       double eps, int relu, int M, int C, int W, int slot, int max_ctas, uint64_t stream, int dtype,
+                       uint64_t res) {
     if (C % 4 != 0) throw std::runtime_error("bn_forward: channel count must be a multiple of 4");
     if (slot < 0) throw std::runtime_error("bn_forward: negative slot");
+    if (res != 0 && (W != 0 || !relu)) throw std::runtime_error("bn_forward: a residual needs relu = 1 and no pool");
     ck(launch_bn_forward(P_<const void>(x), P_<void>(y), P_<unsigned char>(arg), P_<float>(partial), P_<const float>(gamma),
                          P_<const float>(beta), P_<const float>(cbias), P_<float>(save_mean), P_<float>(save_invstd),
                          P_<float>(rmean), P_<float>(rvar), P_<long long>(nbt), (float)momentum, (float)eps, relu, M, C, W, slot,
-                         max_ctas, bn_dtype(dtype, "bn_forward"), S_(stream)), "bn_forward");
+                         max_ctas, bn_dtype(dtype, "bn_forward"), S_(stream), P_<const void>(res)), "bn_forward");
 }
 static void bn_backward(uint64_t x, uint64_t dy, uint64_t arg, uint64_t dx, uint64_t partial, uint64_t gamma, uint64_t beta,
                         uint64_t save_mean, uint64_t save_invstd, uint64_t dgamma, uint64_t dbeta, int relu, int M, int C, int W,
-                        int slot, int max_ctas, uint64_t stream, int dtype) {
+                        int slot, int max_ctas, uint64_t stream, int dtype, uint64_t res, uint64_t dres) {
     if (slot < 0) throw std::runtime_error("bn_backward: negative slot");
+    if ((res == 0) != (dres == 0)) throw std::runtime_error("bn_backward: res and dres go together");
+    if (res != 0 && (W != 0 || !relu)) throw std::runtime_error("bn_backward: a residual needs relu = 1 and no pool");
     ck(launch_bn_backward(P_<const void>(x), P_<const void>(dy), P_<const unsigned char>(arg), P_<void>(dx), P_<float>(partial),
                           P_<const float>(gamma), P_<const float>(beta), P_<const float>(save_mean), P_<const float>(save_invstd),
                           P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, bn_dtype(dtype, "bn_backward"),
-                          S_(stream)), "bn_backward");
+                          S_(stream), P_<const void>(res), P_<void>(dres)), "bn_backward");
 }
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
     if ((C % 4) || (H % 2) || (W % 2)) throw std::runtime_error("maxpool2_fwd: needs C % 4 == 0 and even H, W");
@@ -638,8 +644,14 @@ PYBIND11_MODULE(_C, m) {
     m.attr("VERDICT_OFFSET") = offsetof(ScaleSync, verdict);
     m.def("maxpool2_fwd", &maxpool2_fwd);
     m.def("maxpool2_bwd", &maxpool2_bwd);
-    m.def("bn_forward", &bn_forward);
-    m.def("bn_backward", &bn_backward);
+    m.def("bn_forward", &bn_forward, py::arg("x"), py::arg("y"), py::arg("arg"), py::arg("partial"), py::arg("gamma"),
+          py::arg("beta"), py::arg("cbias"), py::arg("save_mean"), py::arg("save_invstd"), py::arg("rmean"), py::arg("rvar"),
+          py::arg("nbt"), py::arg("momentum"), py::arg("eps"), py::arg("relu"), py::arg("M"), py::arg("C"), py::arg("W"),
+          py::arg("slot"), py::arg("max_ctas"), py::arg("stream"), py::arg("dtype"), py::arg("res") = 0);
+    m.def("bn_backward", &bn_backward, py::arg("x"), py::arg("dy"), py::arg("arg"), py::arg("dx"), py::arg("partial"),
+          py::arg("gamma"), py::arg("beta"), py::arg("save_mean"), py::arg("save_invstd"), py::arg("dgamma"), py::arg("dbeta"),
+          py::arg("relu"), py::arg("M"), py::arg("C"), py::arg("W"), py::arg("slot"), py::arg("max_ctas"), py::arg("stream"),
+          py::arg("dtype"), py::arg("res") = 0, py::arg("dres") = 0);
     m.def("bn_tile_rows", &bn_tile_rows);
     m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;

@@ -1,4 +1,4 @@
-// Fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations, training mode,
+// Fused (conv-bias +) BatchNorm [+ residual] + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations, training mode,
 // forward and backward: one cooperative kernel per pass.
 //
 // The CNN zoo of the reference (VGG/models/vgg.py:28-36 and the ResNets) is stacks of  Conv2d -> BatchNorm2d -> ReLU
@@ -27,6 +27,14 @@
 // A bias added before a batch-norm cancels exactly: BN(x + b) = BN(x) with the batch mean shifted by b.  The forward pass
 // therefore never adds it (only running_mean sees it), and its gradient -- identically zero, since the loss does not depend
 // on it -- is not "computed" by a reduction over dy that can only return rounding noise.
+//
+// Residual (kRes, the end of a ResNet block: y = relu(bn(x) + r)): r is [M, C] in x's type and layout.  The statistics,
+// running statistics and conv-bias rule are unchanged: the batch-norm only sees x.
+//   forward : (3) writes  y = max(0, fma(x, a, b) + r)  (fp32 add of the widened r), reading r as y is stored;
+//   backward: (1) recomputes the mask  [fma(x, a, b) + r > 0]  bit for bit, writes  dres = dy [mask]  (exact: dy or 0)
+//                 and takes dbeta / dgamma over it; a held tile keeps the masked gradient on chip;
+//             (3) dx by the same formula from the masked gradient: held, or the dres this CTA wrote in (1), read back.
+// kRes and kPool never combine (no ResNet pools after the add); kRes = false compiles to the kernels without it.
 //
 // Layout: x is [M, C] row-major (NHWC with M = N*H*W), C a multiple of 4; each thread owns 4 consecutive channels
 // (128-bit accesses) and strides over rows; tiles are contiguous row ranges.  With a pool, a tile is a whole number of
@@ -235,10 +243,12 @@ struct BnFwdArgs {
     int relu;
     unsigned int* sync;
     BnGeom g;
+    const T* res;               // kRes only: the residual [M, C], added after the batch-norm, before the ReLU
 };
 
-template <bool kPool, typename T>
+template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p) {
+    static_assert(!(kPool && kRes), "no pool follows a residual add");
     using A = BnAct<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals, then a = gamma/std, b = beta - mean a | pool: held y
@@ -315,11 +325,19 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
     }
     __syncthreads();
 
-    // (3) y = max(0, a x + b), or its 2x2 max-pool
+    // (3) y = max(0, a x + b), or its 2x2 max-pool, or with a residual r  y = max(0, (a x + b) + r)
     const float4* ab4 = s_dyn;                // [cv] a | [cv] b
     auto yval = [&](const float4& xin, int col) {
         float4 v = f4_fma(xin, ab4[col], ab4[g.cv + col]);
         if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+        return v;
+    };
+    const V* r4 = reinterpret_cast<const V*>(p.res);
+    auto ldr = [&](size_t o) { return A::wide(__ldg(r4 + o)); };
+    auto yres = [&](const float4& xin, const float4& rin, int col) {
+        float4 v = f4_fma(xin, ab4[col], ab4[g.cv + col]);
+        v.x += rin.x; v.y += rin.y; v.z += rin.z; v.w += rin.w;
+        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
         return v;
     };
     V* y4 = reinterpret_cast<V*>(p.y);
@@ -332,18 +350,39 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
                 if (ty >= g.rpi || col >= g.cv) continue;
                 int r = row0 + ty;
                 if (held) {
+                    if constexpr (kRes) {
+                        float4 q[kBnHold];
 #pragma unroll
-                    for (int k = 0; k < kBnHold; ++k)
-                        if (r + k * g.rpi < row1) y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(yval(A::wide(h[k]), col));
+                        for (int k = 0; k < kBnHold; ++k)
+                            if (r + k * g.rpi < row1) q[k] = ldr((size_t)(r + k * g.rpi) * g.cv + col);
+#pragma unroll
+                        for (int k = 0; k < kBnHold; ++k)
+                            if (r + k * g.rpi < row1)
+                                y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(yres(A::wide(h[k]), q[k], col));
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < kBnHold; ++k)
+                            if (r + k * g.rpi < row1) y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(yval(A::wide(h[k]), col));
+                    }
                     continue;
                 }
                 for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                     const size_t o = (size_t)r * g.cv + col;
                     const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
-                    y4[o] = A::narrow(yval(v0, col)); y4[o + st1] = A::narrow(yval(v1, col));
-                    y4[o + 2 * st1] = A::narrow(yval(v2, col)); y4[o + 3 * st1] = A::narrow(yval(v3, col));
+                    if constexpr (kRes) {
+                        const float4 q0 = ldr(o), q1 = ldr(o + st1), q2 = ldr(o + 2 * st1), q3 = ldr(o + 3 * st1);
+                        y4[o] = A::narrow(yres(v0, q0, col)); y4[o + st1] = A::narrow(yres(v1, q1, col));
+                        y4[o + 2 * st1] = A::narrow(yres(v2, q2, col)); y4[o + 3 * st1] = A::narrow(yres(v3, q3, col));
+                    } else {
+                        y4[o] = A::narrow(yval(v0, col)); y4[o + st1] = A::narrow(yval(v1, col));
+                        y4[o + 2 * st1] = A::narrow(yval(v2, col)); y4[o + 3 * st1] = A::narrow(yval(v3, col));
+                    }
                 }
-                for (; r < row1; r += g.rpi) { const size_t o = (size_t)r * g.cv + col; y4[o] = A::narrow(yval(ldx(o), col)); }
+                for (; r < row1; r += g.rpi) {
+                    const size_t o = (size_t)r * g.cv + col;
+                    if constexpr (kRes) y4[o] = A::narrow(yres(ldx(o), ldr(o), col));
+                    else y4[o] = A::narrow(yval(ldx(o), col));
+                }
             }
         } else {
             // a held tile is staged in shared memory (its windows span threads); the window of pooled pixel pp is the
@@ -390,10 +429,13 @@ struct BnBwdArgs {
     int relu;
     unsigned int* sync;
     BnGeom g;
+    const T* res;               // kRes only: the forward's residual [M, C]
+    T* dres;                    // kRes only: its gradient dy * [z > 0], [M, C]
 };
 
-template <bool kPool, typename T>
+template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p) {
+    static_assert(!(kPool && kRes), "no pool follows a residual add");
     using A = BnAct<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals
@@ -440,8 +482,21 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
         return make_float4((v.x - k.mean.x) * k.istd.x, (v.y - k.mean.y) * k.istd.y, (v.z - k.mean.z) * k.istd.z,
                            (v.w - k.mean.w) * k.istd.w);
     };
+    // with a residual the forward output was max(0, fma(x, a, b) + r): the same mask, bit for bit, and the gradient of
+    // both the batch-norm output and the residual is dy masked by it, which is written out as dres (exact)
+    const V* r4 = reinterpret_cast<const V*>(p.res);
+    V* dr4 = reinterpret_cast<V*>(p.dres);
+    auto ldr = [&](size_t o) { return A::wide(__ldg(r4 + o)); };
+    auto gate = [&](const Col& k, const float4& v, const float4& q, size_t o, float4& d) {
+        if (!(fmaf(v.x, k.a.x, k.b.x) + q.x > 0.f)) d.x = 0.f;
+        if (!(fmaf(v.y, k.a.y, k.b.y) + q.y > 0.f)) d.y = 0.f;
+        if (!(fmaf(v.z, k.a.z, k.b.z) + q.z > 0.f)) d.z = 0.f;
+        if (!(fmaf(v.w, k.a.w, k.b.w) + q.w > 0.f)) d.w = 0.f;
+        dr4[o] = A::narrow(d);
+    };
     V hx[kBnHold];                            // the CTA's first tile: x as stored
-    float4 hd[kBnHold];                       // and the incoming gradient (with a pool: expanded at the arg-max)
+    float4 hd[kBnHold];                       // and the incoming gradient (with a pool: expanded at the arg-max; with a
+                                              // residual: already masked)
 
     // (1) partials, eight or more independent 128-bit loads in flight per thread
     for (int t = blockIdx.x; t < g.nblk; t += gridDim.x) {
@@ -454,7 +509,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                 const Col k = column(col);
                 auto acc = [&](const float4& v, float4 d) {
                     const float4 xh = xhat(k, v);
-                    mask(k, v, d);
+                    if constexpr (!kRes) mask(k, v, d);
                     sb.x += d.x; sb.y += d.y; sb.z += d.z; sb.w += d.w;
                     sg.x = fmaf(d.x, xh.x, sg.x); sg.y = fmaf(d.y, xh.y, sg.y); sg.z = fmaf(d.z, xh.z, sg.z); sg.w = fmaf(d.w, xh.w, sg.w);
                 };
@@ -466,6 +521,14 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                         hx[j] = rr < row1 ? __ldg(x4 + (size_t)rr * g.cv + col) : V{};
                         hd[j] = rr < row1 ? grad(row0, rr, col) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
+                    if constexpr (kRes) {
+#pragma unroll
+                        for (int j = 0; j < kBnHold; ++j)
+                            if (r + j * g.rpi < row1) {
+                                const size_t o = (size_t)(r + j * g.rpi) * g.cv + col;
+                                gate(k, A::wide(hx[j]), ldr(o), o, hd[j]);
+                            }
+                    }
 #pragma unroll
                     for (int j = 0; j < kBnHold; ++j)
                         if (r + j * g.rpi < row1) acc(A::wide(hx[j]), hd[j]);
@@ -473,11 +536,26 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                     for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                         const size_t o = (size_t)r * g.cv + col;
                         const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
-                        const float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
-                                     e3 = grad(row0, r + 3 * g.rpi, col);
+                        float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
+                               e3 = grad(row0, r + 3 * g.rpi, col);
+                        if constexpr (kRes) {
+                            const float4 q0 = ldr(o), q1 = ldr(o + st1), q2 = ldr(o + 2 * st1), q3 = ldr(o + 3 * st1);
+                            gate(k, v0, q0, o, e0); gate(k, v1, q1, o + st1, e1);
+                            gate(k, v2, q2, o + 2 * st1, e2); gate(k, v3, q3, o + 3 * st1, e3);
+                        }
                         acc(v0, e0); acc(v1, e1); acc(v2, e2); acc(v3, e3);
                     }
-                    for (; r < row1; r += g.rpi) acc(ldx((size_t)r * g.cv + col), grad(row0, r, col));
+                    for (; r < row1; r += g.rpi) {
+                        if constexpr (kRes) {
+                            const size_t o = (size_t)r * g.cv + col;
+                            const float4 v = ldx(o);
+                            float4 e = grad(row0, r, col);
+                            gate(k, v, ldr(o), o, e);
+                            acc(v, e);
+                        } else {
+                            acc(ldx((size_t)r * g.cv + col), grad(row0, r, col));
+                        }
+                    }
                 }
             }
             bn_tile_partial(sb, sg, tx, ty, col, g, s_red, p.partial, t);
@@ -510,7 +588,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
             V* o4 = reinterpret_cast<V*>(p.dx);
             auto out = [&](size_t off, const float4& v, float4 d) {
                 const float4 xh = xhat(k, v);
-                mask(k, v, d);
+                if constexpr (!kRes) mask(k, v, d);
                 o4[off] = A::narrow(make_float4(k.a.x * (d.x - mb.x - xh.x * mg.x), k.a.y * (d.y - mb.y - xh.y * mg.y),
                                                 k.a.z * (d.z - mb.z - xh.z * mg.z), k.a.w * (d.w - mb.w - xh.w * mg.w)));
             };
@@ -521,14 +599,18 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                     if (r + j * g.rpi < row1) out((size_t)(r + j * g.rpi) * g.cv + col, A::wide(hx[j]), hd[j]);
                 continue;
             }
+            // with a residual, the masked gradient is the dres this thread wrote in (1): a coherent load, not __ldg
+            auto grad3 = [&](int r3) -> float4 {
+                if constexpr (kRes) return A::wide(__ldcg(dr4 + (size_t)r3 * g.cv + col));
+                else return grad(row0, r3, col);
+            };
             for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                 const size_t o = (size_t)r * g.cv + col;
                 const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
-                const float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
-                             e3 = grad(row0, r + 3 * g.rpi, col);
+                const float4 e0 = grad3(r), e1 = grad3(r + g.rpi), e2 = grad3(r + 2 * g.rpi), e3 = grad3(r + 3 * g.rpi);
                 out(o, v0, e0); out(o + st1, v1, e1); out(o + 2 * st1, v2, e2); out(o + 3 * st1, v3, e3);
             }
-            for (; r < row1; r += g.rpi) out((size_t)r * g.cv + col, ldx((size_t)r * g.cv + col), grad(row0, r, col));
+            for (; r < row1; r += g.rpi) out((size_t)r * g.cv + col, ldx((size_t)r * g.cv + col), grad3(r));
         }
     }
 }
@@ -580,45 +662,50 @@ template <typename T>
 static cudaError_t bn_forward_t(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma,
                                 const float* beta, const float* cbias, float* save_mean, float* save_invstd, float* rmean,
                                 float* rvar, long long* nbt, float momentum, float eps, int relu, int M, int C, int W, int slot,
-                                int max_ctas, cudaStream_t stream) {
+                                int max_ctas, cudaStream_t stream, const void* res) {
+    if (res != nullptr && (W > 0 || !relu)) return cudaErrorInvalidValue;      // a residual is always followed by the ReLU
     BnFwdArgs<T> p{static_cast<const T*>(x), static_cast<T*>(y), arg, partial, gamma, beta, cbias, save_mean, save_invstd,
-                   rmean, rvar, nbt, momentum, eps, relu, nullptr, {}};
+                   rmean, rvar, nbt, momentum, eps, relu, nullptr, {}, static_cast<const T*>(res)};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
     size_t smem = sizeof(float) * 2 * C;
     if (W > 0 && p.g.hold) smem += sizeof(float4) * p.g.rows_per_block * p.g.cv;
-    return W > 0 ? bn_launch(bn_fwd_kernel<true, T>, p, smem, max_ctas, stream)
-                 : bn_launch(bn_fwd_kernel<false, T>, p, smem, max_ctas, stream);
+    if (W > 0) return bn_launch(bn_fwd_kernel<true, false, T>, p, smem, max_ctas, stream);
+    return res != nullptr ? bn_launch(bn_fwd_kernel<false, true, T>, p, smem, max_ctas, stream)
+                          : bn_launch(bn_fwd_kernel<false, false, T>, p, smem, max_ctas, stream);
 }
 
 template <typename T>
 static cudaError_t bn_backward_t(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
                                  const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
                                  float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas,
-                                 cudaStream_t stream) {
+                                 cudaStream_t stream, const void* res, void* dres) {
+    if ((res == nullptr) != (dres == nullptr) || (res != nullptr && (W > 0 || !relu))) return cudaErrorInvalidValue;
     BnBwdArgs<T> p{static_cast<const T*>(x), static_cast<const T*>(dy), arg, static_cast<T*>(dx), partial, gamma, beta,
-                   save_mean, save_invstd, dgamma, dbeta, relu, nullptr, {}};
+                   save_mean, save_invstd, dgamma, dbeta, relu, nullptr, {}, static_cast<const T*>(res),
+                   static_cast<T*>(dres)};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
     const size_t smem = sizeof(float) * 2 * C;
-    return W > 0 ? bn_launch(bn_bwd_kernel<true, T>, p, smem, max_ctas, stream)
-                 : bn_launch(bn_bwd_kernel<false, T>, p, smem, max_ctas, stream);
+    if (W > 0) return bn_launch(bn_bwd_kernel<true, false, T>, p, smem, max_ctas, stream);
+    return res != nullptr ? bn_launch(bn_bwd_kernel<false, true, T>, p, smem, max_ctas, stream)
+                          : bn_launch(bn_bwd_kernel<false, false, T>, p, smem, max_ctas, stream);
 }
 
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
                               float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
-                              cudaStream_t stream) {
+                              cudaStream_t stream, const void* res) {
     switch (dtype) {
         case BnDtype::kF32:
             return bn_forward_t<float>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
-                                       momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+                                       momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
         case BnDtype::kBF16:
             return bn_forward_t<__nv_bfloat16>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar,
-                                               nbt, momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+                                               nbt, momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
         case BnDtype::kF16:
             return bn_forward_t<__half>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
-                                        momentum, eps, relu, M, C, W, slot, max_ctas, stream);
+                                        momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
     }
     return cudaErrorInvalidValue;
 }
@@ -626,17 +713,17 @@ cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float*
 cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
                                const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
                                float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
-                               cudaStream_t stream) {
+                               cudaStream_t stream, const void* res, void* dres) {
     switch (dtype) {
         case BnDtype::kF32:
             return bn_backward_t<float>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
-                                        M, C, W, slot, max_ctas, stream);
+                                        M, C, W, slot, max_ctas, stream, res, dres);
         case BnDtype::kBF16:
             return bn_backward_t<__nv_bfloat16>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta,
-                                                relu, M, C, W, slot, max_ctas, stream);
+                                                relu, M, C, W, slot, max_ctas, stream, res, dres);
         case BnDtype::kF16:
             return bn_backward_t<__half>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
-                                         M, C, W, slot, max_ctas, stream);
+                                         M, C, W, slot, max_ctas, stream, res, dres);
     }
     return cudaErrorInvalidValue;
 }

@@ -345,17 +345,19 @@ struct LandParams {
 cudaError_t launch_land(const LandParams& lp, float* bucket, cudaStream_t stream);
 // fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool when W > 0], channels_last, training mode (csrc/bnrelu.cu):
 // one cooperative kernel per pass.  `slot` names the call site's grid hand-off counters; max_ctas > 0 caps the grid.
-// x, y, dy and dx are of type `dtype`; parameters, statistics, partials and dgamma / dbeta are fp32.
+// x, y, dy and dx are of type `dtype`; parameters, statistics, partials and dgamma / dbeta are fp32.  A non-null `res`
+// (same type and [M, C] layout as x; W == 0 and relu only) makes it  y = relu(bn(x) + res)  and the backward writes the
+// residual's gradient `dres`.
 enum class BnDtype : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 int bn_tile_rows(int M, int C);
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
                               float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
-                              cudaStream_t stream);
+                              cudaStream_t stream, const void* res = nullptr);
 cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
                                const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
                                float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
-                               cudaStream_t stream);
+                               cudaStream_t stream, const void* res = nullptr, void* dres = nullptr);
 cudaError_t launch_maxpool2_fwd(const float* x, float* y, unsigned char* arg, int N, int H, int W, int C, cudaStream_t stream);
 cudaError_t launch_maxpool2_bwd(const float* dy, const unsigned char* arg, float* dx, int N, int H, int W, int C,
                                 cudaStream_t stream);

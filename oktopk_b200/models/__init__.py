@@ -15,8 +15,14 @@ DNNS = ["vgg16", "vgg19", "vgg11", "vgg13", "resnet20", "resnet32", "resnet44", 
         "resnet101", "resnet152", "mnistnet", "lstman4", "lstm", "bert_base", "bert"]
 
 
+# the ResNets whose batch-norms take the fused kernels with ``fuse_bn=True`` (VGG fuses by default; the ImageNet
+# ResNets keep the stock modules, see ROADMAP)
+FUSED_BN_RESNETS = ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110")
+
+
 def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
-    """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set)."""
+    """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
+    ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``)."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
@@ -53,4 +59,7 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
         net = BertForPreTraining(cfg, kwargs.get("depth", 4), recompute=bool(kwargs.get("recompute", False)))
     else:
         raise ValueError("unknown dnn %r (have %s)" % (dnn, DNNS))
+    if d in FUSED_BN_RESNETS:
+        net.fuse = bool(kwargs.get("fuse_bn", False))
+        net.fuse_fp16 = bool(kwargs.get("fuse_fp16", False))
     return net, ext

@@ -31,10 +31,24 @@ class _BasicA(nn.Module):
             x = F.pad(x, (0, 0, 0, 0, self.pad // 2, self.pad - self.pad // 2))
         return F.relu(x + y, inplace=True)
 
+    def forward_fused(self, x, fp16: bool = False):
+        """``forward`` through the fused batch-norm kernels, the residual add and ReLU folded into the second one."""
+        from ..ops.fused_bn import conv_bn_relu
+        y = conv_bn_relu(x, self.c1, self.b1, fp16=fp16)
+        if self.stride != 1 or self.pad:
+            x = x[:, :, ::self.stride, ::self.stride]
+            x = F.pad(x, (0, 0, 0, 0, self.pad // 2, self.pad - self.pad // 2))
+        return conv_bn_relu(y, self.c2, self.b2, fp16=fp16, residual=x)
+
 
 class CifarResNet(nn.Module):
+    """``net.fuse`` (default off; ``create_net(..., fuse_bn=True)``) runs every conv -> BN [+ shortcut] -> ReLU through
+    the fused batch-norm kernels in training on the GPU, ``net.fuse_fp16`` adds fp16 activations to that path (as for
+    VGG).  The option-A shortcut (stride slice + channel zero-pad) stays stock torch ops."""
+
     def __init__(self, depth: int = 20, num_classes: int = 10):
         super().__init__()
+        self.fuse, self.fuse_fp16 = False, False
         assert (depth - 2) % 6 == 0
         n = (depth - 2) // 6
         self.stem = nn.Sequential(nn.Conv2d(3, 16, 3, 1, 1, bias=False), nn.BatchNorm2d(16), nn.ReLU(inplace=True))
@@ -50,6 +64,12 @@ class CifarResNet(nn.Module):
                 nn.init.kaiming_normal_(m.weight)
 
     def forward(self, x):
+        if self.fuse and x.is_cuda and self.training:
+            from ..ops.fused_bn import conv_bn_relu
+            x = conv_bn_relu(x, self.stem[0], self.stem[1], fp16=self.fuse_fp16)
+            for b in self.blocks:
+                x = b.forward_fused(x, self.fuse_fp16)
+            return self.fc(torch.flatten(F.adaptive_avg_pool2d(x, 1), 1))
         x = self.blocks(self.stem(x))
         return self.fc(torch.flatten(F.adaptive_avg_pool2d(x, 1), 1))
 

@@ -1,4 +1,4 @@
-"""Fused (conv-bias +) BatchNorm2d + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations
+"""Fused (conv-bias +) BatchNorm2d [+ residual] + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations
 (``csrc/bnrelu.cu``).
 
 ``bias_bn_relu(x, bn, conv_bias, relu=True, pool=None)`` replaces ``pool(relu(bn(x + conv_bias)))`` in training mode on
@@ -9,6 +9,12 @@ never stored.  The convolution is then called WITHOUT its bias: a bias in front 
 (``BN(x + b) = BN(x)``, the batch mean absorbs it), so it only enters the running-mean update, and its gradient is
 identically zero (returned as ``None``; autograd's own reduction over ``dy`` returns rounding noise for it).
 Parameters, buffers and ``state_dict`` keys are the stock modules' ones.
+
+Residual: ``bias_bn_relu(..., residual=r)`` / ``conv_bn_relu(..., residual=r)`` compute ``relu(bn(x) + r)``, the end of a
+ResNet block, in the same two kernels (``relu=True`` and no pool only; anything else is a ``ValueError``).  The
+statistics are ``x``'s alone; the backward kernel also writes ``dr = dy * [bn(x) + r > 0]``, which is exact.  ``r`` must
+be on ``x``'s device with its shape and dtype (a non-channels_last ``r`` is made contiguous once); otherwise, and
+wherever the fast path does not apply, the stock ``F.relu(bn(x) + r)`` runs.
 
 bf16: under ``torch.autocast("cuda", torch.bfloat16)`` (or with bf16 activations and autocast off) the convolution
 returns bf16 and the kernels' bf16 instantiation runs.  As torch's batch-norm does under autocast, it takes bf16
@@ -94,9 +100,13 @@ def _pool_fusable(x: torch.Tensor, pool: torch.nn.MaxPool2d) -> bool:
             and ext.require().bn_tile_rows(N * H * W, C) % (2 * W) == 0)
 
 
+def _residual_ok(x: torch.Tensor, residual: torch.Tensor) -> bool:
+    return residual.device == x.device and residual.shape == x.shape and residual.dtype == x.dtype
+
+
 class _BiasBNReLUPool(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, gamma, beta, cbias, rmean, rvar, nbt, momentum, eps, relu, pool, slot):
+    def forward(ctx, x, gamma, beta, cbias, rmean, rvar, nbt, momentum, eps, relu, pool, slot, res=None):
         C = ext.require()
         N, Ch, H, W = x.shape
         M = N * H * W
@@ -115,15 +125,15 @@ class _BiasBNReLUPool(torch.autograd.Function):
                      beta.data_ptr(), 0 if cbias is None else cbias.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch,
                      0 if rmean is None else rmean.data_ptr(), 0 if rvar is None else rvar.data_ptr(),
                      0 if nbt is None else nbt.data_ptr(), float(momentum), float(eps), int(relu), M, Ch,
-                     W if pool else 0, slot, MAX_CTAS, s, dtype)
-        ctx.save_for_backward(x, gamma, beta, stats, arg)
+                     W if pool else 0, slot, MAX_CTAS, s, dtype, 0 if res is None else res.data_ptr())
+        ctx.save_for_backward(x, gamma, beta, stats, arg, res)
         ctx.relu, ctx.pool, ctx.slot, ctx.dtype = bool(relu), bool(pool), slot, dtype
         return y
 
     @staticmethod
     def backward(ctx, dy):
         C = ext.require()
-        x, gamma, beta, stats, arg = ctx.saved_tensors
+        x, gamma, beta, stats, arg, res = ctx.saved_tensors
         N, Ch, H, W = x.shape
         M = N * H * W
         assert dy.dtype == x.dtype, (dy.dtype, x.dtype)          # y was allocated in x.dtype
@@ -133,46 +143,64 @@ class _BiasBNReLUPool(torch.autograd.Function):
         rows = C.bn_tile_rows(M, Ch)
         partial = torch.empty((M + rows - 1) // rows * 2 * Ch, dtype=torch.float32, device=x.device)
         dgb = torch.empty(2 * Ch, dtype=torch.float32, device=x.device)         # [dgamma | dbeta]
+        dres = None if res is None else torch.empty_like(x)                       # dy masked by the ReLU
         s = torch.cuda.current_stream().cuda_stream
         C.bn_backward(x.data_ptr(), dy.data_ptr(), 0 if arg is None else arg.data_ptr(), dx.data_ptr(), partial.data_ptr(),
                       gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch, dgb.data_ptr(),
                       dgb.data_ptr() + 4 * Ch, int(ctx.relu), M, Ch, W if ctx.pool else 0, ctx.slot, MAX_CTAS, s,
-                      ctx.dtype)
+                      ctx.dtype, 0 if res is None else res.data_ptr(), 0 if dres is None else dres.data_ptr())
         # conv bias: the loss does not depend on it (see module docstring) -> no gradient
-        return dx, dgb[:Ch], dgb[Ch:], None, None, None, None, None, None, None, None, None
+        return dx, dgb[:Ch], dgb[Ch:], None, None, None, None, None, None, None, None, None, dres
+
+
+def _check_residual(residual: Optional[torch.Tensor], relu: bool, pool: Optional[torch.nn.MaxPool2d]) -> None:
+    if residual is not None and (not relu or pool is not None):
+        raise ValueError("a residual is added before the ReLU: it needs relu=True and pool=None")
 
 
 def bias_bn_relu(x: torch.Tensor, bn: torch.nn.BatchNorm2d, conv_bias: Optional[torch.Tensor] = None,
-                 relu: bool = True, pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False) -> torch.Tensor:
+                 relu: bool = True, pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False,
+                 residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``pool(relu(bn(x + conv_bias)))`` (``relu=False``: without the ReLU; ``pool=None``: without the pool;
-    ``fp16``: fp16 activations and fp16 autocast take the fused kernels too)."""
-    if _fast_path_ok(x, bn, fp16) and (conv_bias is None or conv_bias.dtype == torch.float32):
+    ``fp16``: fp16 activations and fp16 autocast take the fused kernels too).  With a ``residual`` (the end of a
+    ResNet block; ``relu=True`` and ``pool=None`` only): ``relu(bn(x + conv_bias) + residual)``."""
+    _check_residual(residual, relu, pool)
+    if (_fast_path_ok(x, bn, fp16) and (conv_bias is None or conv_bias.dtype == torch.float32)
+            and (residual is None or _residual_ok(x, residual))):
+        if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
+            residual = residual.contiguous(memory_format=torch.channels_last)
         track = bn.track_running_stats and bn.running_mean is not None
         fuse = pool is not None and _pool_fusable(x, pool)
         y = _BiasBNReLUPool.apply(x, bn.weight, bn.bias, conv_bias, bn.running_mean if track else None,
                                   bn.running_var if track else None, bn.num_batches_tracked if track else None,
-                                  bn.momentum, bn.eps, relu, fuse, _sync_slot(bn))
+                                  bn.momentum, bn.eps, relu, fuse, _sync_slot(bn), residual)
         return y if pool is None or fuse else max_pool_2x2(y, pool)
     if conv_bias is not None:
         x = x + conv_bias.view(1, -1, 1, 1)
     y = bn(x)
+    if residual is not None:
+        return F.relu(y + residual)
     y = F.relu(y) if relu else y
     return y if pool is None else max_pool_2x2(y, pool)
 
 
 def conv_bn_relu(x: torch.Tensor, conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, relu: bool = True,
-                 pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False) -> torch.Tensor:
+                 pool: Optional[torch.nn.MaxPool2d] = None, fp16: bool = False,
+                 residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``pool(relu(bn(conv(x))))`` with the convolution's bias folded into the fused batch-norm when the fast path
-    applies (``fp16``: see ``bias_bn_relu``)."""
+    applies (``fp16``: see ``bias_bn_relu``); with a ``residual``, ``relu(bn(conv(x)) + residual)``."""
+    _check_residual(residual, relu, pool)
     if _fast_path_ok_pre(x, conv, bn, fp16):
         z = F.conv2d(x, conv.weight, None, conv.stride, conv.padding, conv.dilation, conv.groups)
         if _fast_path_ok(z, bn, fp16):
-            return bias_bn_relu(z, bn, conv.bias, relu, pool, fp16)
+            return bias_bn_relu(z, bn, conv.bias, relu, pool, fp16, residual)
         if conv.bias is not None:
             z = z + conv.bias.view(1, -1, 1, 1)
         y = bn(z)
     else:
         y = bn(conv(x))
+    if residual is not None:
+        return F.relu(y + residual)
     y = F.relu(y) if relu else y
     return y if pool is None else max_pool_2x2(y, pool)
 

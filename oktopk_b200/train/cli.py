@@ -66,7 +66,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--bf16", action="store_true", help="bf16 autocast")
     p.add_argument("--fused-bn-fp16", action="store_true",
                    help="with --fp16: VGG's Conv -> BN -> ReLU [-> pool] blocks take the fused fp16 batch-norm kernels "
-                        "(default: stock modules under fp16)")
+                        "(default: stock modules under fp16; a ResNet also needs --fused-bn)")
+    p.add_argument("--fused-bn", action="store_true",
+                   help="CIFAR ResNets (resnet20 ... resnet110): every conv -> BN [+ shortcut] -> ReLU takes the fused "
+                        "batch-norm kernels (default: stock modules; VGG always fuses)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -96,7 +99,18 @@ def model_args(args: argparse.Namespace):
         model_kwargs["recompute"] = True
     if args.fused_bn_fp16:
         model_kwargs["fuse_fp16"] = True
+    if args.fused_bn:
+        model_kwargs["fuse_bn"] = True
     return dnn, model_kwargs
+
+
+def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
+    """``--fused-bn`` is for the CIFAR ResNets only; on one of them, ``--fused-bn-fp16`` needs it."""
+    from ..models import FUSED_BN_RESNETS
+    if args.fused_bn and args.dnn not in FUSED_BN_RESNETS:
+        parser.error("--fused-bn applies to %s (VGG fuses by default), not %s" % (", ".join(FUSED_BN_RESNETS), args.dnn))
+    if args.fused_bn_fp16 and args.dnn in FUSED_BN_RESNETS and not args.fused_bn:
+        parser.error("--fused-bn-fp16 on %s needs --fused-bn" % args.dnn)
 
 
 def main(argv=None) -> int:
@@ -104,6 +118,7 @@ def main(argv=None) -> int:
     args = parser.parse_args(argv)
     if args.fused_bn_fp16 and not args.fp16:
         parser.error("--fused-bn-fp16 needs --fp16")
+    check_fused_bn_args(parser, args)
     import oktopk_b200 as okt
     from .trainer import preset_for, robust_ssgd
     okt.init()
