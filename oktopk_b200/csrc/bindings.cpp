@@ -527,6 +527,35 @@ static void bn_backward(uint64_t x, uint64_t dy, uint64_t arg, uint64_t dx, uint
                           P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, bn_dtype(dtype, "bn_backward"),
                           S_(stream), P_<const void>(res), P_<void>(dres)), "bn_backward");
 }
+// y = LayerNorm(x + dropout(a)) over R rows of H: x, y, gamma, beta, mean, rstd (and in the backward dy, dx, dgamma,
+// dbeta) fp32; a and da of type a_dtype (codes as bn_dtype).  seed: one int64 in device memory, read by the kernels;
+// p_keep_thr = floor((1-p) 2^32), or 2^32 for no dropout (seed may then be 0).  partial: ln_bwd_grid(R) * 2H floats.
+static void ln_check(const char* what, int R, int H, long long p_keep_thr, uint64_t seed, uint64_t mean, uint64_t rstd,
+                     std::initializer_list<uint64_t> vec_ptrs) {
+    if (R <= 0 || !ln_supported_h(H)) throw std::runtime_error(std::string(what) + ": needs R > 0 and H in 128, 256, ..., 1024");
+    if (p_keep_thr < 0 || p_keep_thr > (1LL << 32)) throw std::runtime_error(std::string(what) + ": p_keep_thr out of range");
+    if (p_keep_thr < (1LL << 32) && seed == 0) throw std::runtime_error(std::string(what) + ": dropout needs the seed");
+    if (mean == 0 || rstd == 0) throw std::runtime_error(std::string(what) + ": mean and rstd are needed");
+    for (uint64_t p : vec_ptrs)            // accessed as 128-bit (8-byte for a 16-bit a) vectors
+        if (p == 0 || (p & 15)) throw std::runtime_error(std::string(what) + ": tensors must be non-null and 16-byte aligned");
+}
+static void ln_forward(uint64_t x, uint64_t a, uint64_t y, uint64_t gamma, uint64_t beta, uint64_t mean, uint64_t rstd,
+                       uint64_t seed, int R, int H, long long p_keep_thr, double scale, double eps, int a_dtype,
+                       uint64_t stream) {
+    ln_check("ln_forward", R, H, p_keep_thr, seed, mean, rstd, {x, a, y, gamma, beta});
+    ck(launch_ln_forward(P_<const float>(x), P_<const void>(a), P_<float>(y), P_<const float>(gamma), P_<const float>(beta),
+                         P_<float>(mean), P_<float>(rstd), P_<const unsigned long long>(seed), R, H, p_keep_thr, (float)scale,
+                         (float)eps, bn_dtype(a_dtype, "ln_forward"), S_(stream)), "ln_forward");
+}
+static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uint64_t mean, uint64_t rstd, uint64_t seed,
+                        uint64_t dx, uint64_t da, uint64_t partial, uint64_t dgamma, uint64_t dbeta, int R, int H,
+                        long long p_keep_thr, double scale, int a_dtype, uint64_t stream) {
+    ln_check("ln_backward", R, H, p_keep_thr, seed, mean, rstd, {x, a, dy, gamma, dx, da, partial, dgamma, dbeta});
+    ck(launch_ln_backward(P_<const float>(x), P_<const void>(a), P_<const float>(dy), P_<const float>(gamma),
+                          P_<const float>(mean), P_<const float>(rstd), P_<const unsigned long long>(seed), P_<float>(dx),
+                          P_<void>(da), P_<float>(partial), P_<float>(dgamma), P_<float>(dbeta), R, H, p_keep_thr,
+                          (float)scale, bn_dtype(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
+}
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
     if ((C % 4) || (H % 2) || (W % 2)) throw std::runtime_error("maxpool2_fwd: needs C % 4 == 0 and even H, W");
     ck(launch_maxpool2_fwd(P_<const float>(x), P_<float>(y), P_<unsigned char>(arg), N, H, W, C, S_(stream)), "maxpool2_fwd");
@@ -653,6 +682,15 @@ PYBIND11_MODULE(_C, m) {
           py::arg("relu"), py::arg("M"), py::arg("C"), py::arg("W"), py::arg("slot"), py::arg("max_ctas"), py::arg("stream"),
           py::arg("dtype"), py::arg("res") = 0, py::arg("dres") = 0);
     m.def("bn_tile_rows", &bn_tile_rows);
+    m.def("ln_forward", &ln_forward, py::arg("x"), py::arg("a"), py::arg("y"), py::arg("gamma"), py::arg("beta"),
+          py::arg("mean"), py::arg("rstd"), py::arg("seed"), py::arg("R"), py::arg("H"), py::arg("p_keep_thr"),
+          py::arg("scale"), py::arg("eps"), py::arg("a_dtype"), py::arg("stream"));
+    m.def("ln_backward", &ln_backward, py::arg("x"), py::arg("a"), py::arg("dy"), py::arg("gamma"), py::arg("mean"),
+          py::arg("rstd"), py::arg("seed"), py::arg("dx"), py::arg("da"), py::arg("partial"), py::arg("dgamma"),
+          py::arg("dbeta"), py::arg("R"), py::arg("H"), py::arg("p_keep_thr"), py::arg("scale"), py::arg("a_dtype"),
+          py::arg("stream"));
+    m.def("ln_bwd_grid", &ln_bwd_grid);
+    m.def("ln_supported_h", &ln_supported_h);
     m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;

@@ -335,5 +335,20 @@ __device__ __forceinline__ void pull_chunks(const ChunkSrc* srcs, int nsrc, bool
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., SC'11, with Random123's constants and round order): four 32-bit words from a 128-bit
+// counter and a 64-bit key.  Counter 0 and key 0 give 6627e8d5 e169c58d bc57ac4c 9b00dbd8.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        if (r > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    }
+    return c;
+}
+
 
 }  // namespace okt

@@ -361,6 +361,18 @@ cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned cha
 cudaError_t launch_maxpool2_fwd(const float* x, float* y, unsigned char* arg, int N, int H, int W, int C, cudaStream_t stream);
 cudaError_t launch_maxpool2_bwd(const float* dy, const unsigned char* arg, float* dx, int N, int H, int W, int C,
                                 cudaStream_t stream);
+// fused  y = LayerNorm(x + dropout(a))  over rows of H elements (csrc/layernorm.cu): x, y, dx, gamma, beta, dgamma,
+// dbeta, mean and rstd are fp32; a and da are of type `a_dtype` (BnDtype's codes).  keep_thr >= 2^32 turns the dropout
+// off (seed may then be null).  The backward pass writes its [ln_bwd_grid(R), 2H] column partials to `partial`.
+bool ln_supported_h(int H);
+int ln_bwd_grid(int R);
+cudaError_t launch_ln_forward(const float* x, const void* a, float* y, const float* gamma, const float* beta, float* mean,
+                              float* rstd, const unsigned long long* seed, int R, int H, long long keep_thr, float scale,
+                              float eps, BnDtype a_dtype, cudaStream_t stream);
+cudaError_t launch_ln_backward(const float* x, const void* a, const float* dy, const float* gamma, const float* mean,
+                               const float* rstd, const unsigned long long* seed, float* dx, void* da, float* partial,
+                               float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, BnDtype a_dtype,
+                               cudaStream_t stream);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
 cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
 cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);

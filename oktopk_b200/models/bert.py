@@ -7,7 +7,8 @@ self-attention, ``BertLayer``, pooler, ``BertPreTrainingHeads``) and with the st
 parameter, ``depth=4/__init__.py:17``) => BERT-base has 133,547,324 parameters, the paper's 133.5 M.
 
 Fresh implementation: fused QKV projection, ``F.scaled_dot_product_attention`` (the reference does
-matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm`` instead of apex.
+matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm`` instead of apex, or with
+``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``.
 """
 from __future__ import annotations
 
@@ -85,8 +86,12 @@ class BertSelfAttention(nn.Module):
 
 
 class BertLayer(nn.Module):
+    """``fuse_ln`` (default off) runs both ``LayerNorm(x + dropout(a))`` sites through the fused kernels of
+    ``ops/fused_ln.py``; parameters, buffers and ``state_dict`` keys are the same either way."""
+
     def __init__(self, c: BertConfig):
         super().__init__()
+        self.fuse_ln = False
         self.attention = BertSelfAttention(c)
         self.attn_out = nn.Linear(c.hidden_size, c.hidden_size)
         self.attn_norm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
@@ -97,6 +102,11 @@ class BertLayer(nn.Module):
         self.act = _act(c.hidden_act)
 
     def forward(self, x: torch.Tensor, mask: Optional[torch.Tensor]) -> torch.Tensor:
+        if self.fuse_ln:
+            from ..ops.fused_ln import residual_dropout_layer_norm
+            p = self.dropout.p if self.training else 0.0
+            x = residual_dropout_layer_norm(x, self.attn_out(self.attention(x, mask)), self.attn_norm, p)
+            return residual_dropout_layer_norm(x, self.output(self.act(self.intermediate(x))), self.out_norm, p)
         a = self.dropout(self.attn_out(self.attention(x, mask)))
         x = self.attn_norm(x + a)
         f = self.dropout(self.output(self.act(self.intermediate(x))))
@@ -196,7 +206,10 @@ class PretrainingCriterion(nn.Module):
 
 
 class BertForPreTraining(nn.Module):
-    def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False):
+    """``fuse_ln=True`` (or ``net.fuse_ln = True`` at any time) sets ``BertLayer.fuse_ln`` on every encoder layer."""
+
+    def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False,
+                 fuse_ln: bool = False):
         super().__init__()
         self.config = config or BertConfig()
         self.recompute = recompute           # ``--recompute_step`` (BERT/runtime.py:546-557, modeling.py:414-431)
@@ -204,6 +217,18 @@ class BertForPreTraining(nn.Module):
         self.criterion = PretrainingCriterion(self.config.vocab_size)
         self.apply(self._init)
         nn.init.normal_(self.stages[-1].heads.decoder_weight, std=self.config.initializer_range)
+        self.fuse_ln = fuse_ln
+
+    @property
+    def fuse_ln(self) -> bool:
+        """True when every encoder layer runs its two residual LayerNorms through the fused kernels."""
+        return all(m.fuse_ln for m in self.modules() if isinstance(m, BertLayer))
+
+    @fuse_ln.setter
+    def fuse_ln(self, on: bool) -> None:
+        for m in self.modules():
+            if isinstance(m, BertLayer):
+                m.fuse_ln = bool(on)
 
     def _init(self, m: nn.Module) -> None:
         if isinstance(m, (nn.Linear, nn.Embedding)):

@@ -70,6 +70,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-bn", action="store_true",
                    help="CIFAR ResNets (resnet20 ... resnet110): every conv -> BN [+ shortcut] -> ReLU takes the fused "
                         "batch-norm kernels (default: stock modules; VGG always fuses)")
+    p.add_argument("--fused-ln", action="store_true",
+                   help="BERT: both LayerNorm(x + dropout(a)) sites of every encoder layer take the fused dropout + "
+                        "residual + LayerNorm kernels (default: stock ops)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -101,6 +104,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["fuse_fp16"] = True
     if args.fused_bn:
         model_kwargs["fuse_bn"] = True
+    if args.fused_ln:
+        model_kwargs["fuse_ln"] = True
     return dnn, model_kwargs
 
 
@@ -113,12 +118,20 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
         parser.error("--fused-bn-fp16 on %s needs --fused-bn" % args.dnn)
 
 
+def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
+    """``--fused-ln`` is for BERT only (``--dnn bert_base`` / ``bert``, or a ``--module models.bertN.depth=M``)."""
+    dnn = model_args(args)[0]
+    if args.fused_ln and dnn not in ("bert", "bert_base"):
+        parser.error("--fused-ln applies to BERT (bert_base, bert), not %s" % dnn)
+
+
 def main(argv=None) -> int:
     parser = build_parser()
     args = parser.parse_args(argv)
     if args.fused_bn_fp16 and not args.fp16:
         parser.error("--fused-bn-fp16 needs --fp16")
     check_fused_bn_args(parser, args)
+    check_fused_ln_args(parser, args)
     import oktopk_b200 as okt
     from .trainer import preset_for, robust_ssgd
     okt.init()
