@@ -556,6 +556,28 @@ static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uin
                           P_<void>(da), P_<float>(partial), P_<float>(dgamma), P_<float>(dbeta), R, H, p_keep_thr,
                           (float)scale, bn_dtype(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
 }
+// Softmax cross-entropy over R rows of V logits (x, dx of type dtype, codes as bn_dtype), targets t int64, mean over the
+// rows whose target is not ignore_index.  lse: R + 1 floats (the rows' log-sum-exp, then n); rowloss: R floats; loss and
+// g: one float each, in device memory.
+static void xent_check(const char* what, int R, long long V, std::initializer_list<uint64_t> ptrs, uint64_t x, uint64_t t) {
+    if (R <= 0 || V <= 0) throw std::runtime_error(std::string(what) + ": needs R > 0 and V > 0");
+    for (uint64_t p : ptrs)
+        if (p == 0) throw std::runtime_error(std::string(what) + ": null pointer");
+    if ((x & 15) || (t & 7)) throw std::runtime_error(std::string(what) + ": logits must be 16-byte aligned, targets 8-byte");
+}
+static void xent_forward(uint64_t x, uint64_t t, uint64_t lse, uint64_t rowloss, uint64_t loss, int R, long long V,
+                         long long ignore_index, int dtype, uint64_t stream) {
+    xent_check("xent_forward", R, V, {x, t, lse, rowloss, loss}, x, t);
+    ck(launch_xent_forward(P_<const void>(x), P_<const long long>(t), P_<float>(lse), P_<float>(rowloss), P_<float>(loss),
+                           R, V, ignore_index, bn_dtype(dtype, "xent_forward"), S_(stream)), "xent_forward");
+}
+static void xent_backward(uint64_t x, uint64_t t, uint64_t lse, uint64_t g, uint64_t dx, int R, long long V,
+                          long long ignore_index, int dtype, uint64_t stream) {
+    xent_check("xent_backward", R, V, {x, t, lse, g, dx}, x, t);
+    if (dx & 15) throw std::runtime_error("xent_backward: the gradient must be 16-byte aligned");
+    ck(launch_xent_backward(P_<const void>(x), P_<const long long>(t), P_<const float>(lse), P_<const float>(g), P_<void>(dx),
+                            R, V, ignore_index, bn_dtype(dtype, "xent_backward"), S_(stream)), "xent_backward");
+}
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
     if ((C % 4) || (H % 2) || (W % 2)) throw std::runtime_error("maxpool2_fwd: needs C % 4 == 0 and even H, W");
     ck(launch_maxpool2_fwd(P_<const float>(x), P_<float>(y), P_<unsigned char>(arg), N, H, W, C, S_(stream)), "maxpool2_fwd");
@@ -691,6 +713,10 @@ PYBIND11_MODULE(_C, m) {
           py::arg("stream"));
     m.def("ln_bwd_grid", &ln_bwd_grid);
     m.def("ln_supported_h", &ln_supported_h);
+    m.def("xent_forward", &xent_forward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("rowloss"), py::arg("loss"),
+          py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
+    m.def("xent_backward", &xent_backward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("g"), py::arg("dx"),
+          py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
     m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;

@@ -373,6 +373,13 @@ cudaError_t launch_ln_backward(const float* x, const void* a, const float* dy, c
                                const float* rstd, const unsigned long long* seed, float* dx, void* da, float* partial,
                                float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, BnDtype a_dtype,
                                cudaStream_t stream);
+// fused softmax cross-entropy, mean over the rows whose target is not ignore_index (csrc/xent.cu): x and dx [R, V] of
+// type `dtype` (BnDtype's codes), 16-byte aligned; t [R] int64; lse [R + 1] fp32 (per-row log-sum-exp, then n);
+// rowloss [R] fp32 scratch; loss and g one fp32 each.  Two launches forward, one backward.
+cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, float* rowloss, float* loss, int R,
+                                long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
+cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
+                                 long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
 cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
 cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);

@@ -23,7 +23,7 @@ FUSED_BN_RESNETS = ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110")
 def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
     ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``); for BERT,
-    ``fuse_ln=True`` turns on ``net.fuse_ln``."""
+    ``fuse_ln=True`` turns on ``net.fuse_ln`` and ``fuse_xent=True`` ``net.fuse_xent``."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
@@ -58,7 +58,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
             import dataclasses
             cfg = dataclasses.replace(cfg, num_hidden_layers=int(kwargs["num_hidden_layers"]))
         net = BertForPreTraining(cfg, kwargs.get("depth", 4), recompute=bool(kwargs.get("recompute", False)),
-                                 fuse_ln=bool(kwargs.get("fuse_ln", False)))
+                                 fuse_ln=bool(kwargs.get("fuse_ln", False)),
+                                 fuse_xent=bool(kwargs.get("fuse_xent", False)))
     else:
         raise ValueError("unknown dnn %r (have %s)" % (dnn, DNNS))
     if d in FUSED_BN_RESNETS:

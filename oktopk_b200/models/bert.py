@@ -8,7 +8,8 @@ parameter, ``depth=4/__init__.py:17``) => BERT-base has 133,547,324 parameters, 
 
 Fresh implementation: fused QKV projection, ``F.scaled_dot_product_attention`` (the reference does
 matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm`` instead of apex, or with
-``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``.
+``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``, and
+with ``fuse_xent=True`` the masked-LM loss on the fused softmax cross-entropy of ``ops/fused_xent.py``.
 """
 from __future__ import annotations
 
@@ -193,23 +194,31 @@ def build_stages(c: BertConfig, depth: int = 4) -> List[nn.Module]:
 
 
 class PretrainingCriterion(nn.Module):
-    """CE(MLM, ignore_index=-1) + CE(NSP) (``BERT/runtime.py:585-596``)."""
+    """CE(MLM, ignore_index=-1) + CE(NSP) (``BERT/runtime.py:585-596``).  ``fuse_xent`` (default off) runs the MLM term
+    through the fused softmax cross-entropy of ``ops/fused_xent.py``; the NSP term stays stock."""
 
     def __init__(self, vocab_size: int):
         super().__init__()
         self.vocab_size = vocab_size
+        self.fuse_xent = False
 
     def forward(self, prediction_scores, seq_relationship_score, masked_lm_labels, next_sentence_labels):
-        mlm = F.cross_entropy(prediction_scores.view(-1, self.vocab_size), masked_lm_labels.view(-1), ignore_index=-1)
+        scores, labels = prediction_scores.view(-1, self.vocab_size), masked_lm_labels.view(-1)
+        if self.fuse_xent:
+            from ..ops.fused_xent import softmax_cross_entropy
+            mlm = softmax_cross_entropy(scores, labels, ignore_index=-1)
+        else:
+            mlm = F.cross_entropy(scores, labels, ignore_index=-1)
         nsp = F.cross_entropy(seq_relationship_score.view(-1, 2), next_sentence_labels.view(-1))
         return mlm + nsp
 
 
 class BertForPreTraining(nn.Module):
-    """``fuse_ln=True`` (or ``net.fuse_ln = True`` at any time) sets ``BertLayer.fuse_ln`` on every encoder layer."""
+    """``fuse_ln=True`` (or ``net.fuse_ln = True`` at any time) sets ``BertLayer.fuse_ln`` on every encoder layer;
+    ``fuse_xent=True`` (or ``net.fuse_xent``) sets ``PretrainingCriterion.fuse_xent``."""
 
     def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False,
-                 fuse_ln: bool = False):
+                 fuse_ln: bool = False, fuse_xent: bool = False):
         super().__init__()
         self.config = config or BertConfig()
         self.recompute = recompute           # ``--recompute_step`` (BERT/runtime.py:546-557, modeling.py:414-431)
@@ -218,6 +227,16 @@ class BertForPreTraining(nn.Module):
         self.apply(self._init)
         nn.init.normal_(self.stages[-1].heads.decoder_weight, std=self.config.initializer_range)
         self.fuse_ln = fuse_ln
+        self.fuse_xent = fuse_xent
+
+    @property
+    def fuse_xent(self) -> bool:
+        """True when the masked-LM loss runs through the fused softmax cross-entropy."""
+        return self.criterion.fuse_xent
+
+    @fuse_xent.setter
+    def fuse_xent(self, on: bool) -> None:
+        self.criterion.fuse_xent = bool(on)
 
     @property
     def fuse_ln(self) -> bool:

@@ -163,16 +163,24 @@ class BertForQuestionAnswering(_Head):
 
 
 class BertForMaskedLM(_Head):
-    def __init__(self, config: Optional[BertConfig] = None):
+    """``fuse_xent`` (default off, a run-time switch) computes the loss with the fused softmax cross-entropy of
+    ``ops/fused_xent.py``."""
+
+    def __init__(self, config: Optional[BertConfig] = None, fuse_xent: bool = False):
         super().__init__(config)
         self.heads = BertPreTrainingHeads(self.config)
+        self.fuse_xent = fuse_xent
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None, masked_lm_labels=None):
         seq, pooled = self.bert(input_ids, token_type_ids, attention_mask)
         scores, _ = self.heads(seq, pooled)
         if masked_lm_labels is None:
             return scores
-        return F.cross_entropy(scores.view(-1, self.config.vocab_size), masked_lm_labels.view(-1), ignore_index=-1)
+        scores, labels = scores.view(-1, self.config.vocab_size), masked_lm_labels.view(-1)
+        if self.fuse_xent:
+            from ..ops.fused_xent import softmax_cross_entropy
+            return softmax_cross_entropy(scores, labels, ignore_index=-1)
+        return F.cross_entropy(scores, labels, ignore_index=-1)
 
 
 class BertForNextSentencePrediction(_Head):

@@ -73,6 +73,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-ln", action="store_true",
                    help="BERT: both LayerNorm(x + dropout(a)) sites of every encoder layer take the fused dropout + "
                         "residual + LayerNorm kernels (default: stock ops)")
+    p.add_argument("--fused-xent", action="store_true",
+                   help="BERT: the masked-LM loss takes the fused softmax cross-entropy kernels, which read only the "
+                        "labelled rows (default: stock cross_entropy)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -106,6 +109,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["fuse_bn"] = True
     if args.fused_ln:
         model_kwargs["fuse_ln"] = True
+    if args.fused_xent:
+        model_kwargs["fuse_xent"] = True
     return dnn, model_kwargs
 
 
@@ -119,10 +124,12 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln`` is for BERT only (``--dnn bert_base`` / ``bert``, or a ``--module models.bertN.depth=M``)."""
+    """``--fused-ln`` and ``--fused-xent`` are for BERT only (``--dnn bert_base`` / ``bert``, or a
+    ``--module models.bertN.depth=M``)."""
     dnn = model_args(args)[0]
-    if args.fused_ln and dnn not in ("bert", "bert_base"):
-        parser.error("--fused-ln applies to BERT (bert_base, bert), not %s" % dnn)
+    for flag, on in (("--fused-ln", args.fused_ln), ("--fused-xent", args.fused_xent)):
+        if on and dnn not in ("bert", "bert_base"):
+            parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
 
 
 def main(argv=None) -> int:
