@@ -704,6 +704,7 @@ PYBIND11_MODULE(_C, m) {
           py::arg("relu"), py::arg("M"), py::arg("C"), py::arg("W"), py::arg("slot"), py::arg("max_ctas"), py::arg("stream"),
           py::arg("dtype"), py::arg("res") = 0, py::arg("dres") = 0);
     m.def("bn_tile_rows", &bn_tile_rows);
+    m.def("bn_sliced", &bn_sliced, py::arg("M"), py::arg("C"), py::arg("W"));
     m.def("ln_forward", &ln_forward, py::arg("x"), py::arg("a"), py::arg("y"), py::arg("gamma"), py::arg("beta"),
           py::arg("mean"), py::arg("rstd"), py::arg("seed"), py::arg("R"), py::arg("H"), py::arg("p_keep_thr"),
           py::arg("scale"), py::arg("eps"), py::arg("a_dtype"), py::arg("stream"));

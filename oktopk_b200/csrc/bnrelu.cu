@@ -1,5 +1,6 @@
 // Fused (conv-bias +) BatchNorm [+ residual] + ReLU [+ 2x2 max-pool] for channels_last fp32, bf16 or fp16 activations, training mode,
-// forward and backward: one cooperative kernel per pass.
+// forward and backward: one kernel per pass -- cooperative with a grid-wide hand-off, or, on small layers, channel-sliced
+// with none.
 //
 // The CNN zoo of the reference (VGG/models/vgg.py:28-36 and the ResNets) is stacks of  Conv2d -> BatchNorm2d -> ReLU
 // [-> MaxPool2d].  Run through stock framework ops, a VGG-16 step at 16 images per GPU spends a quarter of its time in the
@@ -23,6 +24,24 @@
 // for the combine.  A CTA's tiles after its first (only when tiles outnumber co-resident CTAs), and tiles larger than
 // kBnHold float4 per thread, are read again from global memory in (3).  The tile partition, the per-thread summation
 // order and the combine order do not depend on the grid, so neither do the results.
+//
+// Summation tree.  Every per-channel sum (x, x^2; dbeta, dgamma) is added in one fixed fp32 tree that depends on (M, C)
+// alone, with bn_geom's tiles of rows_per_block rows and rpi row lanes:
+//   1. per tile t and lane ty: the rows  t rows_per_block + ty + k rpi,  k ascending, one after the other (x^2 and dgamma
+//      by fmaf into the running sum);
+//   2. per tile: lanes ty = 0 .. rpi-1 in ascending order (bn_tile_partial);
+//   3. across tiles (bn_combine_partials): the partial row is [sum | second sum], C/2 float4 columns, taken in chunks of
+//      256 columns; in the chunk at c0,  w = min(256, C/2 - c0)  and  groups = 256 / w;  group j adds tiles j, j + groups,
+//      ... in order, starting from 0.f, and the groups are then added in ascending order.
+// Mean and 1/std come from the totals in double (bn_stats).
+//
+// Channel-sliced kernels (bn_fwd_sliced_kernel, bn_bwd_sliced_kernel; chosen by bn_geom's sc, see there).  Statistics are
+// per channel, so a CTA that owns sc float4 columns and ALL rows needs nobody else: thread (column of the slice, tile,
+// lane) does step 1 privately on rows it holds in registers, bn_slice_reduce does steps 2 and 3 in shared memory, and
+// the CTA computes the statistics of its channels and writes y / dx from the held rows.  No partials, no g_bn_sync, no
+// wait on another CTA, a plain launch.  Same tree and the same per-element device functions as the cooperative kernels,
+// hence the same bits.  A grid cap (max_ctas > 0) always selects the cooperative kernels.  Layers with fewer than
+// 2 kBnMinSlices float4 columns or more rows than a CTA's threads can hold stay cooperative.
 //
 // A bias added before a batch-norm cancels exactly: BN(x + b) = BN(x) with the batch mean shifted by b.  The forward pass
 // therefore never adds it (only running_mean sees it), and its gradient -- identically zero, since the loss does not depend
@@ -68,6 +87,7 @@ constexpr int kBnThreads = 256;
 constexpr int kBnMaxBlocks = 512;
 constexpr int kBnHold = 8;             // float4 per thread and tensor held on chip: a whole ~8 K-element tile (bn_geom)
 constexpr int kBnSyncSlots = 1024;
+constexpr int kBnMinSlices = 32;       // channel-sliced kernels: at least this many CTAs, or the cooperative kernels run
 
 // {arrival ticket, release generation} per call site (the caller picks the slot).  Zero at module load; every kernel
 // leaves its ticket at zero and only advances the generation, so a CUDA graph replays the kernels without a reset node.
@@ -79,6 +99,7 @@ struct BnGeom {
     int rows_per_block, nblk;
     int hold;              // a tile fits in kBnHold float4 per thread (one column tile)
     int W;                 // > 0: a 2x2 / stride-2 max-pool over images of width W follows
+    int sc;                // > 0: the channel-sliced kernels can run, with sc float4 columns per CTA (2 .. 8)
 };
 
 __host__ __device__ inline BnGeom bn_geom(int M, int C) {
@@ -98,6 +119,15 @@ __host__ __device__ inline BnGeom bn_geom(int M, int C) {
     g.nblk = (M + rpb - 1) / rpb;
     g.hold = g.cv <= kBnThreads && rpb / g.rpi <= kBnHold;
     g.W = 0;
+    // Channel-sliced: one thread per (column of the slice, tile, row lane), so a CTA of sc columns has sc * nblk * rpi
+    // threads.  The widest power-of-two slice that fits a CTA and still leaves kBnMinSlices CTAs; a one-column slice
+    // (16 bytes per row, half a sector) does not qualify.
+    g.sc = 0;
+    if (g.hold) {
+        int sc = 1;
+        while (2 * sc * g.nblk * g.rpi <= kBnThreads && g.cv / (2 * sc) >= kBnMinSlices) sc *= 2;
+        if (sc >= 2 && g.cv % sc == 0) g.sc = sc;
+    }
     return g;
 }
 
@@ -142,6 +172,36 @@ __device__ __forceinline__ void pool_step(float4& m, uchar4& a, const float4& v,
     if (v.y > m.y || v.y != v.y) { m.y = v.y; a.y = k; }
     if (v.z > m.z || v.z != v.z) { m.z = v.z; a.z = k; }
     if (v.w > m.w || v.w != v.w) { m.w = v.w; a.w = k; }
+}
+
+// The 2x2 window of a pooled pixel whose first row is lr: at(lr, c), at(lr + 1, c), at(lr + W, c), at(lr + W + 1, c).
+template <typename At>
+__device__ __forceinline__ void pool_window(At at, int lr, int W, int c, float4& m, uchar4& a) {
+    const float4 v1 = at(lr + 1, c), v2 = at(lr + W, c), v3 = at(lr + W + 1, c);
+    m = at(lr, c);
+    a = make_uchar4(0, 0, 0, 0);
+    pool_step(m, a, v1, 1);
+    pool_step(m, a, v2, 2);
+    pool_step(m, a, v3, 3);
+}
+
+// One row's term of a thread's private sums of x and x^2.
+__device__ __forceinline__ void bn_sum_sq(float4& s, float4& q, const float4& v) {
+    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+    q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
+}
+
+// y = a x + b [ReLU], and with a residual y = max(0, (a x + b) + r)
+__device__ __forceinline__ float4 bn_y(const float4& x, const float4& a, const float4& b, int relu) {
+    float4 v = f4_fma(x, a, b);
+    if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+    return v;
+}
+__device__ __forceinline__ float4 bn_y_res(const float4& x, const float4& r, const float4& a, const float4& b) {
+    float4 v = f4_fma(x, a, b);
+    v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+    v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+    return v;
 }
 
 // Combine the per-tile partials [nblk][2C] into s_tot[2C] with ALL threads of the block: a tile of up to 256 float4
@@ -197,6 +257,42 @@ __device__ __forceinline__ void bn_tile_partial(float4 s, float4 q, int tx, int 
     __syncthreads();
 }
 
+// Channel-sliced CTA: thread (tile t, lane ty, column cx of the slice) = threadIdx.x = (t * rpi + ty) * sc + cx holds its
+// private sums (s, q).  Adds them in the order of the summation tree (file header), which is what bn_tile_partial and
+// bn_combine_partials do across CTAs, and leaves the totals in s_tot: [sc] of s, then [sc] of q.
+// s_scr: 2 * blockDim + 2 * nblk * sc float4 of scratch, free again on return.
+__device__ __forceinline__ void bn_slice_reduce(const float4& s, const float4& q, const BnGeom& g, float4* s_scr,
+                                                float4* s_tot) {
+    const int sc = g.sc, lanes = g.nblk * g.rpi;
+    float4* s_lane = s_scr;
+    float4* s_tile = s_scr + 2 * blockDim.x;
+    auto add = [](float4& a, const float4& b) { a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w; };
+    s_lane[threadIdx.x] = s;
+    s_lane[lanes * sc + threadIdx.x] = q;
+    __syncthreads();
+    for (int i = threadIdx.x; i < 2 * g.nblk * sc; i += blockDim.x) {           // a tile's lanes, ascending
+        const int which = i / (g.nblk * sc), t = i / sc % g.nblk, cx = i % sc;
+        const float4* src = s_lane + (which * lanes + t * g.rpi) * sc + cx;
+        float4 v = src[0];
+        for (int j = 1; j < g.rpi; ++j) add(v, src[j * sc]);
+        s_tile[i] = v;                                                          // [which][t][cx]
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 2 * sc; i += blockDim.x) {                    // tiles j, j + groups, ...; then the groups
+        const int which = i / sc, cx = i % sc;
+        const int pcol = which * g.cv + blockIdx.x * sc + cx;                   // float4 column of a partial row [2C]
+        const int groups = kBnThreads / min(kBnThreads, 2 * g.cv - pcol / kBnThreads * kBnThreads);
+        float4 tot;
+        for (int j = 0; j < groups; ++j) {
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int b = j; b < g.nblk; b += groups) add(acc, s_tile[(which * g.nblk + b) * sc + cx]);
+            if (j == 0) tot = acc; else add(tot, acc);
+        }
+        s_tot[i] = tot;
+    }
+    __syncthreads();
+}
+
 // Grid-wide hand-off.  bn_arrive: once every CTA has written its partials, exactly one CTA (the last to arrive) gets
 // true and does the combine.  bn_release: that CTA publishes its results; every other CTA waits there for them.  The
 // generation is read before arriving, and the last CTA can only advance it after every arrival.
@@ -246,6 +342,33 @@ struct BnFwdArgs {
     const T* res;               // kRes only: the residual [M, C], added after the batch-norm, before the ReLU
 };
 
+// Channel c from its sums s of x and q of x^2 over the M rows: mean and 1/std in double, saved; running statistics with
+// the unbiased variance and the conv-bias-shifted mean.
+template <typename T>
+__device__ __forceinline__ void bn_stats(const BnFwdArgs<T>& p, int c, float sf, float qf) {
+    const BnGeom& g = p.g;
+    const double s = (double)sf, q = (double)qf;
+    const double mean = s / (double)g.M;
+    double var = q / (double)g.M - mean * mean;
+    if (var < 0.0) var = 0.0;
+    const float invstd = (float)(1.0 / sqrt(var + (double)p.eps));
+    p.save_mean[c] = (float)mean;
+    p.save_invstd[c] = invstd;
+    if (p.rmean != nullptr) {
+        const float mb = (float)mean + (p.cbias != nullptr ? __ldg(p.cbias + c) : 0.f);
+        const double unb = g.M > 1 ? var * (double)g.M / (double)(g.M - 1) : var;
+        p.rmean[c] = fmaf(p.momentum, mb, __fmul_rn(1.f - p.momentum, p.rmean[c]));
+        p.rvar[c] = fmaf(p.momentum, (float)unb, __fmul_rn(1.f - p.momentum, p.rvar[c]));
+    }
+}
+
+// a = gamma / std, b = beta - mean a of channel c
+template <typename T>
+__device__ __forceinline__ void bn_scale_shift(const BnFwdArgs<T>& p, int c, float mean, float invstd, float& a, float& b) {
+    a = __fmul_rn(__ldg(p.gamma + c), invstd);
+    b = __fsub_rn(__ldg(p.beta + c), __fmul_rn(mean, a));      // no fma: backward recomputes it
+}
+
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
@@ -268,10 +391,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
             const int col = c0 + tx;
             float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
             if (ty < g.rpi && col < g.cv) {
-                auto acc = [&](const float4& v) {
-                    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-                    q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
-                };
+                auto acc = [&](const float4& v) { bn_sum_sq(s, q, v); };
                 int r = row0 + ty;
                 if (held) {
 #pragma unroll
@@ -300,45 +420,21 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
     if (last) {
         float* s_tot = s_ab;                  // overwritten by a, b only after bn_release's barrier
         bn_combine_partials(p.partial, g.nblk, g.C, s_tot, s_red);
-        for (int c = threadIdx.x; c < g.C; c += kBnThreads) {
-            const double s = (double)s_tot[c], q = (double)s_tot[g.C + c];
-            const double mean = s / (double)g.M;
-            double var = q / (double)g.M - mean * mean;
-            if (var < 0.0) var = 0.0;
-            const float invstd = (float)(1.0 / sqrt(var + (double)p.eps));
-            p.save_mean[c] = (float)mean;
-            p.save_invstd[c] = invstd;
-            if (p.rmean != nullptr) {
-                const float mb = (float)mean + (p.cbias != nullptr ? __ldg(p.cbias + c) : 0.f);
-                const double unb = g.M > 1 ? var * (double)g.M / (double)(g.M - 1) : var;
-                p.rmean[c] = fmaf(p.momentum, mb, __fmul_rn(1.f - p.momentum, p.rmean[c]));
-                p.rvar[c] = fmaf(p.momentum, (float)unb, __fmul_rn(1.f - p.momentum, p.rvar[c]));
-            }
-        }
+        for (int c = threadIdx.x; c < g.C; c += kBnThreads) bn_stats(p, c, s_tot[c], s_tot[g.C + c]);
         if (threadIdx.x == 0 && p.nbt != nullptr) *p.nbt += 1;
     }
     bn_release(p.sync, last, gen);
-    for (int c = threadIdx.x; c < g.C; c += kBnThreads) {
-        const float a = __fmul_rn(__ldg(p.gamma + c), __ldcg(p.save_invstd + c));
-        s_ab[c] = a;
-        s_ab[g.C + c] = __fsub_rn(__ldg(p.beta + c), __fmul_rn(__ldcg(p.save_mean + c), a));   // no fma: backward recomputes it
-    }
+    for (int c = threadIdx.x; c < g.C; c += kBnThreads)
+        bn_scale_shift(p, c, __ldcg(p.save_mean + c), __ldcg(p.save_invstd + c), s_ab[c], s_ab[g.C + c]);
     __syncthreads();
 
     // (3) y = max(0, a x + b), or its 2x2 max-pool, or with a residual r  y = max(0, (a x + b) + r)
     const float4* ab4 = s_dyn;                // [cv] a | [cv] b
-    auto yval = [&](const float4& xin, int col) {
-        float4 v = f4_fma(xin, ab4[col], ab4[g.cv + col]);
-        if (p.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-        return v;
-    };
+    auto yval = [&](const float4& xin, int col) { return bn_y(xin, ab4[col], ab4[g.cv + col], p.relu); };
     const V* r4 = reinterpret_cast<const V*>(p.res);
     auto ldr = [&](size_t o) { return A::wide(__ldg(r4 + o)); };
     auto yres = [&](const float4& xin, const float4& rin, int col) {
-        float4 v = f4_fma(xin, ab4[col], ab4[g.cv + col]);
-        v.x += rin.x; v.y += rin.y; v.z += rin.z; v.w += rin.w;
-        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-        return v;
+        return bn_y_res(xin, rin, ab4[col], ab4[g.cv + col]);
     };
     V* y4 = reinterpret_cast<V*>(p.y);
     for (int t = blockIdx.x; t < g.nblk; t += gridDim.x) {
@@ -402,16 +498,89 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
             for (int i = threadIdx.x; i < npool; i += kBnThreads) {
                 const int c = i % g.cv, pp = i / g.cv;
                 const int lr = (pp / Wo) * 2 * W + (pp % Wo) * 2;
-                const float4 v1 = at(lr + 1, c), v2 = at(lr + W, c), v3 = at(lr + W + 1, c);
-                float4 m = at(lr, c);
-                uchar4 a = make_uchar4(0, 0, 0, 0);
-                pool_step(m, a, v1, 1);
-                pool_step(m, a, v2, 2);
-                pool_step(m, a, v3, 3);
+                float4 m;
+                uchar4 a;
+                pool_window(at, lr, W, c, m, a);
                 const size_t o = (size_t)(row0 / 4 + pp) * g.cv + c;
                 y4[o] = A::narrow(m);
                 a4[o] = a;
             }
+        }
+    }
+}
+
+// Channel-sliced forward (g.sc > 0): CTA b owns float4 columns [b sc, (b + 1) sc) and every row; blockDim = sc nblk rpi.
+// No partials, no hand-off: the statistics of the owned channels never leave the CTA.
+template <bool kPool, bool kRes, typename T>
+__global__ void __launch_bounds__(kBnThreads) bn_fwd_sliced_kernel(const BnFwdArgs<T> p) {
+    static_assert(!(kPool && kRes), "no pool follows a residual add");
+    using A = BnAct<T>;
+    using V = typename A::V;
+    extern __shared__ float4 s_dyn[];         // bn_slice_reduce's scratch, then with a pool the slice's y, [M][sc]
+    __shared__ float4 s_tot[2 * 8], s_ab[2 * 8];   // the owned columns' totals [sc] | [sc]; a = gamma/std [sc] | b [sc]
+    const BnGeom& g = p.g;
+    const int sc = g.sc, cx = threadIdx.x % sc, ln = threadIdx.x / sc, col = blockIdx.x * sc + cx;
+    const int row0 = ln / g.rpi * g.rows_per_block, row1 = min(g.M, row0 + g.rows_per_block), r = row0 + ln % g.rpi;
+    const V* x4 = reinterpret_cast<const V*>(p.x);
+
+    // (1) the thread's rows, held; their sums in row order
+    V h[kBnHold];
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
+#pragma unroll
+    for (int k = 0; k < kBnHold; ++k) h[k] = r + k * g.rpi < row1 ? __ldg(x4 + (size_t)(r + k * g.rpi) * g.cv + col) : V{};
+#pragma unroll
+    for (int k = 0; k < kBnHold; ++k)
+        if (r + k * g.rpi < row1) bn_sum_sq(s, q, A::wide(h[k]));
+
+    // (2) totals of the owned channels, their statistics, a and b
+    bn_slice_reduce(s, q, g, s_dyn, s_tot);
+    const float* s_f = reinterpret_cast<const float*>(s_tot);
+    float* s_abf = reinterpret_cast<float*>(s_ab);
+    for (int i = threadIdx.x; i < 4 * sc; i += blockDim.x) {        // a CTA can have fewer threads than channels
+        const int c = blockIdx.x * 4 * sc + i;
+        bn_stats(p, c, s_f[i], s_f[4 * sc + i]);
+        bn_scale_shift(p, c, p.save_mean[c], p.save_invstd[c], s_abf[i], s_abf[4 * sc + i]);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0 && p.nbt != nullptr) *p.nbt += 1;
+    __syncthreads();
+
+    // (3) y from the held rows
+    const float4 a4 = s_ab[cx], b4 = s_ab[sc + cx];
+    V* y4 = reinterpret_cast<V*>(p.y);
+    if constexpr (kRes) {
+        const V* r4 = reinterpret_cast<const V*>(p.res);
+#pragma unroll
+        for (int k0 = 0; k0 < kBnHold; k0 += 4) {               // four residual loads in flight beside the held rows
+            float4 rr[4];
+#pragma unroll
+            for (int k = k0; k < k0 + 4; ++k)
+                if (r + k * g.rpi < row1) rr[k - k0] = A::wide(__ldg(r4 + (size_t)(r + k * g.rpi) * g.cv + col));
+#pragma unroll
+            for (int k = k0; k < k0 + 4; ++k)
+                if (r + k * g.rpi < row1)
+                    y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(bn_y_res(A::wide(h[k]), rr[k - k0], a4, b4));
+        }
+    } else if constexpr (!kPool) {
+#pragma unroll
+        for (int k = 0; k < kBnHold; ++k)
+            if (r + k * g.rpi < row1) y4[(size_t)(r + k * g.rpi) * g.cv + col] = A::narrow(bn_y(A::wide(h[k]), a4, b4, p.relu));
+    } else {
+        // every 2x2 window of the owned columns lies in this CTA; rows and pooled pixels are global (the first row is 0)
+#pragma unroll
+        for (int k = 0; k < kBnHold; ++k)
+            if (r + k * g.rpi < row1) s_dyn[(r + k * g.rpi) * sc + cx] = bn_y(A::wide(h[k]), a4, b4, p.relu);
+        __syncthreads();
+        auto at = [&](int lr, int c) { return s_dyn[lr * sc + c]; };
+        const int W = g.W, Wo = W >> 1;
+        uchar4* arg4 = reinterpret_cast<uchar4*>(p.arg);
+        for (int i = threadIdx.x; i < g.M / 4 * sc; i += blockDim.x) {
+            const int c = i % sc, pp = i / sc;
+            float4 m;
+            uchar4 am;
+            pool_window(at, (pp / Wo) * 2 * W + (pp % Wo) * 2, W, c, m, am);
+            const size_t o = (size_t)pp * g.cv + blockIdx.x * sc + c;
+            y4[o] = A::narrow(m);
+            arg4[o] = am;
         }
     }
 }
@@ -433,6 +602,84 @@ struct BnBwdArgs {
     T* dres;                    // kRes only: its gradient dy * [z > 0], [M, C]
 };
 
+// Per-element arithmetic of the backward pass, shared by the cooperative and the channel-sliced kernels.
+// Per-column constants; the forward output was max(0, fma(x, a, b)): same a, b, same fma => the same mask, bit for bit.
+struct BnCol { float4 mean, istd, a, b; };
+
+template <bool kPool, bool kRes, typename T>
+struct BnBwdElem {
+    using A = BnAct<T>;
+    using V = typename A::V;
+    const BnBwdArgs<T>& p;
+
+    // the gradient reaching the batch-norm output at row r: dy, or the pooled dy at the window's arg-max and 0 elsewhere
+    // (row0: the first row of r's tile, a multiple of 2W; 0 takes r as a global row)
+    __device__ __forceinline__ float4 grad(int row0, int r, int col) const {
+        const BnGeom& g = p.g;
+        const V* d4 = reinterpret_cast<const V*>(p.dy);
+        if (!kPool) return A::wide(__ldg(d4 + (size_t)r * g.cv + col));
+        const int lr = r - row0, hl = lr / g.W, w = lr - hl * g.W;
+        const size_t o = (size_t)(row0 / 4 + (hl >> 1) * (g.W >> 1) + (w >> 1)) * g.cv + col;
+        const int k = (hl & 1) * 2 + (w & 1);
+        const float4 d = A::wide(__ldg(d4 + o));
+        const uchar4 a = __ldg(reinterpret_cast<const uchar4*>(p.arg) + o);
+        return make_float4(a.x == k ? d.x : 0.f, a.y == k ? d.y : 0.f, a.z == k ? d.z : 0.f, a.w == k ? d.w : 0.f);
+    }
+    __device__ __forceinline__ BnCol column(int col) const {
+        BnCol k;
+        k.mean = __ldg(reinterpret_cast<const float4*>(p.save_mean) + col);
+        k.istd = __ldg(reinterpret_cast<const float4*>(p.save_invstd) + col);
+        const float4 gm = __ldg(reinterpret_cast<const float4*>(p.gamma) + col);
+        const float4 bt = __ldg(reinterpret_cast<const float4*>(p.beta) + col);
+        k.a = make_float4(__fmul_rn(gm.x, k.istd.x), __fmul_rn(gm.y, k.istd.y), __fmul_rn(gm.z, k.istd.z), __fmul_rn(gm.w, k.istd.w));
+        k.b = make_float4(__fsub_rn(bt.x, __fmul_rn(k.mean.x, k.a.x)), __fsub_rn(bt.y, __fmul_rn(k.mean.y, k.a.y)),
+                          __fsub_rn(bt.z, __fmul_rn(k.mean.z, k.a.z)), __fsub_rn(bt.w, __fmul_rn(k.mean.w, k.a.w)));
+        return k;
+    }
+    __device__ __forceinline__ void mask(const BnCol& k, const float4& v, float4& d) const {
+        if (p.relu) {
+            if (!(fmaf(v.x, k.a.x, k.b.x) > 0.f)) d.x = 0.f;
+            if (!(fmaf(v.y, k.a.y, k.b.y) > 0.f)) d.y = 0.f;
+            if (!(fmaf(v.z, k.a.z, k.b.z) > 0.f)) d.z = 0.f;
+            if (!(fmaf(v.w, k.a.w, k.b.w) > 0.f)) d.w = 0.f;
+        }
+    }
+    static __device__ __forceinline__ float4 xhat(const BnCol& k, const float4& v) {
+        return make_float4((v.x - k.mean.x) * k.istd.x, (v.y - k.mean.y) * k.istd.y, (v.z - k.mean.z) * k.istd.z,
+                           (v.w - k.mean.w) * k.istd.w);
+    }
+    // with a residual the forward output was max(0, fma(x, a, b) + r): the same mask, bit for bit, and the gradient of
+    // both the batch-norm output and the residual is dy masked by it, which is written out as dres (exact)
+    __device__ __forceinline__ void gate(const BnCol& k, const float4& v, const float4& q, size_t o, float4& d) const {
+        if (!(fmaf(v.x, k.a.x, k.b.x) + q.x > 0.f)) d.x = 0.f;
+        if (!(fmaf(v.y, k.a.y, k.b.y) + q.y > 0.f)) d.y = 0.f;
+        if (!(fmaf(v.z, k.a.z, k.b.z) + q.z > 0.f)) d.z = 0.f;
+        if (!(fmaf(v.w, k.a.w, k.b.w) + q.w > 0.f)) d.w = 0.f;
+        reinterpret_cast<V*>(p.dres)[o] = A::narrow(d);
+    }
+    // one row's term of a thread's private sums of dbeta and dgamma (d with a residual: already gated)
+    __device__ __forceinline__ void acc(const BnCol& k, const float4& v, float4 d, float4& sb, float4& sg) const {
+        const float4 xh = xhat(k, v);
+        if constexpr (!kRes) mask(k, v, d);
+        sb.x += d.x; sb.y += d.y; sb.z += d.z; sb.w += d.w;
+        sg.x = fmaf(d.x, xh.x, sg.x); sg.y = fmaf(d.y, xh.y, sg.y); sg.z = fmaf(d.z, xh.z, sg.z); sg.w = fmaf(d.w, xh.w, sg.w);
+    }
+    __device__ __forceinline__ float4 over_m(const float4& t) const {
+        const double M = (double)p.g.M;
+        return make_float4((float)(t.x / M), (float)(t.y / M), (float)(t.z / M), (float)(t.w / M));
+    }
+    // dx at offset off from x = v and the gradient d, with mb = dbeta / M and mg = dgamma / M
+    __device__ __forceinline__ void dx(const BnCol& k, const float4& mb, const float4& mg, size_t off, const float4& v,
+                                       float4 d) const {
+        const float4 xh = xhat(k, v);
+        if constexpr (!kRes) mask(k, v, d);
+        reinterpret_cast<V*>(p.dx)[off] =
+            A::narrow(make_float4(k.a.x * (d.x - mb.x - xh.x * mg.x), k.a.y * (d.y - mb.y - xh.y * mg.y),
+                                  k.a.z * (d.z - mb.z - xh.z * mg.z), k.a.w * (d.w - mb.w - xh.w * mg.w)));
+    }
+};
+
+
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
@@ -442,58 +689,13 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
     __shared__ float4 s_red[2 * kBnThreads];
     const BnGeom& g = p.g;
     const int tx = threadIdx.x % g.tpr, ty = threadIdx.x / g.tpr;
+    const BnBwdElem<kPool, kRes, T> el{p};
     const V* x4 = reinterpret_cast<const V*>(p.x);
-    const V* d4 = reinterpret_cast<const V*>(p.dy);
-    const uchar4* a4 = reinterpret_cast<const uchar4*>(p.arg);
-    auto ldx = [&](size_t o) { return A::wide(__ldg(x4 + o)); };
-    const size_t st1 = (size_t)g.rpi * g.cv;
-    // the gradient reaching the batch-norm output at row r: dy, or the pooled dy at the window's arg-max and 0 elsewhere
-    auto grad = [&](int row0, int r, int col) -> float4 {
-        if (!kPool) return A::wide(__ldg(d4 + (size_t)r * g.cv + col));
-        const int lr = r - row0, hl = lr / g.W, w = lr - hl * g.W;
-        const size_t o = (size_t)(row0 / 4 + (hl >> 1) * (g.W >> 1) + (w >> 1)) * g.cv + col;
-        const int k = (hl & 1) * 2 + (w & 1);
-        const float4 d = A::wide(__ldg(d4 + o));
-        const uchar4 a = __ldg(a4 + o);
-        return make_float4(a.x == k ? d.x : 0.f, a.y == k ? d.y : 0.f, a.z == k ? d.z : 0.f, a.w == k ? d.w : 0.f);
-    };
-    // per-column constants; the forward output was max(0, fma(x, a, b)): same a, b, same fma => the same mask, bit for bit
-    struct Col { float4 mean, istd, a, b; };
-    auto column = [&](int col) {
-        Col k;
-        k.mean = __ldg(reinterpret_cast<const float4*>(p.save_mean) + col);
-        k.istd = __ldg(reinterpret_cast<const float4*>(p.save_invstd) + col);
-        const float4 gm = __ldg(reinterpret_cast<const float4*>(p.gamma) + col);
-        const float4 bt = __ldg(reinterpret_cast<const float4*>(p.beta) + col);
-        k.a = make_float4(__fmul_rn(gm.x, k.istd.x), __fmul_rn(gm.y, k.istd.y), __fmul_rn(gm.z, k.istd.z), __fmul_rn(gm.w, k.istd.w));
-        k.b = make_float4(__fsub_rn(bt.x, __fmul_rn(k.mean.x, k.a.x)), __fsub_rn(bt.y, __fmul_rn(k.mean.y, k.a.y)),
-                          __fsub_rn(bt.z, __fmul_rn(k.mean.z, k.a.z)), __fsub_rn(bt.w, __fmul_rn(k.mean.w, k.a.w)));
-        return k;
-    };
-    auto mask = [&](const Col& k, const float4& v, float4& d) {
-        if (p.relu) {
-            if (!(fmaf(v.x, k.a.x, k.b.x) > 0.f)) d.x = 0.f;
-            if (!(fmaf(v.y, k.a.y, k.b.y) > 0.f)) d.y = 0.f;
-            if (!(fmaf(v.z, k.a.z, k.b.z) > 0.f)) d.z = 0.f;
-            if (!(fmaf(v.w, k.a.w, k.b.w) > 0.f)) d.w = 0.f;
-        }
-    };
-    auto xhat = [&](const Col& k, const float4& v) {
-        return make_float4((v.x - k.mean.x) * k.istd.x, (v.y - k.mean.y) * k.istd.y, (v.z - k.mean.z) * k.istd.z,
-                           (v.w - k.mean.w) * k.istd.w);
-    };
-    // with a residual the forward output was max(0, fma(x, a, b) + r): the same mask, bit for bit, and the gradient of
-    // both the batch-norm output and the residual is dy masked by it, which is written out as dres (exact)
     const V* r4 = reinterpret_cast<const V*>(p.res);
     V* dr4 = reinterpret_cast<V*>(p.dres);
+    auto ldx = [&](size_t o) { return A::wide(__ldg(x4 + o)); };
     auto ldr = [&](size_t o) { return A::wide(__ldg(r4 + o)); };
-    auto gate = [&](const Col& k, const float4& v, const float4& q, size_t o, float4& d) {
-        if (!(fmaf(v.x, k.a.x, k.b.x) + q.x > 0.f)) d.x = 0.f;
-        if (!(fmaf(v.y, k.a.y, k.b.y) + q.y > 0.f)) d.y = 0.f;
-        if (!(fmaf(v.z, k.a.z, k.b.z) + q.z > 0.f)) d.z = 0.f;
-        if (!(fmaf(v.w, k.a.w, k.b.w) + q.w > 0.f)) d.w = 0.f;
-        dr4[o] = A::narrow(d);
-    };
+    const size_t st1 = (size_t)g.rpi * g.cv;
     V hx[kBnHold];                            // the CTA's first tile: x as stored
     float4 hd[kBnHold];                       // and the incoming gradient (with a pool: expanded at the arg-max; with a
                                               // residual: already masked)
@@ -506,27 +708,22 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
             const int col = c0 + tx;
             float4 sb = make_float4(0.f, 0.f, 0.f, 0.f), sg = sb;
             if (ty < g.rpi && col < g.cv) {
-                const Col k = column(col);
-                auto acc = [&](const float4& v, float4 d) {
-                    const float4 xh = xhat(k, v);
-                    if constexpr (!kRes) mask(k, v, d);
-                    sb.x += d.x; sb.y += d.y; sb.z += d.z; sb.w += d.w;
-                    sg.x = fmaf(d.x, xh.x, sg.x); sg.y = fmaf(d.y, xh.y, sg.y); sg.z = fmaf(d.z, xh.z, sg.z); sg.w = fmaf(d.w, xh.w, sg.w);
-                };
+                const BnCol k = el.column(col);
+                auto acc = [&](const float4& v, const float4& d) { el.acc(k, v, d, sb, sg); };
                 int r = row0 + ty;
                 if (held) {
 #pragma unroll
                     for (int j = 0; j < kBnHold; ++j) {
                         const int rr = r + j * g.rpi;
                         hx[j] = rr < row1 ? __ldg(x4 + (size_t)rr * g.cv + col) : V{};
-                        hd[j] = rr < row1 ? grad(row0, rr, col) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        hd[j] = rr < row1 ? el.grad(row0, rr, col) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
                     if constexpr (kRes) {
 #pragma unroll
                         for (int j = 0; j < kBnHold; ++j)
                             if (r + j * g.rpi < row1) {
                                 const size_t o = (size_t)(r + j * g.rpi) * g.cv + col;
-                                gate(k, A::wide(hx[j]), ldr(o), o, hd[j]);
+                                el.gate(k, A::wide(hx[j]), ldr(o), o, hd[j]);
                             }
                     }
 #pragma unroll
@@ -536,12 +733,12 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                     for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                         const size_t o = (size_t)r * g.cv + col;
                         const float4 v0 = ldx(o), v1 = ldx(o + st1), v2 = ldx(o + 2 * st1), v3 = ldx(o + 3 * st1);
-                        float4 e0 = grad(row0, r, col), e1 = grad(row0, r + g.rpi, col), e2 = grad(row0, r + 2 * g.rpi, col),
-                               e3 = grad(row0, r + 3 * g.rpi, col);
+                        float4 e0 = el.grad(row0, r, col), e1 = el.grad(row0, r + g.rpi, col), e2 = el.grad(row0, r + 2 * g.rpi, col),
+                               e3 = el.grad(row0, r + 3 * g.rpi, col);
                         if constexpr (kRes) {
                             const float4 q0 = ldr(o), q1 = ldr(o + st1), q2 = ldr(o + 2 * st1), q3 = ldr(o + 3 * st1);
-                            gate(k, v0, q0, o, e0); gate(k, v1, q1, o + st1, e1);
-                            gate(k, v2, q2, o + 2 * st1, e2); gate(k, v3, q3, o + 3 * st1, e3);
+                            el.gate(k, v0, q0, o, e0); el.gate(k, v1, q1, o + st1, e1);
+                            el.gate(k, v2, q2, o + 2 * st1, e2); el.gate(k, v3, q3, o + 3 * st1, e3);
                         }
                         acc(v0, e0); acc(v1, e1); acc(v2, e2); acc(v3, e3);
                     }
@@ -549,11 +746,11 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
                         if constexpr (kRes) {
                             const size_t o = (size_t)r * g.cv + col;
                             const float4 v = ldx(o);
-                            float4 e = grad(row0, r, col);
-                            gate(k, v, ldr(o), o, e);
+                            float4 e = el.grad(row0, r, col);
+                            el.gate(k, v, ldr(o), o, e);
                             acc(v, e);
                         } else {
-                            acc(ldx((size_t)r * g.cv + col), grad(row0, r, col));
+                            acc(ldx((size_t)r * g.cv + col), el.grad(row0, r, col));
                         }
                     }
                 }
@@ -579,19 +776,11 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
         for (int c0 = 0; c0 < g.cv; c0 += g.tpr) {
             const int col = c0 + tx;
             if (ty >= g.rpi || col >= g.cv) continue;
-            const Col k = column(col);
+            const BnCol k = el.column(col);
             const float4 db = __ldcg(reinterpret_cast<const float4*>(p.dbeta) + col);
             const float4 dg = __ldcg(reinterpret_cast<const float4*>(p.dgamma) + col);
-            const double M = (double)g.M;
-            const float4 mb = make_float4((float)(db.x / M), (float)(db.y / M), (float)(db.z / M), (float)(db.w / M));
-            const float4 mg = make_float4((float)(dg.x / M), (float)(dg.y / M), (float)(dg.z / M), (float)(dg.w / M));
-            V* o4 = reinterpret_cast<V*>(p.dx);
-            auto out = [&](size_t off, const float4& v, float4 d) {
-                const float4 xh = xhat(k, v);
-                if constexpr (!kRes) mask(k, v, d);
-                o4[off] = A::narrow(make_float4(k.a.x * (d.x - mb.x - xh.x * mg.x), k.a.y * (d.y - mb.y - xh.y * mg.y),
-                                                k.a.z * (d.z - mb.z - xh.z * mg.z), k.a.w * (d.w - mb.w - xh.w * mg.w)));
-            };
+            const float4 mb = el.over_m(db), mg = el.over_m(dg);
+            auto out = [&](size_t off, const float4& v, const float4& d) { el.dx(k, mb, mg, off, v, d); };
             int r = row0 + ty;
             if (held) {
 #pragma unroll
@@ -602,7 +791,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
             // with a residual, the masked gradient is the dres this thread wrote in (1): a coherent load, not __ldg
             auto grad3 = [&](int r3) -> float4 {
                 if constexpr (kRes) return A::wide(__ldcg(dr4 + (size_t)r3 * g.cv + col));
-                else return grad(row0, r3, col);
+                else return el.grad(row0, r3, col);
             };
             for (; r + 3 * g.rpi < row1; r += 4 * g.rpi) {
                 const size_t o = (size_t)r * g.cv + col;
@@ -615,8 +804,64 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
     }
 }
 
+// Channel-sliced backward (g.sc > 0): the thread layout of bn_fwd_sliced_kernel.
+template <bool kPool, bool kRes, typename T>
+__global__ void __launch_bounds__(kBnThreads) bn_bwd_sliced_kernel(const BnBwdArgs<T> p) {
+    static_assert(!(kPool && kRes), "no pool follows a residual add");
+    using A = BnAct<T>;
+    using V = typename A::V;
+    extern __shared__ float4 s_dyn[];         // bn_slice_reduce's scratch
+    __shared__ float4 s_tot[2 * 8];           // [sc] dbeta | [sc] dgamma of the owned columns
+    const BnGeom& g = p.g;
+    const int sc = g.sc, cx = threadIdx.x % sc, ln = threadIdx.x / sc, col = blockIdx.x * sc + cx;
+    const int row0 = ln / g.rpi * g.rows_per_block, row1 = min(g.M, row0 + g.rows_per_block), r = row0 + ln % g.rpi;
+    const BnBwdElem<kPool, kRes, T> el{p};
+    const V* x4 = reinterpret_cast<const V*>(p.x);
+    const BnCol k = el.column(col);
+
+    // (1) the thread's rows of x and of the gradient (pooled: expanded; residual: gated, dres written), held; their sums
+    V hx[kBnHold];
+    float4 hd[kBnHold];
+    float4 sb = make_float4(0.f, 0.f, 0.f, 0.f), sg = sb;
+#pragma unroll
+    for (int j = 0; j < kBnHold; ++j) {
+        const int rr = r + j * g.rpi;
+        hx[j] = rr < row1 ? __ldg(x4 + (size_t)rr * g.cv + col) : V{};
+        hd[j] = rr < row1 ? el.grad(0, rr, col) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if constexpr (kRes) {
+        const V* r4 = reinterpret_cast<const V*>(p.res);
+#pragma unroll
+        for (int j = 0; j < kBnHold; ++j)
+            if (r + j * g.rpi < row1) {
+                const size_t o = (size_t)(r + j * g.rpi) * g.cv + col;
+                el.gate(k, A::wide(hx[j]), A::wide(__ldg(r4 + o)), o, hd[j]);
+            }
+    }
+#pragma unroll
+    for (int j = 0; j < kBnHold; ++j)
+        if (r + j * g.rpi < row1) el.acc(k, A::wide(hx[j]), hd[j], sb, sg);
+
+    // (2) dbeta, dgamma of the owned columns
+    bn_slice_reduce(sb, sg, g, s_dyn, s_tot);
+    if (threadIdx.x < sc) {
+        reinterpret_cast<float4*>(p.dbeta)[blockIdx.x * sc + threadIdx.x] = s_tot[threadIdx.x];
+        reinterpret_cast<float4*>(p.dgamma)[blockIdx.x * sc + threadIdx.x] = s_tot[sc + threadIdx.x];
+    }
+
+    // (3) input gradient
+    const float4 mb = el.over_m(s_tot[cx]), mg = el.over_m(s_tot[sc + cx]);
+#pragma unroll
+    for (int j = 0; j < kBnHold; ++j)
+        if (r + j * g.rpi < row1) el.dx(k, mb, mg, (size_t)(r + j * g.rpi) * g.cv + col, A::wide(hx[j]), hd[j]);
+}
+
 // ---------------------------------------------------------------------------------------------- launchers
 int bn_tile_rows(int M, int C) { return bn_geom(M, C).rows_per_block; }
+
+// Whether a call without a grid cap runs the channel-sliced kernels.  A pool of width W > 0 only has to be one the fused
+// kernels take at all: a pooled slice's y, M * sc float4, never exceeds kBnHold * kBnThreads of them (32 KB).
+bool bn_sliced(int M, int C, int W) { return bn_geom(M, C).sc > 0 && (W == 0 || (W % 2 == 0 && M % (2 * W) == 0)); }
 
 static unsigned int* bn_sync_slot(int slot) {
     static unsigned int* base[64] = {nullptr};
@@ -650,6 +895,17 @@ static cudaError_t bn_launch(void (*kernel)(const Args), Args p, size_t smem, in
     return e;
 }
 
+// Plain launch of a channel-sliced kernel: cv / sc CTAs of sc * nblk * rpi threads; `stage`: bytes of the pooled y.
+template <typename Args>
+static cudaError_t bn_launch_sliced(void (*kernel)(const Args), const Args& p, size_t stage, cudaStream_t stream) {
+    const BnGeom& g = p.g;
+    const int threads = g.sc * g.nblk * g.rpi;
+    size_t smem = sizeof(float4) * (2 * threads + 2 * g.nblk * g.sc);           // bn_slice_reduce's scratch
+    if (smem < stage) smem = stage;
+    kernel<<<g.cv / g.sc, threads, smem, stream>>>(p);
+    return cudaGetLastError();
+}
+
 static cudaError_t bn_prepare(BnGeom& g, unsigned int*& sync, int M, int C, int W, int slot) {
     g = bn_geom(M, C);
     g.W = W;
@@ -668,6 +924,11 @@ static cudaError_t bn_forward_t(const void* x, void* y, unsigned char* arg, floa
                    rmean, rvar, nbt, momentum, eps, relu, nullptr, {}, static_cast<const T*>(res)};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
+    if (p.g.sc > 0 && max_ctas <= 0) {           // a grid cap asks for the cooperative kernels' loop over tiles
+        if (W > 0) return bn_launch_sliced(bn_fwd_sliced_kernel<true, false, T>, p, sizeof(float4) * M * p.g.sc, stream);
+        return res != nullptr ? bn_launch_sliced(bn_fwd_sliced_kernel<false, true, T>, p, 0, stream)
+                              : bn_launch_sliced(bn_fwd_sliced_kernel<false, false, T>, p, 0, stream);
+    }
     size_t smem = sizeof(float) * 2 * C;
     if (W > 0 && p.g.hold) smem += sizeof(float4) * p.g.rows_per_block * p.g.cv;
     if (W > 0) return bn_launch(bn_fwd_kernel<true, false, T>, p, smem, max_ctas, stream);
@@ -686,6 +947,11 @@ static cudaError_t bn_backward_t(const void* x, const void* dy, const unsigned c
                    static_cast<T*>(dres)};
     cudaError_t e = bn_prepare(p.g, p.sync, M, C, W, slot);
     if (e != cudaSuccess) return e;
+    if (p.g.sc > 0 && max_ctas <= 0) {
+        if (W > 0) return bn_launch_sliced(bn_bwd_sliced_kernel<true, false, T>, p, 0, stream);
+        return res != nullptr ? bn_launch_sliced(bn_bwd_sliced_kernel<false, true, T>, p, 0, stream)
+                              : bn_launch_sliced(bn_bwd_sliced_kernel<false, false, T>, p, 0, stream);
+    }
     const size_t smem = sizeof(float) * 2 * C;
     if (W > 0) return bn_launch(bn_bwd_kernel<true, false, T>, p, smem, max_ctas, stream);
     return res != nullptr ? bn_launch(bn_bwd_kernel<false, true, T>, p, smem, max_ctas, stream)

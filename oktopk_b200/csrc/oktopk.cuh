@@ -350,6 +350,7 @@ cudaError_t launch_land(const LandParams& lp, float* bucket, cudaStream_t stream
 // residual's gradient `dres`.
 enum class BnDtype : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 int bn_tile_rows(int M, int C);
+bool bn_sliced(int M, int C, int W);      // the channel-sliced kernels run (given max_ctas <= 0): no `partial`, no hand-off
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
                               float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,

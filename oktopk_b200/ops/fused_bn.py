@@ -8,7 +8,8 @@ stride-2 ``pool`` the forward kernel writes only the pooled output and a one-byt
 never stored.  The convolution is then called WITHOUT its bias: a bias in front of a batch-norm cancels exactly
 (``BN(x + b) = BN(x)``, the batch mean absorbs it), so it only enters the running-mean update, and its gradient is
 identically zero (returned as ``None``; autograd's own reduction over ``dy`` returns rounding noise for it).
-Parameters, buffers and ``state_dict`` keys are the stock modules' ones.
+Parameters, buffers and ``state_dict`` keys are the stock modules' ones.  Small layers (``bn_sliced(M, C, W)``: VGG-16's
+layers 5 - 13 at 16 images) run the channel-sliced kernels, which have no grid hand-off and compute the same bits.
 
 Residual: ``bias_bn_relu(..., residual=r)`` / ``conv_bn_relu(..., residual=r)`` compute ``relu(bn(x) + r)``, the end of a
 ResNet block, in the same two kernels (``relu=True`` and no pool only; anything else is a ``ValueError``).  The
@@ -47,7 +48,8 @@ import torch.nn.functional as F
 from . import ext
 
 # > 0 caps the grid of the fused batch-norm kernels, so that each CTA loops over several tiles (tests use it to cover
-# that path on a GPU whose co-resident grid exceeds the tile count)
+# that path on a GPU whose co-resident grid exceeds the tile count).  A cap also keeps a shape the channel-sliced kernels
+# would take on the cooperative ones (1 << 30 caps nothing: the cooperative kernels exactly as without a cap).
 MAX_CTAS = 0
 
 _SLOTS = itertools.count()
@@ -104,6 +106,14 @@ def _residual_ok(x: torch.Tensor, residual: torch.Tensor) -> bool:
     return residual.device == x.device and residual.shape == x.shape and residual.dtype == x.dtype
 
 
+def _partial(C, x: torch.Tensor, M: int, Ch: int, W: int) -> Optional[torch.Tensor]:
+    """The cooperative kernels' per-tile partials; the channel-sliced kernels need none."""
+    if MAX_CTAS <= 0 and C.bn_sliced(M, Ch, W):
+        return None
+    rows = C.bn_tile_rows(M, Ch)
+    return torch.empty((M + rows - 1) // rows * 2 * Ch, dtype=torch.float32, device=x.device)
+
+
 class _BiasBNReLUPool(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gamma, beta, cbias, rmean, rvar, nbt, momentum, eps, relu, pool, slot, res=None):
@@ -117,11 +127,11 @@ class _BiasBNReLUPool(torch.autograd.Function):
         else:
             y = torch.empty_like(x)                   # preserves channels_last
             arg = None
-        rows = C.bn_tile_rows(M, Ch)
-        partial = torch.empty((M + rows - 1) // rows * 2 * Ch, dtype=torch.float32, device=x.device)
+        partial = _partial(C, x, M, Ch, W if pool else 0)
         stats = torch.empty(2 * Ch, dtype=torch.float32, device=x.device)       # [mean | invstd]
         s = torch.cuda.current_stream().cuda_stream
-        C.bn_forward(x.data_ptr(), y.data_ptr(), 0 if arg is None else arg.data_ptr(), partial.data_ptr(), gamma.data_ptr(),
+        C.bn_forward(x.data_ptr(), y.data_ptr(), 0 if arg is None else arg.data_ptr(),
+                     0 if partial is None else partial.data_ptr(), gamma.data_ptr(),
                      beta.data_ptr(), 0 if cbias is None else cbias.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch,
                      0 if rmean is None else rmean.data_ptr(), 0 if rvar is None else rvar.data_ptr(),
                      0 if nbt is None else nbt.data_ptr(), float(momentum), float(eps), int(relu), M, Ch,
@@ -140,14 +150,13 @@ class _BiasBNReLUPool(torch.autograd.Function):
         if not dy.is_contiguous(memory_format=torch.channels_last):
             dy = dy.contiguous(memory_format=torch.channels_last)
         dx = torch.empty_like(x)
-        rows = C.bn_tile_rows(M, Ch)
-        partial = torch.empty((M + rows - 1) // rows * 2 * Ch, dtype=torch.float32, device=x.device)
+        partial = _partial(C, x, M, Ch, W if ctx.pool else 0)
         dgb = torch.empty(2 * Ch, dtype=torch.float32, device=x.device)         # [dgamma | dbeta]
         dres = None if res is None else torch.empty_like(x)                       # dy masked by the ReLU
         s = torch.cuda.current_stream().cuda_stream
-        C.bn_backward(x.data_ptr(), dy.data_ptr(), 0 if arg is None else arg.data_ptr(), dx.data_ptr(), partial.data_ptr(),
-                      gamma.data_ptr(), beta.data_ptr(), stats.data_ptr(), stats.data_ptr() + 4 * Ch, dgb.data_ptr(),
-                      dgb.data_ptr() + 4 * Ch, int(ctx.relu), M, Ch, W if ctx.pool else 0, ctx.slot, MAX_CTAS, s,
+        C.bn_backward(x.data_ptr(), dy.data_ptr(), 0 if arg is None else arg.data_ptr(), dx.data_ptr(),
+                      0 if partial is None else partial.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+                      stats.data_ptr(), stats.data_ptr() + 4 * Ch, dgb.data_ptr(), dgb.data_ptr() + 4 * Ch, int(ctx.relu), M, Ch, W if ctx.pool else 0, ctx.slot, MAX_CTAS, s,
                       ctx.dtype, 0 if res is None else res.data_ptr(), 0 if dres is None else dres.data_ptr())
         # conv bias: the loss does not depend on it (see module docstring) -> no gradient
         return dx, dgb[:Ch], dgb[Ch:], None, None, None, None, None, None, None, None, None, dres
