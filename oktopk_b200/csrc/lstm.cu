@@ -1,0 +1,282 @@
+// Persistent LSTM recurrence (fp32, time-major T x N, torch's gate order i, f, g, o, zero initial state):
+//
+//   a_t = gx_t + W_hh h_{t-1}                  gx = x W_ih^T + b_ih + b_hh for all t: one GEMM in torch beforehand
+//   i, f, o = sigmoid(a_i, a_f, a_o), g = tanh(a_g),   c_t = f c_{t-1} + i g,   h_t = o tanh(c_t)
+//
+// Utterance b has length len_b: y_t = h_t for t < len_b and exactly 0 after (what pad_packed_sequence gives).
+//
+// cuDNN's fp32 RNN runs this as a small GEMM and an element-wise kernel per timestep and pass, each re-reading the
+// 4H x H recurrent matrix from L2.  Here one cooperative kernel walks all timesteps of a pass, and the matrix stays in
+// shared memory: CTA b owns the u hidden units [b u, b u + u) (u = ceil(H / #SMs): H = 800 on 132 SMs gives u = 7 on
+// 115 CTAs, 89.6 KB of weights each).
+//
+// Forward (lstm_fwd_kernel): the CTA keeps the 4u rows of W_hh of its units' gates and their cell states c.  At step t
+// it stages h_{t-1} = y_{t-1} (all N x H of it, `rows` batch rows at a time) from L2 into shared memory, forms its 4u x N
+// gate sums, then its units' c_t and h_t; it writes y_t, the activated gates and c_t (for the backward pass) and crosses
+// the grid barrier, after which every CTA can read all of y_t.
+//
+// Backward (lstm_bwd_kernel), t from T-1 down to 0: the CTA keeps the 4H x u columns of W_hh of the same units, so that
+// dh_rec[j] = sum_k W_hh[k, j] dgates_{t+1}[k] is local.  At step t it stages dgates_{t+1} (N x 4H) and forms its u x N
+// dh_rec; with dy_t, the saved gates and c, and its carried dc it writes dgates_t for its units' 4 gate rows and crosses
+// the barrier.  For t >= len_b, dgates and the carried dc are exactly 0.  dx, dW_ih, dW_hh and the bias gradients are
+// GEMMs and sums over dgates in torch.
+//
+// The barrier is common.cuh's ticket grid_sync on a counter the caller zeroes: one per step, the only cross-CTA
+// dependency being the whole of y_t (dgates_t), which every CTA reads.  Operands written by other CTAs in this launch
+// are read with ld.global.cg (L2), never through L1.
+//
+// Every sum has a fixed order: lane l of a warp adds the float4 columns l, l + 32, ... of a dot product in order, and the
+// 32 lanes are combined by a fixed butterfly.  No atomics touch data, so results are bitwise reproducible.
+#include "common.cuh"
+#include "oktopk.cuh"
+
+namespace okt {
+
+constexpr int kLstmThreads = 512;                // ops/fused_lstm.py LSTM_THREADS
+constexpr int kLstmWarps = kLstmThreads / 32;
+constexpr int kLstmNB = 4;                       // batch rows of one warp task in lstm_dots
+
+struct LstmFwdArgs {
+    const float* gx;
+    const float* whh;
+    const int* len;
+    float* y;
+    float* gates;
+    float* cs;
+    unsigned long long* bar;
+    int T, N, H, u, rows;
+};
+
+struct LstmBwdArgs {
+    const float* dy;
+    const float* gates;
+    const float* cs;
+    const float* whh;
+    const int* len;
+    float* dg;
+    unsigned long long* bar;
+    int T, N, H, u, rows;
+};
+
+__device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+
+// Copy `nrows` rows of K floats (K % 4 == 0, 16-byte aligned) that other CTAs wrote in this launch to shared memory.
+__device__ __forceinline__ void lstm_stage(float* __restrict__ sV, const float* __restrict__ g, int nrows, int K) {
+    float4* d = reinterpret_cast<float4*>(sV);
+    const float4* s = reinterpret_cast<const float4*>(g);
+    const int n4 = nrows * (K >> 2);
+    for (int i = threadIdx.x; i < n4; i += kLstmThreads) d[i] = __ldcg(s + i);
+}
+
+// out[r N + n0 + j] = sum_k sW[r K + k] sV[j K + k] for r < R, j < nc.  A warp takes one (r, kLstmNB rows of sV) task at
+// a time; the order of every sum is fixed (see the file header), whichever warp runs it.
+__device__ __forceinline__ void lstm_dots(const float* __restrict__ sW, const float* __restrict__ sV,
+                                          float* __restrict__ out, int R, int K, int nc, int n0, int N) {
+    const int K4 = K >> 2, lane = lane_id(), warp = threadIdx.x >> 5;
+    const int nb = (nc + kLstmNB - 1) / kLstmNB;
+    const float4* W4 = reinterpret_cast<const float4*>(sW);
+    const float4* V4 = reinterpret_cast<const float4*>(sV);
+    for (int task = warp; task < R * nb; task += kLstmWarps) {
+        const int r = task / nb, j0 = (task - r * nb) * kLstmNB;
+        const float4* w = W4 + (size_t)r * K4;
+        float acc[kLstmNB];
+#pragma unroll
+        for (int j = 0; j < kLstmNB; ++j) acc[j] = 0.f;
+        for (int k = lane; k < K4; k += 32) {
+            const float4 a = w[k];
+#pragma unroll
+            for (int j = 0; j < kLstmNB; ++j) {
+                if (j0 + j < nc) {
+                    const float4 b = V4[(size_t)(j0 + j) * K4 + k];
+                    acc[j] = fmaf(a.x, b.x, acc[j]);
+                    acc[j] = fmaf(a.y, b.y, acc[j]);
+                    acc[j] = fmaf(a.z, b.z, acc[j]);
+                    acc[j] = fmaf(a.w, b.w, acc[j]);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kLstmNB; ++j) acc[j] = warp_sum_f(acc[j]);
+        if (lane == 0) {
+#pragma unroll
+            for (int j = 0; j < kLstmNB; ++j)
+                if (j0 + j < nc) out[r * N + n0 + j0 + j] = acc[j];
+        }
+    }
+}
+
+// out[r N + n] = sum_k sW[r K + k] V[n K + k] over all N rows of V (global, written in this launch), `rows` at a time.
+__device__ __forceinline__ void lstm_matvec(const float* __restrict__ sW, float* __restrict__ sV, const float* V,
+                                            float* __restrict__ out, int R, int K, int N, int rows) {
+    for (int n0 = 0; n0 < N; n0 += rows) {
+        const int nc = min(rows, N - n0);
+        lstm_stage(sV, V + (size_t)n0 * K, nc, K);
+        __syncthreads();
+        lstm_dots(sW, sV, out, R, K, nc, n0, N);
+        __syncthreads();
+    }
+}
+
+// Shared memory: W [4u][H] | h_{t-1} rows [rows][H] | gate sums [4u][N] | c [u][N].
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwdArgs p) {
+    extern __shared__ float4 lstm_smem[];
+    const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2;
+    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    float* sW = reinterpret_cast<float*>(lstm_smem);
+    float* sV = sW + (size_t)R * H;
+    float* sG = sV + (size_t)p.rows * H;
+    float* sC = sG + R * N;
+    for (int i = threadIdx.x; i < R * H4; i += kLstmThreads) {      // local row q u + j = W_hh row q H + u0 + j
+        const int lr = i / H4, k = i - lr * H4, q = lr / u, j = lr - q * u;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (j < nu) v = __ldg(reinterpret_cast<const float4*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
+        reinterpret_cast<float4*>(sW)[i] = v;
+    }
+    for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sC[i] = 0.f;
+    for (int t = 0; t < p.T; ++t) {
+        if (t == 0) {
+            for (int i = threadIdx.x; i < R * N; i += kLstmThreads) sG[i] = 0.f;
+            __syncthreads();
+        } else {
+            lstm_matvec(sW, sV, p.y + (size_t)(t - 1) * N * H, sG, R, H, N, p.rows);
+        }
+        for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
+            const int j = i / N, n = i - j * N, unit = u0 + j;
+            const size_t row = (size_t)t * N + n;
+            const float* gx = p.gx + row * 4 * H + unit;
+            float* gs = p.gates + row * 4 * H + unit;
+            const size_t o = row * H + unit;
+            if (t < __ldg(p.len + n)) {
+                const float gi = lstm_sigmoid(sG[(0 * u + j) * N + n] + __ldg(gx));
+                const float gf = lstm_sigmoid(sG[(1 * u + j) * N + n] + __ldg(gx + H));
+                const float gg = tanhf(sG[(2 * u + j) * N + n] + __ldg(gx + 2 * H));
+                const float go = lstm_sigmoid(sG[(3 * u + j) * N + n] + __ldg(gx + 3 * H));
+                const float c = gf * sC[j * N + n] + gi * gg;
+                sC[j * N + n] = c;
+                gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
+                p.cs[o] = c;
+                p.y[o] = go * tanhf(c);
+            } else {
+                gs[0] = 0.f; gs[H] = 0.f; gs[2 * H] = 0.f; gs[3 * H] = 0.f;
+                p.cs[o] = 0.f;
+                p.y[o] = 0.f;
+            }
+        }
+        if (t + 1 < p.T) grid_sync(p.bar);
+    }
+}
+
+// Shared memory: W^T [u][4H] | dgates_{t+1} rows [rows][4H] | dh_rec [u][N] | carried dc [u][N].
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwdArgs p) {
+    extern __shared__ float4 lstm_smem[];
+    const int H = p.H, N = p.N, u = p.u, G = 4 * H;
+    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    float* sW = reinterpret_cast<float*>(lstm_smem);
+    float* sV = sW + (size_t)u * G;
+    float* sD = sV + (size_t)p.rows * G;
+    float* sDC = sD + u * N;
+    for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
+        const int k = i / u, j = i - k * u;
+        sW[(size_t)j * G + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : 0.f;
+    }
+    for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sDC[i] = 0.f;
+    for (int t = p.T - 1; t >= 0; --t) {
+        if (t == p.T - 1) {
+            for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sD[i] = 0.f;
+            __syncthreads();
+        } else {
+            lstm_matvec(sW, sV, p.dg + (size_t)(t + 1) * N * G, sD, u, G, N, p.rows);
+        }
+        for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
+            const int j = i / N, n = i - j * N, unit = u0 + j;
+            const size_t row = (size_t)t * N + n;
+            const size_t o = row * H + unit;
+            float* dg = p.dg + row * G + unit;
+            if (t < __ldg(p.len + n)) {
+                const float* gs = p.gates + row * G + unit;
+                const float gi = __ldg(gs), gf = __ldg(gs + H), gg = __ldg(gs + 2 * H), go = __ldg(gs + 3 * H);
+                const float tc = tanhf(__ldg(p.cs + o));
+                const float cp = t > 0 ? __ldg(p.cs + o - (size_t)N * H) : 0.f;
+                const float dh = __ldg(p.dy + o) + sD[j * N + n];
+                const float dc = dh * go * (1.f - tc * tc) + sDC[j * N + n];
+                dg[0] = dc * gg * gi * (1.f - gi);
+                dg[H] = dc * cp * gf * (1.f - gf);
+                dg[2 * H] = dc * gi * (1.f - gg * gg);
+                dg[3 * H] = dh * tc * go * (1.f - go);
+                sDC[j * N + n] = dc * gf;
+            } else {
+                dg[0] = 0.f; dg[H] = 0.f; dg[2 * H] = 0.f; dg[3 * H] = 0.f;
+                sDC[j * N + n] = 0.f;
+            }
+        }
+        if (t > 0) grid_sync(p.bar);
+    }
+}
+
+// What a launch needs to know about the device and the kernel, queried once per device (the SM count), per larger
+// shared-memory size (the kernel's opt-in limit only ever grows) and per new size (the occupancy): the eager AN4 step
+// launches these kernels ten times, and its host side is what limits it.
+constexpr int kLstmMaxDevices = 64;
+struct LstmLaunchCache {
+    int sms = 0;
+    size_t smem_set = 0;
+    size_t occ_smem = 0;
+    int occ_per = 0;
+};
+
+// Cooperative launch of `grid` CTAs with `smem` bytes each; an error if they cannot all be co-resident.
+template <typename Args>
+static cudaError_t lstm_launch(void (*kernel)(const Args), const Args& p, int grid, size_t smem, cudaStream_t stream) {
+    static LstmLaunchCache cache[kLstmMaxDevices];             // one table per kernel: Args differs between the two
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 0 || dev >= kLstmMaxDevices) return cudaErrorInvalidDevice;
+    LstmLaunchCache& c = cache[dev];
+    if (c.sms == 0) e = cudaDeviceGetAttribute(&c.sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess && smem > c.smem_set) {
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess) c.smem_set = smem;
+    }
+    if (e == cudaSuccess && smem != c.occ_smem) {
+        int per = 0;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kernel, kLstmThreads, smem);
+        if (e == cudaSuccess) {
+            c.occ_smem = smem;
+            c.occ_per = per;
+        }
+    }
+    if (e != cudaSuccess) {
+        c.sms = 0;
+        (void)cudaGetLastError();
+        return e;
+    }
+    if (c.occ_per * c.sms < grid) return cudaErrorCooperativeLaunchTooLarge;
+    void* args[] = {(void*)&p};
+    e = cudaLaunchCooperativeKernel((void*)kernel, dim3(grid), dim3(kLstmThreads), args, smem, stream);
+    (void)cudaGetLastError();       // a failed launch must not surface again at the next launcher's error check
+    return e;
+}
+
+static bool lstm_shape_ok(int T, int N, int H, int u, int rows) {
+    return T > 0 && N > 0 && H > 0 && H % 4 == 0 && u > 0 && u <= H && rows > 0 && rows <= N;
+}
+
+cudaError_t launch_lstm_forward(const float* gx, const float* whh, const int* len, float* y, float* gates, float* cs,
+                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream) {
+    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
+    const LstmFwdArgs p{gx, whh, len, y, gates, cs, bar, T, N, H, u, rows};
+    const size_t smem = sizeof(float) * ((size_t)4 * u * H + (size_t)rows * H + (size_t)5 * u * N);
+    return lstm_launch(lstm_fwd_kernel, p, (H + u - 1) / u, smem, stream);
+}
+
+cudaError_t launch_lstm_backward(const float* dy, const float* gates, const float* cs, const float* whh, const int* len,
+                                 float* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                 cudaStream_t stream) {
+    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
+    const LstmBwdArgs p{dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows};
+    const size_t smem = sizeof(float) * ((size_t)4 * u * H + (size_t)rows * 4 * H + (size_t)2 * u * N);
+    return lstm_launch(lstm_bwd_kernel, p, (H + u - 1) / u, smem, stream);
+}
+
+}  // namespace okt

@@ -23,7 +23,8 @@ FUSED_BN_RESNETS = ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110")
 def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
     ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``); for BERT,
-    ``fuse_ln=True`` turns on ``net.fuse_ln`` and ``fuse_xent=True`` ``net.fuse_xent``."""
+    ``fuse_ln=True`` turns on ``net.fuse_ln`` and ``fuse_xent=True`` ``net.fuse_xent``; for ``lstman4``,
+    ``fuse_lstm=True`` turns on ``net.fuse_lstm``."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
@@ -45,7 +46,10 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     elif d == "mnistnet":
         net = zoo.MnistNet()
     elif d == "lstman4":
-        net = lstman4(**kwargs)
+        kw = dict(kwargs)
+        fuse_lstm = bool(kw.pop("fuse_lstm", False))
+        net = lstman4(**kw)
+        net.fuse_lstm = fuse_lstm
         ext = {"labels": AN4_LABELS}
     elif d == "lstm":
         net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20))

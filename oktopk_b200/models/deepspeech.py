@@ -6,15 +6,21 @@ Architecture parity with ``VGG/models/lstm_models.py:148-239`` and the factory d
 BatchNorm+LSTM layers on packed sequences, a look-ahead convolution, BatchNorm + bias-free Linear.
 27,569,568 parameters in 40 tensors.  Input ``(B, 1, 161, T)`` + lengths; output ``(B, T', classes)``
 logits (softmax only in eval mode) + output lengths; trained with CTC.
+
+``fuse_lstm=True`` (or ``net.fuse_lstm = True`` at any time) runs the uni-directional LSTM layers on the persistent
+recurrence kernels of ``ops/fused_lstm.py`` instead of packing the sequences for cuDNN; parameters, buffers and
+``state_dict`` keys are the same either way.
 """
 from __future__ import annotations
 
 import math
-from typing import Tuple
+from typing import Optional, Tuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from ..ops.fused_lstm import lstm_layer, stock_layer
 
 AN4_LABELS = "_'ABCDEFGHIJKLMNOPQRSTUVWXYZ "     # 29 symbols, index 0 = CTC blank
 
@@ -49,23 +55,24 @@ class _SeqBN(nn.Module):
 
 
 class BatchRNN(nn.Module):
+    """``fuse`` (default off) runs the recurrence through ``ops/fused_lstm.lstm_layer``, which falls back to the stock
+    pack -> rnn -> pad sequence wherever its kernels do not apply."""
+
     def __init__(self, input_size: int, hidden_size: int, rnn_type=nn.LSTM, bidirectional: bool = False,
-                 batch_norm: bool = True):
+                 batch_norm: bool = True, fuse: bool = False):
         super().__init__()
         self.bidirectional = bidirectional
+        self.fuse = fuse
         self.batch_norm = _SeqBN(nn.BatchNorm1d(input_size)) if batch_norm else None
         self.rnn = rnn_type(input_size=input_size, hidden_size=hidden_size, bidirectional=bidirectional, bias=True)
 
-    def forward(self, x: torch.Tensor, lengths: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, lengths: torch.Tensor, dev_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``lengths``: host int tensor; ``dev_lengths``: optionally the same as int32 on the device (fused path)."""
         if self.batch_norm is not None:
             x = self.batch_norm(x)
-        total = x.size(0)
-        x = nn.utils.rnn.pack_padded_sequence(x, lengths.cpu(), enforce_sorted=False)
-        x, _ = self.rnn(x)
-        x, _ = nn.utils.rnn.pad_packed_sequence(x, total_length=total)
-        if self.bidirectional:
-            x = x.view(x.size(0), x.size(1), 2, -1).sum(2)
-        return x
+        if self.fuse:
+            return lstm_layer(x, lengths, self.rnn, dev_lengths)
+        return stock_layer(x, lengths, self.rnn)
 
 
 class Lookahead(nn.Module):
@@ -89,7 +96,7 @@ class Lookahead(nn.Module):
 class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
-                 window_size: float = 0.02):
+                 window_size: float = 0.02, fuse_lstm: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -111,6 +118,17 @@ class DeepSpeech(nn.Module):
             Lookahead(rnn_hidden_size, context=context), nn.Hardtanh(0, 20, inplace=True))
         self.fc = _SeqBN(nn.Sequential(nn.BatchNorm1d(rnn_hidden_size),
                                        nn.Linear(rnn_hidden_size, num_classes, bias=False)))
+        self.fuse_lstm = fuse_lstm
+
+    @property
+    def fuse_lstm(self) -> bool:
+        """Whether every ``BatchRNN`` layer takes the fused recurrence kernels (``ops/fused_lstm.py``)."""
+        return all(m.fuse for m in self.rnns)
+
+    @fuse_lstm.setter
+    def fuse_lstm(self, on: bool) -> None:
+        for m in self.rnns:
+            m.fuse = bool(on)
 
     def get_seq_lens(self, input_length: torch.Tensor) -> torch.Tensor:
         seq = input_length
@@ -124,8 +142,10 @@ class DeepSpeech(nn.Module):
         x = self.conv(x, out_lens)
         b, c, d, t = x.size()
         x = x.view(b, c * d, t).permute(2, 0, 1).contiguous()        # T x N x H
+        # the fused layers read the lengths on the device: one copy for all of them
+        dev_lens = out_lens.to(x.device) if x.is_cuda and any(m.fuse for m in self.rnns) else None
         for rnn in self.rnns:
-            x = rnn(x, out_lens)
+            x = rnn(x, out_lens, dev_lens)
         if self.lookahead is not None:
             x = self.lookahead(x)
         x = self.fc(x).transpose(0, 1)                                # N x T x classes
@@ -134,9 +154,11 @@ class DeepSpeech(nn.Module):
         return x, out_lens
 
 
-def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False) -> DeepSpeech:
+def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
+            fuse_lstm: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
-    return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional)
+    return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
+                      fuse_lstm=fuse_lstm)
 
 
 class PTBLSTM(nn.Module):

@@ -76,6 +76,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-xent", action="store_true",
                    help="BERT: the masked-LM loss takes the fused softmax cross-entropy kernels, which read only the "
                         "labelled rows (default: stock cross_entropy)")
+    p.add_argument("--fused-lstm", action="store_true",
+                   help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
+                        "and pass, instead of packed sequences through cuDNN (default: stock)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -111,6 +114,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["fuse_ln"] = True
     if args.fused_xent:
         model_kwargs["fuse_xent"] = True
+    if args.fused_lstm:
+        model_kwargs["fuse_lstm"] = True
     return dnn, model_kwargs
 
 
@@ -132,6 +137,12 @@ def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespac
             parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
 
 
+def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
+    """``--fused-lstm`` is for the AN4 DeepSpeech model (``--dnn lstman4``) only."""
+    if args.fused_lstm and model_args(args)[0] != "lstman4":
+        parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
+
+
 def main(argv=None) -> int:
     parser = build_parser()
     args = parser.parse_args(argv)
@@ -139,6 +150,7 @@ def main(argv=None) -> int:
         parser.error("--fused-bn-fp16 needs --fp16")
     check_fused_bn_args(parser, args)
     check_fused_ln_args(parser, args)
+    check_fused_lstm_args(parser, args)
     import oktopk_b200 as okt
     from .trainer import preset_for, robust_ssgd
     okt.init()
