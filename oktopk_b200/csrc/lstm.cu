@@ -1,4 +1,4 @@
-// Persistent LSTM recurrence (fp32, time-major T x N, torch's gate order i, f, g, o, zero initial state):
+// Persistent LSTM recurrence (time-major T x N, torch's gate order i, f, g, o, zero initial state):
 //
 //   a_t = gx_t + W_hh h_{t-1}                  gx = x W_ih^T + b_ih + b_hh for all t: one GEMM in torch beforehand
 //   i, f, o = sigmoid(a_i, a_f, a_o), g = tanh(a_g),   c_t = f c_{t-1} + i g,   h_t = o tanh(c_t)
@@ -25,8 +25,18 @@
 // dependency being the whole of y_t (dgates_t), which every CTA reads.  Operands written by other CTAs in this launch
 // are read with ld.global.cg (L2), never through L1.
 //
-// Every sum has a fixed order: lane l of a warp adds the float4 columns l, l + 32, ... of a dot product in order, and the
-// 32 lanes are combined by a fixed butterfly.  No atomics touch data, so results are bitwise reproducible.
+// Every sum has a fixed order: lane l of a warp adds the four-element columns l, l + 32, ... of a dot product in order,
+// and the 32 lanes are combined by a fixed butterfly.  No atomics touch data, so results are bitwise reproducible.
+//
+// Storage type S (float, __nv_bfloat16 or __half) is that of the five tensors that are 16-bit under autocast: W_hh (in
+// global and in shared memory), gx, y, dy and dgates, and so of the staged h_{t-1} and dgates_{t+1}.  The saved gates and
+// c, the gate and dh sums, the cell state, the carried dc and every accumulator are fp32 whatever S is.  A 16-bit
+// element is widened on load and enters the same fmaf chain in the same order, so a 16-bit launch is the fp32 kernel run
+// on the widened operands, except where a y or dgates it stored (rounded to nearest even, not saturated: an fp16
+// overflow is inf) is read back at the next step.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "oktopk.cuh"
 
@@ -36,58 +46,98 @@ constexpr int kLstmThreads = 512;                // ops/fused_lstm.py LSTM_THREA
 constexpr int kLstmWarps = kLstmThreads / 32;
 constexpr int kLstmNB = 4;                       // batch rows of one warp task in lstm_dots
 
+template <typename S>
 struct LstmFwdArgs {
-    const float* gx;
-    const float* whh;
+    const S* gx;
+    const S* whh;
     const int* len;
-    float* y;
+    S* y;
     float* gates;
     float* cs;
     unsigned long long* bar;
     int T, N, H, u, rows;
 };
 
+template <typename S>
 struct LstmBwdArgs {
-    const float* dy;
+    const S* dy;
     const float* gates;
     const float* cs;
-    const float* whh;
+    const S* whh;
     const int* len;
-    float* dg;
+    S* dg;
     unsigned long long* bar;
     int T, N, H, u, rows;
 };
 
 __device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
-// Copy `nrows` rows of K floats (K % 4 == 0, 16-byte aligned) that other CTAs wrote in this launch to shared memory.
-__device__ __forceinline__ void lstm_stage(float* __restrict__ sV, const float* __restrict__ g, int nrows, int K) {
-    float4* d = reinterpret_cast<float4*>(sV);
-    const float4* s = reinterpret_cast<const float4*>(g);
+// Storage type S: Vec holds four elements (16 bytes of float, 8 bytes of a 16-bit type), widen() makes them floats,
+// narrow() rounds one float to nearest even without saturating.
+template <typename S> struct LstmEl;
+template <> struct LstmEl<float> {
+    using Vec = float4;
+    static __device__ __forceinline__ Vec zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+    static __device__ __forceinline__ float4 widen(const Vec& v) { return v; }
+    static __device__ __forceinline__ float ld(const float* p) { return __ldg(p); }
+    static __device__ __forceinline__ float narrow(float v) { return v; }
+};
+template <> struct LstmEl<__nv_bfloat16> {
+    using Vec = uint2;
+    static __device__ __forceinline__ Vec zero() { return make_uint2(0u, 0u); }
+    static __device__ __forceinline__ float4 widen(const Vec& v) {
+        const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.x));
+        const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.y));
+        return make_float4(lo.x, lo.y, hi.x, hi.y);
+    }
+    static __device__ __forceinline__ float ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+    static __device__ __forceinline__ __nv_bfloat16 narrow(float v) { return __float2bfloat16_rn(v); }
+};
+template <> struct LstmEl<__half> {
+    using Vec = uint2;
+    static __device__ __forceinline__ Vec zero() { return make_uint2(0u, 0u); }
+    static __device__ __forceinline__ float4 widen(const Vec& v) {
+        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+        return make_float4(lo.x, lo.y, hi.x, hi.y);
+    }
+    static __device__ __forceinline__ float ld(const __half* p) { return __half2float(__ldg(p)); }
+    static __device__ __forceinline__ __half narrow(float v) { return __float2half_rn(v); }
+};
+
+// Copy `nrows` rows of K elements (K % 4 == 0, Vec-aligned) that other CTAs wrote in this launch to shared memory.
+template <typename S>
+__device__ __forceinline__ void lstm_stage(S* __restrict__ sV, const S* __restrict__ g, int nrows, int K) {
+    using Vec = typename LstmEl<S>::Vec;
+    Vec* d = reinterpret_cast<Vec*>(sV);
+    const Vec* s = reinterpret_cast<const Vec*>(g);
     const int n4 = nrows * (K >> 2);
     for (int i = threadIdx.x; i < n4; i += kLstmThreads) d[i] = __ldcg(s + i);
 }
 
 // out[r N + n0 + j] = sum_k sW[r K + k] sV[j K + k] for r < R, j < nc.  A warp takes one (r, kLstmNB rows of sV) task at
 // a time; the order of every sum is fixed (see the file header), whichever warp runs it.
-__device__ __forceinline__ void lstm_dots(const float* __restrict__ sW, const float* __restrict__ sV,
+template <typename S>
+__device__ __forceinline__ void lstm_dots(const S* __restrict__ sW, const S* __restrict__ sV,
                                           float* __restrict__ out, int R, int K, int nc, int n0, int N) {
+    using El = LstmEl<S>;
+    using Vec = typename El::Vec;
     const int K4 = K >> 2, lane = lane_id(), warp = threadIdx.x >> 5;
     const int nb = (nc + kLstmNB - 1) / kLstmNB;
-    const float4* W4 = reinterpret_cast<const float4*>(sW);
-    const float4* V4 = reinterpret_cast<const float4*>(sV);
+    const Vec* W4 = reinterpret_cast<const Vec*>(sW);
+    const Vec* V4 = reinterpret_cast<const Vec*>(sV);
     for (int task = warp; task < R * nb; task += kLstmWarps) {
         const int r = task / nb, j0 = (task - r * nb) * kLstmNB;
-        const float4* w = W4 + (size_t)r * K4;
+        const Vec* w = W4 + (size_t)r * K4;
         float acc[kLstmNB];
 #pragma unroll
         for (int j = 0; j < kLstmNB; ++j) acc[j] = 0.f;
         for (int k = lane; k < K4; k += 32) {
-            const float4 a = w[k];
+            const float4 a = El::widen(w[k]);
 #pragma unroll
             for (int j = 0; j < kLstmNB; ++j) {
                 if (j0 + j < nc) {
-                    const float4 b = V4[(size_t)(j0 + j) * K4 + k];
+                    const float4 b = El::widen(V4[(size_t)(j0 + j) * K4 + k]);
                     acc[j] = fmaf(a.x, b.x, acc[j]);
                     acc[j] = fmaf(a.y, b.y, acc[j]);
                     acc[j] = fmaf(a.z, b.z, acc[j]);
@@ -106,7 +156,8 @@ __device__ __forceinline__ void lstm_dots(const float* __restrict__ sW, const fl
 }
 
 // out[r N + n] = sum_k sW[r K + k] V[n K + k] over all N rows of V (global, written in this launch), `rows` at a time.
-__device__ __forceinline__ void lstm_matvec(const float* __restrict__ sW, float* __restrict__ sV, const float* V,
+template <typename S>
+__device__ __forceinline__ void lstm_matvec(const S* __restrict__ sW, S* __restrict__ sV, const S* V,
                                             float* __restrict__ out, int R, int K, int N, int rows) {
     for (int n0 = 0; n0 < N; n0 += rows) {
         const int nc = min(rows, N - n0);
@@ -117,20 +168,24 @@ __device__ __forceinline__ void lstm_matvec(const float* __restrict__ sW, float*
     }
 }
 
-// Shared memory: W [4u][H] | h_{t-1} rows [rows][H] | gate sums [4u][N] | c [u][N].
-__global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwdArgs p) {
+// Shared memory: W [4u][H] and h_{t-1} rows [rows][H] of S | gate sums [4u][N] | c [u][N] of float.  H % 4 == 0 makes
+// the two S sections multiples of 8 bytes, so the float sections are aligned for either S.
+template <typename S>
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwdArgs<S> p) {
+    using El = LstmEl<S>;
+    using Vec = typename El::Vec;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2;
     const int u0 = blockIdx.x * u, nu = min(u, H - u0);
-    float* sW = reinterpret_cast<float*>(lstm_smem);
-    float* sV = sW + (size_t)R * H;
-    float* sG = sV + (size_t)p.rows * H;
+    S* sW = reinterpret_cast<S*>(lstm_smem);
+    S* sV = sW + (size_t)R * H;
+    float* sG = reinterpret_cast<float*>(sV + (size_t)p.rows * H);
     float* sC = sG + R * N;
     for (int i = threadIdx.x; i < R * H4; i += kLstmThreads) {      // local row q u + j = W_hh row q H + u0 + j
         const int lr = i / H4, k = i - lr * H4, q = lr / u, j = lr - q * u;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < nu) v = __ldg(reinterpret_cast<const float4*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
-        reinterpret_cast<float4*>(sW)[i] = v;
+        Vec v = El::zero();
+        if (j < nu) v = __ldg(reinterpret_cast<const Vec*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
+        reinterpret_cast<Vec*>(sW)[i] = v;
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sC[i] = 0.f;
     for (int t = 0; t < p.T; ++t) {
@@ -143,41 +198,43 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
         for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
             const int j = i / N, n = i - j * N, unit = u0 + j;
             const size_t row = (size_t)t * N + n;
-            const float* gx = p.gx + row * 4 * H + unit;
+            const S* gx = p.gx + row * 4 * H + unit;
             float* gs = p.gates + row * 4 * H + unit;
             const size_t o = row * H + unit;
             if (t < __ldg(p.len + n)) {
-                const float gi = lstm_sigmoid(sG[(0 * u + j) * N + n] + __ldg(gx));
-                const float gf = lstm_sigmoid(sG[(1 * u + j) * N + n] + __ldg(gx + H));
-                const float gg = tanhf(sG[(2 * u + j) * N + n] + __ldg(gx + 2 * H));
-                const float go = lstm_sigmoid(sG[(3 * u + j) * N + n] + __ldg(gx + 3 * H));
+                const float gi = lstm_sigmoid(sG[(0 * u + j) * N + n] + El::ld(gx));
+                const float gf = lstm_sigmoid(sG[(1 * u + j) * N + n] + El::ld(gx + H));
+                const float gg = tanhf(sG[(2 * u + j) * N + n] + El::ld(gx + 2 * H));
+                const float go = lstm_sigmoid(sG[(3 * u + j) * N + n] + El::ld(gx + 3 * H));
                 const float c = gf * sC[j * N + n] + gi * gg;
                 sC[j * N + n] = c;
                 gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
                 p.cs[o] = c;
-                p.y[o] = go * tanhf(c);
+                p.y[o] = El::narrow(go * tanhf(c));
             } else {
                 gs[0] = 0.f; gs[H] = 0.f; gs[2 * H] = 0.f; gs[3 * H] = 0.f;
                 p.cs[o] = 0.f;
-                p.y[o] = 0.f;
+                p.y[o] = El::narrow(0.f);
             }
         }
         if (t + 1 < p.T) grid_sync(p.bar);
     }
 }
 
-// Shared memory: W^T [u][4H] | dgates_{t+1} rows [rows][4H] | dh_rec [u][N] | carried dc [u][N].
-__global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwdArgs p) {
+// Shared memory: W^T [u][4H] and dgates_{t+1} rows [rows][4H] of S | dh_rec [u][N] | carried dc [u][N] of float.
+template <typename S>
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwdArgs<S> p) {
+    using El = LstmEl<S>;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, G = 4 * H;
     const int u0 = blockIdx.x * u, nu = min(u, H - u0);
-    float* sW = reinterpret_cast<float*>(lstm_smem);
-    float* sV = sW + (size_t)u * G;
-    float* sD = sV + (size_t)p.rows * G;
+    S* sW = reinterpret_cast<S*>(lstm_smem);
+    S* sV = sW + (size_t)u * G;
+    float* sD = reinterpret_cast<float*>(sV + (size_t)p.rows * G);
     float* sDC = sD + u * N;
     for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
         const int k = i / u, j = i - k * u;
-        sW[(size_t)j * G + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : 0.f;
+        sW[(size_t)j * G + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : El::narrow(0.f);
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sDC[i] = 0.f;
     for (int t = p.T - 1; t >= 0; --t) {
@@ -191,21 +248,21 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
             const int j = i / N, n = i - j * N, unit = u0 + j;
             const size_t row = (size_t)t * N + n;
             const size_t o = row * H + unit;
-            float* dg = p.dg + row * G + unit;
+            S* dg = p.dg + row * G + unit;
             if (t < __ldg(p.len + n)) {
                 const float* gs = p.gates + row * G + unit;
                 const float gi = __ldg(gs), gf = __ldg(gs + H), gg = __ldg(gs + 2 * H), go = __ldg(gs + 3 * H);
                 const float tc = tanhf(__ldg(p.cs + o));
                 const float cp = t > 0 ? __ldg(p.cs + o - (size_t)N * H) : 0.f;
-                const float dh = __ldg(p.dy + o) + sD[j * N + n];
+                const float dh = El::ld(p.dy + o) + sD[j * N + n];
                 const float dc = dh * go * (1.f - tc * tc) + sDC[j * N + n];
-                dg[0] = dc * gg * gi * (1.f - gi);
-                dg[H] = dc * cp * gf * (1.f - gf);
-                dg[2 * H] = dc * gi * (1.f - gg * gg);
-                dg[3 * H] = dh * tc * go * (1.f - go);
+                dg[0] = El::narrow(dc * gg * gi * (1.f - gi));
+                dg[H] = El::narrow(dc * cp * gf * (1.f - gf));
+                dg[2 * H] = El::narrow(dc * gi * (1.f - gg * gg));
+                dg[3 * H] = El::narrow(dh * tc * go * (1.f - go));
                 sDC[j * N + n] = dc * gf;
             } else {
-                dg[0] = 0.f; dg[H] = 0.f; dg[2 * H] = 0.f; dg[3 * H] = 0.f;
+                dg[0] = dg[H] = dg[2 * H] = dg[3 * H] = El::narrow(0.f);
                 sDC[j * N + n] = 0.f;
             }
         }
@@ -227,7 +284,7 @@ struct LstmLaunchCache {
 // Cooperative launch of `grid` CTAs with `smem` bytes each; an error if they cannot all be co-resident.
 template <typename Args>
 static cudaError_t lstm_launch(void (*kernel)(const Args), const Args& p, int grid, size_t smem, cudaStream_t stream) {
-    static LstmLaunchCache cache[kLstmMaxDevices];             // one table per kernel: Args differs between the two
+    static LstmLaunchCache cache[kLstmMaxDevices];             // one table per kernel: Args differs between all six
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
@@ -262,21 +319,49 @@ static bool lstm_shape_ok(int T, int N, int H, int u, int rows) {
     return T > 0 && N > 0 && H > 0 && H % 4 == 0 && u > 0 && u <= H && rows > 0 && rows <= N;
 }
 
-cudaError_t launch_lstm_forward(const float* gx, const float* whh, const int* len, float* y, float* gates, float* cs,
-                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream) {
-    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    const LstmFwdArgs p{gx, whh, len, y, gates, cs, bar, T, N, H, u, rows};
-    const size_t smem = sizeof(float) * ((size_t)4 * u * H + (size_t)rows * H + (size_t)5 * u * N);
-    return lstm_launch(lstm_fwd_kernel, p, (H + u - 1) / u, smem, stream);
+template <typename S>
+static cudaError_t lstm_forward_t(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
+                                  unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream) {
+    const LstmFwdArgs<S> p{static_cast<const S*>(gx), static_cast<const S*>(whh), len, static_cast<S*>(y), gates, cs, bar,
+                           T, N, H, u, rows};
+    const size_t smem = sizeof(S) * ((size_t)4 * u * H + (size_t)rows * H) + sizeof(float) * (size_t)5 * u * N;
+    return lstm_launch(lstm_fwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
 }
 
-cudaError_t launch_lstm_backward(const float* dy, const float* gates, const float* cs, const float* whh, const int* len,
-                                 float* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                 cudaStream_t stream) {
+template <typename S>
+static cudaError_t lstm_backward_t(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
+                                   void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                   cudaStream_t stream) {
+    const LstmBwdArgs<S> p{static_cast<const S*>(dy), gates, cs, static_cast<const S*>(whh), len, static_cast<S*>(dg), bar,
+                           T, N, H, u, rows};
+    const size_t smem = sizeof(S) * ((size_t)4 * u * H + (size_t)rows * 4 * H) + sizeof(float) * (size_t)2 * u * N;
+    return lstm_launch(lstm_bwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
+}
+
+cudaError_t launch_lstm_forward(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
+                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
+                                BnDtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    const LstmBwdArgs p{dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows};
-    const size_t smem = sizeof(float) * ((size_t)4 * u * H + (size_t)rows * 4 * H + (size_t)2 * u * N);
-    return lstm_launch(lstm_bwd_kernel, p, (H + u - 1) / u, smem, stream);
+    switch (dtype) {
+        case BnDtype::kF32: return lstm_forward_t<float>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+        case BnDtype::kBF16:
+            return lstm_forward_t<__nv_bfloat16>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF16: return lstm_forward_t<__half>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
+                                 void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                 cudaStream_t stream, BnDtype dtype) {
+    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
+    switch (dtype) {
+        case BnDtype::kF32: return lstm_backward_t<float>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
+        case BnDtype::kBF16:
+            return lstm_backward_t<__nv_bfloat16>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF16: return lstm_backward_t<__half>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
+    }
+    return cudaErrorInvalidValue;
 }
 
 }  // namespace okt

@@ -381,15 +381,17 @@ cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, f
                                 long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
 cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
                                  long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
-// persistent LSTM recurrence, fp32, time-major (csrc/lstm.cu): one cooperative launch per pass, ceil(H / u) CTAs of u
-// hidden units each, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H] (the
-// input projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg
-// [T, N, 4H].  `bar` is a zeroed 64-bit grid-barrier counter.  whh, y and dg 16-byte aligned, H % 4 == 0.
-cudaError_t launch_lstm_forward(const float* gx, const float* whh, const int* len, float* y, float* gates, float* cs,
-                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream);
-cudaError_t launch_lstm_backward(const float* dy, const float* gates, const float* cs, const float* whh, const int* len,
-                                 float* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                 cudaStream_t stream);
+// persistent LSTM recurrence, time-major (csrc/lstm.cu): one cooperative launch per pass, ceil(H / u) CTAs of u hidden
+// units each, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H] (the input
+// projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg
+// [T, N, 4H].  gx, whh, y, dy and dg are of type `dtype` (BnDtype's codes); gates and cs are fp32.  `bar` is a zeroed
+// 64-bit grid-barrier counter.  whh, y and dg aligned to four elements (16 bytes in fp32, 8 in bf16 / fp16), H % 4 == 0.
+cudaError_t launch_lstm_forward(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
+                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
+                                BnDtype dtype);
+cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
+                                 void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                 cudaStream_t stream, BnDtype dtype);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
 cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
 cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);

@@ -24,7 +24,7 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
     ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``); for BERT,
     ``fuse_ln=True`` turns on ``net.fuse_ln`` and ``fuse_xent=True`` ``net.fuse_xent``; for ``lstman4``,
-    ``fuse_lstm=True`` turns on ``net.fuse_lstm``."""
+    ``fuse_lstm=True`` turns on ``net.fuse_lstm`` and ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast``."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):

@@ -9,7 +9,8 @@ logits (softmax only in eval mode) + output lengths; trained with CTC.
 
 ``fuse_lstm=True`` (or ``net.fuse_lstm = True`` at any time) runs the uni-directional LSTM layers on the persistent
 recurrence kernels of ``ops/fused_lstm.py`` instead of packing the sequences for cuDNN; parameters, buffers and
-``state_dict`` keys are the same either way.
+``state_dict`` keys are the same either way.  Under bf16 / fp16 autocast those layers are stock again unless
+``fuse_lstm_autocast=True`` (``net.fuse_lstm_autocast``) is set as well, which runs the 16-bit forms of the kernels.
 """
 from __future__ import annotations
 
@@ -56,13 +57,15 @@ class _SeqBN(nn.Module):
 
 class BatchRNN(nn.Module):
     """``fuse`` (default off) runs the recurrence through ``ops/fused_lstm.lstm_layer``, which falls back to the stock
-    pack -> rnn -> pad sequence wherever its kernels do not apply."""
+    pack -> rnn -> pad sequence wherever its kernels do not apply; with ``fuse_autocast`` (default off) it takes the
+    16-bit kernels under bf16 / fp16 autocast, where ``fuse`` alone is stock."""
 
     def __init__(self, input_size: int, hidden_size: int, rnn_type=nn.LSTM, bidirectional: bool = False,
-                 batch_norm: bool = True, fuse: bool = False):
+                 batch_norm: bool = True, fuse: bool = False, fuse_autocast: bool = False):
         super().__init__()
         self.bidirectional = bidirectional
         self.fuse = fuse
+        self.fuse_autocast = fuse_autocast
         self.batch_norm = _SeqBN(nn.BatchNorm1d(input_size)) if batch_norm else None
         self.rnn = rnn_type(input_size=input_size, hidden_size=hidden_size, bidirectional=bidirectional, bias=True)
 
@@ -71,7 +74,7 @@ class BatchRNN(nn.Module):
         if self.batch_norm is not None:
             x = self.batch_norm(x)
         if self.fuse:
-            return lstm_layer(x, lengths, self.rnn, dev_lengths)
+            return lstm_layer(x, lengths, self.rnn, dev_lengths, autocast=self.fuse_autocast)
         return stock_layer(x, lengths, self.rnn)
 
 
@@ -96,7 +99,7 @@ class Lookahead(nn.Module):
 class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
-                 window_size: float = 0.02, fuse_lstm: bool = False):
+                 window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -119,6 +122,7 @@ class DeepSpeech(nn.Module):
         self.fc = _SeqBN(nn.Sequential(nn.BatchNorm1d(rnn_hidden_size),
                                        nn.Linear(rnn_hidden_size, num_classes, bias=False)))
         self.fuse_lstm = fuse_lstm
+        self.fuse_lstm_autocast = fuse_lstm_autocast
 
     @property
     def fuse_lstm(self) -> bool:
@@ -129,6 +133,16 @@ class DeepSpeech(nn.Module):
     def fuse_lstm(self, on: bool) -> None:
         for m in self.rnns:
             m.fuse = bool(on)
+
+    @property
+    def fuse_lstm_autocast(self) -> bool:
+        """Whether every fused ``BatchRNN`` layer keeps its kernels (their 16-bit forms) under bf16 / fp16 autocast."""
+        return all(m.fuse_autocast for m in self.rnns)
+
+    @fuse_lstm_autocast.setter
+    def fuse_lstm_autocast(self, on: bool) -> None:
+        for m in self.rnns:
+            m.fuse_autocast = bool(on)
 
     def get_seq_lens(self, input_length: torch.Tensor) -> torch.Tensor:
         seq = input_length
@@ -155,10 +169,10 @@ class DeepSpeech(nn.Module):
 
 
 def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
-            fuse_lstm: bool = False) -> DeepSpeech:
+            fuse_lstm: bool = False, fuse_lstm_autocast: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
     return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
-                      fuse_lstm=fuse_lstm)
+                      fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast)
 
 
 class PTBLSTM(nn.Module):
