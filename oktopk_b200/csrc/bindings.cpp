@@ -578,6 +578,33 @@ static void xent_backward(uint64_t x, uint64_t t, uint64_t lse, uint64_t g, uint
     ck(launch_xent_backward(P_<const void>(x), P_<const long long>(t), P_<const float>(lse), P_<const float>(g), P_<void>(dx),
                             R, V, ignore_index, bn_dtype(dtype, "xent_backward"), S_(stream)), "xent_backward");
 }
+// Fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels [R] int64, rows [M] int32, tgt [M]
+// int64, slot [R] int32, count one int64, overflow one int64 or 0; x / dx [R, H] and out / dout [M, H] of type dtype.
+static void mlm_select(uint64_t labels, uint64_t rows, uint64_t tgt, uint64_t slot, uint64_t count, uint64_t overflow,
+                       int R, int M, long long ignore_index, uint64_t stream) {
+    if (R <= 0 || M <= 0) throw std::runtime_error("mlm_select: needs R > 0 and M > 0");
+    if (!labels || !rows || !tgt || !slot || !count) throw std::runtime_error("mlm_select: null pointer");
+    if ((labels & 7) || (tgt & 7) || (count & 7) || (overflow & 7) || (rows & 3) || (slot & 3))
+        throw std::runtime_error("mlm_select: misaligned pointer");
+    ck(launch_mlm_select(P_<const long long>(labels), R, ignore_index, M, P_<int>(rows), P_<long long>(tgt),
+                         P_<int>(slot), P_<long long>(count), P_<long long>(overflow), S_(stream)), "mlm_select");
+}
+static void mlm_copy_check(const char* what, int nrows, int H, uint64_t src, uint64_t idx, uint64_t dst, BnDtype dt) {
+    if (nrows <= 0 || H <= 0) throw std::runtime_error(std::string(what) + ": needs rows > 0 and H > 0");
+    if (!src || !idx || !dst) throw std::runtime_error(std::string(what) + ": null pointer");
+    const uint64_t mask = dt == BnDtype::kF32 ? 3 : 1;
+    if ((src & mask) || (dst & mask) || (idx & 3)) throw std::runtime_error(std::string(what) + ": misaligned pointer");
+}
+static void mlm_gather(uint64_t x, uint64_t rows, uint64_t out, int M, int H, int dtype, uint64_t stream) {
+    const BnDtype dt = bn_dtype(dtype, "mlm_gather");
+    mlm_copy_check("mlm_gather", M, H, x, rows, out, dt);
+    ck(launch_mlm_gather(P_<const void>(x), P_<const int>(rows), P_<void>(out), M, H, dt, S_(stream)), "mlm_gather");
+}
+static void mlm_scatter(uint64_t dout, uint64_t slot, uint64_t dx, int R, int H, int dtype, uint64_t stream) {
+    const BnDtype dt = bn_dtype(dtype, "mlm_scatter");
+    mlm_copy_check("mlm_scatter", R, H, dout, slot, dx, dt);
+    ck(launch_mlm_scatter(P_<const void>(dout), P_<const int>(slot), P_<void>(dx), R, H, dt, S_(stream)), "mlm_scatter");
+}
 // Persistent LSTM recurrence (csrc/lstm.cu), time-major: gx [T, N, 4H], whh [4H, H], len [N] int32 in [1, T],
 // y / cs [T, N, H], gates / dy / dg as named; bar: one zeroed int64.  u hidden units per CTA, `rows` batch rows staged at
 // a time (ops/fused_lstm.lstm_geometry).  gx, whh, y, dy and dg are of type dtype (codes as bn_dtype), gates and cs fp32.
@@ -748,6 +775,12 @@ PYBIND11_MODULE(_C, m) {
           py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
     m.def("xent_backward", &xent_backward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("g"), py::arg("dx"),
           py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
+    m.def("mlm_select", &mlm_select, py::arg("labels"), py::arg("rows"), py::arg("tgt"), py::arg("slot"), py::arg("count"),
+          py::arg("overflow"), py::arg("R"), py::arg("M"), py::arg("ignore_index"), py::arg("stream"));
+    m.def("mlm_gather", &mlm_gather, py::arg("x"), py::arg("rows"), py::arg("out"), py::arg("M"), py::arg("H"),
+          py::arg("dtype"), py::arg("stream"));
+    m.def("mlm_scatter", &mlm_scatter, py::arg("dout"), py::arg("slot"), py::arg("dx"), py::arg("R"), py::arg("H"),
+          py::arg("dtype"), py::arg("stream"));
     m.def("lstm_forward", &lstm_forward, py::arg("gx"), py::arg("whh"), py::arg("len"), py::arg("y"), py::arg("gates"),
           py::arg("cs"), py::arg("bar"), py::arg("T"), py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"),
           py::arg("stream"), py::arg("dtype") = 0);

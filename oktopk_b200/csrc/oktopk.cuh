@@ -381,6 +381,14 @@ cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, f
                                 long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
 cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
                                  long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
+// fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels and tgt int64, rows [M] and slot
+// [R] int32, count one int64, overflow one int64 that accumulates max(count - M, 0) (or null); x [R, H] and out [M, H],
+// dout [M, H] and dx [R, H] of type `dtype` (BnDtype's codes).  One launch each.
+cudaError_t launch_mlm_select(const long long* labels, int R, long long ignore_index, int M, int* rows, long long* tgt,
+                              int* slot, long long* count, long long* overflow, cudaStream_t stream);
+cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, int H, BnDtype dtype, cudaStream_t stream);
+cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, BnDtype dtype,
+                               cudaStream_t stream);
 // persistent LSTM recurrence, time-major (csrc/lstm.cu): one cooperative launch per pass, ceil(H / u) CTAs of u hidden
 // units each, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H] (the input
 // projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg

@@ -9,14 +9,15 @@ parameter, ``depth=4/__init__.py:17``) => BERT-base has 133,547,324 parameters, 
 Fresh implementation: fused QKV projection, ``F.scaled_dot_product_attention`` (the reference does
 matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm`` instead of apex, or with
 ``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``, and
-with ``fuse_xent=True`` the masked-LM loss on the fused softmax cross-entropy of ``ops/fused_xent.py``.
+with ``fuse_xent=True`` the masked-LM loss on the fused softmax cross-entropy of ``ops/fused_xent.py``, and with
+``sparse_mlm=True`` the masked-LM head on the labelled rows only, gathered by ``ops/mlm_gather.py``.
 """
 from __future__ import annotations
 
 import json
 import math
 from dataclasses import dataclass
-from typing import List, Optional, Tuple
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
@@ -125,7 +126,13 @@ class BertPooler(nn.Module):
 
 class BertPreTrainingHeads(nn.Module):
     """MLM head (dense + act + LN + decoder) and NSP head.  ``decoder_weight`` is an independent
-    ``[vocab, hidden]`` parameter (untied, see module docstring) plus a vocab-sized bias."""
+    ``[vocab, hidden]`` parameter (untied, see module docstring) plus a vocab-sized bias.
+
+    ``forward(seq, pooled)`` returns ``(scores [B, S, V], nsp)``.  Given the masked-LM labels ``[B, S]`` (-1 = not
+    masked) it also returns the targets of the scores' rows: with ``sparse_mlm`` off ``(scores [B, S, V], nsp,
+    labels)``; with it on the MLM head runs on the labelled rows only, gathered by ``ops/mlm_gather.py`` into
+    ``capacity_rows(B S, mlm_capacity)`` rows, and returns ``(scores [M, V], nsp, tgt [M])``.  Labelled rows past the
+    capacity are left out of the loss and counted in the non-persistent buffer ``mlm_overflow``."""
 
     def __init__(self, c: BertConfig):
         super().__init__()
@@ -135,10 +142,20 @@ class BertPreTrainingHeads(nn.Module):
         self.decoder_weight = nn.Parameter(torch.empty(c.vocab_size, c.hidden_size).normal_(std=c.initializer_range))
         self.decoder_bias = nn.Parameter(torch.zeros(c.vocab_size))
         self.seq_relationship = nn.Linear(c.hidden_size, 2)
+        self.sparse_mlm = False
+        self.mlm_capacity = 0.25
+        self.register_buffer("mlm_overflow", torch.zeros(1, dtype=torch.int64), persistent=False)
 
-    def forward(self, seq: torch.Tensor, pooled: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    def forward(self, seq: torch.Tensor, pooled: torch.Tensor, labels: Optional[torch.Tensor] = None):
+        if labels is not None and self.sparse_mlm:
+            from ..ops.mlm_gather import capacity_rows, gather_labelled
+            m = capacity_rows(labels.numel(), self.mlm_capacity)
+            xg, tgt = gather_labelled(seq.reshape(-1, seq.size(-1)), labels.reshape(-1), m, -1, self.mlm_overflow)
+            h = self.transform_norm(self.act(self.transform(xg)))
+            return F.linear(h, self.decoder_weight, self.decoder_bias), self.seq_relationship(pooled), tgt
         h = self.transform_norm(self.act(self.transform(seq)))
-        return F.linear(h, self.decoder_weight, self.decoder_bias), self.seq_relationship(pooled)
+        scores, nsp = F.linear(h, self.decoder_weight, self.decoder_bias), self.seq_relationship(pooled)
+        return (scores, nsp) if labels is None else (scores, nsp, labels)
 
 
 def extended_attention_mask(input_mask: torch.Tensor, dtype=torch.float32) -> torch.Tensor:
@@ -178,10 +195,10 @@ class EndingStage(nn.Module):
         self.pooler = BertPooler(c)
         self.heads = BertPreTrainingHeads(c)
 
-    def forward(self, x, mask):
+    def forward(self, x, mask, labels=None):
         for l in self.layers:
             x = l(x, mask)
-        return self.heads(x, self.pooler(x))
+        return self.heads(x, self.pooler(x), labels)
 
 
 def build_stages(c: BertConfig, depth: int = 4) -> List[nn.Module]:
@@ -215,10 +232,12 @@ class PretrainingCriterion(nn.Module):
 
 class BertForPreTraining(nn.Module):
     """``fuse_ln=True`` (or ``net.fuse_ln = True`` at any time) sets ``BertLayer.fuse_ln`` on every encoder layer;
-    ``fuse_xent=True`` (or ``net.fuse_xent``) sets ``PretrainingCriterion.fuse_xent``."""
+    ``fuse_xent=True`` (or ``net.fuse_xent``) sets ``PretrainingCriterion.fuse_xent``; ``sparse_mlm=True`` (or
+    ``net.sparse_mlm``) runs the masked-LM head on the labelled rows only when labels are given, gathered into
+    ``mlm_capacity`` (or ``net.mlm_capacity``) times B·S rows, rounded up to a multiple of 8 (``BertPreTrainingHeads``)."""
 
     def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False,
-                 fuse_ln: bool = False, fuse_xent: bool = False):
+                 fuse_ln: bool = False, fuse_xent: bool = False, sparse_mlm: bool = False, mlm_capacity: float = 0.25):
         super().__init__()
         self.config = config or BertConfig()
         self.recompute = recompute           # ``--recompute_step`` (BERT/runtime.py:546-557, modeling.py:414-431)
@@ -228,6 +247,28 @@ class BertForPreTraining(nn.Module):
         nn.init.normal_(self.stages[-1].heads.decoder_weight, std=self.config.initializer_range)
         self.fuse_ln = fuse_ln
         self.fuse_xent = fuse_xent
+        self.sparse_mlm = sparse_mlm
+        self.mlm_capacity = mlm_capacity
+
+    @property
+    def sparse_mlm(self) -> bool:
+        """True when the masked-LM head runs on the gathered labelled rows only."""
+        return self.stages[-1].heads.sparse_mlm
+
+    @sparse_mlm.setter
+    def sparse_mlm(self, on: bool) -> None:
+        self.stages[-1].heads.sparse_mlm = bool(on)
+
+    @property
+    def mlm_capacity(self) -> float:
+        """The gathered rows of the sparse masked-LM head, as a fraction of the batch's B·S token rows."""
+        return self.stages[-1].heads.mlm_capacity
+
+    @mlm_capacity.setter
+    def mlm_capacity(self, fraction: float) -> None:
+        from ..ops.mlm_gather import capacity_rows
+        capacity_rows(1, fraction)                           # validates: 0 < fraction <= 1
+        self.stages[-1].heads.mlm_capacity = float(fraction)
 
     @property
     def fuse_xent(self) -> bool:
@@ -270,6 +311,9 @@ class BertForPreTraining(nn.Module):
                 x = checkpoint(st, x, mask, use_reentrant=False)
             else:
                 x = st(x, mask)
+        if self.sparse_mlm and masked_lm_labels is not None and next_sentence_label is not None:
+            scores, nsp, tgt = self.stages[-1](x, mask, masked_lm_labels)
+            return self.criterion(scores, nsp, tgt, next_sentence_label)
         scores, nsp = self.stages[-1](x, mask)
         if masked_lm_labels is not None and next_sentence_label is not None:
             return self.criterion(scores, nsp, masked_lm_labels, next_sentence_label)

@@ -164,19 +164,41 @@ class BertForQuestionAnswering(_Head):
 
 class BertForMaskedLM(_Head):
     """``fuse_xent`` (default off, a run-time switch) computes the loss with the fused softmax cross-entropy of
-    ``ops/fused_xent.py``."""
+    ``ops/fused_xent.py``; ``sparse_mlm`` (default off, a run-time switch) runs the head on the labelled rows only,
+    gathered into ``mlm_capacity`` times B·S rows, when labels are given (``BertPreTrainingHeads``)."""
 
-    def __init__(self, config: Optional[BertConfig] = None, fuse_xent: bool = False):
+    def __init__(self, config: Optional[BertConfig] = None, fuse_xent: bool = False, sparse_mlm: bool = False,
+                 mlm_capacity: float = 0.25):
         super().__init__(config)
         self.heads = BertPreTrainingHeads(self.config)
         self.fuse_xent = fuse_xent
+        self.sparse_mlm = sparse_mlm
+        self.mlm_capacity = mlm_capacity
+
+    @property
+    def sparse_mlm(self) -> bool:
+        return self.heads.sparse_mlm
+
+    @sparse_mlm.setter
+    def sparse_mlm(self, on: bool) -> None:
+        self.heads.sparse_mlm = bool(on)
+
+    @property
+    def mlm_capacity(self) -> float:
+        return self.heads.mlm_capacity
+
+    @mlm_capacity.setter
+    def mlm_capacity(self, fraction: float) -> None:
+        from ..ops.mlm_gather import capacity_rows
+        capacity_rows(1, fraction)                           # validates: 0 < fraction <= 1
+        self.heads.mlm_capacity = float(fraction)
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None, masked_lm_labels=None):
         seq, pooled = self.bert(input_ids, token_type_ids, attention_mask)
-        scores, _ = self.heads(seq, pooled)
         if masked_lm_labels is None:
-            return scores
-        scores, labels = scores.view(-1, self.config.vocab_size), masked_lm_labels.view(-1)
+            return self.heads(seq, pooled)[0]
+        scores, _, labels = self.heads(seq, pooled, masked_lm_labels)
+        scores, labels = scores.view(-1, self.config.vocab_size), labels.view(-1)
         if self.fuse_xent:
             from ..ops.fused_xent import softmax_cross_entropy
             return softmax_cross_entropy(scores, labels, ignore_index=-1)

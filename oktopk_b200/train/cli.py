@@ -76,6 +76,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-xent", action="store_true",
                    help="BERT: the masked-LM loss takes the fused softmax cross-entropy kernels, which read only the "
                         "labelled rows (default: stock cross_entropy)")
+    p.add_argument("--sparse-mlm", action="store_true",
+                   help="BERT: the masked-LM head (transform, LayerNorm, decoder GEMM) runs on the labelled rows only, "
+                        "gathered into a fixed number of rows (default: every token row)")
+    p.add_argument("--mlm-capacity", type=float, default=None,
+                   help="with --sparse-mlm: the gathered rows as a fraction of the batch's tokens, rounded up to a "
+                        "multiple of 8 (default 0.25; labelled rows past it stop training with an error; 1.0 never "
+                        "overflows)")
     p.add_argument("--fused-lstm", action="store_true",
                    help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
                         "and pass, instead of packed sequences through cuDNN (default: stock)")
@@ -117,6 +124,10 @@ def model_args(args: argparse.Namespace):
         model_kwargs["fuse_ln"] = True
     if args.fused_xent:
         model_kwargs["fuse_xent"] = True
+    if args.sparse_mlm:
+        model_kwargs["sparse_mlm"] = True
+    if args.mlm_capacity is not None:
+        model_kwargs["mlm_capacity"] = args.mlm_capacity
     if args.fused_lstm:
         model_kwargs["fuse_lstm"] = True
     if args.fused_lstm_autocast:
@@ -134,12 +145,18 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln`` and ``--fused-xent`` are for BERT only (``--dnn bert_base`` / ``bert``, or a
-    ``--module models.bertN.depth=M``)."""
+    """``--fused-ln``, ``--fused-xent``, ``--sparse-mlm`` and ``--mlm-capacity`` are for BERT only (``--dnn bert_base`` /
+    ``bert``, or a ``--module models.bertN.depth=M``); ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
     dnn = model_args(args)[0]
-    for flag, on in (("--fused-ln", args.fused_ln), ("--fused-xent", args.fused_xent)):
+    for flag, on in (("--fused-ln", args.fused_ln), ("--fused-xent", args.fused_xent),
+                     ("--sparse-mlm", args.sparse_mlm), ("--mlm-capacity", args.mlm_capacity is not None)):
         if on and dnn not in ("bert", "bert_base"):
             parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
+    if args.mlm_capacity is not None:
+        if not args.sparse_mlm:
+            parser.error("--mlm-capacity needs --sparse-mlm")
+        if not 0.0 < args.mlm_capacity <= 1.0:
+            parser.error("--mlm-capacity must be in (0, 1], got %r" % args.mlm_capacity)
 
 
 def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:

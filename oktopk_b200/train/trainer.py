@@ -22,6 +22,7 @@ import torch.nn.functional as F
 from .. import compression as _comp
 from ..config import LossScale, OkTopkConfig, preset as _preset
 from ..models import create_net
+from ..models.bert import BertPreTrainingHeads
 from ..optimizer import BertAdam, DistributedOptimizer, broadcast_parameters
 from ..parallel.world import World, world as _world
 from ..utils.logging import get_logger
@@ -81,6 +82,8 @@ class Trainer:
         self.loss_scale = LossScale.parse(loss_scale)
         self.net = net.to(self.device)
         self.is_bert = dnn.startswith("bert")
+        # masked-LM heads whose overflow counter check_mlm_overflow() reads when their sparse_mlm switch is on
+        self._mlm_heads = [m for m in self.net.modules() if isinstance(m, BertPreTrainingHeads)]
         # CNN zoo on the GPU: channels_last weights and activations.  cuDNN's TF32/fp32 convolution kernels are NHWC: with
         # NCHW tensors every convolution is bracketed by nchwToNhwc / nhwcToNchw transposes.  Numerics are unchanged (same kernels, no layout conversion).
         self.channels_last = (self.device.type == "cuda" and not self.is_bert and dnn not in ("lstman4", "lstm")
@@ -281,8 +284,21 @@ class Trainer:
                     self._loss_ev[i].synchronize()
                     self._loss_hist.append(float(self._loss_pin[i]))
                     self._loss_ev[i] = None
+        self.check_mlm_overflow()
         out, self._loss_hist = self._loss_hist, []
         return out
+
+    def check_mlm_overflow(self) -> None:
+        """Raise ``RuntimeError`` if a masked-LM head with ``sparse_mlm`` on has left labelled rows past its capacity
+        out of the loss.  Reads the head's device counter, so it waits for the work queued so far: call it where the
+        host reads values back anyway (``flush_losses``, the logging points and the end of ``robust_ssgd``)."""
+        for h in self._mlm_heads:
+            if h.sparse_mlm:
+                n = int(h.mlm_overflow)
+                if n:
+                    raise RuntimeError("the sparse masked-LM head left %d labelled rows out of the loss: more rows were "
+                                       "labelled than its capacity of %g of the batch's tokens holds; raise "
+                                       "--mlm-capacity (mlm_capacity; 1.0 never overflows)" % (n, h.mlm_capacity))
 
     def update_model(self) -> None:
         if self.dnn == "lstman4":                # LSTM/main_trainer.py:94-99: clip the *reduced* gradient
@@ -455,6 +471,7 @@ def robust_ssgd(dnn: str, dataset: Optional[str], data_dir: Optional[str], nwork
             if done % log_every == 0:
                 loss = tr.last_loss()
                 tr.optimizer.check_faults()
+                tr.check_mlm_overflow()
                 dt = (time.perf_counter() - t_last) / log_every
                 t_last = time.perf_counter()
                 if w.rank == 0:
@@ -469,4 +486,5 @@ def robust_ssgd(dnn: str, dataset: Optional[str], data_dir: Optional[str], nwork
         if max_iters is not None and done >= max_iters:
             break
     tr.optimizer.stop()
+    tr.check_mlm_overflow()
     return tr
