@@ -93,6 +93,12 @@ class OkTopkConfig:
     comm_ctas: int = 0                  # CTAs of the persistent kernel (0 => 1 per SM)
     pull_mode: str = "tma"              # 'tma' (cp.async.bulk of remote chunks) | 'ldg' (128-bit peer loads)
     overlap: bool = True                # launch a bucket's exchange as soon as its last grad lands
+    # threshold-reuse Ok-Topk calls pack a bucket's ready gradients during backward (parallel/early_pack.py): one segment
+    # once early_pack_frac of the bucket is ready and unpacked, on at most early_pack_ctas CTAs.  OKTOPK_EARLY_PACK=0 in the
+    # environment turns it off.
+    early_pack: bool = True
+    early_pack_frac: float = 0.85
+    early_pack_ctas: int = 32
     gselect_mode: str = "auto"          # global selection over the reduced region: 'list' | 'scan' | 'auto' (density <= 0.5 % -> list)
     peer_timeout_s: float = 60.0        # bound of every cross-GPU flag wait inside the kernels (0 = wait forever)
 

@@ -364,6 +364,31 @@ static void oktopk_run(uint64_t g, uint64_t res, uint64_t st, const std::vector<
         p.nsrc = 1;
         p.zero_g = 1;
     }
+    if (o.contains("pack_ranges")) {
+        // early pack: element ranges [lo, hi) at multiples of 4 inside the bucket's whole float4 vectors.  A segment launch
+        // (segment=1) packs its ranges; the call packs only its ranges, the rest having been packed by segments.
+        auto rs = o["pack_ranges"].cast<std::vector<std::pair<long long, long long>>>();
+        if (rs.size() > (size_t)kPackRangeMax) throw std::runtime_error("oktopk_run: more pack ranges than kPackRangeMax");
+        long long end = 0;
+        for (size_t i = 0; i < rs.size(); ++i) {
+            const long long lo = rs[i].first, hi = rs[i].second;
+            if (lo < end || hi < lo || (lo & 3) || (hi & 3) || hi > ((long long)n & ~3LL))
+                throw std::runtime_error("oktopk_run: pack ranges must be ordered, disjoint, at multiples of 4 elements, "
+                                         "inside the bucket's whole vectors");
+            p.pk_lo[i] = (int)(lo >> 2);
+            p.pk_hi[i] = (int)(hi >> 2);
+            end = hi;
+        }
+        p.pk_mode = 1;
+        p.pk_nr = (int)rs.size();
+        if (geti("segment", 0)) {
+            if (rs.empty() || p.zero_g || p.L.cap > 0 || p.residual_mode != RES_OKTOPK)
+                throw std::runtime_error("oktopk_run: a segment launch takes ranges of an Ok-Topk bucket read from its "
+                                         "sources in the lossless layout");
+            ck(launch_oktopk_segment(p, geti("seg_ctas", 32), S_(stream)), "oktopk segment launch");
+            return;
+        }
+    }
     if (geti("split_phases", 0)) {
         // ablation / debugging: one launch per phase instead of the single persistent kernel
         for (int ph = p.phase_begin; ph < p.phase_end; ++ph) {
@@ -792,5 +817,6 @@ PYBIND11_MODULE(_C, m) {
     m.attr("TRACE_LEN") = kTraceLen;
     m.attr("LAND_MAX") = kLandMax;
     m.attr("SRC_SEG_MAX") = kSrcSegMax;
+    m.attr("PACK_RANGE_MAX") = kPackRangeMax;
     m.attr("CHUNK") = kChunk;
 }

@@ -67,6 +67,275 @@ __device__ __forceinline__ float4 grad4_at(const SrcSeg* s, int ns, int v) {
     return out;
 }
 
+// shared-memory copy of the gradient-source table and the list of its partial last vectors (length % 4 != 0), which the
+// streaming pass patches from global memory.  Ends with a block barrier.
+__device__ __forceinline__ void load_src_table(const OktParams& p, SrcSeg* s_src, int* s_tail_v, int* s_tail_q, int* s_ntail) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nsrc = p.nsrc, n4 = p.n >> 2;
+    for (int q = tid; q < nsrc; q += blockDim.x) s_src[q] = SrcSeg{p.src[q], p.src_off[q], p.src_len[q]};
+    if (warp == 0) {
+        int cnt = 0;
+        for (int q0 = 0; q0 < nsrc; q0 += 32) {
+            const int q = q0 + lane;
+            const int end = q < nsrc ? p.src_off[q] + p.src_len[q] : 0;
+            const bool part = q < nsrc && (end & 3) != 0 && (end >> 2) < n4;
+            const unsigned m = __ballot_sync(0xffffffffu, part);
+            if (part) { const int t = cnt + __popc(m & ((1u << lane) - 1u)); s_tail_v[t] = end >> 2; s_tail_q[t] = q; }
+            cnt += __popc(m);
+        }
+        if (lane == 0) *s_ntail = cnt;
+    }
+    __syncthreads();
+}
+
+// The tiles of the streaming pass: float4 ranges [lo[r], hi[r]) cut into tiles of kTileV vectors from each range's start;
+// range r holds tiles first[r] .. first[r + 1] - 1.  One range [0, n4) is the whole bucket.
+struct TileMap { const int* lo; const int* hi; const int* first; int nr; };
+
+// thread 0: ranges -> tile prefix (shared arrays of kPackRangeMax / kPackRangeMax + 1 entries); ends with a block barrier
+__device__ __forceinline__ TileMap tile_map_build(int nr, const int* lo_in, const int* hi_in, int* lo, int* hi, int* first) {
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int r = 0; r < nr; ++r) {
+            lo[r] = lo_in[r]; hi[r] = hi_in[r]; first[r] = t;
+            t += (hi[r] - lo[r] + kTileV - 1) / kTileV;
+        }
+        first[nr] = t;
+    }
+    __syncthreads();
+    return TileMap{lo, hi, first, nr};
+}
+
+// first vector and end of tile t
+__device__ __forceinline__ void tile_at(const TileMap& m, int t, int* base, int* end) {
+    int r = 0;
+    while (t >= m.first[r + 1]) ++r;
+    *base = m.lo[r] + (t - m.first[r]) * kTileV;
+    *end = min(*base + kTileV, m.hi[r]);
+}
+
+struct PackRing { float4* r; float4* g; uint64_t* full; uint64_t* empty; };   // [STAGES][kTileV] each; STAGES barriers each
+struct PackSrc { const SrcSeg* seg; int nseg; const int* tail_v; const int* tail_q; int ntail; };
+struct PackSel {                  // selection: threshold, ladder, region edges, send-slot offsets and buffers
+    float thr; LadderCfg lc; const float* lthr; int* lcnt;
+    const int* edges; const int* soff; int* sidx; float* sval; int P;
+};
+
+// The streaming pack pass over this CTA's tiles of `tm` (tile = blockIdx.x + j * gridDim.x): acc = g + residual ->
+// residual (the gradient assembled from the source segments), |acc| > thr appended to the destination's send slot
+// through st->send_cursor, ladder tallies into sel.lcnt.  res_only: the accumulator is already in the residual buffer.
+// clear_g: write zeros over the bucket (the gradient was landed there).  ring_it counts the tiles ever pushed through the
+// ring (its mbarrier phases run on across calls of the same CTA).  Returns the number of tiles this CTA consumed.
+//
+// Fed by TMA: the CTA walks its tiles (kPackTile x 512 float4 = 16 KB of the gradient + 16 KB of the residual each)
+// through a STAGES-deep shared-memory ring.  One elected thread arms the stage's mbarrier (expect_tx) and issues the bulk
+// loads STAGES-1 tiles ahead, so the reads in flight per SM do not depend on occupancy or the register budget; consumers
+// read the tile with conflict-free LDS.128, write the accumulator (and, when the gradient was landed in the bucket, zeros
+// over it) back with streaming 128-bit stores (posted), and run the selection.  HBM traffic: 12 B/element when the
+// gradient is read from autograd's tensors (gradient + residual in, residual out), 16 B/element when it was landed (+ the
+// bucket cleared).  The gradient half of a tile is assembled from the source segments that overlap it, one bulk copy per
+// piece; what no segment covers (padding, parameters without a gradient, the last 1-3 elements of a segment whose length
+// is not a multiple of 4) is copied from the bucket, which is all-zero in that mode, and the partial last vector of a
+// segment is patched by the consumer from global memory (never read past a source's end).
+template <int STAGES>
+__device__ __forceinline__ int pack_stream(const OktParams& p, const TileMap& tm, const PackRing& ring, int ring_it,
+                                           bool res_only, bool clear_g, const PackSrc& src, const PackSel& sel,
+                                           int& dropped) {
+    OktState* st = p.st;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n = p.n;
+    float4* g4 = reinterpret_cast<float4*>(p.g);
+    float4* r4 = reinterpret_cast<float4*>(p.res);
+    const int ntiles = tm.first[tm.nr];
+    const int G = gridDim.x;
+    const int nmine = (ntiles > (int)blockIdx.x) ? (ntiles - (int)blockIdx.x + G - 1) / G : 0;
+    const SrcSeg* s_src = src.seg;
+    const int nsrc = src.nseg;
+    const float thr_sel = sel.thr;
+    const LadderCfg& lc = sel.lc;
+
+    auto arm = [&](int j) {                                         // thread 0 only; j = tile number of THIS pass
+        int base, end;
+        tile_at(tm, blockIdx.x + j * G, &base, &end);
+        const int stg = (ring_it + j) % STAGES;
+        const uint32_t bytes = (uint32_t)(end - base) * 16u;
+        fence_proxy_async_all();
+        mbar_expect_tx(&ring.full[stg], res_only ? bytes : 2u * bytes);
+        tma_load_1d(ring.r + stg * kTileV, r4 + (size_t)base, bytes, &ring.full[stg]);
+        if (res_only) return;
+        float4* dst = ring.g + stg * kTileV;
+        const int e0 = base * 4, e1 = e0 + (int)(bytes >> 2);
+        // first segment whose whole vectors reach past e0
+        int lo = 0, hi = nsrc;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (s_src[mid].off + (s_src[mid].len & ~3) <= e0) lo = mid + 1; else hi = mid;
+        }
+        int q = lo, e = e0;
+        while (e < e1) {
+            if (q < nsrc && s_src[q].off <= e) {                    // inside segment q
+                const int stop = min(e1, s_src[q].off + (s_src[q].len & ~3));
+                if (stop > e) {
+                    tma_load_1d(dst + ((e - e0) >> 2), s_src[q].src + (e - s_src[q].off), (uint32_t)(stop - e) * 4u,
+                                &ring.full[stg]);
+                    e = stop;
+                }
+                ++q;
+            } else {                                                // not covered: zeros from the bucket
+                const int stop = q < nsrc ? min(e1, s_src[q].off) : e1;
+                tma_load_1d(dst + ((e - e0) >> 2), p.g + e, (uint32_t)(stop - e) * 4u, &ring.full[stg]);
+                e = stop;
+            }
+        }
+    };
+    if (tid == 0)
+        for (int j = 0; j < min(nmine, STAGES - 1); ++j) {
+            // a stage used by the previous pass must have been released by all warps before it is re-armed
+            const int q = ring_it + j;
+            if (q >= STAGES) mbar_wait(&ring.empty[q % STAGES], (uint32_t)(q / STAGES - 1) & 1u);
+            arm(j);
+        }
+    for (int j = 0; j < nmine; ++j) {
+        // Producer (thread 0): re-arm the stage tile j-1 used, once all kWarps warps have released it (per-stage
+        // "empty" mbarrier; no block-wide barrier per tile, so a warp waiting for its slot reservation does not
+        // hold up the other 15 -- they may run up to STAGES-1 tiles ahead).
+        if (tid == 0 && j + STAGES - 1 < nmine) {
+            const int q = ring_it + j + STAGES - 1;                 // ring slot sequence number being armed
+            if (q >= STAGES) mbar_wait(&ring.empty[q % STAGES], (uint32_t)(q / STAGES - 1) & 1u);
+            arm(j + STAGES - 1);
+        }
+        const int qj = ring_it + j;
+        const int stg = qj % STAGES;
+        mbar_wait(&ring.full[stg], (uint32_t)(qj / STAGES) & 1u);
+        int base, tend;
+        tile_at(tm, blockIdx.x + j * G, &base, &tend);
+        float4 a[kPackTile];
+        bool in[kPackTile];
+#pragma unroll
+        for (int u = 0; u < kPackTile; ++u) {
+            const int v = base + u * kThreads + tid;
+            in[u] = v < tend;
+            a[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (in[u]) {
+                a[u] = ring.r[stg * kTileV + u * kThreads + tid];
+                if (!res_only) {
+                    float4 gq = ring.g[stg * kTileV + u * kThreads + tid];
+                    for (int t = 0; t < src.ntail; ++t)
+                        if (src.tail_v[t] == v) {                   // a segment ends inside this vector
+                            const SrcSeg sg = s_src[src.tail_q[t]];
+                            const float* sp = sg.src + (sg.len & ~3);
+                            const int c = sg.len & 3;
+                            gq.x = sp[0];
+                            if (c > 1) gq.y = sp[1];
+                            if (c > 2) gq.z = sp[2];
+                        }
+                    a[u].x += gq.x; a[u].y += gq.y; a[u].z += gq.z; a[u].w += gq.w;
+                    st_stream_f4(r4 + v, a[u]);
+                }
+                if (clear_g) st_stream_f4(g4 + v, make_float4(0.f, 0.f, 0.f, 0.f));
+            }
+        }
+        __syncwarp();                                               // the warp's part of the tile is in registers:
+        if (lane == 0) mbar_arrive(&ring.empty[stg]);               // release the stage (1 of kWarps arrivals)
+        // ---- selection: one slot reservation per (warp, trip, destination) ------------------------------
+        // 16 element flags per lane -> 16 ballots; the warp's trip covers 4 windows of 128 consecutive elements,
+        // which (regions being contiguous ranges) almost always belong to ONE destination, so the append costs
+        // one global atomic per trip instead of one per selected vector component.
+        unsigned msk[kPackTile * 4];
+        unsigned mybits = 0u;
+        int tot = 0;
+#pragma unroll
+        for (int u = 0; u < kPackTile; ++u) {
+            const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const bool pred = in[u] && fabsf(xs[c]) > thr_sel;
+                // TopkDSA zeroes the residual at the exact top-k INCLUDING the k-th element itself, which the
+                // strict '>' select does not send (reference quirk, SURVEY B.4-3).  On a tie at the k-th
+                // magnitude the top-k holds only k - #(|x| > thr) of the tied elements -- the radix select's
+                // remaining rank, sel_krem -- so a ticket bounds the clears to that many (which ones is unspecified)
+                if (p.residual_mode == RES_LOCAL_GE && in[u] && xs[c] != 0.f && fabsf(xs[c]) == thr_sel &&
+                    atomicAdd(&st->tie_cursor, 1) < (int)__ldcg(&st->sel_krem))
+                    p.res[4 * (base + u * kThreads + tid) + c] = 0.f;
+                const unsigned m = __ballot_sync(0xffffffffu, pred);
+                msk[u * 4 + c] = m;
+                tot += __popc(m);
+                if (pred) mybits |= 1u << (u * 4 + c);
+            }
+        }
+        if (tot == 0) continue;
+        // ladder tallies of my selected elements (shared-memory atomics: only selected elements get here)
+        if (lc.n_total > 1) {
+#pragma unroll
+            for (int u = 0; u < kPackTile; ++u) {
+                const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (mybits & (1u << (u * 4 + c)))
+                        atomicAdd(&sel.lcnt[ladder_rung(sel.lthr, lc.n_total, fabsf(xs[c]))], 1);
+            }
+        } else if (lane == 0) {
+            atomicAdd(&sel.lcnt[0], tot);                          // one rung: the warp's count in one go
+        }
+        const int e_first = 4 * (base + (warp << 5));
+        const int e_last = min(n - 1, 4 * (base + (kPackTile - 1) * kThreads + (warp << 5) + 31) + 3);
+        const int dlo = region_of(sel.edges, sel.P, e_first), dhi = region_of(sel.edges, sel.P, e_last);
+        for (int d = dlo; d <= dhi; ++d) {
+            unsigned md[kPackTile * 4];
+            unsigned mine = mybits;
+            int cnt = 0;
+            if (dlo == dhi) {
+#pragma unroll
+                for (int q = 0; q < kPackTile * 4; ++q) { md[q] = msk[q]; cnt += __popc(md[q]); }
+            } else {
+                const int lo_d = sel.edges[d], hi_d = sel.edges[d + 1];
+                mine = 0u;
+#pragma unroll
+                for (int u = 0; u < kPackTile; ++u) {
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        const int i = 4 * (base + u * kThreads + tid) + c;
+                        const bool pd = ((mybits >> (u * 4 + c)) & 1u) && i >= lo_d && i < hi_d;
+                        md[u * 4 + c] = __ballot_sync(0xffffffffu, pd);
+                        cnt += __popc(md[u * 4 + c]);
+                        if (pd) mine |= 1u << (u * 4 + c);
+                    }
+                }
+            }
+            if (cnt == 0) continue;
+            int run = 0;
+            if (lane == 0) run = atomicAdd(&st->send_cursor[d], cnt);
+            run = __shfl_sync(0xffffffffu, run, 0);
+            const int scap_d = sel.soff[d + 1] - sel.soff[d];
+            int* sidx = sel.sidx + sel.soff[d];
+            float* sval = sel.sval + sel.soff[d];
+            const int off_d = sel.edges[d];
+            const unsigned lt = (1u << lane) - 1u;
+#pragma unroll
+            for (int u = 0; u < kPackTile; ++u) {
+                const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const int q = u * 4 + c;
+                    if ((mine >> q) & 1u) {
+                        const int pos = run + __popc(md[q] & lt);
+                        const int i = 4 * (base + u * kThreads + tid) + c;
+                        if (pos < scap_d) {
+                            sidx[pos] = i - off_d;
+                            sval[pos] = xs[c];
+                            if (p.residual_mode != RES_OKTOPK) p.res[i] = 0.f;   // sent => cleared (classic rule)
+                        } else {
+                            dropped++;                                           // stays in the residual
+                        }
+                    }
+                    run += __popc(md[q]);
+                }
+            }
+        }
+    }
+    return nmine;
+}
+
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(const OktParams p) {
     __shared__ uint32_t s_hist[kHistBins];
     __shared__ int s_w[kWarps + 1];
@@ -87,6 +356,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     __shared__ SrcSeg s_src[kSrcSegMax];                    // gradient-source table
     __shared__ int s_tail_v[kSrcSegMax], s_tail_q[kSrcSegMax];   // vectors where a segment ends mid-way (length % 4 != 0)
     __shared__ int s_ntail;
+    __shared__ int s_rlo[kPackRangeMax], s_rhi[kPackRangeMax], s_rfirst[kPackRangeMax + 1];   // tiles of the pack pass
     extern __shared__ __align__(128) float4 dyn_pk[];       // TMA ring of the streaming pass (kPackSmemBytes)
 
     if (verdict_set(p.skip)) return;
@@ -122,23 +392,14 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
     }
     const int n4 = n >> 2;
     const int nsrc = p.nsrc;
-    for (int q = tid; q < nsrc; q += kThreads) s_src[q] = SrcSeg{p.src[q], p.src_off[q], p.src_len[q]};
-    if (warp == 0) {                     // list the partial last vectors of the segments (the streaming pass patches them)
-        int cnt = 0;
-        for (int q0 = 0; q0 < nsrc; q0 += 32) {
-            const int q = q0 + lane;
-            const int end = q < nsrc ? p.src_off[q] + p.src_len[q] : 0;
-            const bool part = q < nsrc && (end & 3) != 0 && (end >> 2) < n4;
-            const unsigned m = __ballot_sync(0xffffffffu, part);
-            if (part) { const int t = cnt + __popc(m & ((1u << lane) - 1u)); s_tail_v[t] = end >> 2; s_tail_q[t] = q; }
-            cnt += __popc(m);
-        }
-        if (lane == 0) s_ntail = cnt;
-    }
-    __syncthreads();
+    load_src_table(p, s_src, s_tail_v, s_tail_q, &s_ntail);
     const int ntail = s_ntail;
+    // what the pack pass streams: the whole bucket, or (a threshold-reuse call after segment launches) what they left
+    const int whole[2] = {0, n4};
+    const bool ranged = p.pk_mode && !two_pass;
+    const TileMap tmap = tile_map_build(ranged ? p.pk_nr : 1, ranged ? p.pk_lo : whole, ranged ? p.pk_hi : whole + 1,
+                                        s_rlo, s_rhi, s_rfirst);
 
-    float4* g4 = reinterpret_cast<float4*>(p.g);
     float4* r4 = reinterpret_cast<float4*>(p.res);
 
     // ======================================================================== PH_LOCAL
@@ -372,11 +633,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
         int dropped = 0;
         if (blockIdx.x == 0 && tid == 0) { st->stat_global_count = 0; st->stat_recv_total = 0; st->stat_dense_fallback = 0; }
 
-        float4* pk_r = dyn_pk;                                          // [kPackStages][kTileV]
-        float4* pk_g = dyn_pk + kPackStages * kTileV;                   // [kPackStages][kTileV]
-        const int ntiles = (n4 + kTileV - 1) / kTileV;
-        const int G = gridDim.x;
-        const int nmine = (ntiles > (int)blockIdx.x) ? (ntiles - (int)blockIdx.x + G - 1) / G : 0;
+        const PackRing ring{dyn_pk, dyn_pk + kPackStages * kTileV, s_pk_bar, s_pk_empty};   // [kPackStages][kTileV] each
         int ring_it = 0;                                                // tiles this CTA has pushed through the ring so far
 
         while (true) {
@@ -419,196 +676,9 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
                 }
             };
 
-            // Streaming pass fed by TMA: the CTA walks its tiles (kPackTile x 512 float4 = 16 KB of the gradient + 16 KB of
-            // the residual each) through a kPackStages-deep shared-memory ring.  One elected thread arms the stage's mbarrier
-            // (expect_tx) and issues the two cp.async.bulk loads kPackStages-1 tiles ahead, so ~96 KB of reads per SM are in
-            // flight independent of occupancy/register budget; consumers read the tile with conflict-free LDS.128, write the
-            // accumulator (and, when the gradient was landed in the bucket, zeros over it) back with streaming 128-bit
-            // stores (posted), and run the selection.  HBM traffic: 12 B/element when the gradient is read from autograd's
-            // tensors (gradient + residual in, residual out), 16 B/element when it was landed (+ the bucket cleared).
-            // The gradient half of a tile is assembled from the source segments that overlap it, one bulk copy per piece;
-            // what no segment covers (padding, parameters without a gradient, the last 1-3 elements of a segment whose
-            // length is not a multiple of 4) is copied from the bucket, which is all-zero in that mode, and the partial
-            // last vector of a segment is patched by the consumer from global memory (never read past a source's end).
-            // (The ring's mbarrier phases run on across redo passes: ring_it counts every tile ever pushed through.)
-            auto arm = [&](int j) {                                         // thread 0 only; j = tile number of THIS pass
-                const int tile = blockIdx.x + j * G;
-                const int stg = (ring_it + j) % kPackStages;
-                const uint32_t bytes = (uint32_t)min(kTileV, n4 - tile * kTileV) * 16u;
-                fence_proxy_async_all();
-                mbar_expect_tx(&s_pk_bar[stg], res_only ? bytes : 2u * bytes);
-                tma_load_1d(pk_r + stg * kTileV, r4 + (size_t)tile * kTileV, bytes, &s_pk_bar[stg]);
-                if (res_only) return;
-                float4* dst = pk_g + stg * kTileV;
-                const int e0 = tile * kTileV * 4, e1 = e0 + (int)(bytes >> 2);
-                // first segment whose whole vectors reach past e0
-                int lo = 0, hi = nsrc;
-                while (lo < hi) {
-                    const int mid = (lo + hi) >> 1;
-                    if (s_src[mid].off + (s_src[mid].len & ~3) <= e0) lo = mid + 1; else hi = mid;
-                }
-                int q = lo, e = e0;
-                while (e < e1) {
-                    if (q < nsrc && s_src[q].off <= e) {                    // inside segment q
-                        const int stop = min(e1, s_src[q].off + (s_src[q].len & ~3));
-                        if (stop > e) {
-                            tma_load_1d(dst + ((e - e0) >> 2), s_src[q].src + (e - s_src[q].off), (uint32_t)(stop - e) * 4u,
-                                        &s_pk_bar[stg]);
-                            e = stop;
-                        }
-                        ++q;
-                    } else {                                                // not covered: zeros from the bucket
-                        const int stop = q < nsrc ? min(e1, s_src[q].off) : e1;
-                        tma_load_1d(dst + ((e - e0) >> 2), p.g + e, (uint32_t)(stop - e) * 4u, &s_pk_bar[stg]);
-                        e = stop;
-                    }
-                }
-            };
-            if (tid == 0)
-                for (int j = 0; j < min(nmine, kPackStages - 1); ++j) {
-                    // a stage used by the previous pass must have been released by all warps before it is re-armed
-                    const int q = ring_it + j;
-                    if (q >= kPackStages) mbar_wait(&s_pk_empty[q % kPackStages], (uint32_t)(q / kPackStages - 1) & 1u);
-                    arm(j);
-                }
-            for (int j = 0; j < nmine; ++j) {
-                // Producer (thread 0): re-arm the stage tile j-1 used, once all kWarps warps have released it (per-stage
-                // "empty" mbarrier; no block-wide barrier per tile, so a warp waiting for its slot reservation does not
-                // hold up the other 15 -- they may run up to kPackStages-1 tiles ahead).
-                if (tid == 0 && j + kPackStages - 1 < nmine) {
-                    const int q = ring_it + j + kPackStages - 1;           // ring slot sequence number being armed
-                    if (q >= kPackStages) mbar_wait(&s_pk_empty[q % kPackStages], (uint32_t)(q / kPackStages - 1) & 1u);
-                    arm(j + kPackStages - 1);
-                }
-                const int qj = ring_it + j;
-                const int stg = qj % kPackStages;
-                mbar_wait(&s_pk_bar[stg], (uint32_t)(qj / kPackStages) & 1u);
-                const int base = (blockIdx.x + j * G) * kTileV;
-                float4 a[kPackTile];
-                bool in[kPackTile];
-#pragma unroll
-                for (int u = 0; u < kPackTile; ++u) {
-                    const int v = base + u * kThreads + tid;
-                    in[u] = v < n4;
-                    a[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (in[u]) {
-                        a[u] = pk_r[stg * kTileV + u * kThreads + tid];
-                        if (!res_only) {
-                            float4 gq = pk_g[stg * kTileV + u * kThreads + tid];
-                            for (int t = 0; t < ntail; ++t)
-                                if (s_tail_v[t] == v) {                     // a segment ends inside this vector
-                                    const SrcSeg sg = s_src[s_tail_q[t]];
-                                    const float* src = sg.src + (sg.len & ~3);
-                                    const int c = sg.len & 3;
-                                    gq.x = src[0];
-                                    if (c > 1) gq.y = src[1];
-                                    if (c > 2) gq.z = src[2];
-                                }
-                            a[u].x += gq.x; a[u].y += gq.y; a[u].z += gq.z; a[u].w += gq.w;
-                            st_stream_f4(r4 + v, a[u]);
-                        }
-                        if (attempt == 0 && p.zero_g) st_stream_f4(g4 + v, make_float4(0.f, 0.f, 0.f, 0.f));
-                    }
-                }
-                __syncwarp();                                               // the warp's part of the tile is in registers:
-                if (lane == 0) mbar_arrive(&s_pk_empty[stg]);               // release the stage (1 of kWarps arrivals)
-                // ---- selection: one slot reservation per (warp, trip, destination) ------------------------------
-                // 16 element flags per lane -> 16 ballots; the warp's trip covers 4 windows of 128 consecutive elements,
-                // which (regions being contiguous ranges) almost always belong to ONE destination, so the append costs
-                // one global atomic per trip instead of one per selected vector component.
-                unsigned msk[kPackTile * 4];
-                unsigned mybits = 0u;
-                int tot = 0;
-#pragma unroll
-                for (int u = 0; u < kPackTile; ++u) {
-                    const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const bool pred = in[u] && fabsf(xs[c]) > thr_sel;
-                        // TopkDSA zeroes the residual at the exact top-k INCLUDING the k-th element itself, which the
-                        // strict '>' select does not send (reference quirk, SURVEY B.4-3).  On a tie at the k-th
-                        // magnitude the top-k holds only k - #(|x| > thr) of the tied elements -- the radix select's
-                        // remaining rank, sel_krem -- so a ticket bounds the clears to that many (which ones is unspecified)
-                        if (p.residual_mode == RES_LOCAL_GE && in[u] && xs[c] != 0.f && fabsf(xs[c]) == thr_sel &&
-                            atomicAdd(&st->tie_cursor, 1) < (int)__ldcg(&st->sel_krem))
-                            p.res[4 * (base + u * kThreads + tid) + c] = 0.f;
-                        const unsigned m = __ballot_sync(0xffffffffu, pred);
-                        msk[u * 4 + c] = m;
-                        tot += __popc(m);
-                        if (pred) mybits |= 1u << (u * 4 + c);
-                    }
-                }
-                if (tot == 0) continue;
-                // ladder tallies of my selected elements (shared-memory atomics: only selected elements get here)
-                if (lc.n_total > 1) {
-#pragma unroll
-                    for (int u = 0; u < kPackTile; ++u) {
-                        const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
-#pragma unroll
-                        for (int c = 0; c < 4; ++c)
-                            if (mybits & (1u << (u * 4 + c)))
-                                atomicAdd(&s_lcnt[ladder_rung(s_lthr, lc.n_total, fabsf(xs[c]))], 1);
-                    }
-                } else if (lane == 0) {
-                    atomicAdd(&s_lcnt[0], tot);                            // one rung: the warp's count in one go
-                }
-                const int e_first = 4 * (base + (warp << 5));
-                const int e_last = min(n - 1, 4 * (base + (kPackTile - 1) * kThreads + (warp << 5) + 31) + 3);
-                const int dlo = region_of(s_edges, P, e_first), dhi = region_of(s_edges, P, e_last);
-                for (int d = dlo; d <= dhi; ++d) {
-                    unsigned md[kPackTile * 4];
-                    unsigned mine = mybits;
-                    int cnt = 0;
-                    if (dlo == dhi) {
-#pragma unroll
-                        for (int q = 0; q < kPackTile * 4; ++q) { md[q] = msk[q]; cnt += __popc(md[q]); }
-                    } else {
-                        const int lo_d = s_edges[d], hi_d = s_edges[d + 1];
-                        mine = 0u;
-#pragma unroll
-                        for (int u = 0; u < kPackTile; ++u) {
-#pragma unroll
-                            for (int c = 0; c < 4; ++c) {
-                                const int i = 4 * (base + u * kThreads + tid) + c;
-                                const bool pd = ((mybits >> (u * 4 + c)) & 1u) && i >= lo_d && i < hi_d;
-                                md[u * 4 + c] = __ballot_sync(0xffffffffu, pd);
-                                cnt += __popc(md[u * 4 + c]);
-                                if (pd) mine |= 1u << (u * 4 + c);
-                            }
-                        }
-                    }
-                    if (cnt == 0) continue;
-                    int run = 0;
-                    if (lane == 0) run = atomicAdd(&st->send_cursor[d], cnt);
-                    run = __shfl_sync(0xffffffffu, run, 0);
-                    const int scap_d = s_soff[d + 1] - s_soff[d];
-                    int* sidx = my_sidx + s_soff[d];
-                    float* sval = my_sval + s_soff[d];
-                    const int off_d = s_edges[d];
-                    const unsigned lt = (1u << lane) - 1u;
-#pragma unroll
-                    for (int u = 0; u < kPackTile; ++u) {
-                        const float xs[4] = {a[u].x, a[u].y, a[u].z, a[u].w};
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) {
-                            const int q = u * 4 + c;
-                            if ((mine >> q) & 1u) {
-                                const int pos = run + __popc(md[q] & lt);
-                                const int i = 4 * (base + u * kThreads + tid) + c;
-                                if (pos < scap_d) {
-                                    sidx[pos] = i - off_d;
-                                    sval[pos] = xs[c];
-                                    if (p.residual_mode != RES_OKTOPK) p.res[i] = 0.f;   // sent => cleared (classic rule)
-                                } else {
-                                    dropped++;                                           // stays in the residual
-                                }
-                            }
-                            run += __popc(md[q]);
-                        }
-                    }
-                }
-            }
-            ring_it += nmine;
+            const PackSrc src{s_src, nsrc, s_tail_v, s_tail_q, ntail};
+            const PackSel sel{thr_sel, lc, s_lthr, s_lcnt, s_edges, s_soff, my_sidx, my_sval, P};
+            ring_it += pack_stream<kPackStages>(p, tmap, ring, ring_it, res_only, attempt == 0 && p.zero_g, src, sel, dropped);
             if (blockIdx.x == 0 && warp == 0 && (n & 3)) {
                 int i = n4 * 4 + lane;
                 bool in = i < n;
@@ -975,6 +1045,53 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) oktopk_fused_kernel(cons
 }
 
 // ------------------------------------------------------------------------------------------
+// Early pack: the threshold-reuse pack pass over some ranges of the bucket, launched while backward is still running
+// (their gradients exist; the rest of the bucket's may not).  It does exactly the per-element work of the call's pack
+// pass (pack_stream) with the carried threshold, appends to the same send slots through st->send_cursor and adds its
+// ladder tallies to st->guard_counts; the call that follows packs only what no segment covered and publishes.  It must
+// co-run with backward without holding it up: an ordinary (non-cooperative) grid of a few dozen CTAs with a 64 KB ring
+// leaves most SMs to the backward kernels (cuDNN's take far more shared memory, so an SM that hosts a segment CTA hosts
+// none of theirs).  A carried threshold of 0 makes the call recompute the exact threshold over the whole bucket: the
+// segment then does nothing.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) oktopk_segment_kernel(const OktParams p) {
+    __shared__ int s_edges[OKT_MAXP + 1];
+    __shared__ int s_soff[OKT_MAXP + 1];
+    __shared__ float s_lthr[kGuardMax];
+    __shared__ int s_lcnt[kGuardMax];
+    __shared__ __align__(8) uint64_t s_full[kSegStages];
+    __shared__ __align__(8) uint64_t s_empty[kSegStages];
+    __shared__ SrcSeg s_src[kSrcSegMax];
+    __shared__ int s_tail_v[kSrcSegMax], s_tail_q[kSrcSegMax];
+    __shared__ int s_ntail;
+    __shared__ int s_rlo[kPackRangeMax], s_rhi[kPackRangeMax], s_rfirst[kPackRangeMax + 1];
+    extern __shared__ __align__(128) float4 dyn_seg[];      // [2][kSegStages][kTileV]
+
+    if (verdict_set(p.skip)) return;
+    OktState* st = p.st;
+    const float thr = st->local_thr;
+    if (thr == 0.f) return;
+    const int tid = threadIdx.x, P = p.P;
+    if (tid == 0) {
+        for (int q = 0; q < kSegStages; ++q) { mbar_init(&s_full[q], 1); mbar_init(&s_empty[q], kWarps); }
+        mbar_fence_init();
+    }
+    if (tid <= P) s_edges[tid] = st->edges[tid];
+    load_src_table(p, s_src, s_tail_v, s_tail_q, &s_ntail);
+    if (tid <= P) s_soff[tid] = (tid < P) ? slot_off(p.L, s_edges, tid) : slot_off(p.L, s_edges, P);
+    const TileMap tmap = tile_map_build(p.pk_nr, p.pk_lo, p.pk_hi, s_rlo, s_rhi, s_rfirst);
+    const LadderCfg lc = ladder_cfg(p, true);
+    ladder_build(s_lthr, s_lcnt, lc, thr);
+    char* me = p.peers[p.rank];
+    const PackRing ring{dyn_seg, dyn_seg + kSegStages * kTileV, s_full, s_empty};
+    const PackSrc src{s_src, p.nsrc, s_tail_v, s_tail_q, s_ntail};
+    const PackSel sel{thr, lc, s_lthr, s_lcnt, s_edges, s_soff, send_idx_base(me, p.L), send_val_base(me, p.L), P};
+    int dropped = 0;
+    pack_stream<kSegStages>(p, tmap, ring, 0, false, false, src, sel, dropped);
+    ladder_flush(st, s_lcnt);
+}
+
+// ------------------------------------------------------------------------------------------
 // standalone exact k-th |x| (used by tests and by the dist/NCCL baseline on CUDA tensors)
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads, 2) kth_abs_kernel(const float* x, int n, int k, OktState* st, float* out) {
@@ -1011,6 +1128,24 @@ cudaError_t launch_oktopk(const OktParams& p, int grid, cudaStream_t stream) {
     }
     void* args[] = {(void*)&p};
     return cudaLaunchCooperativeKernel((void*)oktopk_fused_kernel, dim3(grid), dim3(kThreads), args, kPackSmemBytes, stream);
+}
+
+cudaError_t launch_oktopk_segment(const OktParams& p, int max_ctas, cudaStream_t stream) {
+    constexpr int kSmem = kSegStages * 2 * kTileV * 16;
+    static bool attr_set[64] = {false};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(oktopk_segment_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+        if (e != cudaSuccess) return e;
+        attr_set[dev] = true;
+    }
+    int ntiles = 0;
+    for (int r = 0; r < p.pk_nr; ++r) ntiles += (p.pk_hi[r] - p.pk_lo[r] + kTileV - 1) / kTileV;
+    if (ntiles <= 0) return cudaSuccess;
+    const int grid = std::min((ntiles + kSegTiles - 1) / kSegTiles, std::max(max_ctas, 1));
+    oktopk_segment_kernel<<<grid, kThreads, kSmem, stream>>>(p);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_kth_abs(const float* x, int n, int k, OktState* st, float* out_thr, int grid, cudaStream_t stream) {

@@ -161,6 +161,11 @@ enum GlobalMode : int { GLB_THRESHOLD = 0, GLB_EXACT_TOPK = 1, GLB_ALL_NONZERO =
 // addresses of its capture.  Sized for the largest bucket of the bench workloads (BERT-base: 132 tensors) with the
 // whole OktParams under the classic 4 KB kernel-parameter limit.
 constexpr int kSrcSegMax = 160;
+// Early pack (see oktopk_segment_kernel): a threshold-reuse call whose bucket was partly packed during backward by segment
+// launches gets the vector ranges that are still to be packed; a segment launch gets its one range.
+constexpr int kPackRangeMax = 32;
+constexpr int kSegStages = 2;           // TMA ring depth of a segment launch (64 KB of shared memory)
+constexpr int kSegTiles = 4;            // tiles per CTA of a segment launch: short-lived CTAs, no cooperative grid ...
 
 struct OktParams {
     float* g;            // gradient bucket (result written in place)
@@ -203,6 +208,11 @@ struct OktParams {
     int src_off[kSrcSegMax];
     int src_len[kSrcSegMax];
     const float* src[kSrcSegMax];
+    // 0: the pack pass covers the whole bucket.  1: it covers only the float4 ranges [pk_lo[r], pk_hi[r]), r < pk_nr
+    // (pk_nr may be 0); the rest was packed by segment launches of this call.  Ignored by two-pass calls.
+    int pk_mode, pk_nr;
+    int pk_lo[kPackRangeMax];
+    int pk_hi[kPackRangeMax];
 };
 static_assert(sizeof(OktParams) <= 4096, "OktParams must fit the 4 KB kernel-parameter limit");
 
@@ -271,6 +281,9 @@ struct DenseParams {
 // ---- host-callable launchers (implemented in the .cu files) ----------------------------------------
 int okt_max_coop_grid(int device);
 cudaError_t launch_oktopk(const OktParams& p, int grid, cudaStream_t stream);
+// threshold-reuse pack of the ranges p.pk_lo[r] .. p.pk_hi[r], r < p.pk_nr, ahead of the call (no publish), on one
+// CTA per kSegTiles tiles but at most max_ctas
+cudaError_t launch_oktopk_segment(const OktParams& p, int max_ctas, cudaStream_t stream);
 cudaError_t launch_gather_scheme(const GatherParams& p, int grid, cudaStream_t stream);
 cudaError_t launch_gtopk(const TreeParams& p, int grid, cudaStream_t stream);
 int gtopk_max_coop_grid(int device);

@@ -33,6 +33,7 @@ from .config import LossScale, OkTopkConfig
 from .ops import ext
 from .parallel.allreducer import AllReducer
 from .parallel.buckets import Bucket, attach, build_buckets
+from .parallel.early_pack import PackPlanner
 from .parallel.world import World, world as _world
 
 
@@ -170,6 +171,18 @@ class _BucketedComm:
                 self._update = None
         self._direct = (self._land and self._update is not None and allreducer.compressor.name == "oktopk"
                         and all(b.flat_param is not None for b in self._buckets))
+        # Early pack (parallel/early_pack.py): on a threshold-reuse Ok-Topk step the hooks pack the ready gradients on the
+        # communication stream, once early_pack_frac of the bucket has them, while backward goes on
+        self._packs = {}
+        self._pos_in_bucket = {p: i for b in self._buckets for i, p in enumerate(b.params)}
+        if self._direct and self._use_streams:
+            for b in self._buckets:
+                if len(b.params) <= ext.require().SRC_SEG_MAX:
+                    self._packs[b.index] = PackPlanner(b.offsets, b.numel,
+                                                       math.ceil(self._cfg.early_pack_frac * b.numel),
+                                                       ext.require().PACK_RANGE_MAX)
+            for b in self._buckets:
+                b.packing = None                  # this step: None undecided, else whether its hooks pack early
         if self._use_streams:
             # high priority: a bucket's (SM-partitioned) communication kernel should get its SMs as soon as backward
             # kernels retire CTAs, not after the whole backward queue
@@ -254,7 +267,39 @@ class _BucketedComm:
             b.pending -= 1
             if b.pending == 0:
                 self._launch_ready()
+            elif b.index in self._packs:
+                self._pack_early(b, p)
         return hook
+
+    def _pack_early(self, b: Bucket, p) -> None:
+        """Parameter ``p`` of bucket ``b`` has its gradient: pack the ready, unpacked gradients now if they are enough
+        (``PackPlanner``), on the communication stream behind the work that produced them."""
+        if b.packing is None:
+            b.packing = (self._direct and not self.momentum_correction and self._ls is None
+                         and self._allreducer.reads_sources(b.name) and self._allreducer.packs_early(b.name))
+        if not b.packing:
+            return
+        planner = self._packs[b.index]
+        ranges = planner.ready(self._pos_in_bucket[p])
+        if ranges is None:
+            return
+        ptrs, offs, lens = [], [], []
+        for q, o, v in sorted(zip(b.params, b.offsets, b.grad_views), key=lambda t: t[1]):
+            g = q.grad
+            if not any(lo <= o < hi for lo, hi in ranges) or g is None or g.numel() == 0:
+                continue
+            if (g.data_ptr() == v.data_ptr() or g.dtype != torch.float32 or not g.is_cuda or g.stride() != v.stride()
+                    or g.data_ptr() % 16):
+                raise RuntimeError("early pack: the gradient of %s cannot be read in place; set "
+                                   "OkTopkConfig.early_pack=False" % self._parameter_names.get(q, "?"))
+            ptrs.append(g.data_ptr())
+            offs.append(o)
+            lens.append(g.numel())
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream())
+        self._comm_stream.wait_event(ev)
+        with torch.cuda.stream(self._comm_stream):
+            self._allreducer.pack_segment(b.name, ranges, (ptrs, offs, lens), stream=self._comm_stream)
 
     def _launch_ready(self) -> None:
         # strictly in bucket order on every rank: the fused kernels spin on peers' flags, so two
@@ -317,6 +362,12 @@ class _BucketedComm:
         srcs = None
         if self._direct and not self.momentum_correction and self._allreducer.reads_sources(b.name):
             srcs = self._source_table(b)
+        rest = None
+        if b.index in self._packs and self._packs[b.index].segments:
+            if srcs is None:
+                raise RuntimeError("early pack: bucket %s was partly packed from its gradients but its last call cannot "
+                                   "read them in place; set OkTopkConfig.early_pack=False" % b.name)
+            rest = self._packs[b.index].rest()
         if srcs is None and self._land:
             self._land_bucket(b)
         if self.momentum_correction:
@@ -326,7 +377,8 @@ class _BucketedComm:
             ev.record(torch.cuda.current_stream())
             self._comm_stream.wait_event(ev)
             with torch.cuda.stream(self._comm_stream):
-                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream, srcs=srcs, scale=self._ls)
+                self._allreducer.reduce_bucket(b.name, b.grad, stream=self._comm_stream, srcs=srcs, scale=self._ls,
+                                               pack_ranges=rest)
                 b.event.record(self._comm_stream)
         else:
             self._allreducer.reduce_bucket(b.name, b.grad, srcs=srcs, scale=self._ls)
@@ -406,6 +458,9 @@ class _BucketedComm:
         for b in self._buckets:
             b.pending = len(b.params)
             b.launched = False
+            if b.index in self._packs:
+                self._packs[b.index].reset()
+                b.packing = None
         self._next_launch = 0
         self._synced = False
         self._allreducer.poll_faults()           # pinned host flag, no sync: a timed-out peer wait surfaces at once

@@ -95,7 +95,20 @@ class AllReducer:
             return False
         return eng.reads_sources(self.compressor.name, self.get_current_density())
 
-    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None, srcs=None, scale=None) -> torch.Tensor:
+    def packs_early(self, name: str) -> bool:
+        """True if the next reduction of bucket ``name`` may pack ready gradients during backward (``pack_segment``);
+        the caller reads the gradient from its sources and runs without loss scaling."""
+        from ..utils import settings
+        eng = self._engines.get(name)
+        if eng is None or settings.PROFILING or settings.PROFILING_GRAD or settings.PROFILING_NORM:
+            return False
+        return eng.packs_early(self.compressor.name, self.get_current_density())
+
+    def pack_segment(self, name: str, ranges, srcs, stream=None) -> None:
+        self._engines[name].pack_segment(self.compressor.name, ranges, srcs, self.get_current_density(), stream)
+
+    def reduce_bucket(self, name: str, flat: torch.Tensor, stream=None, srcs=None, scale=None,
+                      pack_ranges=None) -> torch.Tensor:
         """Reduce bucket ``name`` in place.  ``srcs = (pointers, offsets, lengths)``: the gradient is in these fp32
         tensors rather than in ``flat``, which must then be all-zero (only where ``reads_sources(name)``).
 
@@ -121,7 +134,7 @@ class AllReducer:
             return self._reduce_profiled(name, flat, stream, density, skip)
         if name in self._engines:
             out = self._engines[name].reduce(self.compressor.name, density, stream=stream, g=flat, srcs=srcs,
-                                             skip=skip)
+                                             skip=skip, pack_ranges=pack_ranges)
             if settings.PROFILING:
                 self._profile_iteration(name)
             return out

@@ -12,6 +12,7 @@ Memory per bucket (one IPC allocation, mapped by every peer):
 """
 from __future__ import annotations
 
+import os
 from typing import Dict, List, Optional
 
 import torch
@@ -114,6 +115,7 @@ class CudaBucketEngine:
         self.last_mode = ""
         self._res_clean = False                  # True while the residual is known to be all-zero (dense-switch calls)
         self._skip = 0                           # bucket verdict address of the running call (loss scaling), 0 = off
+        self.early_pack = bool(cfg.early_pack) and os.environ.get("OKTOPK_EARLY_PACK", "1") != "0"
 
     # ------------------------------------------------------------------ helpers
     def _stream(self, stream: Optional[torch.cuda.Stream]) -> int:
@@ -136,6 +138,23 @@ class CudaBucketEngine:
         the bucket: an Ok-Topk call of the fused kernel, whose pack pass then reads every source once and leaves the bucket
         alone.  The bucket must be all-zero when such a call starts."""
         return compressor == "oktopk" and self._plan(compressor, density).kind == "fused"
+
+    def packs_early(self, compressor: str, density: Optional[float] = None) -> bool:
+        """True if the next ``reduce`` call may be preceded by ``pack_segment`` launches (parallel/early_pack.py): an
+        Ok-Topk threshold-reuse call of the fused kernel in the lossless slot layout.  The caller also makes sure that it
+        reads the gradient from its sources and that loss scaling is off."""
+        if not (self.early_pack and compressor == "oktopk" and self.cap == 0 and self.cfg.fused):
+            return False
+        plan = self._plan(compressor, density)
+        return plan.kind == "fused" and not plan.exact_local and not plan.repartition
+
+    def pack_segment(self, compressor: str, ranges, srcs: tuple, density: Optional[float] = None,
+                     stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Pack the bucket ranges ``ranges = [(lo, hi), ...]`` of the next call now, from the gradient sources ``srcs``
+        that cover them (only where ``packs_early``).  Enqueue it behind the previous call and ahead of the next one on
+        the same stream."""
+        self._fused(compressor, self._plan(compressor, density), density, self._stream(stream), self.grad, srcs,
+                    pack_ranges=list(ranges), segment=True)
 
     def enable_loss_scaling(self) -> None:
         """Allocate the device words of ``unscale_check`` (before any graph capture; a no-op when already done)."""
@@ -164,12 +183,13 @@ class CudaBucketEngine:
 
     def reduce(self, compressor: str, density: Optional[float] = None,
                stream: Optional[torch.cuda.Stream] = None, g: Optional[torch.Tensor] = None,
-               srcs: Optional[tuple] = None, skip: int = 0) -> torch.Tensor:
+               srcs: Optional[tuple] = None, skip: int = 0, pack_ranges: Optional[list] = None) -> torch.Tensor:
         """Allreduce this bucket in place (``self.grad`` unless an external ``g`` is given).
 
         ``srcs = (pointers, offsets, lengths)``: the gradient is not in the bucket but in these fp32 tensors, at these
         element offsets of the bucket (Ok-Topk only, see ``reads_sources``); the result is written into the bucket.
-        ``skip``: device address of the bucket verdict of loss scaling (0 = off); when set the kernels return at entry."""
+        ``skip``: device address of the bucket verdict of loss scaling (0 = off); when set the kernels return at entry.
+        ``pack_ranges``: after ``pack_segment`` launches, the element ranges they left for this call to pack."""
         ext_g = g is not None and g.data_ptr() != self.grad.data_ptr()
         plan = self._plan(compressor, density)
         if srcs is not None and (ext_g or compressor != "oktopk" or plan.kind != "fused"):
@@ -195,7 +215,7 @@ class CudaBucketEngine:
         else:
             self._res_clean = False
             if plan.kind == "fused":
-                self._fused(compressor, plan, density, s, out, srcs)
+                self._fused(compressor, plan, density, s, out, srcs, pack_ranges)
             elif plan.kind == "gather":
                 self._gather(compressor, plan, density, s, out)
             else:
@@ -211,7 +231,7 @@ class CudaBucketEngine:
                          self.host_flag_dev, self._skip)
 
     def _fused(self, compressor: str, plan: CallPlan, density: Optional[float], s: int, g: torch.Tensor,
-               srcs: Optional[tuple] = None) -> None:
+               srcs: Optional[tuple] = None, pack_ranges: Optional[list] = None, segment: bool = False) -> None:
         cfg = self.cfg
         k = self.k_now(density)
         o: Dict = {"pull_tma": 1 if cfg.pull_mode == "tma" else 0, "deterministic": int(cfg.deterministic),
@@ -251,9 +271,14 @@ class CudaBucketEngine:
             o["srcs"] = srcs
         if self._skip:
             o["skip"] = self._skip
+        if pack_ranges is not None:
+            o["pack_ranges"] = [(int(a), int(b)) for a, b in pack_ranges]
+            o["segment"] = int(segment)
+            o["seg_ctas"] = int(cfg.early_pack_ctas)
         self.C.oktopk_run(g.data_ptr(), self.residual.data_ptr(), self.state_ptr, self.peer_comm, self.n,
                           self.rank, k, self.cap, self.gcap, o, self.grid, s)
-        self.last_mode = compressor
+        if not segment:
+            self.last_mode = compressor
 
     def _gather(self, compressor: str, plan: CallPlan, density: Optional[float], s: int, g: torch.Tensor) -> None:
         cfg = self.cfg
