@@ -581,6 +581,37 @@ static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uin
                           P_<void>(da), P_<float>(partial), P_<float>(dgamma), P_<float>(dbeta), R, H, p_keep_thr,
                           (float)scale, bn_dtype(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
 }
+// Fused self-attention, head dim 64 (csrc/attention.cu): qkv / dqkv [B, S, 3 H 64] and out / dout [B, S, H 64] of type
+// dtype (codes as bn_dtype), 16-byte aligned; mask [B, S] fp32 or 0; lse / delta [B, H, S] fp32.  p_keep_thr and seed as
+// for ln_forward; scale = 1 / (1 - p).
+static void attn_check(const char* what, int B, int S, int H, long long p_keep_thr, uint64_t seed,
+                       std::initializer_list<uint64_t> vec_ptrs, std::initializer_list<uint64_t> f32_ptrs) {
+    if (!attn_supported(B, S, H)) throw std::runtime_error(std::string(what) + ": needs B, H >= 1 and 1 <= S <= 512");
+    if (p_keep_thr < 0 || p_keep_thr > (1LL << 32)) throw std::runtime_error(std::string(what) + ": p_keep_thr out of range");
+    if (p_keep_thr < (1LL << 32) && seed == 0) throw std::runtime_error(std::string(what) + ": dropout needs the seed");
+    for (uint64_t p : vec_ptrs)
+        if (p == 0 || (p & 15)) throw std::runtime_error(std::string(what) + ": tensors must be non-null and 16-byte aligned");
+    for (uint64_t p : f32_ptrs)
+        if (p == 0 || (p & 3)) throw std::runtime_error(std::string(what) + ": lse / delta must be non-null fp32");
+}
+static void attn_forward(uint64_t qkv, uint64_t mask, uint64_t seed, uint64_t out, uint64_t lse, int B, int S, int H,
+                         long long p_keep_thr, double scale, int dtype, uint64_t stream) {
+    attn_check("attn_forward", B, S, H, p_keep_thr, seed, {qkv, out}, {lse});
+    if (mask & 3) throw std::runtime_error("attn_forward: the mask must be fp32");
+    ck(launch_attn_forward(P_<const void>(qkv), P_<const float>(mask), P_<const unsigned long long>(seed), P_<void>(out),
+                           P_<float>(lse), B, S, H, p_keep_thr, (float)scale, bn_dtype(dtype, "attn_forward"), S_(stream)),
+       "attn_forward");
+}
+static void attn_backward(uint64_t qkv, uint64_t out, uint64_t dout, uint64_t mask, uint64_t seed, uint64_t lse,
+                          uint64_t delta, uint64_t dqkv, int B, int S, int H, long long p_keep_thr, double scale, int dtype,
+                          uint64_t stream) {
+    attn_check("attn_backward", B, S, H, p_keep_thr, seed, {qkv, out, dout, dqkv}, {lse, delta});
+    if (mask & 3) throw std::runtime_error("attn_backward: the mask must be fp32");
+    ck(launch_attn_backward(P_<const void>(qkv), P_<const void>(out), P_<const void>(dout), P_<const float>(mask),
+                            P_<const unsigned long long>(seed), P_<const float>(lse), P_<float>(delta), P_<void>(dqkv), B, S,
+                            H, p_keep_thr, (float)scale, bn_dtype(dtype, "attn_backward"), S_(stream)),
+       "attn_backward");
+}
 // Softmax cross-entropy over R rows of V logits (x, dx of type dtype, codes as bn_dtype), targets t int64, mean over the
 // rows whose target is not ignore_index.  lse: R + 1 floats (the rows' log-sum-exp, then n); rowloss: R floats; loss and
 // g: one float each, in device memory.
@@ -796,6 +827,13 @@ PYBIND11_MODULE(_C, m) {
           py::arg("stream"));
     m.def("ln_bwd_grid", &ln_bwd_grid);
     m.def("ln_supported_h", &ln_supported_h);
+    m.def("attn_forward", &attn_forward, py::arg("qkv"), py::arg("mask"), py::arg("seed"), py::arg("out"), py::arg("lse"),
+          py::arg("B"), py::arg("S"), py::arg("H"), py::arg("p_keep_thr"), py::arg("scale"), py::arg("dtype"),
+          py::arg("stream"));
+    m.def("attn_backward", &attn_backward, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("mask"), py::arg("seed"),
+          py::arg("lse"), py::arg("delta"), py::arg("dqkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("p_keep_thr"),
+          py::arg("scale"), py::arg("dtype"), py::arg("stream"));
+    m.def("attn_supported", &attn_supported);
     m.def("xent_forward", &xent_forward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("rowloss"), py::arg("loss"),
           py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
     m.def("xent_backward", &xent_backward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("g"), py::arg("dx"),

@@ -413,6 +413,16 @@ cudaError_t launch_lstm_forward(const void* gx, const void* whh, const int* len,
 cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
                                  void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
                                  cudaStream_t stream, BnDtype dtype);
+// fused self-attention, head dim 64 (csrc/attention.cu): qkv and dqkv [B, S, 3 H 64], out and dout [B, S, H 64], all of
+// type `dtype` (BnDtype's codes), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
+// fp32 (lse written by the forward pass, delta scratch of the backward pass).  keep_thr >= 2^32 turns the dropout off
+// (seed may then be null); `scale` is the kept elements' 1 / (1 - p).  One launch forward, two backward.
+bool attn_supported(int B, int S, int H);
+cudaError_t launch_attn_forward(const void* qkv, const float* mask, const unsigned long long* seed, void* out, float* lse,
+                                int B, int S, int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream);
+cudaError_t launch_attn_backward(const void* qkv, const void* out, const void* dout, const float* mask,
+                                 const unsigned long long* seed, const float* lse, float* delta, void* dqkv, int B, int S,
+                                 int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
 cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
 cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);

@@ -10,7 +10,8 @@ Fresh implementation: fused QKV projection, ``F.scaled_dot_product_attention`` (
 matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm`` instead of apex, or with
 ``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``, and
 with ``fuse_xent=True`` the masked-LM loss on the fused softmax cross-entropy of ``ops/fused_xent.py``, and with
-``sparse_mlm=True`` the masked-LM head on the labelled rows only, gathered by ``ops/mlm_gather.py``.
+``sparse_mlm=True`` the masked-LM head on the labelled rows only, gathered by ``ops/mlm_gather.py``, and with
+``fuse_attn=True`` self-attention on the fused kernels of ``ops/fused_attn.py``.
 """
 from __future__ import annotations
 
@@ -74,13 +75,20 @@ class BertEmbeddings(nn.Module):
 
 
 class BertSelfAttention(nn.Module):
+    """``fuse_attn`` (default off) runs the attention of the packed projection through the fused kernels of
+    ``ops/fused_attn.py``; parameters, buffers and ``state_dict`` keys are the same either way."""
+
     def __init__(self, c: BertConfig):
         super().__init__()
         self.h, self.dh = c.num_attention_heads, c.hidden_size // c.num_attention_heads
         self.qkv = nn.Linear(c.hidden_size, 3 * c.hidden_size)          # same parameter count as 3 separate projections
         self.p_drop = c.attention_probs_dropout_prob
+        self.fuse_attn = False
 
     def forward(self, x: torch.Tensor, mask: Optional[torch.Tensor]) -> torch.Tensor:
+        if self.fuse_attn:
+            from ..ops.fused_attn import self_attention
+            return self_attention(self.qkv(x), self.h, mask, self.p_drop if self.training else 0.0)
         b, s, _ = x.shape
         q, k, v = self.qkv(x).view(b, s, 3, self.h, self.dh).permute(2, 0, 3, 1, 4)
         o = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=self.p_drop if self.training else 0.0)
@@ -234,10 +242,12 @@ class BertForPreTraining(nn.Module):
     """``fuse_ln=True`` (or ``net.fuse_ln = True`` at any time) sets ``BertLayer.fuse_ln`` on every encoder layer;
     ``fuse_xent=True`` (or ``net.fuse_xent``) sets ``PretrainingCriterion.fuse_xent``; ``sparse_mlm=True`` (or
     ``net.sparse_mlm``) runs the masked-LM head on the labelled rows only when labels are given, gathered into
-    ``mlm_capacity`` (or ``net.mlm_capacity``) times B·S rows, rounded up to a multiple of 8 (``BertPreTrainingHeads``)."""
+    ``mlm_capacity`` (or ``net.mlm_capacity``) times B·S rows, rounded up to a multiple of 8 (``BertPreTrainingHeads``);
+    ``fuse_attn=True`` (or ``net.fuse_attn``) sets ``BertSelfAttention.fuse_attn`` on every encoder layer."""
 
     def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False,
-                 fuse_ln: bool = False, fuse_xent: bool = False, sparse_mlm: bool = False, mlm_capacity: float = 0.25):
+                 fuse_ln: bool = False, fuse_xent: bool = False, sparse_mlm: bool = False, mlm_capacity: float = 0.25,
+                 fuse_attn: bool = False):
         super().__init__()
         self.config = config or BertConfig()
         self.recompute = recompute           # ``--recompute_step`` (BERT/runtime.py:546-557, modeling.py:414-431)
@@ -249,6 +259,18 @@ class BertForPreTraining(nn.Module):
         self.fuse_xent = fuse_xent
         self.sparse_mlm = sparse_mlm
         self.mlm_capacity = mlm_capacity
+        self.fuse_attn = fuse_attn
+
+    @property
+    def fuse_attn(self) -> bool:
+        """True when every encoder layer runs its self-attention through the fused kernels."""
+        return all(m.fuse_attn for m in self.modules() if isinstance(m, BertSelfAttention))
+
+    @fuse_attn.setter
+    def fuse_attn(self, on: bool) -> None:
+        for m in self.modules():
+            if isinstance(m, BertSelfAttention):
+                m.fuse_attn = bool(on)
 
     @property
     def sparse_mlm(self) -> bool:

@@ -83,6 +83,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="with --sparse-mlm: the gathered rows as a fraction of the batch's tokens, rounded up to a "
                         "multiple of 8 (default 0.25; labelled rows past it stop training with an error; 1.0 never "
                         "overflows)")
+    p.add_argument("--fused-attn", action="store_true",
+                   help="BERT: the self-attention of every encoder layer takes the fused attention kernels, which read "
+                        "the packed QKV projection and regenerate the dropout mask (default: stock "
+                        "scaled_dot_product_attention)")
     p.add_argument("--fused-lstm", action="store_true",
                    help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
                         "and pass, instead of packed sequences through cuDNN (default: stock)")
@@ -128,6 +132,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["sparse_mlm"] = True
     if args.mlm_capacity is not None:
         model_kwargs["mlm_capacity"] = args.mlm_capacity
+    if args.fused_attn:
+        model_kwargs["fuse_attn"] = True
     if args.fused_lstm:
         model_kwargs["fuse_lstm"] = True
     if args.fused_lstm_autocast:
@@ -145,11 +151,12 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln``, ``--fused-xent``, ``--sparse-mlm`` and ``--mlm-capacity`` are for BERT only (``--dnn bert_base`` /
-    ``bert``, or a ``--module models.bertN.depth=M``); ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
+    """``--fused-ln``, ``--fused-xent``, ``--sparse-mlm``, ``--mlm-capacity`` and ``--fused-attn`` are for BERT only
+    (``--dnn bert_base`` / ``bert``, or a ``--module models.bertN.depth=M``); ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
     dnn = model_args(args)[0]
     for flag, on in (("--fused-ln", args.fused_ln), ("--fused-xent", args.fused_xent),
-                     ("--sparse-mlm", args.sparse_mlm), ("--mlm-capacity", args.mlm_capacity is not None)):
+                     ("--sparse-mlm", args.sparse_mlm), ("--mlm-capacity", args.mlm_capacity is not None),
+                     ("--fused-attn", args.fused_attn)):
         if on and dnn not in ("bert", "bert_base"):
             parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
     if args.mlm_capacity is not None:
