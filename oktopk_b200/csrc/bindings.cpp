@@ -664,8 +664,11 @@ static void mlm_scatter(uint64_t dout, uint64_t slot, uint64_t dx, int R, int H,
 // Persistent LSTM recurrence (csrc/lstm.cu), time-major: gx [T, N, 4H], whh [4H, H], len [N] int32 in [1, T],
 // y / cs [T, N, H], gates / dy / dg as named; bar: one zeroed int64.  u hidden units per CTA, `rows` batch rows staged at
 // a time (ops/fused_lstm.lstm_geometry).  gx, whh, y, dy and dg are of type dtype (codes as bn_dtype), gates and cs fp32.
+// whh_rev != 0 (the reverse direction's W_hh) runs both directions of a bidirectional layer in the one launch: gx, y,
+// cs, gates and dg are then [2, T, N, .], forward direction first, dy is the same [T, N, H] for both, and bar is two
+// zeroed int64, one per direction.
 static void lstm_check(const char* what, int T, int N, int H, int u, int rows, BnDtype dtype,
-                       std::initializer_list<uint64_t> ptrs, std::initializer_list<uint64_t> vec_ptrs) {
+                       std::initializer_list<uint64_t> ptrs, std::initializer_list<uint64_t> vec_ptrs, uint64_t bar) {
     if (T <= 0 || N <= 0 || H <= 0 || H % 4 || u <= 0 || rows <= 0 || rows > N)
         throw std::runtime_error(std::string(what) + ": needs T, N > 0, H > 0 a multiple of 4, u > 0 and 0 < rows <= N");
     for (uint64_t p : ptrs)
@@ -673,22 +676,26 @@ static void lstm_check(const char* what, int T, int N, int H, int u, int rows, B
     const uint64_t mask = dtype == BnDtype::kF32 ? 15 : 7;            // read four elements at a time
     for (uint64_t p : vec_ptrs)
         if (p & mask)
-            throw std::runtime_error(std::string(what) + ": W_hh and the staged operand must be " +
+            throw std::runtime_error(std::string(what) + ": W_hh (both directions') and the staged operand must be " +
                                      std::to_string(mask + 1) + "-byte aligned");
+    if (bar & 7) throw std::runtime_error(std::string(what) + ": bar must be 8-byte aligned (one int64 per direction)");
 }
 static void lstm_forward(uint64_t gx, uint64_t whh, uint64_t len, uint64_t y, uint64_t gates, uint64_t cs, uint64_t bar,
-                         int T, int N, int H, int u, int rows, uint64_t stream, int dtype) {
+                         int T, int N, int H, int u, int rows, uint64_t stream, int dtype, uint64_t whh_rev) {
     const BnDtype dt = bn_dtype(dtype, "lstm_forward");
-    lstm_check("lstm_forward", T, N, H, u, rows, dt, {gx, whh, len, y, gates, cs, bar}, {whh, y});
-    ck(launch_lstm_forward(P_<const void>(gx), P_<const void>(whh), P_<const int>(len), P_<void>(y), P_<float>(gates),
-                           P_<float>(cs), P_<unsigned long long>(bar), T, N, H, u, rows, S_(stream), dt), "lstm_forward");
+    lstm_check("lstm_forward", T, N, H, u, rows, dt, {gx, whh, len, y, gates, cs, bar}, {whh, whh_rev, y}, bar);
+    ck(launch_lstm_forward(P_<const void>(gx), P_<const void>(whh), P_<const void>(whh_rev), P_<const int>(len),
+                           P_<void>(y), P_<float>(gates), P_<float>(cs), P_<unsigned long long>(bar), T, N, H, u, rows,
+                           S_(stream), dt),
+       "lstm_forward");
 }
 static void lstm_backward(uint64_t dy, uint64_t gates, uint64_t cs, uint64_t whh, uint64_t len, uint64_t dg, uint64_t bar,
-                          int T, int N, int H, int u, int rows, uint64_t stream, int dtype) {
+                          int T, int N, int H, int u, int rows, uint64_t stream, int dtype, uint64_t whh_rev) {
     const BnDtype dt = bn_dtype(dtype, "lstm_backward");
-    lstm_check("lstm_backward", T, N, H, u, rows, dt, {dy, gates, cs, whh, len, dg, bar}, {dg});
+    lstm_check("lstm_backward", T, N, H, u, rows, dt, {dy, gates, cs, whh, len, dg, bar}, {dg}, bar);
     ck(launch_lstm_backward(P_<const void>(dy), P_<const float>(gates), P_<const float>(cs), P_<const void>(whh),
-                            P_<const int>(len), P_<void>(dg), P_<unsigned long long>(bar), T, N, H, u, rows, S_(stream), dt),
+                            P_<const void>(whh_rev), P_<const int>(len), P_<void>(dg), P_<unsigned long long>(bar), T, N,
+                            H, u, rows, S_(stream), dt),
        "lstm_backward");
 }
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
@@ -846,10 +853,10 @@ PYBIND11_MODULE(_C, m) {
           py::arg("dtype"), py::arg("stream"));
     m.def("lstm_forward", &lstm_forward, py::arg("gx"), py::arg("whh"), py::arg("len"), py::arg("y"), py::arg("gates"),
           py::arg("cs"), py::arg("bar"), py::arg("T"), py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"),
-          py::arg("stream"), py::arg("dtype") = 0);
+          py::arg("stream"), py::arg("dtype") = 0, py::arg("whh_rev") = 0);
     m.def("lstm_backward", &lstm_backward, py::arg("dy"), py::arg("gates"), py::arg("cs"), py::arg("whh"), py::arg("len"),
           py::arg("dg"), py::arg("bar"), py::arg("T"), py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"),
-          py::arg("stream"), py::arg("dtype") = 0);
+          py::arg("stream"), py::arg("dtype") = 0, py::arg("whh_rev") = 0);
     m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;

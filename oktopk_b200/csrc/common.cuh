@@ -134,13 +134,14 @@ __device__ __forceinline__ uint64_t make_mail(uint32_t epoch, uint32_t payload) 
 
 // ----------------------------------------------------------------------------------------
 // grid barrier (all CTAs co-resident: cooperative launch). 64-bit ticket counter: each barrier
-// consumes exactly gridDim.x tickets, so the target is derived from one's own ticket and the
-// counter never has to be reset.
+// consumes exactly G tickets, so the target is derived from one's own ticket and the counter
+// never has to be reset.  G is the number of CTAs that sync on `bar`: the whole grid, or a
+// group of CTAs that shares nothing with the rest of the grid between barriers and has a
+// counter of its own.
 // ----------------------------------------------------------------------------------------
-__device__ __forceinline__ void grid_sync(unsigned long long* bar) {
+__device__ __forceinline__ void grid_sync(unsigned long long* bar, unsigned long long G) {
     __syncthreads();
     if (threadIdx.x == 0) {
-        const unsigned long long G = gridDim.x;
         __threadfence();
         unsigned long long old = atomicAdd(bar, 1ULL);
         unsigned long long target = (old / G + 1ULL) * G;
@@ -149,6 +150,7 @@ __device__ __forceinline__ void grid_sync(unsigned long long* bar) {
     }
     __syncthreads();
 }
+__device__ __forceinline__ void grid_sync(unsigned long long* bar) { grid_sync(bar, gridDim.x); }
 
 // "Last CTA done" ticket: every CTA calls it once when it has finished a phase; exactly one call -- the last one of
 // the grid -- returns true, with all other CTAs' prior global writes visible to it (and, through a subsequent

@@ -34,6 +34,16 @@
 // element is widened on load and enters the same fmaf chain in the same order, so a 16-bit launch is the fp32 kernel run
 // on the widened operands, except where a y or dgates it stored (rounded to nearest even, not saturated: an fp16
 // overflow is inf) is read back at the next step.
+//
+// Directions: a bidirectional layer runs both of its directions in one launch of dirs * g CTAs (g = ceil(H / u)).  CTA
+// b serves direction d = b / g with units [(b % g) u, ...) of that direction's own W_hh.  Every per-timestep tensor is
+// direction-major, [dirs, T, N, .], so direction 0 sees exactly the one-direction layout; dy is shared, since the layer's
+// output is y[0] + y[1].  The two recurrences are independent: each direction syncs only its own g CTAs, on its own
+// counter bar[d].  At step s, row n of direction d works on time t = pi_d,n(s) (lstm_time): s forward; len_n - 1 - s
+// for s < len_n and s after that in reverse.  pi is a permutation of [0, T), so the reverse direction starts from a zero
+// state at len_n - 1 (packed-sequence semantics), writes every time once, and writes exact zeros at t >= len_n like the
+// forward one.  What the forward direction indexes by t (gx, gates, c, y, dy, dgates; h_{t-1} = y at pi(s - 1),
+// dgates_{t+1} at pi(s + 1), c_{t-1} at pi(s - 1)) the reverse one indexes by pi.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -46,16 +56,17 @@ constexpr int kLstmThreads = 512;                // ops/fused_lstm.py LSTM_THREA
 constexpr int kLstmWarps = kLstmThreads / 32;
 constexpr int kLstmNB = 4;                       // batch rows of one warp task in lstm_dots
 
+// whh[1] is null for a one-direction layer; g = ceil(H / u) CTAs per direction.
 template <typename S>
 struct LstmFwdArgs {
     const S* gx;
-    const S* whh;
+    const S* whh[2];
     const int* len;
     S* y;
     float* gates;
     float* cs;
     unsigned long long* bar;
-    int T, N, H, u, rows;
+    int T, N, H, u, rows, g;
 };
 
 template <typename S>
@@ -63,14 +74,17 @@ struct LstmBwdArgs {
     const S* dy;
     const float* gates;
     const float* cs;
-    const S* whh;
+    const S* whh[2];
     const int* len;
     S* dg;
     unsigned long long* bar;
-    int T, N, H, u, rows;
+    int T, N, H, u, rows, g;
 };
 
 __device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+
+// The time that row n (length L) of a direction works on at step s (the file header's pi).
+__device__ __forceinline__ int lstm_time(int s, int L, bool rev) { return rev && s < L ? L - 1 - s : s; }
 
 // Storage type S: Vec holds four elements (16 bytes of float, 8 bytes of a 16-bit type), widen() makes them floats,
 // narrow() rounds one float to nearest even without saturating.
@@ -105,14 +119,25 @@ template <> struct LstmEl<__half> {
     static __device__ __forceinline__ __half narrow(float v) { return __float2half_rn(v); }
 };
 
-// Copy `nrows` rows of K elements (K % 4 == 0, Vec-aligned) that other CTAs wrote in this launch to shared memory.
+// Copy batch rows [n0, n0 + nrows) of the [T, N, K] tensor V (K % 4 == 0, Vec-aligned), which other CTAs wrote in this
+// launch, to shared memory: row n from time lstm_time(s, len_n, rev).  Forward that is one contiguous block; in
+// reverse each row has its own time.
 template <typename S>
-__device__ __forceinline__ void lstm_stage(S* __restrict__ sV, const S* __restrict__ g, int nrows, int K) {
+__device__ __forceinline__ void lstm_stage(S* __restrict__ sV, const S* V, int n0, int nrows, int K, int N, int s,
+                                           const int* __restrict__ len, bool rev) {
     using Vec = typename LstmEl<S>::Vec;
     Vec* d = reinterpret_cast<Vec*>(sV);
-    const Vec* s = reinterpret_cast<const Vec*>(g);
-    const int n4 = nrows * (K >> 2);
-    for (int i = threadIdx.x; i < n4; i += kLstmThreads) d[i] = __ldcg(s + i);
+    const int K4 = K >> 2, n4 = nrows * K4;
+    if (!rev) {
+        const Vec* src = reinterpret_cast<const Vec*>(V + (size_t)s * N * K + (size_t)n0 * K);
+        for (int i = threadIdx.x; i < n4; i += kLstmThreads) d[i] = __ldcg(src + i);
+        return;
+    }
+    for (int i = threadIdx.x; i < n4; i += kLstmThreads) {
+        const int r = i / K4, k = i - r * K4, n = n0 + r;
+        const size_t t = lstm_time(s, __ldg(len + n), true);
+        d[i] = __ldcg(reinterpret_cast<const Vec*>(V + (t * N + n) * K) + k);
+    }
 }
 
 // out[r N + n0 + j] = sum_k sW[r K + k] sV[j K + k] for r < R, j < nc.  A warp takes one (r, kLstmNB rows of sV) task at
@@ -155,13 +180,15 @@ __device__ __forceinline__ void lstm_dots(const S* __restrict__ sW, const S* __r
     }
 }
 
-// out[r N + n] = sum_k sW[r K + k] V[n K + k] over all N rows of V (global, written in this launch), `rows` at a time.
+// out[r N + n] = sum_k sW[r K + k] V[t_n, n, k] over all N rows of V (global [T, N, K], written in this launch), `rows`
+// at a time, t_n = lstm_time(s, len_n, rev).
 template <typename S>
 __device__ __forceinline__ void lstm_matvec(const S* __restrict__ sW, S* __restrict__ sV, const S* V,
-                                            float* __restrict__ out, int R, int K, int N, int rows) {
+                                            float* __restrict__ out, int R, int K, int N, int rows, int s,
+                                            const int* __restrict__ len, bool rev) {
     for (int n0 = 0; n0 < N; n0 += rows) {
         const int nc = min(rows, N - n0);
-        lstm_stage(sV, V + (size_t)n0 * K, nc, K);
+        lstm_stage(sV, V, n0, nc, K, N, s, len, rev);
         __syncthreads();
         lstm_dots(sW, sV, out, R, K, nc, n0, N);
         __syncthreads();
@@ -176,7 +203,16 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
     using Vec = typename El::Vec;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2;
-    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    const int d = blockIdx.x / p.g;
+    const bool rev = d != 0;
+    const int u0 = (blockIdx.x - d * p.g) * u, nu = min(u, H - u0);
+    const size_t dTNH = (size_t)d * p.T * N * H;                     // this direction's [T, N, .] blocks
+    const S* whh = rev ? p.whh[1] : p.whh[0];
+    const S* gx0 = p.gx + 4 * dTNH;
+    S* y = p.y + dTNH;
+    float* gates = p.gates + 4 * dTNH;
+    float* cs = p.cs + dTNH;
+    unsigned long long* bar = p.bar + d;
     S* sW = reinterpret_cast<S*>(lstm_smem);
     S* sV = sW + (size_t)R * H;
     float* sG = reinterpret_cast<float*>(sV + (size_t)p.rows * H);
@@ -184,24 +220,25 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
     for (int i = threadIdx.x; i < R * H4; i += kLstmThreads) {      // local row q u + j = W_hh row q H + u0 + j
         const int lr = i / H4, k = i - lr * H4, q = lr / u, j = lr - q * u;
         Vec v = El::zero();
-        if (j < nu) v = __ldg(reinterpret_cast<const Vec*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
+        if (j < nu) v = __ldg(reinterpret_cast<const Vec*>(whh + (size_t)(q * H + u0 + j) * H) + k);
         reinterpret_cast<Vec*>(sW)[i] = v;
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sC[i] = 0.f;
-    for (int t = 0; t < p.T; ++t) {
-        if (t == 0) {
+    for (int s = 0; s < p.T; ++s) {
+        if (s == 0) {
             for (int i = threadIdx.x; i < R * N; i += kLstmThreads) sG[i] = 0.f;
             __syncthreads();
         } else {
-            lstm_matvec(sW, sV, p.y + (size_t)(t - 1) * N * H, sG, R, H, N, p.rows);
+            lstm_matvec(sW, sV, y, sG, R, H, N, p.rows, s - 1, p.len, rev);         // h_{t-1}: y at pi(s - 1)
         }
         for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
             const int j = i / N, n = i - j * N, unit = u0 + j;
-            const size_t row = (size_t)t * N + n;
-            const S* gx = p.gx + row * 4 * H + unit;
-            float* gs = p.gates + row * 4 * H + unit;
+            const int L = __ldg(p.len + n);
+            const size_t row = (size_t)lstm_time(s, L, rev) * N + n;
+            const S* gx = gx0 + row * 4 * H + unit;
+            float* gs = gates + row * 4 * H + unit;
             const size_t o = row * H + unit;
-            if (t < __ldg(p.len + n)) {
+            if (s < L) {
                 const float gi = lstm_sigmoid(sG[(0 * u + j) * N + n] + El::ld(gx));
                 const float gf = lstm_sigmoid(sG[(1 * u + j) * N + n] + El::ld(gx + H));
                 const float gg = tanhf(sG[(2 * u + j) * N + n] + El::ld(gx + 2 * H));
@@ -209,15 +246,15 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
                 const float c = gf * sC[j * N + n] + gi * gg;
                 sC[j * N + n] = c;
                 gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
-                p.cs[o] = c;
-                p.y[o] = El::narrow(go * tanhf(c));
+                cs[o] = c;
+                y[o] = El::narrow(go * tanhf(c));
             } else {
                 gs[0] = 0.f; gs[H] = 0.f; gs[2 * H] = 0.f; gs[3 * H] = 0.f;
-                p.cs[o] = 0.f;
-                p.y[o] = El::narrow(0.f);
+                cs[o] = 0.f;
+                y[o] = El::narrow(0.f);
             }
         }
-        if (t + 1 < p.T) grid_sync(p.bar);
+        if (s + 1 < p.T) grid_sync(bar, p.g);
     }
 }
 
@@ -227,33 +264,42 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
     using El = LstmEl<S>;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, G = 4 * H;
-    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    const int d = blockIdx.x / p.g;
+    const bool rev = d != 0;
+    const int u0 = (blockIdx.x - d * p.g) * u, nu = min(u, H - u0);
+    const size_t dTNH = (size_t)d * p.T * N * H;                     // this direction's [T, N, .] blocks; dy is shared
+    const S* whh = rev ? p.whh[1] : p.whh[0];
+    const float* gates = p.gates + 4 * dTNH;
+    const float* cs = p.cs + dTNH;
+    S* dg0 = p.dg + 4 * dTNH;
+    unsigned long long* bar = p.bar + d;
     S* sW = reinterpret_cast<S*>(lstm_smem);
     S* sV = sW + (size_t)u * G;
     float* sD = reinterpret_cast<float*>(sV + (size_t)p.rows * G);
     float* sDC = sD + u * N;
     for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
         const int k = i / u, j = i - k * u;
-        sW[(size_t)j * G + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : El::narrow(0.f);
+        sW[(size_t)j * G + k] = j < nu ? __ldg(whh + (size_t)k * H + u0 + j) : El::narrow(0.f);
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sDC[i] = 0.f;
-    for (int t = p.T - 1; t >= 0; --t) {
-        if (t == p.T - 1) {
+    for (int s = p.T - 1; s >= 0; --s) {
+        if (s == p.T - 1) {
             for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sD[i] = 0.f;
             __syncthreads();
         } else {
-            lstm_matvec(sW, sV, p.dg + (size_t)(t + 1) * N * G, sD, u, G, N, p.rows);
+            lstm_matvec(sW, sV, dg0, sD, u, G, N, p.rows, s + 1, p.len, rev);       // dgates at pi(s + 1)
         }
         for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
             const int j = i / N, n = i - j * N, unit = u0 + j;
-            const size_t row = (size_t)t * N + n;
+            const int L = __ldg(p.len + n);
+            const size_t row = (size_t)lstm_time(s, L, rev) * N + n;
             const size_t o = row * H + unit;
-            S* dg = p.dg + row * G + unit;
-            if (t < __ldg(p.len + n)) {
-                const float* gs = p.gates + row * G + unit;
+            S* dg = dg0 + row * G + unit;
+            if (s < L) {
+                const float* gs = gates + row * G + unit;
                 const float gi = __ldg(gs), gf = __ldg(gs + H), gg = __ldg(gs + 2 * H), go = __ldg(gs + 3 * H);
-                const float tc = tanhf(__ldg(p.cs + o));
-                const float cp = t > 0 ? __ldg(p.cs + o - (size_t)N * H) : 0.f;
+                const float tc = tanhf(__ldg(cs + o));
+                const float cp = s > 0 ? __ldg(cs + ((size_t)lstm_time(s - 1, L, rev) * N + n) * H + unit) : 0.f;
                 const float dh = El::ld(p.dy + o) + sD[j * N + n];
                 const float dc = dh * go * (1.f - tc * tc) + sDC[j * N + n];
                 dg[0] = El::narrow(dc * gg * gi * (1.f - gi));
@@ -266,7 +312,7 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
                 sDC[j * N + n] = 0.f;
             }
         }
-        if (t > 0) grid_sync(p.bar);
+        if (s > 0) grid_sync(bar, p.g);
     }
 }
 
@@ -319,47 +365,56 @@ static bool lstm_shape_ok(int T, int N, int H, int u, int rows) {
     return T > 0 && N > 0 && H > 0 && H % 4 == 0 && u > 0 && u <= H && rows > 0 && rows <= N;
 }
 
+// whh_rev null: one direction, g = ceil(H / u) CTAs; else both, 2 g CTAs.
 template <typename S>
-static cudaError_t lstm_forward_t(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
-                                  unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream) {
-    const LstmFwdArgs<S> p{static_cast<const S*>(gx), static_cast<const S*>(whh), len, static_cast<S*>(y), gates, cs, bar,
-                           T, N, H, u, rows};
+static cudaError_t lstm_forward_t(const void* gx, const void* whh, const void* whh_rev, const int* len, void* y,
+                                  float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                  cudaStream_t stream) {
+    const int g = (H + u - 1) / u;
+    const LstmFwdArgs<S> p{static_cast<const S*>(gx), {static_cast<const S*>(whh), static_cast<const S*>(whh_rev)}, len,
+                           static_cast<S*>(y), gates, cs, bar, T, N, H, u, rows, g};
     const size_t smem = sizeof(S) * ((size_t)4 * u * H + (size_t)rows * H) + sizeof(float) * (size_t)5 * u * N;
-    return lstm_launch(lstm_fwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
+    return lstm_launch(lstm_fwd_kernel<S>, p, whh_rev ? 2 * g : g, smem, stream);
 }
 
 template <typename S>
-static cudaError_t lstm_backward_t(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
-                                   void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                   cudaStream_t stream) {
-    const LstmBwdArgs<S> p{static_cast<const S*>(dy), gates, cs, static_cast<const S*>(whh), len, static_cast<S*>(dg), bar,
-                           T, N, H, u, rows};
+static cudaError_t lstm_backward_t(const void* dy, const float* gates, const float* cs, const void* whh,
+                                   const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
+                                   int H, int u, int rows, cudaStream_t stream) {
+    const int g = (H + u - 1) / u;
+    const LstmBwdArgs<S> p{static_cast<const S*>(dy), gates, cs,
+                           {static_cast<const S*>(whh), static_cast<const S*>(whh_rev)}, len, static_cast<S*>(dg), bar,
+                           T, N, H, u, rows, g};
     const size_t smem = sizeof(S) * ((size_t)4 * u * H + (size_t)rows * 4 * H) + sizeof(float) * (size_t)2 * u * N;
-    return lstm_launch(lstm_bwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
+    return lstm_launch(lstm_bwd_kernel<S>, p, whh_rev ? 2 * g : g, smem, stream);
 }
 
-cudaError_t launch_lstm_forward(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
-                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
-                                BnDtype dtype) {
+cudaError_t launch_lstm_forward(const void* gx, const void* whh, const void* whh_rev, const int* len, void* y,
+                                float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                cudaStream_t stream, BnDtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
     switch (dtype) {
-        case BnDtype::kF32: return lstm_forward_t<float>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF32:
+            return lstm_forward_t<float>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
         case BnDtype::kBF16:
-            return lstm_forward_t<__nv_bfloat16>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
-        case BnDtype::kF16: return lstm_forward_t<__half>(gx, whh, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+            return lstm_forward_t<__nv_bfloat16>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF16:
+            return lstm_forward_t<__half>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
     }
     return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
-                                 void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                 cudaStream_t stream, BnDtype dtype) {
+cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh,
+                                 const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
+                                 int H, int u, int rows, cudaStream_t stream, BnDtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
     switch (dtype) {
-        case BnDtype::kF32: return lstm_backward_t<float>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF32:
+            return lstm_backward_t<float>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
         case BnDtype::kBF16:
-            return lstm_backward_t<__nv_bfloat16>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
-        case BnDtype::kF16: return lstm_backward_t<__half>(dy, gates, cs, whh, len, dg, bar, T, N, H, u, rows, stream);
+            return lstm_backward_t<__nv_bfloat16>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
+        case BnDtype::kF16:
+            return lstm_backward_t<__half>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
     }
     return cudaErrorInvalidValue;
 }

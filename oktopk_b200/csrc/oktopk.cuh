@@ -403,16 +403,18 @@ cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, 
 cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, BnDtype dtype,
                                cudaStream_t stream);
 // persistent LSTM recurrence, time-major (csrc/lstm.cu): one cooperative launch per pass, ceil(H / u) CTAs of u hidden
-// units each, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H] (the input
-// projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg
+// units each per direction, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H]
+// (the input projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg
 // [T, N, 4H].  gx, whh, y, dy and dg are of type `dtype` (BnDtype's codes); gates and cs are fp32.  `bar` is a zeroed
 // 64-bit grid-barrier counter.  whh, y and dg aligned to four elements (16 bytes in fp32, 8 in bf16 / fp16), H % 4 == 0.
-cudaError_t launch_lstm_forward(const void* gx, const void* whh, const int* len, void* y, float* gates, float* cs,
-                                unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
-                                BnDtype dtype);
-cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh, const int* len,
-                                 void* dg, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                 cudaStream_t stream, BnDtype dtype);
+// whh_rev non-null runs a bidirectional layer, whh_rev being the reverse direction's W_hh: gx, y, cs, gates and dg are
+// then [2, T, N, .] (forward direction first), dy stays [T, N, H] (the same for both), and bar holds two counters.
+cudaError_t launch_lstm_forward(const void* gx, const void* whh, const void* whh_rev, const int* len, void* y,
+                                float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u, int rows,
+                                cudaStream_t stream, BnDtype dtype);
+cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh,
+                                 const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
+                                 int H, int u, int rows, cudaStream_t stream, BnDtype dtype);
 // fused self-attention, head dim 64 (csrc/attention.cu): qkv and dqkv [B, S, 3 H 64], out and dout [B, S, H 64], all of
 // type `dtype` (BnDtype's codes), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
 // fp32 (lse written by the forward pass, delta scratch of the backward pass).  keep_thr >= 2^32 turns the dropout off

@@ -26,7 +26,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ``fuse_ln=True`` turns on ``net.fuse_ln``, ``fuse_xent=True`` ``net.fuse_xent`` and ``sparse_mlm=True``
     ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``) and ``fuse_attn=True`` ``net.fuse_attn``; for
     ``lstman4``,
-    ``fuse_lstm=True`` turns on ``net.fuse_lstm`` and ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast``."""
+    ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
+    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``)."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):

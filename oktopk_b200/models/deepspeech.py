@@ -11,6 +11,9 @@ logits (softmax only in eval mode) + output lengths; trained with CTC.
 recurrence kernels of ``ops/fused_lstm.py`` instead of packing the sequences for cuDNN; parameters, buffers and
 ``state_dict`` keys are the same either way.  Under bf16 / fp16 autocast those layers are stock again unless
 ``fuse_lstm_autocast=True`` (``net.fuse_lstm_autocast``) is set as well, which runs the 16-bit forms of the kernels.
+The bidirectional network (``bidirectional=True``) keeps stock layers under ``fuse_lstm`` unless
+``fuse_lstm_bidirectional=True`` (``net.fuse_lstm_bidirectional``) is set as well, which runs both directions of each
+layer in one launch of the kernels.
 """
 from __future__ import annotations
 
@@ -58,14 +61,17 @@ class _SeqBN(nn.Module):
 class BatchRNN(nn.Module):
     """``fuse`` (default off) runs the recurrence through ``ops/fused_lstm.lstm_layer``, which falls back to the stock
     pack -> rnn -> pad sequence wherever its kernels do not apply; with ``fuse_autocast`` (default off) it takes the
-    16-bit kernels under bf16 / fp16 autocast, where ``fuse`` alone is stock."""
+    16-bit kernels under bf16 / fp16 autocast, where ``fuse`` alone is stock; with ``fuse_bidirectional`` (default off)
+    a bidirectional layer takes them too, where ``fuse`` alone is stock."""
 
     def __init__(self, input_size: int, hidden_size: int, rnn_type=nn.LSTM, bidirectional: bool = False,
-                 batch_norm: bool = True, fuse: bool = False, fuse_autocast: bool = False):
+                 batch_norm: bool = True, fuse: bool = False, fuse_autocast: bool = False,
+                 fuse_bidirectional: bool = False):
         super().__init__()
         self.bidirectional = bidirectional
         self.fuse = fuse
         self.fuse_autocast = fuse_autocast
+        self.fuse_bidirectional = fuse_bidirectional
         self.batch_norm = _SeqBN(nn.BatchNorm1d(input_size)) if batch_norm else None
         self.rnn = rnn_type(input_size=input_size, hidden_size=hidden_size, bidirectional=bidirectional, bias=True)
 
@@ -74,7 +80,8 @@ class BatchRNN(nn.Module):
         if self.batch_norm is not None:
             x = self.batch_norm(x)
         if self.fuse:
-            return lstm_layer(x, lengths, self.rnn, dev_lengths, autocast=self.fuse_autocast)
+            return lstm_layer(x, lengths, self.rnn, dev_lengths, autocast=self.fuse_autocast,
+                              bidirectional=self.fuse_bidirectional)
         return stock_layer(x, lengths, self.rnn)
 
 
@@ -99,7 +106,8 @@ class Lookahead(nn.Module):
 class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
-                 window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False):
+                 window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
+                 fuse_lstm_bidirectional: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -123,6 +131,7 @@ class DeepSpeech(nn.Module):
                                        nn.Linear(rnn_hidden_size, num_classes, bias=False)))
         self.fuse_lstm = fuse_lstm
         self.fuse_lstm_autocast = fuse_lstm_autocast
+        self.fuse_lstm_bidirectional = fuse_lstm_bidirectional
 
     @property
     def fuse_lstm(self) -> bool:
@@ -143,6 +152,16 @@ class DeepSpeech(nn.Module):
     def fuse_lstm_autocast(self, on: bool) -> None:
         for m in self.rnns:
             m.fuse_autocast = bool(on)
+
+    @property
+    def fuse_lstm_bidirectional(self) -> bool:
+        """Whether every fused bidirectional ``BatchRNN`` layer runs both directions on the kernels (one launch)."""
+        return all(m.fuse_bidirectional for m in self.rnns)
+
+    @fuse_lstm_bidirectional.setter
+    def fuse_lstm_bidirectional(self, on: bool) -> None:
+        for m in self.rnns:
+            m.fuse_bidirectional = bool(on)
 
     def get_seq_lens(self, input_length: torch.Tensor) -> torch.Tensor:
         seq = input_length
@@ -169,10 +188,12 @@ class DeepSpeech(nn.Module):
 
 
 def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
-            fuse_lstm: bool = False, fuse_lstm_autocast: bool = False) -> DeepSpeech:
+            fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
+            fuse_lstm_bidirectional: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
     return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
-                      fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast)
+                      fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast,
+                      fuse_lstm_bidirectional=fuse_lstm_bidirectional)
 
 
 class PTBLSTM(nn.Module):

@@ -1,4 +1,4 @@
-"""Persistent LSTM recurrence for DeepSpeech's uni-directional layers (``csrc/lstm.cu``).
+"""Persistent LSTM recurrence for DeepSpeech's LSTM layers (``csrc/lstm.cu``).
 
 ``lstm_layer(x, lengths, rnn)`` returns what ``BatchRNN`` returns after its batch norm: ``rnn`` run over the time-major
 ``x`` (T x N x I) with per-utterance ``lengths`` through ``pack_padded_sequence`` / ``pad_packed_sequence``, i.e. the
@@ -17,9 +17,16 @@ The native path runs one cooperative kernel per pass instead of cuDNN's small GE
 Everything is summed in fp32 in a fixed order (no atomics), so results are bitwise reproducible.  The native path
 needs: CUDA fp32 tensors with autocast off, the native extension, ``rnn`` a single-layer, uni-directional ``nn.LSTM``
 with bias, ``proj_size == 0`` and ``batch_first=False``, lengths in [1, T], and an (H, N) that ``lstm_geometry``
-accepts on the current device.  Everything else -- the CPU, fp64, bidirectional layers, and in fp32 the PTB model's
-H = 1500, whose 288 KB of recurrent weights per CTA do not fit on chip -- runs the stock pack -> ``rnn`` -> pad sequence
-and returns exactly what ``BatchRNN`` returns without the switch.
+accepts on the current device.  Everything else -- the CPU, fp64, bidirectional layers (unless asked for, below), and
+in fp32 the PTB model's H = 1500, whose 288 KB of recurrent weights per CTA do not fit on chip -- runs the stock pack ->
+``rnn`` -> pad sequence and returns exactly what ``BatchRNN`` returns without the switch.
+
+``lstm_layer(..., bidirectional=True)`` takes a single-layer bidirectional ``nn.LSTM`` too, on the same conditions.  Both
+directions run in one launch per pass, each on half of the SMs (``lstm_geometry`` at ``sms // 2``, so H = 800 on an H100
+is u = 13 on 62 + 62 CTAs): the reverse direction is the forward recurrence run over each utterance's own
+``len - 1, ..., 0``, so it starts from a zero state at the last frame, as the packed stock layer does.  Each direction
+has its own input projection GEMM; the output is the sum of the two directions' y, which is what ``BatchRNN`` returns,
+and ``dx`` is two accumulating GEMMs.  A layer whose two directions do not fit together runs stock.
 
 Under bf16 / fp16 CUDA autocast the layer is stock too, unless ``lstm_layer(..., autocast=True)`` asks for the 16-bit
 kernels: ``x``, ``W_ih``, ``W_hh`` and ``b_ih + b_hh`` are cast to the autocast type (the parameters stay fp32), the
@@ -75,9 +82,10 @@ def lstm_geometry(H: int, N: int, sms: int, smem_per_block: int, elem: int = 4) 
     return LstmGeometry(u, grid, fr, br, fwd_fixed + elem * H * fr, bwd_fixed + 4 * elem * H * br)
 
 
-def _device_geometry(H: int, N: int, dev: torch.device, elem: int = 4) -> Optional[LstmGeometry]:
+def _device_geometry(H: int, N: int, dev: torch.device, elem: int = 4, dirs: int = 1) -> Optional[LstmGeometry]:
+    """The geometry of one direction of a ``dirs``-direction layer: the directions split the SMs between them."""
     p = torch.cuda.get_device_properties(dev)
-    return lstm_geometry(H, N, p.multi_processor_count, p.shared_memory_per_block_optin, elem)
+    return lstm_geometry(H, N, p.multi_processor_count // dirs, p.shared_memory_per_block_optin, elem)
 
 
 _DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}      # csrc/oktopk.cuh BnDtype
@@ -95,10 +103,10 @@ def stock_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module) -> torch
     return x
 
 
-def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module,
-               autocast: bool) -> Optional[Tuple[LstmGeometry, torch.dtype]]:
-    """The geometry and the kernels' storage type when the native path applies, else None."""
-    if not (isinstance(rnn, nn.LSTM) and rnn.num_layers == 1 and not rnn.bidirectional and rnn.bias
+def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, autocast: bool,
+               bidirectional: bool) -> Optional[Tuple[LstmGeometry, torch.dtype]]:
+    """The geometry (of one direction) and the kernels' storage type when the native path applies, else None."""
+    if not (isinstance(rnn, nn.LSTM) and rnn.num_layers == 1 and (bidirectional or not rnn.bidirectional) and rnn.bias
             and rnn.proj_size == 0 and not rnn.batch_first):
         return None
     if not (x.is_cuda and x.dim() == 3 and x.size(2) == rnn.input_size):
@@ -110,8 +118,7 @@ def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module,
             return None
     if x.dtype not in (torch.float32, dt) or not ext.available():
         return None
-    ps = (rnn.weight_ih_l0, rnn.weight_hh_l0, rnn.bias_ih_l0, rnn.bias_hh_l0)
-    if any(p.dtype != torch.float32 or p.device != x.device for p in ps):
+    if any(p.dtype != torch.float32 or p.device != x.device for p in _params(rnn)):
         return None
     T, N = x.size(0), x.size(1)
     if lengths.dim() != 1 or lengths.numel() != N or T == 0:
@@ -119,73 +126,105 @@ def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module,
     host = lengths.cpu()
     if int(host.min()) < 1 or int(host.max()) > T:          # stock raises on these; let it
         return None
-    geom = _device_geometry(rnn.hidden_size, N, x.device, dt.itemsize)
+    geom = _device_geometry(rnn.hidden_size, N, x.device, dt.itemsize, 2 if rnn.bidirectional else 1)
     return None if geom is None else (geom, dt)
+
+
+def _params(rnn: nn.LSTM) -> Tuple[torch.Tensor, ...]:
+    """W_ih, W_hh, b_ih, b_hh of each direction, forward direction first."""
+    return tuple(getattr(rnn, n + sfx) for sfx in (("_l0", "_l0_reverse") if rnn.bidirectional else ("_l0",))
+                 for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
 
 
 class _LstmLayer(torch.autograd.Function):
     """``dt``: the kernels' storage type.  fp32: every tensor is fp32.  bf16 / fp16: x and the parameters are cast to it
-    here, once per forward, and both passes run with autocast off, so that neither depends on the ambient state."""
+    here, once per forward, and both passes run with autocast off, so that neither depends on the ambient state.
+    ``ps``: W_ih, W_hh, b_ih, b_hh of one direction, or of the forward then the reverse direction."""
 
     @staticmethod
-    def forward(ctx, x, lens, w_ih, w_hh, b_ih, b_hh, geom, dt):
+    def forward(ctx, x, lens, geom, dt, *ps):
         C = ext.require()
         T, N, I = x.shape
-        H = w_hh.size(1)
+        dirs = len(ps) // 4
+        H = ps[1].size(1)
         with torch.autocast(x.device.type, enabled=False):
-            xs, w_ih, w_hh, b = x.to(dt), w_ih.to(dt), w_hh.to(dt), (b_ih + b_hh).to(dt)
-            gx = torch.addmm(b, xs.reshape(T * N, I), w_ih.t())                # (T N) x 4H
-        y = torch.empty(T, N, H, device=x.device, dtype=dt)
-        gates = torch.empty(T, N, 4 * H, device=x.device, dtype=torch.float32)
-        cs = torch.empty(T, N, H, device=x.device, dtype=torch.float32)
-        bar = torch.zeros(1, dtype=torch.int64, device=x.device)
-        C.lstm_forward(gx.data_ptr(), w_hh.data_ptr(), lens.data_ptr(), y.data_ptr(), gates.data_ptr(), cs.data_ptr(),
-                       bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows, torch.cuda.current_stream().cuda_stream,
-                       _DTYPE_CODE[dt])
-        ctx.save_for_backward(xs, lens, w_ih, w_hh, y, gates, cs)
+            xs = x.to(dt)
+            w_ih = [ps[4 * d].to(dt) for d in range(dirs)]
+            w_hh = [ps[4 * d + 1].to(dt) for d in range(dirs)]
+            gx = torch.empty(dirs, T * N, 4 * H, device=x.device, dtype=dt)
+            for d in range(dirs):
+                b = (ps[4 * d + 2] + ps[4 * d + 3]).to(dt)
+                torch.addmm(b, xs.reshape(T * N, I), w_ih[d].t(), out=gx[d])        # (T N) x 4H
+        y = torch.empty(dirs * T, N, H, device=x.device, dtype=dt)       # [dirs, T, N, H]; one direction: the output
+        gates = torch.empty(dirs, T, N, 4 * H, device=x.device, dtype=torch.float32)
+        cs = torch.empty(dirs, T, N, H, device=x.device, dtype=torch.float32)
+        bar = torch.zeros(dirs, dtype=torch.int64, device=x.device)
+        C.lstm_forward(gx.data_ptr(), w_hh[0].data_ptr(), lens.data_ptr(), y.data_ptr(), gates.data_ptr(),
+                       cs.data_ptr(), bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows,
+                       torch.cuda.current_stream().cuda_stream, _DTYPE_CODE[dt], w_hh[1].data_ptr() if dirs == 2 else 0)
+        ctx.save_for_backward(xs, lens, y, gates, cs, *w_ih, *w_hh)
         ctx.geom = geom
         ctx.x_dtype = x.dtype
-        return y
+        return y if dirs == 1 else y[:T] + y[T:]                 # stock_layer's sum of the two directions
 
     @staticmethod
     def backward(ctx, dy):
         C = ext.require()
-        x, lens, w_ih, w_hh, y, gates, cs = ctx.saved_tensors
+        x, lens, y, gates, cs, *ws = ctx.saved_tensors
+        dirs = len(ws) // 2
+        w_ih, w_hh = ws[:dirs], ws[dirs:]
         T, N, I = x.shape
-        H = w_hh.size(1)
+        y = y.view(dirs, T, N, -1)
+        H = w_hh[0].size(1)
         dt = y.dtype
         dy = dy.to(dt).contiguous()
-        dg = torch.empty(T, N, 4 * H, device=x.device, dtype=dt)
-        bar = torch.zeros(1, dtype=torch.int64, device=x.device)
-        C.lstm_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), w_hh.data_ptr(), lens.data_ptr(), dg.data_ptr(),
-                        bar.data_ptr(), T, N, H, ctx.geom.units, ctx.geom.bwd_rows,
-                        torch.cuda.current_stream().cuda_stream, _DTYPE_CODE[dt])
-        g2 = dg.view(T * N, 4 * H)
+        dg = torch.empty(dirs, T, N, 4 * H, device=x.device, dtype=dt)
+        bar = torch.zeros(dirs, dtype=torch.int64, device=x.device)
+        C.lstm_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), w_hh[0].data_ptr(), lens.data_ptr(),
+                        dg.data_ptr(), bar.data_ptr(), T, N, H, ctx.geom.units, ctx.geom.bwd_rows,
+                        torch.cuda.current_stream().cuda_stream, _DTYPE_CODE[dt],
+                        w_hh[1].data_ptr() if dirs == 2 else 0)
         need = ctx.needs_input_grad
+        grads = []
+        dx = None
         with torch.autocast(x.device.type, enabled=False):      # GEMMs in dt; the parameters' gradients come back fp32
-            dx = (g2 @ w_ih).view(T, N, I).to(ctx.x_dtype) if need[0] else None
-            dw_ih = (g2.t() @ x.reshape(T * N, I)).float() if need[2] else None
-            # h_{t-1} = y_{t-1}
-            dw_hh = (dg[1:].reshape(-1, 4 * H).t() @ y[:-1].reshape(-1, H)).float() if need[3] else None
-            db = g2.sum(0, dtype=torch.float32) if need[4] or need[5] else None
-        db_ih = db if need[4] else None
-        db_hh = (db.clone() if need[4] else db) if need[5] else None             # two tensors, never one aliased
-        return dx, None, dw_ih, dw_hh, db_ih, db_hh, None, None
+            for d in range(dirs):
+                g2 = dg[d].view(T * N, 4 * H)
+                n_ih, n_hh, n_bih, n_bhh = need[4 + 4 * d:8 + 4 * d]
+                if need[0]:
+                    dx = g2 @ w_ih[d] if d == 0 else dx.addmm_(g2, w_ih[d])
+                dw_ih = (g2.t() @ x.reshape(T * N, I)).float() if n_ih else None
+                # h_{t-1} = y_{t-1} forward; in reverse the previous step's h is y_{t+1}, which is 0 at t + 1 >= len
+                if d == 0:
+                    dw_hh = (dg[0, 1:].reshape(-1, 4 * H).t() @ y[0, :-1].reshape(-1, H)).float() if n_hh else None
+                else:
+                    dw_hh = (dg[1, :-1].reshape(-1, 4 * H).t() @ y[1, 1:].reshape(-1, H)).float() if n_hh else None
+                db = g2.sum(0, dtype=torch.float32) if n_bih or n_bhh else None
+                db_ih = db if n_bih else None
+                db_hh = (db.clone() if n_bih else db) if n_bhh else None         # two tensors, never one aliased
+                grads += [dw_ih, dw_hh, db_ih, db_hh]
+        if dx is not None:
+            dx = dx.view(T, N, I).to(ctx.x_dtype)
+        return (dx, None, None, None, *grads)
 
 
 def lstm_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, dev_lengths: Optional[torch.Tensor] = None,
-               autocast: bool = False) -> torch.Tensor:
+               autocast: bool = False, bidirectional: bool = False) -> torch.Tensor:
     """``rnn`` over ``x`` (T x N x I) with per-utterance ``lengths`` (host int tensor), as ``BatchRNN`` runs it; see the
     module docstring.  ``dev_lengths``: the same lengths as int32 on ``x``'s device, to share one copy between
-    layers.  ``autocast``: under bf16 / fp16 CUDA autocast, take the 16-bit kernels instead of the stock layer."""
-    ok = _native_ok(x, lengths, rnn, autocast)
+    layers.  ``autocast``: under bf16 / fp16 CUDA autocast, take the 16-bit kernels instead of the stock layer.
+    ``bidirectional``: a bidirectional ``rnn`` takes the kernels too, both directions in one launch, instead of the stock
+    layer."""
+    ok = _native_ok(x, lengths, rnn, autocast, bidirectional)
     if ok is None:
         return stock_layer(x, lengths, rnn)
     geom, dt = ok
     if dev_lengths is None or dev_lengths.device != x.device or dev_lengths.dtype != torch.int32:
         dev_lengths = lengths.to(device=x.device, dtype=torch.int32)
-    w_hh = rnn.weight_hh_l0.contiguous()
-    if dt == torch.float32 and w_hh.data_ptr() % 16:         # read as 16-byte vectors; a 16-bit copy is a fresh tensor
-        w_hh = w_hh.clone()
-    return _LstmLayer.apply(x.contiguous(), dev_lengths.contiguous(), rnn.weight_ih_l0, w_hh, rnn.bias_ih_l0,
-                            rnn.bias_hh_l0, geom, dt)
+    ps = list(_params(rnn))
+    for i in range(1, len(ps), 4):
+        w_hh = ps[i].contiguous()
+        if dt == torch.float32 and w_hh.data_ptr() % 16:     # read as 16-byte vectors; a 16-bit copy is a fresh tensor
+            w_hh = w_hh.clone()
+        ps[i] = w_hh
+    return _LstmLayer.apply(x.contiguous(), dev_lengths.contiguous(), geom, dt, *ps)

@@ -93,6 +93,12 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-lstm-autocast", action="store_true",
                    help="with --fused-lstm and --bf16 or --fp16: the LSTM layers take the 16-bit fused recurrence kernels "
                         "(default: stock layers under autocast)")
+    p.add_argument("--bidirectional", action="store_true",
+                   help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
+                        "(default: uni-directional)")
+    p.add_argument("--fused-lstm-bidirectional", action="store_true",
+                   help="with --fused-lstm and --bidirectional: both directions of each LSTM layer run on the fused "
+                        "recurrence kernels in one launch (default: stock bidirectional layers)")
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -138,6 +144,10 @@ def model_args(args: argparse.Namespace):
         model_kwargs["fuse_lstm"] = True
     if args.fused_lstm_autocast:
         model_kwargs["fuse_lstm_autocast"] = True
+    if args.bidirectional:
+        model_kwargs["bidirectional"] = True
+    if args.fused_lstm_bidirectional:
+        model_kwargs["fuse_lstm_bidirectional"] = True
     return dnn, model_kwargs
 
 
@@ -167,14 +177,21 @@ def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-lstm`` is for the AN4 DeepSpeech model (``--dnn lstman4``) only; ``--fused-lstm-autocast`` needs it and
-    one of ``--bf16`` / ``--fp16``."""
+    """``--fused-lstm`` and ``--bidirectional`` are for the AN4 DeepSpeech model (``--dnn lstman4``) only;
+    ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
+    needs ``--fused-lstm`` and ``--bidirectional``."""
     if args.fused_lstm and model_args(args)[0] != "lstman4":
         parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
     if args.fused_lstm_autocast and not args.fused_lstm:
         parser.error("--fused-lstm-autocast needs --fused-lstm")
     if args.fused_lstm_autocast and not (args.bf16 or args.fp16):
         parser.error("--fused-lstm-autocast needs --bf16 or --fp16")
+    if args.bidirectional and model_args(args)[0] != "lstman4":
+        parser.error("--bidirectional applies to lstman4, not %s" % model_args(args)[0])
+    if args.fused_lstm_bidirectional and not args.fused_lstm:
+        parser.error("--fused-lstm-bidirectional needs --fused-lstm")
+    if args.fused_lstm_bidirectional and not args.bidirectional:
+        parser.error("--fused-lstm-bidirectional needs --bidirectional")
 
 
 def main(argv=None) -> int:
