@@ -36,11 +36,9 @@
 // past S the log-sum-exp +inf, so their P is exactly 0, and nothing past S is stored.  16-bit stores round to nearest
 // even without saturating, so an overflow arrives as inf.  A sequence whose mask is -inf at every key has l = 0 and
 // lse2 = -inf in every row: its O and d(qkv) are NaN, as softmax over an all -inf row is.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 #include "devlib.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -137,7 +135,7 @@ template <typename T> struct AttnMma16 {        // bf16 / fp16, m16n8k16
     static __device__ __forceinline__ uint32_t pack_raw(const T* lo, const T* hi) {
         return (uint32_t)*reinterpret_cast<const uint16_t*>(lo) | ((uint32_t)*reinterpret_cast<const uint16_t*>(hi) << 16);
     }
-    static __device__ __forceinline__ uint32_t pack(float lo, float hi);
+    static __device__ __forceinline__ uint32_t pack(float lo, float hi) { return Elem<T>::narrow2(lo, hi); }
     static __device__ __forceinline__ A load_a(const T* s, int row0, int k0) {
         const int g = lane_id() >> 2, t = lane_id() & 3;
         const T* p0 = s + (row0 + g) * kAttLd + k0 + 2 * t;
@@ -162,14 +160,6 @@ template <typename T> struct AttnMma16 {        // bf16 / fp16, m16n8k16
     static __device__ __forceinline__ void mma(float (&d)[4], const A& a, const B& b);
 };
 
-template <> __device__ __forceinline__ uint32_t AttnMma16<__nv_bfloat16>::pack(float lo, float hi) {
-    const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&v);
-}
-template <> __device__ __forceinline__ uint32_t AttnMma16<__half>::pack(float lo, float hi) {
-    const __half2 v = __floats2half2_rn(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&v);
-}
 template <> __device__ __forceinline__ void AttnMma16<__nv_bfloat16>::mma(float (&d)[4], const A& a, const B& b) {
     asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
@@ -182,18 +172,6 @@ template <> __device__ __forceinline__ void AttnMma16<__half>::mma(float (&d)[4]
 }
 template <> struct AttnMma<__nv_bfloat16> : AttnMma16<__nv_bfloat16> {};
 template <> struct AttnMma<__half> : AttnMma16<__half> {};
-
-// ---- element access ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float att_f32(float x) { return x; }
-__device__ __forceinline__ float att_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
-__device__ __forceinline__ float att_f32(__half x) { return __half2float(x); }
-
-// two consecutive elements, rounded to nearest even (16-bit: no saturation, past the range -> inf)
-__device__ __forceinline__ void att_store2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
-__device__ __forceinline__ void att_store2(__nv_bfloat16* p, float a, float b) {
-    *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(a, b);
-}
-__device__ __forceinline__ void att_store2(__half* p, float a, float b) { *reinterpret_cast<__half2*>(p) = __floats2half2_rn(a, b); }
 
 // Stage rows [0, n) of a 64 x 64 block (global row stride `stride` elements, 16-byte aligned rows) into a padded
 // shared tile; rows n..63 are zeros.
@@ -345,7 +323,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const T* __restri
         const float inv = 1.f / l[r];
         T* orow = out + ((long long)b * S + i) * HD + h * kAttD + 2 * t;
 #pragma unroll
-        for (int nt = 0; nt < kAttNt; ++nt) att_store2(orow + nt * 8, o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
+        for (int nt = 0; nt < kAttNt; ++nt) Elem<T>::st2(orow + nt * 8, o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
         if (t == 0) lse[bh * S + i] = mx[r] + log2f(l[r]);
     }
 }
@@ -383,7 +361,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __res
             const T* orow = out + ((long long)b * S + i) * HD + h * kAttD + 16 * t;
             const T* drow = sdo + (row0 + g + 8 * r) * kAttLd + 16 * t;
 #pragma unroll
-            for (int x = 0; x < 16; ++x) acc = fmaf(att_f32(drow[x]), att_f32(orow[x]), acc);
+            for (int x = 0; x < 16; ++x) acc = fmaf(Elem<T>::f32(drow[x]), Elem<T>::f32(orow[x]), acc);
         }
         acc += __shfl_xor_sync(0xffffffffu, acc, 1);
         acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -421,7 +399,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __res
         if (i >= S) continue;
         T* row = dqkv + ((long long)b * S + i) * ld3 + h * kAttD + 2 * t;
 #pragma unroll
-        for (int nt = 0; nt < kAttNt; ++nt) att_store2(row + nt * 8, dq[nt][2 * r] * kAttScale, dq[nt][2 * r + 1] * kAttScale);
+        for (int nt = 0; nt < kAttNt; ++nt) Elem<T>::st2(row + nt * 8, dq[nt][2 * r] * kAttScale, dq[nt][2 * r + 1] * kAttScale);
     }
 }
 
@@ -495,8 +473,8 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __re
         T* row = dqkv + ((long long)b * S + j) * ld3 + h * kAttD + 2 * t;
 #pragma unroll
         for (int nt = 0; nt < kAttNt; ++nt) {
-            att_store2(row + HD + nt * 8, dk[nt][2 * r] * kAttScale, dk[nt][2 * r + 1] * kAttScale);
-            att_store2(row + 2 * HD + nt * 8, dv[nt][2 * r], dv[nt][2 * r + 1]);
+            Elem<T>::st2(row + HD + nt * 8, dk[nt][2 * r] * kAttScale, dk[nt][2 * r + 1] * kAttScale);
+            Elem<T>::st2(row + 2 * HD + nt * 8, dv[nt][2 * r], dv[nt][2 * r + 1]);
         }
     }
 }
@@ -563,30 +541,20 @@ static bool attn_args_ok(int B, int S, int H, long long keep_thr, const unsigned
 }
 
 cudaError_t launch_attn_forward(const void* qkv, const float* mask, const unsigned long long* seed, void* out, float* lse,
-                                int B, int S, int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream) {
+                                int B, int S, int H, long long keep_thr, float scale, Dtype dtype, cudaStream_t stream) {
     if (!attn_args_ok(B, S, H, keep_thr, seed)) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32: return attn_forward_t<float>(qkv, mask, seed, out, lse, B, S, H, keep_thr, scale, stream);
-        case BnDtype::kBF16: return attn_forward_t<__nv_bfloat16>(qkv, mask, seed, out, lse, B, S, H, keep_thr, scale, stream);
-        case BnDtype::kF16: return attn_forward_t<__half>(qkv, mask, seed, out, lse, B, S, H, keep_thr, scale, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return attn_forward_t<decltype(e)>(qkv, mask, seed, out, lse, B, S, H, keep_thr, scale, stream);
+    });
 }
 
 cudaError_t launch_attn_backward(const void* qkv, const void* out, const void* dout, const float* mask,
                                  const unsigned long long* seed, const float* lse, float* delta, void* dqkv, int B, int S,
-                                 int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream) {
+                                 int H, long long keep_thr, float scale, Dtype dtype, cudaStream_t stream) {
     if (!attn_args_ok(B, S, H, keep_thr, seed)) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32:
-            return attn_backward_t<float>(qkv, out, dout, mask, seed, lse, delta, dqkv, B, S, H, keep_thr, scale, stream);
-        case BnDtype::kBF16:
-            return attn_backward_t<__nv_bfloat16>(qkv, out, dout, mask, seed, lse, delta, dqkv, B, S, H, keep_thr, scale,
-                                                  stream);
-        case BnDtype::kF16:
-            return attn_backward_t<__half>(qkv, out, dout, mask, seed, lse, delta, dqkv, B, S, H, keep_thr, scale, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return attn_backward_t<decltype(e)>(qkv, out, dout, mask, seed, lse, delta, dqkv, B, S, H, keep_thr, scale, stream);
+    });
 }
 
 }  // namespace okt

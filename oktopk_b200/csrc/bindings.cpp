@@ -525,9 +525,9 @@ static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, do
 // dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case).
 // res (forward and backward) and dres (backward), 0 = absent: y = relu(bn(x) + res) and dres = the residual's gradient,
 // [M, C] in x's dtype, with relu = 1 and W = 0.
-static BnDtype bn_dtype(int dtype, const char* what) {
+static Dtype dtype_arg(int dtype, const char* what) {
     if (dtype < 0 || dtype > 2) throw std::runtime_error(std::string(what) + ": dtype must be 0 (fp32), 1 (bf16) or 2 (fp16)");
-    return static_cast<BnDtype>(dtype);
+    return static_cast<Dtype>(dtype);
 }
 static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, uint64_t gamma, uint64_t beta, uint64_t cbias,
                        uint64_t save_mean, uint64_t save_invstd, uint64_t rmean, uint64_t rvar, uint64_t nbt, double momentum,
@@ -539,7 +539,7 @@ static void bn_forward(uint64_t x, uint64_t y, uint64_t arg, uint64_t partial, u
     ck(launch_bn_forward(P_<const void>(x), P_<void>(y), P_<unsigned char>(arg), P_<float>(partial), P_<const float>(gamma),
                          P_<const float>(beta), P_<const float>(cbias), P_<float>(save_mean), P_<float>(save_invstd),
                          P_<float>(rmean), P_<float>(rvar), P_<long long>(nbt), (float)momentum, (float)eps, relu, M, C, W, slot,
-                         max_ctas, bn_dtype(dtype, "bn_forward"), S_(stream), P_<const void>(res)), "bn_forward");
+                         max_ctas, dtype_arg(dtype, "bn_forward"), S_(stream), P_<const void>(res)), "bn_forward");
 }
 static void bn_backward(uint64_t x, uint64_t dy, uint64_t arg, uint64_t dx, uint64_t partial, uint64_t gamma, uint64_t beta,
                         uint64_t save_mean, uint64_t save_invstd, uint64_t dgamma, uint64_t dbeta, int relu, int M, int C, int W,
@@ -549,11 +549,11 @@ static void bn_backward(uint64_t x, uint64_t dy, uint64_t arg, uint64_t dx, uint
     if (res != 0 && (W != 0 || !relu)) throw std::runtime_error("bn_backward: a residual needs relu = 1 and no pool");
     ck(launch_bn_backward(P_<const void>(x), P_<const void>(dy), P_<const unsigned char>(arg), P_<void>(dx), P_<float>(partial),
                           P_<const float>(gamma), P_<const float>(beta), P_<const float>(save_mean), P_<const float>(save_invstd),
-                          P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, bn_dtype(dtype, "bn_backward"),
+                          P_<float>(dgamma), P_<float>(dbeta), relu, M, C, W, slot, max_ctas, dtype_arg(dtype, "bn_backward"),
                           S_(stream), P_<const void>(res), P_<void>(dres)), "bn_backward");
 }
 // y = LayerNorm(x + dropout(a)) over R rows of H: x, y, gamma, beta, mean, rstd (and in the backward dy, dx, dgamma,
-// dbeta) fp32; a and da of type a_dtype (codes as bn_dtype).  seed: one int64 in device memory, read by the kernels;
+// dbeta) fp32; a and da of type a_dtype (codes as dtype_arg).  seed: one int64 in device memory, read by the kernels;
 // p_keep_thr = floor((1-p) 2^32), or 2^32 for no dropout (seed may then be 0).  partial: ln_bwd_grid(R) * 2H floats.
 static void ln_check(const char* what, int R, int H, long long p_keep_thr, uint64_t seed, uint64_t mean, uint64_t rstd,
                      std::initializer_list<uint64_t> vec_ptrs) {
@@ -570,7 +570,7 @@ static void ln_forward(uint64_t x, uint64_t a, uint64_t y, uint64_t gamma, uint6
     ln_check("ln_forward", R, H, p_keep_thr, seed, mean, rstd, {x, a, y, gamma, beta});
     ck(launch_ln_forward(P_<const float>(x), P_<const void>(a), P_<float>(y), P_<const float>(gamma), P_<const float>(beta),
                          P_<float>(mean), P_<float>(rstd), P_<const unsigned long long>(seed), R, H, p_keep_thr, (float)scale,
-                         (float)eps, bn_dtype(a_dtype, "ln_forward"), S_(stream)), "ln_forward");
+                         (float)eps, dtype_arg(a_dtype, "ln_forward"), S_(stream)), "ln_forward");
 }
 static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uint64_t mean, uint64_t rstd, uint64_t seed,
                         uint64_t dx, uint64_t da, uint64_t partial, uint64_t dgamma, uint64_t dbeta, int R, int H,
@@ -579,10 +579,10 @@ static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uin
     ck(launch_ln_backward(P_<const float>(x), P_<const void>(a), P_<const float>(dy), P_<const float>(gamma),
                           P_<const float>(mean), P_<const float>(rstd), P_<const unsigned long long>(seed), P_<float>(dx),
                           P_<void>(da), P_<float>(partial), P_<float>(dgamma), P_<float>(dbeta), R, H, p_keep_thr,
-                          (float)scale, bn_dtype(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
+                          (float)scale, dtype_arg(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
 }
 // Fused self-attention, head dim 64 (csrc/attention.cu): qkv / dqkv [B, S, 3 H 64] and out / dout [B, S, H 64] of type
-// dtype (codes as bn_dtype), 16-byte aligned; mask [B, S] fp32 or 0; lse / delta [B, H, S] fp32.  p_keep_thr and seed as
+// dtype (codes as dtype_arg), 16-byte aligned; mask [B, S] fp32 or 0; lse / delta [B, H, S] fp32.  p_keep_thr and seed as
 // for ln_forward; scale = 1 / (1 - p).
 static void attn_check(const char* what, int B, int S, int H, long long p_keep_thr, uint64_t seed,
                        std::initializer_list<uint64_t> vec_ptrs, std::initializer_list<uint64_t> f32_ptrs) {
@@ -599,7 +599,7 @@ static void attn_forward(uint64_t qkv, uint64_t mask, uint64_t seed, uint64_t ou
     attn_check("attn_forward", B, S, H, p_keep_thr, seed, {qkv, out}, {lse});
     if (mask & 3) throw std::runtime_error("attn_forward: the mask must be fp32");
     ck(launch_attn_forward(P_<const void>(qkv), P_<const float>(mask), P_<const unsigned long long>(seed), P_<void>(out),
-                           P_<float>(lse), B, S, H, p_keep_thr, (float)scale, bn_dtype(dtype, "attn_forward"), S_(stream)),
+                           P_<float>(lse), B, S, H, p_keep_thr, (float)scale, dtype_arg(dtype, "attn_forward"), S_(stream)),
        "attn_forward");
 }
 static void attn_backward(uint64_t qkv, uint64_t out, uint64_t dout, uint64_t mask, uint64_t seed, uint64_t lse,
@@ -609,10 +609,10 @@ static void attn_backward(uint64_t qkv, uint64_t out, uint64_t dout, uint64_t ma
     if (mask & 3) throw std::runtime_error("attn_backward: the mask must be fp32");
     ck(launch_attn_backward(P_<const void>(qkv), P_<const void>(out), P_<const void>(dout), P_<const float>(mask),
                             P_<const unsigned long long>(seed), P_<const float>(lse), P_<float>(delta), P_<void>(dqkv), B, S,
-                            H, p_keep_thr, (float)scale, bn_dtype(dtype, "attn_backward"), S_(stream)),
+                            H, p_keep_thr, (float)scale, dtype_arg(dtype, "attn_backward"), S_(stream)),
        "attn_backward");
 }
-// Softmax cross-entropy over R rows of V logits (x, dx of type dtype, codes as bn_dtype), targets t int64, mean over the
+// Softmax cross-entropy over R rows of V logits (x, dx of type dtype, codes as dtype_arg), targets t int64, mean over the
 // rows whose target is not ignore_index.  lse: R + 1 floats (the rows' log-sum-exp, then n); rowloss: R floats; loss and
 // g: one float each, in device memory.
 static void xent_check(const char* what, int R, long long V, std::initializer_list<uint64_t> ptrs, uint64_t x, uint64_t t) {
@@ -625,14 +625,14 @@ static void xent_forward(uint64_t x, uint64_t t, uint64_t lse, uint64_t rowloss,
                          long long ignore_index, int dtype, uint64_t stream) {
     xent_check("xent_forward", R, V, {x, t, lse, rowloss, loss}, x, t);
     ck(launch_xent_forward(P_<const void>(x), P_<const long long>(t), P_<float>(lse), P_<float>(rowloss), P_<float>(loss),
-                           R, V, ignore_index, bn_dtype(dtype, "xent_forward"), S_(stream)), "xent_forward");
+                           R, V, ignore_index, dtype_arg(dtype, "xent_forward"), S_(stream)), "xent_forward");
 }
 static void xent_backward(uint64_t x, uint64_t t, uint64_t lse, uint64_t g, uint64_t dx, int R, long long V,
                           long long ignore_index, int dtype, uint64_t stream) {
     xent_check("xent_backward", R, V, {x, t, lse, g, dx}, x, t);
     if (dx & 15) throw std::runtime_error("xent_backward: the gradient must be 16-byte aligned");
     ck(launch_xent_backward(P_<const void>(x), P_<const long long>(t), P_<const float>(lse), P_<const float>(g), P_<void>(dx),
-                            R, V, ignore_index, bn_dtype(dtype, "xent_backward"), S_(stream)), "xent_backward");
+                            R, V, ignore_index, dtype_arg(dtype, "xent_backward"), S_(stream)), "xent_backward");
 }
 // Fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels [R] int64, rows [M] int32, tgt [M]
 // int64, slot [R] int32, count one int64, overflow one int64 or 0; x / dx [R, H] and out / dout [M, H] of type dtype.
@@ -645,35 +645,35 @@ static void mlm_select(uint64_t labels, uint64_t rows, uint64_t tgt, uint64_t sl
     ck(launch_mlm_select(P_<const long long>(labels), R, ignore_index, M, P_<int>(rows), P_<long long>(tgt),
                          P_<int>(slot), P_<long long>(count), P_<long long>(overflow), S_(stream)), "mlm_select");
 }
-static void mlm_copy_check(const char* what, int nrows, int H, uint64_t src, uint64_t idx, uint64_t dst, BnDtype dt) {
+static void mlm_copy_check(const char* what, int nrows, int H, uint64_t src, uint64_t idx, uint64_t dst, Dtype dt) {
     if (nrows <= 0 || H <= 0) throw std::runtime_error(std::string(what) + ": needs rows > 0 and H > 0");
     if (!src || !idx || !dst) throw std::runtime_error(std::string(what) + ": null pointer");
-    const uint64_t mask = dt == BnDtype::kF32 ? 3 : 1;
+    const uint64_t mask = dt == Dtype::kF32 ? 3 : 1;
     if ((src & mask) || (dst & mask) || (idx & 3)) throw std::runtime_error(std::string(what) + ": misaligned pointer");
 }
 static void mlm_gather(uint64_t x, uint64_t rows, uint64_t out, int M, int H, int dtype, uint64_t stream) {
-    const BnDtype dt = bn_dtype(dtype, "mlm_gather");
+    const Dtype dt = dtype_arg(dtype, "mlm_gather");
     mlm_copy_check("mlm_gather", M, H, x, rows, out, dt);
     ck(launch_mlm_gather(P_<const void>(x), P_<const int>(rows), P_<void>(out), M, H, dt, S_(stream)), "mlm_gather");
 }
 static void mlm_scatter(uint64_t dout, uint64_t slot, uint64_t dx, int R, int H, int dtype, uint64_t stream) {
-    const BnDtype dt = bn_dtype(dtype, "mlm_scatter");
+    const Dtype dt = dtype_arg(dtype, "mlm_scatter");
     mlm_copy_check("mlm_scatter", R, H, dout, slot, dx, dt);
     ck(launch_mlm_scatter(P_<const void>(dout), P_<const int>(slot), P_<void>(dx), R, H, dt, S_(stream)), "mlm_scatter");
 }
 // Persistent LSTM recurrence (csrc/lstm.cu), time-major: gx [T, N, 4H], whh [4H, H], len [N] int32 in [1, T],
 // y / cs [T, N, H], gates / dy / dg as named; bar: one zeroed int64.  u hidden units per CTA, `rows` batch rows staged at
-// a time (ops/fused_lstm.lstm_geometry).  gx, whh, y, dy and dg are of type dtype (codes as bn_dtype), gates and cs fp32.
+// a time (ops/fused_lstm.lstm_geometry).  gx, whh, y, dy and dg are of type dtype (codes as dtype_arg), gates and cs fp32.
 // whh_rev != 0 (the reverse direction's W_hh) runs both directions of a bidirectional layer in the one launch: gx, y,
 // cs, gates and dg are then [2, T, N, .], forward direction first, dy is the same [T, N, H] for both, and bar is two
 // zeroed int64, one per direction.
-static void lstm_check(const char* what, int T, int N, int H, int u, int rows, BnDtype dtype,
+static void lstm_check(const char* what, int T, int N, int H, int u, int rows, Dtype dtype,
                        std::initializer_list<uint64_t> ptrs, std::initializer_list<uint64_t> vec_ptrs, uint64_t bar) {
     if (T <= 0 || N <= 0 || H <= 0 || H % 4 || u <= 0 || rows <= 0 || rows > N)
         throw std::runtime_error(std::string(what) + ": needs T, N > 0, H > 0 a multiple of 4, u > 0 and 0 < rows <= N");
     for (uint64_t p : ptrs)
         if (p == 0) throw std::runtime_error(std::string(what) + ": null pointer");
-    const uint64_t mask = dtype == BnDtype::kF32 ? 15 : 7;            // read four elements at a time
+    const uint64_t mask = dtype == Dtype::kF32 ? 15 : 7;            // read four elements at a time
     for (uint64_t p : vec_ptrs)
         if (p & mask)
             throw std::runtime_error(std::string(what) + ": W_hh (both directions') and the staged operand must be " +
@@ -682,7 +682,7 @@ static void lstm_check(const char* what, int T, int N, int H, int u, int rows, B
 }
 static void lstm_forward(uint64_t gx, uint64_t whh, uint64_t len, uint64_t y, uint64_t gates, uint64_t cs, uint64_t bar,
                          int T, int N, int H, int u, int rows, uint64_t stream, int dtype, uint64_t whh_rev) {
-    const BnDtype dt = bn_dtype(dtype, "lstm_forward");
+    const Dtype dt = dtype_arg(dtype, "lstm_forward");
     lstm_check("lstm_forward", T, N, H, u, rows, dt, {gx, whh, len, y, gates, cs, bar}, {whh, whh_rev, y}, bar);
     ck(launch_lstm_forward(P_<const void>(gx), P_<const void>(whh), P_<const void>(whh_rev), P_<const int>(len),
                            P_<void>(y), P_<float>(gates), P_<float>(cs), P_<unsigned long long>(bar), T, N, H, u, rows,
@@ -691,7 +691,7 @@ static void lstm_forward(uint64_t gx, uint64_t whh, uint64_t len, uint64_t y, ui
 }
 static void lstm_backward(uint64_t dy, uint64_t gates, uint64_t cs, uint64_t whh, uint64_t len, uint64_t dg, uint64_t bar,
                           int T, int N, int H, int u, int rows, uint64_t stream, int dtype, uint64_t whh_rev) {
-    const BnDtype dt = bn_dtype(dtype, "lstm_backward");
+    const Dtype dt = dtype_arg(dtype, "lstm_backward");
     lstm_check("lstm_backward", T, N, H, u, rows, dt, {dy, gates, cs, whh, len, dg, bar}, {dg}, bar);
     ck(launch_lstm_backward(P_<const void>(dy), P_<const float>(gates), P_<const float>(cs), P_<const void>(whh),
                             P_<const void>(whh_rev), P_<const int>(len), P_<void>(dg), P_<unsigned long long>(bar), T, N,

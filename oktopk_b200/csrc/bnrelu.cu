@@ -59,26 +59,18 @@
 // (128-bit accesses) and strides over rows; tiles are contiguous row ranges.  With a pool, a tile is a whole number of
 // image row pairs (rows_per_block % 2W == 0), so no 2x2 window straddles two tiles.
 //
-// Activation type (BnAct): x, y, dy and dx are fp32 (one float4 per access), bf16 or fp16 (four 16-bit values in one
-// 8-byte access).  A bf16 or fp16 load is widened to a float4, which is exact, and from there the arithmetic is the fp32
-// kernel's, operation for operation: same tiles, partials, combine, running-statistic fma, ReLU mask, pool arg-max and
-// dx formula.  Only the stores of y and dx round to the 16-bit type (to nearest, ties to even).  The bf16 and fp16
-// kernels are therefore, bit for bit, the fp32 kernel run on x.float() (and dy.float()) with y and dx rounded.  gamma,
-// beta, the conv bias, the running and saved statistics, the partials and dgamma / dbeta stay fp32 in every case, as in
-// torch's batch-norm under autocast.
-//
-// fp16 has three more significand bits than bf16 but a far narrower range, so its range rules are part of the spec:
-//   - overflow: a y or dx whose magnitude rounds past 65504 is stored as +-inf, as torch's .half() does.  Under loss
-//     scaling a too-large scaled gradient overflowing in dx is the normal way an fp16 step overflows; the inf must reach
-//     the optimizer's non-finite check, so nothing is saturated or clamped;
-//   - subnormals: results below 2^-14 in magnitude are rounded to fp16 subnormals, not flushed to zero (cvt.rn.f16x2.f32
-//     without .ftz; the build does not pass -ftz or --use_fast_math), and subnormal inputs widen exactly;
-//   - non-finite inputs: an inf or NaN in x or dy propagates exactly as in the fp32 kernel on the widened input, into
-//     the statistics and the running statistics too (as stock batch-norm does).  There is no extra finite check.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
+// Activation type: x, y, dy and dx are fp32 (one float4 per access), bf16 or fp16 (four 16-bit values in one 8-byte
+// access), converted by elem.cuh's Elem.  A bf16 or fp16 load is widened to a float4, which is exact, and from there the
+// arithmetic is the fp32 kernel's, operation for operation: same tiles, partials, combine, running-statistic fma, ReLU
+// mask, pool arg-max and dx formula.  Only the stores of y and dx round to the 16-bit type, under elem.cuh's contract (to
+// nearest even; an fp16 overflow is +-inf, which under loss scaling is how an fp16 step overflows and must reach the
+// optimizer's non-finite check; fp16 subnormals are kept).  The bf16 and fp16 kernels are therefore, bit for bit, the
+// fp32 kernel run on x.float() (and dy.float()) with y and dx rounded.  An inf or NaN in x or dy propagates as in that
+// kernel, into the statistics and the running statistics too (as stock batch-norm does); there is no extra finite
+// check.  gamma, beta, the conv bias, the running and saved statistics, the partials and dgamma / dbeta stay fp32 in
+// every case, as in torch's batch-norm under autocast.
 #include "common.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -134,37 +126,6 @@ __host__ __device__ inline BnGeom bn_geom(int M, int C) {
 __device__ __forceinline__ float4 f4_fma(const float4& x, const float4& a, const float4& b) {
     return make_float4(fmaf(x.x, a.x, b.x), fmaf(x.y, a.y, b.y), fmaf(x.z, a.z, b.z), fmaf(x.w, a.w, b.w));
 }
-
-// Four consecutive channels of an activation in storage (V), widened to fp32 for arithmetic and narrowed for a store.
-template <typename T> struct BnAct;
-template <> struct BnAct<float> {
-    using V = float4;
-    static __device__ __forceinline__ float4 wide(const float4& v) { return v; }
-    static __device__ __forceinline__ float4 narrow(const float4& v) { return v; }
-};
-template <> struct BnAct<__nv_bfloat16> {
-    using V = uint2;                          // channels 0, 1 in x (low half first), 2, 3 in y
-    static __device__ __forceinline__ float4 wide(const uint2& v) {   // a bf16 is the high half of its fp32: exact
-        return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u), __uint_as_float(v.y << 16),
-                           __uint_as_float(v.y & 0xffff0000u));
-    }
-    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // round to nearest, ties to even
-        const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
-    }
-};
-template <> struct BnAct<__half> {
-    using V = uint2;                          // channels 0, 1 in x (low half first), 2, 3 in y
-    static __device__ __forceinline__ float4 wide(const uint2& v) {   // every fp16, subnormals included, is an fp32: exact
-        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-        return make_float4(lo.x, lo.y, hi.x, hi.y);
-    }
-    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // nearest even; past 65504 -> inf; no flush to zero
-        const __half2 lo = __floats2half2_rn(v.x, v.y), hi = __floats2half2_rn(v.z, v.w);
-        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
-    }
-};
 
 // one step of a 2x2 max-pool window: first maximum in row-major window order wins, NaN propagates (as at::max_pool2d)
 __device__ __forceinline__ void pool_step(float4& m, uchar4& a, const float4& v, unsigned char k) {
@@ -372,7 +333,7 @@ __device__ __forceinline__ void bn_scale_shift(const BnFwdArgs<T>& p, int c, flo
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
-    using A = BnAct<T>;
+    using A = Elem<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals, then a = gamma/std, b = beta - mean a | pool: held y
     __shared__ float4 s_red[2 * kBnThreads];
@@ -514,7 +475,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_fwd_kernel(const BnFwdArgs<T> p
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_fwd_sliced_kernel(const BnFwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
-    using A = BnAct<T>;
+    using A = Elem<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // bn_slice_reduce's scratch, then with a pool the slice's y, [M][sc]
     __shared__ float4 s_tot[2 * 8], s_ab[2 * 8];   // the owned columns' totals [sc] | [sc]; a = gamma/std [sc] | b [sc]
@@ -608,7 +569,7 @@ struct BnCol { float4 mean, istd, a, b; };
 
 template <bool kPool, bool kRes, typename T>
 struct BnBwdElem {
-    using A = BnAct<T>;
+    using A = Elem<T>;
     using V = typename A::V;
     const BnBwdArgs<T>& p;
 
@@ -683,7 +644,7 @@ struct BnBwdElem {
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
-    using A = BnAct<T>;
+    using A = Elem<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // [2][cv] combine totals
     __shared__ float4 s_red[2 * kBnThreads];
@@ -808,7 +769,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_kernel(const BnBwdArgs<T> p
 template <bool kPool, bool kRes, typename T>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_sliced_kernel(const BnBwdArgs<T> p) {
     static_assert(!(kPool && kRes), "no pool follows a residual add");
-    using A = BnAct<T>;
+    using A = Elem<T>;
     using V = typename A::V;
     extern __shared__ float4 s_dyn[];         // bn_slice_reduce's scratch
     __shared__ float4 s_tot[2 * 8];           // [sc] dbeta | [sc] dgamma of the owned columns
@@ -960,38 +921,22 @@ static cudaError_t bn_backward_t(const void* x, const void* dy, const unsigned c
 
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
-                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, Dtype dtype,
                               cudaStream_t stream, const void* res) {
-    switch (dtype) {
-        case BnDtype::kF32:
-            return bn_forward_t<float>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
-                                       momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
-        case BnDtype::kBF16:
-            return bn_forward_t<__nv_bfloat16>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar,
-                                               nbt, momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
-        case BnDtype::kF16:
-            return bn_forward_t<__half>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
-                                        momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return bn_forward_t<decltype(e)>(x, y, arg, partial, gamma, beta, cbias, save_mean, save_invstd, rmean, rvar, nbt,
+                                         momentum, eps, relu, M, C, W, slot, max_ctas, stream, res);
+    });
 }
 
 cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
                                const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
-                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, Dtype dtype,
                                cudaStream_t stream, const void* res, void* dres) {
-    switch (dtype) {
-        case BnDtype::kF32:
-            return bn_backward_t<float>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
-                                        M, C, W, slot, max_ctas, stream, res, dres);
-        case BnDtype::kBF16:
-            return bn_backward_t<__nv_bfloat16>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta,
-                                                relu, M, C, W, slot, max_ctas, stream, res, dres);
-        case BnDtype::kF16:
-            return bn_backward_t<__half>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta, relu,
-                                         M, C, W, slot, max_ctas, stream, res, dres);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return bn_backward_t<decltype(e)>(x, dy, arg, dx, partial, gamma, beta, save_mean, save_invstd, dgamma, dbeta,
+                                          relu, M, C, W, slot, max_ctas, stream, res, dres);
+    });
 }
 
 }  // namespace okt

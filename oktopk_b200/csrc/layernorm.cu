@@ -30,11 +30,9 @@
 // autocast the residual stream and layer_norm stay fp32 while the linear layer hands over 16-bit output).  A 16-bit a is
 // widened on load, exactly; da is rounded once (to nearest even) from the fp32 dz keep s.  The 16-bit kernels are
 // therefore, bit for bit, the fp32 kernel run on a.float() with da rounded.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 #include "devlib.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -44,37 +42,6 @@ constexpr int kLnThreads = 32 * kLnWarps;
 constexpr int kLnFwdMaxBlocks = 8192;
 constexpr int kLnBwdMaxBlocks = 256;           // rows of the backward pass's column partials
 constexpr long long kLnKeepAll = 1LL << 32;
-
-// Four consecutive elements of a (storage V), widened to fp32, and of da, narrowed from fp32.
-template <typename T> struct LnAct;
-template <> struct LnAct<float> {
-    using V = float4;
-    static __device__ __forceinline__ float4 wide(const float4& v) { return v; }
-    static __device__ __forceinline__ float4 narrow(const float4& v) { return v; }
-};
-template <> struct LnAct<__nv_bfloat16> {
-    using V = uint2;                           // elements 0, 1 in x (low half first), 2, 3 in y
-    static __device__ __forceinline__ float4 wide(const uint2& v) {   // a bf16 is the high half of its fp32: exact
-        return make_float4(__uint_as_float(v.x << 16), __uint_as_float(v.x & 0xffff0000u), __uint_as_float(v.y << 16),
-                           __uint_as_float(v.y & 0xffff0000u));
-    }
-    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // round to nearest, ties to even
-        const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
-    }
-};
-template <> struct LnAct<__half> {
-    using V = uint2;
-    static __device__ __forceinline__ float4 wide(const uint2& v) {   // every fp16 is an fp32: exact
-        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-        return make_float4(lo.x, lo.y, hi.x, hi.y);
-    }
-    static __device__ __forceinline__ uint2 narrow(const float4& v) {  // nearest even; past 65504 -> inf; no flush
-        const __half2 lo = __floats2half2_rn(v.x, v.y), hi = __floats2half2_rn(v.z, v.w);
-        return make_uint2(*reinterpret_cast<const unsigned int*>(&lo), *reinterpret_cast<const unsigned int*>(&hi));
-    }
-};
 
 struct LnDrop {
     bool on;
@@ -111,7 +78,7 @@ __device__ __forceinline__ float4 ln_mult(const LnDrop& d, uint32_t keep) {
 template <typename T>
 __device__ __forceinline__ float4 ln_z(const float* x, const T* a, const float4& m, size_t off) {
     const float4 xv = *reinterpret_cast<const float4*>(x + off);
-    const float4 av = LnAct<T>::wide(*reinterpret_cast<const typename LnAct<T>::V*>(a + off));
+    const float4 av = Elem<T>::wide(*reinterpret_cast<const typename Elem<T>::V*>(a + off));
     return make_float4(fmaf(av.x, m.x, xv.x), fmaf(av.y, m.y, xv.y), fmaf(av.z, m.z, xv.z), fmaf(av.w, m.w, xv.w));
 }
 
@@ -200,8 +167,8 @@ __global__ void __launch_bounds__(kLnThreads, 1) ln_bwd_kernel(const float* __re
                                           rs * (g[j].z - c1 - xh[j].z * c2), rs * (g[j].w - c1 - xh[j].w * c2));
             const float4 m = ln_mult(d, keep >> (4 * j));
             *reinterpret_cast<float4*>(dx + base + col) = dz;
-            *reinterpret_cast<typename LnAct<T>::V*>(da + base + col) =
-                LnAct<T>::narrow(make_float4(dz.x * m.x, dz.y * m.y, dz.z * m.z, dz.w * m.w));
+            *reinterpret_cast<typename Elem<T>::V*>(da + base + col) =
+                Elem<T>::narrow(make_float4(dz.x * m.x, dz.y * m.y, dz.z * m.z, dz.w * m.w));
         }
     }
     // the CTA's column partials, warps added in warp order
@@ -299,36 +266,22 @@ static bool ln_args_ok(int R, int H, long long keep_thr, const unsigned long lon
 
 cudaError_t launch_ln_forward(const float* x, const void* a, float* y, const float* gamma, const float* beta, float* mean,
                               float* rstd, const unsigned long long* seed, int R, int H, long long keep_thr, float scale,
-                              float eps, BnDtype a_dtype, cudaStream_t stream) {
+                              float eps, Dtype a_dtype, cudaStream_t stream) {
     if (!ln_args_ok(R, H, keep_thr, seed)) return cudaErrorInvalidValue;
-    switch (a_dtype) {
-        case BnDtype::kF32:
-            return ln_forward_t<float>(x, a, y, gamma, beta, mean, rstd, seed, R, H, keep_thr, scale, eps, stream);
-        case BnDtype::kBF16:
-            return ln_forward_t<__nv_bfloat16>(x, a, y, gamma, beta, mean, rstd, seed, R, H, keep_thr, scale, eps, stream);
-        case BnDtype::kF16:
-            return ln_forward_t<__half>(x, a, y, gamma, beta, mean, rstd, seed, R, H, keep_thr, scale, eps, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(a_dtype, [&](auto e) {
+        return ln_forward_t<decltype(e)>(x, a, y, gamma, beta, mean, rstd, seed, R, H, keep_thr, scale, eps, stream);
+    });
 }
 
 cudaError_t launch_ln_backward(const float* x, const void* a, const float* dy, const float* gamma, const float* mean,
                                const float* rstd, const unsigned long long* seed, float* dx, void* da, float* partial,
-                               float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, BnDtype a_dtype,
+                               float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, Dtype a_dtype,
                                cudaStream_t stream) {
     if (!ln_args_ok(R, H, keep_thr, seed)) return cudaErrorInvalidValue;
-    switch (a_dtype) {
-        case BnDtype::kF32:
-            return ln_backward_t<float>(x, a, dy, gamma, mean, rstd, seed, dx, da, partial, dgamma, dbeta, R, H, keep_thr,
-                                        scale, stream);
-        case BnDtype::kBF16:
-            return ln_backward_t<__nv_bfloat16>(x, a, dy, gamma, mean, rstd, seed, dx, da, partial, dgamma, dbeta, R, H,
-                                                keep_thr, scale, stream);
-        case BnDtype::kF16:
-            return ln_backward_t<__half>(x, a, dy, gamma, mean, rstd, seed, dx, da, partial, dgamma, dbeta, R, H, keep_thr,
-                                         scale, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(a_dtype, [&](auto e) {
+        return ln_backward_t<decltype(e)>(x, a, dy, gamma, mean, rstd, seed, dx, da, partial, dgamma, dbeta, R, H, keep_thr,
+                                          scale, stream);
+    });
 }
 
 }  // namespace okt

@@ -44,10 +44,8 @@
 // state at len_n - 1 (packed-sequence semantics), writes every time once, and writes exact zeros at t >= len_n like the
 // forward one.  What the forward direction indexes by t (gx, gates, c, y, dy, dgates; h_{t-1} = y at pi(s - 1),
 // dgates_{t+1} at pi(s + 1), c_{t-1} at pi(s - 1)) the reverse one indexes by pi.
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include "common.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -86,46 +84,13 @@ __device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + exp
 // The time that row n (length L) of a direction works on at step s (the file header's pi).
 __device__ __forceinline__ int lstm_time(int s, int L, bool rev) { return rev && s < L ? L - 1 - s : s; }
 
-// Storage type S: Vec holds four elements (16 bytes of float, 8 bytes of a 16-bit type), widen() makes them floats,
-// narrow() rounds one float to nearest even without saturating.
-template <typename S> struct LstmEl;
-template <> struct LstmEl<float> {
-    using Vec = float4;
-    static __device__ __forceinline__ Vec zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-    static __device__ __forceinline__ float4 widen(const Vec& v) { return v; }
-    static __device__ __forceinline__ float ld(const float* p) { return __ldg(p); }
-    static __device__ __forceinline__ float narrow(float v) { return v; }
-};
-template <> struct LstmEl<__nv_bfloat16> {
-    using Vec = uint2;
-    static __device__ __forceinline__ Vec zero() { return make_uint2(0u, 0u); }
-    static __device__ __forceinline__ float4 widen(const Vec& v) {
-        const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.x));
-        const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.y));
-        return make_float4(lo.x, lo.y, hi.x, hi.y);
-    }
-    static __device__ __forceinline__ float ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
-    static __device__ __forceinline__ __nv_bfloat16 narrow(float v) { return __float2bfloat16_rn(v); }
-};
-template <> struct LstmEl<__half> {
-    using Vec = uint2;
-    static __device__ __forceinline__ Vec zero() { return make_uint2(0u, 0u); }
-    static __device__ __forceinline__ float4 widen(const Vec& v) {
-        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-        const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-        return make_float4(lo.x, lo.y, hi.x, hi.y);
-    }
-    static __device__ __forceinline__ float ld(const __half* p) { return __half2float(__ldg(p)); }
-    static __device__ __forceinline__ __half narrow(float v) { return __float2half_rn(v); }
-};
-
 // Copy batch rows [n0, n0 + nrows) of the [T, N, K] tensor V (K % 4 == 0, Vec-aligned), which other CTAs wrote in this
 // launch, to shared memory: row n from time lstm_time(s, len_n, rev).  Forward that is one contiguous block; in
 // reverse each row has its own time.
 template <typename S>
 __device__ __forceinline__ void lstm_stage(S* __restrict__ sV, const S* V, int n0, int nrows, int K, int N, int s,
                                            const int* __restrict__ len, bool rev) {
-    using Vec = typename LstmEl<S>::Vec;
+    using Vec = typename Elem<S>::V;
     Vec* d = reinterpret_cast<Vec*>(sV);
     const int K4 = K >> 2, n4 = nrows * K4;
     if (!rev) {
@@ -145,8 +110,8 @@ __device__ __forceinline__ void lstm_stage(S* __restrict__ sV, const S* V, int n
 template <typename S>
 __device__ __forceinline__ void lstm_dots(const S* __restrict__ sW, const S* __restrict__ sV,
                                           float* __restrict__ out, int R, int K, int nc, int n0, int N) {
-    using El = LstmEl<S>;
-    using Vec = typename El::Vec;
+    using El = Elem<S>;
+    using Vec = typename El::V;
     const int K4 = K >> 2, lane = lane_id(), warp = threadIdx.x >> 5;
     const int nb = (nc + kLstmNB - 1) / kLstmNB;
     const Vec* W4 = reinterpret_cast<const Vec*>(sW);
@@ -157,12 +122,13 @@ __device__ __forceinline__ void lstm_dots(const S* __restrict__ sW, const S* __r
         float acc[kLstmNB];
 #pragma unroll
         for (int j = 0; j < kLstmNB; ++j) acc[j] = 0.f;
+#pragma unroll 2                 // two k steps of loads in flight for every S, not left to how costly widening S looks
         for (int k = lane; k < K4; k += 32) {
-            const float4 a = El::widen(w[k]);
+            const float4 a = El::wide(w[k]);
 #pragma unroll
             for (int j = 0; j < kLstmNB; ++j) {
                 if (j0 + j < nc) {
-                    const float4 b = El::widen(V4[(size_t)(j0 + j) * K4 + k]);
+                    const float4 b = El::wide(V4[(size_t)(j0 + j) * K4 + k]);
                     acc[j] = fmaf(a.x, b.x, acc[j]);
                     acc[j] = fmaf(a.y, b.y, acc[j]);
                     acc[j] = fmaf(a.z, b.z, acc[j]);
@@ -199,8 +165,8 @@ __device__ __forceinline__ void lstm_matvec(const S* __restrict__ sW, S* __restr
 // the two S sections multiples of 8 bytes, so the float sections are aligned for either S.
 template <typename S>
 __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwdArgs<S> p) {
-    using El = LstmEl<S>;
-    using Vec = typename El::Vec;
+    using El = Elem<S>;
+    using Vec = typename El::V;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2;
     const int d = blockIdx.x / p.g;
@@ -247,11 +213,11 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
                 sC[j * N + n] = c;
                 gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
                 cs[o] = c;
-                y[o] = El::narrow(go * tanhf(c));
+                y[o] = El::narrow1(go * tanhf(c));
             } else {
                 gs[0] = 0.f; gs[H] = 0.f; gs[2 * H] = 0.f; gs[3 * H] = 0.f;
                 cs[o] = 0.f;
-                y[o] = El::narrow(0.f);
+                y[o] = El::narrow1(0.f);
             }
         }
         if (s + 1 < p.T) grid_sync(bar, p.g);
@@ -261,7 +227,7 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
 // Shared memory: W^T [u][4H] and dgates_{t+1} rows [rows][4H] of S | dh_rec [u][N] | carried dc [u][N] of float.
 template <typename S>
 __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwdArgs<S> p) {
-    using El = LstmEl<S>;
+    using El = Elem<S>;
     extern __shared__ float4 lstm_smem[];
     const int H = p.H, N = p.N, u = p.u, G = 4 * H;
     const int d = blockIdx.x / p.g;
@@ -279,7 +245,7 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
     float* sDC = sD + u * N;
     for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
         const int k = i / u, j = i - k * u;
-        sW[(size_t)j * G + k] = j < nu ? __ldg(whh + (size_t)k * H + u0 + j) : El::narrow(0.f);
+        sW[(size_t)j * G + k] = j < nu ? __ldg(whh + (size_t)k * H + u0 + j) : El::narrow1(0.f);
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sDC[i] = 0.f;
     for (int s = p.T - 1; s >= 0; --s) {
@@ -302,13 +268,13 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
                 const float cp = s > 0 ? __ldg(cs + ((size_t)lstm_time(s - 1, L, rev) * N + n) * H + unit) : 0.f;
                 const float dh = El::ld(p.dy + o) + sD[j * N + n];
                 const float dc = dh * go * (1.f - tc * tc) + sDC[j * N + n];
-                dg[0] = El::narrow(dc * gg * gi * (1.f - gi));
-                dg[H] = El::narrow(dc * cp * gf * (1.f - gf));
-                dg[2 * H] = El::narrow(dc * gi * (1.f - gg * gg));
-                dg[3 * H] = El::narrow(dh * tc * go * (1.f - go));
+                dg[0] = El::narrow1(dc * gg * gi * (1.f - gi));
+                dg[H] = El::narrow1(dc * cp * gf * (1.f - gf));
+                dg[2 * H] = El::narrow1(dc * gi * (1.f - gg * gg));
+                dg[3 * H] = El::narrow1(dh * tc * go * (1.f - go));
                 sDC[j * N + n] = dc * gf;
             } else {
-                dg[0] = dg[H] = dg[2 * H] = dg[3 * H] = El::narrow(0.f);
+                dg[0] = dg[H] = dg[2 * H] = dg[3 * H] = El::narrow1(0.f);
                 sDC[j * N + n] = 0.f;
             }
         }
@@ -391,32 +357,20 @@ static cudaError_t lstm_backward_t(const void* dy, const float* gates, const flo
 
 cudaError_t launch_lstm_forward(const void* gx, const void* whh, const void* whh_rev, const int* len, void* y,
                                 float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                cudaStream_t stream, BnDtype dtype) {
+                                cudaStream_t stream, Dtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32:
-            return lstm_forward_t<float>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
-        case BnDtype::kBF16:
-            return lstm_forward_t<__nv_bfloat16>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
-        case BnDtype::kF16:
-            return lstm_forward_t<__half>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return lstm_forward_t<decltype(e)>(gx, whh, whh_rev, len, y, gates, cs, bar, T, N, H, u, rows, stream);
+    });
 }
 
 cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh,
                                  const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
-                                 int H, int u, int rows, cudaStream_t stream, BnDtype dtype) {
+                                 int H, int u, int rows, cudaStream_t stream, Dtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32:
-            return lstm_backward_t<float>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
-        case BnDtype::kBF16:
-            return lstm_backward_t<__nv_bfloat16>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
-        case BnDtype::kF16:
-            return lstm_backward_t<__half>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return lstm_backward_t<decltype(e)>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
+    });
 }
 
 }  // namespace okt

@@ -24,6 +24,7 @@
 //
 // No host synchronisation anywhere: every launch is graph-capturable.
 #include "common.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -120,8 +121,6 @@ static cudaError_t copy_rows(const void* src, const int* idx, void* dst, int nro
     return copy_rows_t<unsigned short>(src, idx, dst, nrows, H, stream);
 }
 
-static int elem_size(BnDtype dtype) { return dtype == BnDtype::kF32 ? 4 : 2; }
-
 cudaError_t launch_mlm_select(const long long* labels, int R, long long ignore_index, int M, int* rows, long long* tgt,
                               int* slot, long long* count, long long* overflow, cudaStream_t stream) {
     if (R <= 0 || M <= 0) return cudaErrorInvalidValue;
@@ -129,15 +128,15 @@ cudaError_t launch_mlm_select(const long long* labels, int R, long long ignore_i
     return cudaGetLastError();
 }
 
-cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, int H, BnDtype dtype, cudaStream_t stream) {
+cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, int H, Dtype dtype, cudaStream_t stream) {
     if (M <= 0 || H <= 0) return cudaErrorInvalidValue;
-    return copy_rows(x, rows, out, M, H, elem_size(dtype), stream);
+    return with_dtype(dtype, [&](auto e) { return copy_rows(x, rows, out, M, H, sizeof(e), stream); });
 }
 
-cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, BnDtype dtype,
+cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, Dtype dtype,
                                cudaStream_t stream) {
     if (R <= 0 || H <= 0) return cudaErrorInvalidValue;
-    return copy_rows(dout, slot, dx, R, H, elem_size(dtype), stream);
+    return with_dtype(dtype, [&](auto e) { return copy_rows(dout, slot, dx, R, H, sizeof(e), stream); });
 }
 
 }  // namespace okt

@@ -356,75 +356,77 @@ struct LandParams {
     int count;
 };
 cudaError_t launch_land(const LandParams& lp, float* bucket, cudaStream_t stream);
+// The storage type of the fp32 / bf16 / fp16 kernels' tensors: the code ops/ext.DTYPE_CODE passes, made a type by
+// csrc/elem.cuh's with_dtype.
+enum class Dtype : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 // fused (conv-bias +) BatchNorm + ReLU [+ 2x2 max-pool when W > 0], channels_last, training mode (csrc/bnrelu.cu):
 // one cooperative kernel per pass.  `slot` names the call site's grid hand-off counters; max_ctas > 0 caps the grid.
 // x, y, dy and dx are of type `dtype`; parameters, statistics, partials and dgamma / dbeta are fp32.  A non-null `res`
 // (same type and [M, C] layout as x; W == 0 and relu only) makes it  y = relu(bn(x) + res)  and the backward writes the
 // residual's gradient `dres`.
-enum class BnDtype : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 int bn_tile_rows(int M, int C);
 bool bn_sliced(int M, int C, int W);      // the channel-sliced kernels run (given max_ctas <= 0): no `partial`, no hand-off
 cudaError_t launch_bn_forward(const void* x, void* y, unsigned char* arg, float* partial, const float* gamma, const float* beta,
                               const float* cbias, float* save_mean, float* save_invstd, float* rmean, float* rvar, long long* nbt,
-                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                              float momentum, float eps, int relu, int M, int C, int W, int slot, int max_ctas, Dtype dtype,
                               cudaStream_t stream, const void* res = nullptr);
 cudaError_t launch_bn_backward(const void* x, const void* dy, const unsigned char* arg, void* dx, float* partial,
                                const float* gamma, const float* beta, const float* save_mean, const float* save_invstd,
-                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, BnDtype dtype,
+                               float* dgamma, float* dbeta, int relu, int M, int C, int W, int slot, int max_ctas, Dtype dtype,
                                cudaStream_t stream, const void* res = nullptr, void* dres = nullptr);
 cudaError_t launch_maxpool2_fwd(const float* x, float* y, unsigned char* arg, int N, int H, int W, int C, cudaStream_t stream);
 cudaError_t launch_maxpool2_bwd(const float* dy, const unsigned char* arg, float* dx, int N, int H, int W, int C,
                                 cudaStream_t stream);
 // fused  y = LayerNorm(x + dropout(a))  over rows of H elements (csrc/layernorm.cu): x, y, dx, gamma, beta, dgamma,
-// dbeta, mean and rstd are fp32; a and da are of type `a_dtype` (BnDtype's codes).  keep_thr >= 2^32 turns the dropout
+// dbeta, mean and rstd are fp32; a and da are of type `a_dtype` (a Dtype).  keep_thr >= 2^32 turns the dropout
 // off (seed may then be null).  The backward pass writes its [ln_bwd_grid(R), 2H] column partials to `partial`.
 bool ln_supported_h(int H);
 int ln_bwd_grid(int R);
 cudaError_t launch_ln_forward(const float* x, const void* a, float* y, const float* gamma, const float* beta, float* mean,
                               float* rstd, const unsigned long long* seed, int R, int H, long long keep_thr, float scale,
-                              float eps, BnDtype a_dtype, cudaStream_t stream);
+                              float eps, Dtype a_dtype, cudaStream_t stream);
 cudaError_t launch_ln_backward(const float* x, const void* a, const float* dy, const float* gamma, const float* mean,
                                const float* rstd, const unsigned long long* seed, float* dx, void* da, float* partial,
-                               float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, BnDtype a_dtype,
+                               float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, Dtype a_dtype,
                                cudaStream_t stream);
 // fused softmax cross-entropy, mean over the rows whose target is not ignore_index (csrc/xent.cu): x and dx [R, V] of
-// type `dtype` (BnDtype's codes), 16-byte aligned; t [R] int64; lse [R + 1] fp32 (per-row log-sum-exp, then n);
+// type `dtype` (a Dtype), 16-byte aligned; t [R] int64; lse [R + 1] fp32 (per-row log-sum-exp, then n);
 // rowloss [R] fp32 scratch; loss and g one fp32 each.  Two launches forward, one backward.
 cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, float* rowloss, float* loss, int R,
-                                long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
+                                long long V, long long ignore_index, Dtype dtype, cudaStream_t stream);
 cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
-                                 long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream);
+                                 long long V, long long ignore_index, Dtype dtype, cudaStream_t stream);
 // fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels and tgt int64, rows [M] and slot
 // [R] int32, count one int64, overflow one int64 that accumulates max(count - M, 0) (or null); x [R, H] and out [M, H],
-// dout [M, H] and dx [R, H] of type `dtype` (BnDtype's codes).  One launch each.
+// dout [M, H] and dx [R, H] of type `dtype` (a Dtype).  One launch each.
 cudaError_t launch_mlm_select(const long long* labels, int R, long long ignore_index, int M, int* rows, long long* tgt,
                               int* slot, long long* count, long long* overflow, cudaStream_t stream);
-cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, int H, BnDtype dtype, cudaStream_t stream);
-cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, BnDtype dtype,
+cudaError_t launch_mlm_gather(const void* x, const int* rows, void* out, int M, int H, Dtype dtype, cudaStream_t stream);
+cudaError_t launch_mlm_scatter(const void* dout, const int* slot, void* dx, int R, int H, Dtype dtype,
                                cudaStream_t stream);
 // persistent LSTM recurrence, time-major (csrc/lstm.cu): one cooperative launch per pass, ceil(H / u) CTAs of u hidden
 // units each per direction, `rows` batch rows of the per-step operand staged in shared memory at a time.  gx [T, N, 4H]
 // (the input projection with both biases), whh [H4, H] row-major, len [N] int32 in [1, T]; y, cs [T, N, H], gates and dg
-// [T, N, 4H].  gx, whh, y, dy and dg are of type `dtype` (BnDtype's codes); gates and cs are fp32.  `bar` is a zeroed
+// [T, N, 4H].  gx, whh, y, dy and dg are of type `dtype` (a Dtype); gates and cs are fp32.  `bar` is a zeroed
 // 64-bit grid-barrier counter.  whh, y and dg aligned to four elements (16 bytes in fp32, 8 in bf16 / fp16), H % 4 == 0.
 // whh_rev non-null runs a bidirectional layer, whh_rev being the reverse direction's W_hh: gx, y, cs, gates and dg are
 // then [2, T, N, .] (forward direction first), dy stays [T, N, H] (the same for both), and bar holds two counters.
 cudaError_t launch_lstm_forward(const void* gx, const void* whh, const void* whh_rev, const int* len, void* y,
                                 float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u, int rows,
-                                cudaStream_t stream, BnDtype dtype);
+                                cudaStream_t stream, Dtype dtype);
 cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh,
                                  const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
-                                 int H, int u, int rows, cudaStream_t stream, BnDtype dtype);
+                                 int H, int u, int rows, cudaStream_t stream, Dtype dtype);
 // fused self-attention, head dim 64 (csrc/attention.cu): qkv and dqkv [B, S, 3 H 64], out and dout [B, S, H 64], all of
-// type `dtype` (BnDtype's codes), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
+// type `dtype` (a Dtype), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
 // fp32 (lse written by the forward pass, delta scratch of the backward pass).  keep_thr >= 2^32 turns the dropout off
 // (seed may then be null); `scale` is the kept elements' 1 / (1 - p).  One launch forward, two backward.
 bool attn_supported(int B, int S, int H);
 cudaError_t launch_attn_forward(const void* qkv, const float* mask, const unsigned long long* seed, void* out, float* lse,
-                                int B, int S, int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream);
+                                int B, int S, int H, long long keep_thr, float scale, Dtype dtype, cudaStream_t stream);
 cudaError_t launch_attn_backward(const void* qkv, const void* out, const void* dout, const float* mask,
                                  const unsigned long long* seed, const float* lse, float* delta, void* dqkv, int B, int S,
-                                 int H, long long keep_thr, float scale, BnDtype dtype, cudaStream_t stream);
+                                 int H, long long keep_thr, float scale, Dtype dtype, cudaStream_t stream);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
 cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
 cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);

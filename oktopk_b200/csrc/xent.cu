@@ -29,10 +29,8 @@
 // row's lse, loss and gradient NaN; -inf entries contribute exp = 0.  A target outside [0, V) that is not `ignore`
 // counts in n and gives a NaN row loss and a NaN gradient row (torch's kernel device-asserts instead).  An ignored row is
 // never read, so its gradient is 0 even if it holds inf or NaN (stock log_softmax backward makes it NaN).
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include "common.cuh"
+#include "elem.cuh"
 #include "oktopk.cuh"
 
 namespace okt {
@@ -42,66 +40,13 @@ constexpr int kXeBwdThreads = 256;
 constexpr int kXeRedThreads = 256;
 constexpr int kXeMaxBlocks = 8192;
 
-// Element type T: one element, or the kVec elements of a 16-byte vector, widened to fp32 and narrowed back.
-template <typename T> struct XeAct;
-template <> struct XeAct<float> {
-    static constexpr int kVec = 4;
-    static __device__ __forceinline__ float ld(const float* p) { return __ldg(p); }
-    static __device__ __forceinline__ float narrow1(float v) { return v; }
-    static __device__ __forceinline__ void wide(const uint4& u, float (&f)[kVec]) {
-        f[0] = __uint_as_float(u.x); f[1] = __uint_as_float(u.y); f[2] = __uint_as_float(u.z); f[3] = __uint_as_float(u.w);
-    }
-    static __device__ __forceinline__ uint4 narrow(const float (&f)[kVec]) {
-        return make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
-    }
-};
-template <> struct XeAct<__nv_bfloat16> {
-    static constexpr int kVec = 8;
-    static __device__ __forceinline__ float ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
-    static __device__ __forceinline__ __nv_bfloat16 narrow1(float v) { return __float2bfloat16_rn(v); }
-    static __device__ __forceinline__ void wide2(unsigned int w, float& lo, float& hi) {   // exact: a bf16 is the high half
-        lo = __uint_as_float(w << 16);
-        hi = __uint_as_float(w & 0xffff0000u);
-    }
-    static __device__ __forceinline__ unsigned int narrow2(float lo, float hi) {
-        const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-        return *reinterpret_cast<const unsigned int*>(&v);
-    }
-    static __device__ __forceinline__ void wide(const uint4& u, float (&f)[kVec]) {
-        wide2(u.x, f[0], f[1]); wide2(u.y, f[2], f[3]); wide2(u.z, f[4], f[5]); wide2(u.w, f[6], f[7]);
-    }
-    static __device__ __forceinline__ uint4 narrow(const float (&f)[kVec]) {
-        return make_uint4(narrow2(f[0], f[1]), narrow2(f[2], f[3]), narrow2(f[4], f[5]), narrow2(f[6], f[7]));
-    }
-};
-template <> struct XeAct<__half> {
-    static constexpr int kVec = 8;
-    static __device__ __forceinline__ float ld(const __half* p) { return __half2float(__ldg(p)); }
-    static __device__ __forceinline__ __half narrow1(float v) { return __float2half_rn(v); }
-    static __device__ __forceinline__ void wide2(unsigned int w, float& lo, float& hi) {   // exact
-        const float2 v = __half22float2(*reinterpret_cast<const __half2*>(&w));
-        lo = v.x;
-        hi = v.y;
-    }
-    static __device__ __forceinline__ unsigned int narrow2(float lo, float hi) {          // past 65504 -> inf; no flush
-        const __half2 v = __floats2half2_rn(lo, hi);
-        return *reinterpret_cast<const unsigned int*>(&v);
-    }
-    static __device__ __forceinline__ void wide(const uint4& u, float (&f)[kVec]) {
-        wide2(u.x, f[0], f[1]); wide2(u.y, f[2], f[3]); wide2(u.z, f[4], f[5]); wide2(u.w, f[6], f[7]);
-    }
-    static __device__ __forceinline__ uint4 narrow(const float (&f)[kVec]) {
-        return make_uint4(narrow2(f[0], f[1]), narrow2(f[2], f[3]), narrow2(f[4], f[5]), narrow2(f[6], f[7]));
-    }
-};
-
 // A row's scalar head (elements before its first 16-byte boundary) and its count of 16-byte vectors after it; the tail
 // is what is left.  `row` is T-aligned.
 template <typename T>
 __device__ __forceinline__ void xe_split(const T* row, long long V, long long& head, long long& nvec) {
     head = (long long)(((16u - ((unsigned)(uintptr_t)row & 15u)) & 15u) / sizeof(T));
     if (head > V) head = V;
-    nvec = (V - head) / XeAct<T>::kVec;
+    nvec = (V - head) / Elem<T>::kVec;
 }
 
 // Online log-sum-exp state (m, s): the row's running max and sum of exp(x - m).  A pair whose max is unchanged keeps
@@ -132,7 +77,7 @@ template <typename T>
 __global__ void __launch_bounds__(kXeFwdThreads) xent_fwd_kernel(const T* __restrict__ x, const long long* __restrict__ t,
                                                                  float* __restrict__ lse, float* __restrict__ rowloss,
                                                                  int R, long long V, long long ignore) {
-    using A = XeAct<T>;
+    using A = Elem<T>;
     constexpr int kVec = A::kVec, kWarps = kXeFwdThreads / 32, kUnroll = 4;
     __shared__ float s_m[kWarps], s_s[kWarps];
     const int tid = threadIdx.x, lane = lane_id(), warp = tid >> 5;
@@ -199,7 +144,7 @@ template <typename T>
 __global__ void __launch_bounds__(kXeBwdThreads) xent_bwd_kernel(const T* __restrict__ x, const long long* __restrict__ t,
                                                                  const float* __restrict__ lse, const float* __restrict__ g,
                                                                  T* __restrict__ dx, int R, long long V, long long ignore) {
-    using A = XeAct<T>;
+    using A = Elem<T>;
     constexpr int kVec = A::kVec;
     const int tid = threadIdx.x;
     const float gn = __ldg(g) / __ldg(lse + R);
@@ -255,25 +200,17 @@ static cudaError_t xent_backward_t(const void* x, const long long* t, const floa
 }
 
 cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, float* rowloss, float* loss, int R,
-                                long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream) {
+                                long long V, long long ignore_index, Dtype dtype, cudaStream_t stream) {
     if (R <= 0 || V <= 0) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32: return xent_forward_t<float>(x, t, lse, rowloss, loss, R, V, ignore_index, stream);
-        case BnDtype::kBF16: return xent_forward_t<__nv_bfloat16>(x, t, lse, rowloss, loss, R, V, ignore_index, stream);
-        case BnDtype::kF16: return xent_forward_t<__half>(x, t, lse, rowloss, loss, R, V, ignore_index, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
+        return xent_forward_t<decltype(e)>(x, t, lse, rowloss, loss, R, V, ignore_index, stream);
+    });
 }
 
 cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
-                                 long long V, long long ignore_index, BnDtype dtype, cudaStream_t stream) {
+                                 long long V, long long ignore_index, Dtype dtype, cudaStream_t stream) {
     if (R <= 0 || V <= 0) return cudaErrorInvalidValue;
-    switch (dtype) {
-        case BnDtype::kF32: return xent_backward_t<float>(x, t, lse, g, dx, R, V, ignore_index, stream);
-        case BnDtype::kBF16: return xent_backward_t<__nv_bfloat16>(x, t, lse, g, dx, R, V, ignore_index, stream);
-        case BnDtype::kF16: return xent_backward_t<__half>(x, t, lse, g, dx, R, V, ignore_index, stream);
-    }
-    return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) { return xent_backward_t<decltype(e)>(x, t, lse, g, dx, R, V, ignore_index, stream); });
 }
 
 }  // namespace okt

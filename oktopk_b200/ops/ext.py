@@ -7,6 +7,8 @@ import importlib
 import os
 from typing import Optional
 
+import torch
+
 _C = None
 _ERR: Optional[BaseException] = None
 
@@ -60,6 +62,16 @@ def load(build_if_missing: bool = True):
     return _C
 
 
+# The kernels' storage-type code of an fp32 / bf16 / fp16 tensor (csrc/oktopk.cuh Dtype; bindings reject other codes).
+DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+
+
+def dense16(t: torch.Tensor) -> torch.Tensor:
+    """Contiguous and 16-byte aligned (the kernels move 128-bit vectors), copied once if it is not."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def available() -> bool:
     return load() is not None
 
@@ -85,7 +97,6 @@ class DevPtr:
 
 
 def tensor_from_ptr(ptr: int, numel: int, dtype="float32", device=None):
-    import torch
     ts = {"float32": "<f4", "int32": "<i4", "uint8": "|u1", "int64": "<i8"}[dtype]
     dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
     return torch.as_tensor(DevPtr(ptr, numel, ts), device=dev)

@@ -39,13 +39,14 @@ import torch
 import torch.nn.functional as F
 
 from . import ext
-from .fused_ln import _DTYPE_FLAG, _dense, keep_threshold
+from .ext import DTYPE_CODE, dense16
+from .fused_ln import keep_threshold
 
 HEAD_DIM = 64
 
 
 def _fast_path_ok(qkv: torch.Tensor, heads: int, mask, p: float) -> bool:
-    if not (qkv.is_cuda and qkv.dim() == 3 and qkv.dtype in _DTYPE_FLAG and ext.available()):
+    if not (qkv.is_cuda and qkv.dim() == 3 and qkv.dtype in DTYPE_CODE and ext.available()):
         return False
     B, S, W = qkv.shape
     if not (0.0 <= p < 1.0 and heads >= 1 and W == 3 * heads * HEAD_DIM and ext.require().attn_supported(B, S, heads)):
@@ -66,7 +67,7 @@ class _FusedAttention(torch.autograd.Function):
         lse = torch.empty((B, heads, S), dtype=torch.float32, device=qkv.device)
         thr, scale = keep_threshold(p), 1.0 / (1.0 - p)
         C.attn_forward(qkv.data_ptr(), 0 if mask is None else mask.data_ptr(), 0 if seed is None else seed.data_ptr(),
-                       out.data_ptr(), lse.data_ptr(), B, S, heads, thr, scale, _DTYPE_FLAG[qkv.dtype],
+                       out.data_ptr(), lse.data_ptr(), B, S, heads, thr, scale, DTYPE_CODE[qkv.dtype],
                        torch.cuda.current_stream().cuda_stream)
         ctx.save_for_backward(qkv, out, lse, mask, seed)
         ctx.heads, ctx.thr, ctx.scale = heads, thr, scale
@@ -77,12 +78,12 @@ class _FusedAttention(torch.autograd.Function):
         C = ext.require()
         qkv, out, lse, mask, seed = ctx.saved_tensors
         B, S, _ = qkv.shape
-        dout = _dense(dout.to(qkv.dtype))
+        dout = dense16(dout.to(qkv.dtype))
         dqkv = torch.empty_like(qkv)
         delta = torch.empty_like(lse)
         C.attn_backward(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), 0 if mask is None else mask.data_ptr(),
                         0 if seed is None else seed.data_ptr(), lse.data_ptr(), delta.data_ptr(), dqkv.data_ptr(), B, S,
-                        ctx.heads, ctx.thr, ctx.scale, _DTYPE_FLAG[qkv.dtype], torch.cuda.current_stream().cuda_stream)
+                        ctx.heads, ctx.thr, ctx.scale, DTYPE_CODE[qkv.dtype], torch.cuda.current_stream().cuda_stream)
         return dqkv, None, None, None
 
 
@@ -93,8 +94,8 @@ def self_attention(qkv: torch.Tensor, heads: int, mask, p: float) -> torch.Tenso
     p = float(p)
     if _fast_path_ok(qkv, heads, mask, p):
         B, S, _ = qkv.shape
-        m = None if mask is None else _dense(mask.reshape(B, S).float())
-        return _FusedAttention.apply(_dense(qkv), m, int(heads), p)
+        m = None if mask is None else dense16(mask.reshape(B, S).float())
+        return _FusedAttention.apply(dense16(qkv), m, int(heads), p)
     b, s, w = qkv.shape
     dh = w // (3 * heads)
     q, k, v = qkv.view(b, s, 3, heads, dh).permute(2, 0, 3, 1, 4)

@@ -46,6 +46,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ext
+from .ext import DTYPE_CODE
 
 # > 0 caps the grid of the fused batch-norm kernels, so that each CTA loops over several tiles (tests use it to cover
 # that path on a GPU whose co-resident grid exceeds the tile count).  A cap also keeps a shape the channel-sliced kernels
@@ -53,9 +54,6 @@ from . import ext
 MAX_CTAS = 0
 
 _SLOTS = itertools.count()
-
-# the kernels' activation type argument (csrc/bindings.cpp bn_forward / bn_backward)
-_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 
 def _sync_slot(bn: torch.nn.BatchNorm2d) -> int:
@@ -120,7 +118,7 @@ class _BiasBNReLUPool(torch.autograd.Function):
         C = ext.require()
         N, Ch, H, W = x.shape
         M = N * H * W
-        dtype = _DTYPE_FLAG[x.dtype]
+        dtype = DTYPE_CODE[x.dtype]
         if pool:
             y = torch.empty((N, Ch, H // 2, W // 2), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
             arg = torch.empty(y.numel(), dtype=torch.uint8, device=x.device)

@@ -30,9 +30,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ext
-
-# the kernels' type code of ``a`` (csrc/bindings.cpp ln_forward / ln_backward; the batch-norm kernels' codes)
-_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+from .ext import DTYPE_CODE, dense16
 
 
 def keep_threshold(p: float) -> int:
@@ -45,16 +43,10 @@ def _fast_path_ok(x: torch.Tensor, a: torch.Tensor, ln: torch.nn.LayerNorm, p: f
         return False
     H = x.size(-1)
     w, b = ln.weight, ln.bias
-    return (0.0 <= p < 1.0 and x.dtype == torch.float32 and a.dtype in _DTYPE_FLAG and a.device == x.device
+    return (0.0 <= p < 1.0 and x.dtype == torch.float32 and a.dtype in DTYPE_CODE and a.device == x.device
             and a.shape == x.shape and tuple(ln.normalized_shape) == (H,) and H % 128 == 0 and 128 <= H <= 1024
             and w is not None and b is not None and w.dtype == torch.float32 and b.dtype == torch.float32
             and w.device == x.device and b.device == x.device)
-
-
-def _dense(t: torch.Tensor) -> torch.Tensor:
-    """Contiguous and 16-byte aligned (the kernels move 128-bit vectors), copied once if it is not."""
-    t = t.contiguous()
-    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 class _ResidualDropoutLN(torch.autograd.Function):
@@ -69,7 +61,7 @@ class _ResidualDropoutLN(torch.autograd.Function):
         thr, scale = keep_threshold(p), 1.0 / (1.0 - p)
         C.ln_forward(x.data_ptr(), a.data_ptr(), y.data_ptr(), gamma.data_ptr(), beta.data_ptr(), stats[0].data_ptr(),
                      stats[1].data_ptr(), 0 if seed is None else seed.data_ptr(), R, H, thr, scale, eps,
-                     _DTYPE_FLAG[a.dtype], torch.cuda.current_stream().cuda_stream)
+                     DTYPE_CODE[a.dtype], torch.cuda.current_stream().cuda_stream)
         ctx.save_for_backward(x, a, gamma, stats, seed)
         ctx.thr, ctx.scale = thr, scale
         return y
@@ -80,7 +72,7 @@ class _ResidualDropoutLN(torch.autograd.Function):
         x, a, gamma, stats, seed = ctx.saved_tensors
         H = x.size(-1)
         R = x.numel() // H
-        dy = _dense(dy.float())                         # y is fp32, so is its gradient
+        dy = dense16(dy.float())                        # y is fp32, so is its gradient
         dx = torch.empty_like(x)
         da = torch.empty_like(a)
         partial = torch.empty(C.ln_bwd_grid(R) * 2 * H, dtype=torch.float32, device=x.device)
@@ -88,7 +80,7 @@ class _ResidualDropoutLN(torch.autograd.Function):
         C.ln_backward(x.data_ptr(), a.data_ptr(), dy.data_ptr(), gamma.data_ptr(), stats[0].data_ptr(),
                       stats[1].data_ptr(), 0 if seed is None else seed.data_ptr(), dx.data_ptr(), da.data_ptr(),
                       partial.data_ptr(), dgb.data_ptr(), dgb.data_ptr() + 4 * H, R, H, ctx.thr, ctx.scale,
-                      _DTYPE_FLAG[a.dtype], torch.cuda.current_stream().cuda_stream)
+                      DTYPE_CODE[a.dtype], torch.cuda.current_stream().cuda_stream)
         return dx, da, dgb[:H], dgb[H:], None, None
 
 
@@ -96,5 +88,5 @@ def residual_dropout_layer_norm(x: torch.Tensor, a: torch.Tensor, ln: torch.nn.L
     """``ln(x + dropout(a, p))`` (``p = 0``: no dropout, as in eval mode); see the module docstring."""
     p = float(p)
     if _fast_path_ok(x, a, ln, p):
-        return _ResidualDropoutLN.apply(_dense(x), _dense(a), ln.weight, ln.bias, p, float(ln.eps))
+        return _ResidualDropoutLN.apply(dense16(x), dense16(a), ln.weight, ln.bias, p, float(ln.eps))
     return ln(x + F.dropout(a, p, p > 0))

@@ -44,6 +44,7 @@ import torch
 import torch.nn as nn
 
 from . import ext
+from .ext import DTYPE_CODE
 
 LSTM_THREADS = 512          # csrc/lstm.cu kLstmThreads
 MAX_BATCH = 64              # the largest N the native path takes
@@ -86,9 +87,6 @@ def _device_geometry(H: int, N: int, dev: torch.device, elem: int = 4, dirs: int
     """The geometry of one direction of a ``dirs``-direction layer: the directions split the SMs between them."""
     p = torch.cuda.get_device_properties(dev)
     return lstm_geometry(H, N, p.multi_processor_count // dirs, p.shared_memory_per_block_optin, elem)
-
-
-_DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}      # csrc/oktopk.cuh BnDtype
 
 
 def stock_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module) -> torch.Tensor:
@@ -161,7 +159,7 @@ class _LstmLayer(torch.autograd.Function):
         bar = torch.zeros(dirs, dtype=torch.int64, device=x.device)
         C.lstm_forward(gx.data_ptr(), w_hh[0].data_ptr(), lens.data_ptr(), y.data_ptr(), gates.data_ptr(),
                        cs.data_ptr(), bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows,
-                       torch.cuda.current_stream().cuda_stream, _DTYPE_CODE[dt], w_hh[1].data_ptr() if dirs == 2 else 0)
+                       torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt], w_hh[1].data_ptr() if dirs == 2 else 0)
         ctx.save_for_backward(xs, lens, y, gates, cs, *w_ih, *w_hh)
         ctx.geom = geom
         ctx.x_dtype = x.dtype
@@ -182,7 +180,7 @@ class _LstmLayer(torch.autograd.Function):
         bar = torch.zeros(dirs, dtype=torch.int64, device=x.device)
         C.lstm_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), w_hh[0].data_ptr(), lens.data_ptr(),
                         dg.data_ptr(), bar.data_ptr(), T, N, H, ctx.geom.units, ctx.geom.bwd_rows,
-                        torch.cuda.current_stream().cuda_stream, _DTYPE_CODE[dt],
+                        torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt],
                         w_hh[1].data_ptr() if dirs == 2 else 0)
         need = ctx.needs_input_grad
         grads = []

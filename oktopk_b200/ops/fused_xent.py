@@ -28,23 +28,15 @@ import torch
 import torch.nn.functional as F
 
 from . import ext
-
-# the kernels' type code of the logits (csrc/bindings.cpp xent_forward / xent_backward; the batch-norm kernels' codes)
-_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+from .ext import DTYPE_CODE, dense16
 
 
 def _fast_path_ok(logits: torch.Tensor, target: torch.Tensor) -> bool:
     if not (logits.is_cuda and logits.dim() == 2 and ext.available()):
         return False
     R, V = logits.shape
-    return (logits.dtype in _DTYPE_FLAG and 0 < R < 2 ** 31 and V > 0 and target.dtype == torch.int64
+    return (logits.dtype in DTYPE_CODE and 0 < R < 2 ** 31 and V > 0 and target.dtype == torch.int64
             and tuple(target.shape) == (R,) and target.device == logits.device)
-
-
-def _dense(t: torch.Tensor) -> torch.Tensor:
-    """Contiguous and 16-byte aligned (the kernels move 128-bit vectors), copied once if it is not."""
-    t = t.contiguous()
-    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 class _SoftmaxCrossEntropy(torch.autograd.Function):
@@ -56,7 +48,7 @@ class _SoftmaxCrossEntropy(torch.autograd.Function):
         rowloss = torch.empty(R, dtype=torch.float32, device=logits.device)
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
         C.xent_forward(logits.data_ptr(), target.data_ptr(), lse.data_ptr(), rowloss.data_ptr(), loss.data_ptr(), R, V,
-                       ignore_index, _DTYPE_FLAG[logits.dtype], torch.cuda.current_stream().cuda_stream)
+                       ignore_index, DTYPE_CODE[logits.dtype], torch.cuda.current_stream().cuda_stream)
         ctx.save_for_backward(logits, target, lse)
         ctx.ignore_index = ignore_index
         return loss
@@ -69,7 +61,7 @@ class _SoftmaxCrossEntropy(torch.autograd.Function):
         g = g.float().contiguous()                      # the loss is fp32, so is its gradient
         dx = torch.empty_like(logits)
         C.xent_backward(logits.data_ptr(), target.data_ptr(), lse.data_ptr(), g.data_ptr(), dx.data_ptr(), R, V,
-                        ctx.ignore_index, _DTYPE_FLAG[logits.dtype], torch.cuda.current_stream().cuda_stream)
+                        ctx.ignore_index, DTYPE_CODE[logits.dtype], torch.cuda.current_stream().cuda_stream)
         return dx, None, None
 
 
@@ -77,5 +69,5 @@ def softmax_cross_entropy(logits: torch.Tensor, target: torch.Tensor, ignore_ind
     """``F.cross_entropy(logits, target, ignore_index=ignore_index)`` (mean over the labelled rows); see the module
     docstring."""
     if _fast_path_ok(logits, target):
-        return _SoftmaxCrossEntropy.apply(_dense(logits), target.contiguous(), int(ignore_index))
+        return _SoftmaxCrossEntropy.apply(dense16(logits), target.contiguous(), int(ignore_index))
     return F.cross_entropy(logits, target, ignore_index=ignore_index)

@@ -30,9 +30,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import ext
-
-# the kernels' type code of x (csrc/bindings.cpp mlm_gather / mlm_scatter; the batch-norm kernels' codes)
-_DTYPE_FLAG = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+from .ext import DTYPE_CODE
 
 
 def capacity_rows(R: int, fraction: float) -> int:
@@ -50,7 +48,7 @@ def _native_ok(labels: torch.Tensor, capacity: int, x: Optional[torch.Tensor] = 
         return False
     if x is None:
         return True
-    return (x.dim() == 2 and x.size(0) == R and 0 < x.size(1) < 2 ** 31 and x.dtype in _DTYPE_FLAG
+    return (x.dim() == 2 and x.size(0) == R and 0 < x.size(1) < 2 ** 31 and x.dtype in DTYPE_CODE
             and x.device == labels.device)
 
 
@@ -111,7 +109,7 @@ def _copy_rows(src: torch.Tensor, idx: torch.Tensor, native: bool, gather: bool)
         src = src.contiguous()
         out = torch.empty(n, H, dtype=src.dtype, device=src.device)
         fn = C.mlm_gather if gather else C.mlm_scatter
-        fn(src.data_ptr(), idx.data_ptr(), out.data_ptr(), n, H, _DTYPE_FLAG[src.dtype], _stream())
+        fn(src.data_ptr(), idx.data_ptr(), out.data_ptr(), n, H, DTYPE_CODE[src.dtype], _stream())
         return out
     padded = torch.cat([src, src.new_zeros(1, H)])
     return padded[torch.where(idx >= 0, idx.long(), src.size(0))]

@@ -100,8 +100,8 @@ def _kernel_pair_us(C, shape, pooled, dtype, iters):
     nbt = torch.zeros((), dtype=torch.long, device="cuda")
     stats, dgb = torch.empty(2 * Ch, device="cuda"), torch.empty(2 * Ch, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
-    from oktopk_b200.ops.fused_bn import _DTYPE_FLAG
-    flag = _DTYPE_FLAG[dtype]
+    from oktopk_b200.ops.ext import DTYPE_CODE
+    flag = DTYPE_CODE[dtype]
     Wp = W if pooled else 0
 
     def pair():

@@ -149,7 +149,7 @@ def _graph_us(fn, iters):
 def _kernel_pairs(C, shape, dtype, iters):
     """The residual bn_forward + bn_backward pair and the stock sequence it replaces, µs per pair."""
     import torch
-    from oktopk_b200.ops.fused_bn import _DTYPE_FLAG
+    from oktopk_b200.ops.ext import DTYPE_CODE
     N, Ch, H, W = shape
     M = N * H * W
     cl = torch.channels_last
@@ -163,7 +163,7 @@ def _kernel_pairs(C, shape, dtype, iters):
     rm, rv = torch.zeros(Ch, device="cuda"), torch.ones(Ch, device="cuda")
     nbt = torch.zeros((), dtype=torch.long, device="cuda")
     stats, dgb = torch.empty(2 * Ch, device="cuda"), torch.empty(2 * Ch, device="cuda")
-    flag = _DTYPE_FLAG[dtype]
+    flag = DTYPE_CODE[dtype]
 
     def fused():
         s = torch.cuda.current_stream().cuda_stream

@@ -13,11 +13,11 @@ import torch.nn.functional as F
 from oktopk_b200.models import create_net
 from oktopk_b200.models.deepspeech import BatchRNN
 from oktopk_b200.ops import ext, fused_lstm
+from oktopk_b200.ops.ext import DTYPE_CODE
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
-CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 NAMES = ["y", "dx", "dW_ih", "dW_hh", "db_ih", "db_hh"]
 
 
@@ -61,7 +61,7 @@ def _forward(gx, whh, lens, elem):
     bar = torch.zeros(1, dtype=torch.int64, device="cuda")
     C.lstm_forward(gx.data_ptr(), whh.data_ptr(), lens.data_ptr(), y.data_ptr(), gates.data_ptr(), cs.data_ptr(),
                    bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows, torch.cuda.current_stream().cuda_stream,
-                   CODE[gx.dtype])
+                   DTYPE_CODE[gx.dtype])
     return y, gates, cs
 
 
@@ -73,7 +73,7 @@ def _backward(dy, gates, cs, whh, lens, elem):
     bar = torch.zeros(1, dtype=torch.int64, device="cuda")
     C.lstm_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), whh.data_ptr(), lens.data_ptr(), dg.data_ptr(),
                     bar.data_ptr(), T, N, H, geom.units, geom.bwd_rows, torch.cuda.current_stream().cuda_stream,
-                    CODE[dy.dtype])
+                    DTYPE_CODE[dy.dtype])
     return dg
 
 

@@ -118,8 +118,7 @@ def test_scatter_writes_every_row(dtype, H):
     _, _, slot, _ = mlm_gather.select_labelled(labels, M, IGN)
     dout = torch.randn(M, H, device="cuda").to(dtype)
     dx = torch.full((R, H), float("nan"), device="cuda").to(dtype)
-    C.mlm_scatter(dout.data_ptr(), slot.data_ptr(), dx.data_ptr(), R, H, {torch.float32: 0, torch.bfloat16: 1,
-                                                                          torch.float16: 2}[dtype],
+    C.mlm_scatter(dout.data_ptr(), slot.data_ptr(), dx.data_ptr(), R, H, ext.DTYPE_CODE[dtype],
                   torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
     assert not bool(dx.isnan().any())
