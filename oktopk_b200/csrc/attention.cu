@@ -157,19 +157,8 @@ template <typename T> struct AttnMma16 {        // bf16 / fp16, m16n8k16
         return A{{pack(c[2 * kc][0], c[2 * kc][1]), pack(c[2 * kc][2], c[2 * kc][3]), pack(c[2 * kc + 1][0], c[2 * kc + 1][1]),
                   pack(c[2 * kc + 1][2], c[2 * kc + 1][3])}};
     }
-    static __device__ __forceinline__ void mma(float (&d)[4], const A& a, const B& b);
+    static __device__ __forceinline__ void mma(float (&d)[4], const A& a, const B& b) { mma_m16n8k16<T>(d, a.r, b.r); }
 };
-
-template <> __device__ __forceinline__ void AttnMma16<__nv_bfloat16>::mma(float (&d)[4], const A& a, const B& b) {
-    asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a.r[0]), "r"(a.r[1]), "r"(a.r[2]), "r"(a.r[3]), "r"(b.r[0]), "r"(b.r[1]));
-}
-template <> __device__ __forceinline__ void AttnMma16<__half>::mma(float (&d)[4], const A& a, const B& b) {
-    asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a.r[0]), "r"(a.r[1]), "r"(a.r[2]), "r"(a.r[3]), "r"(b.r[0]), "r"(b.r[1]));
-}
 template <> struct AttnMma<__nv_bfloat16> : AttnMma16<__nv_bfloat16> {};
 template <> struct AttnMma<__half> : AttnMma16<__half> {};
 

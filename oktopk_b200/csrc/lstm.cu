@@ -296,7 +296,7 @@ struct LstmLaunchCache {
 // Cooperative launch of `grid` CTAs with `smem` bytes each; an error if they cannot all be co-resident.
 template <typename Args>
 static cudaError_t lstm_launch(void (*kernel)(const Args), const Args& p, int grid, size_t smem, cudaStream_t stream) {
-    static LstmLaunchCache cache[kLstmMaxDevices];             // one table per kernel: Args differs between all six
+    static LstmLaunchCache cache[kLstmMaxDevices];             // one table per kernel: each has its own Args
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
@@ -370,6 +370,295 @@ cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
     return with_dtype(dtype, [&](auto e) {
         return lstm_backward_t<decltype(e)>(dy, gates, cs, whh, whh_rev, len, dg, bar, T, N, H, u, rows, stream);
+    });
+}
+
+// ---- One layer of a stacked language-model LSTM (PTB): carried state, step product on the tensor cores ----------------
+//
+// lstm_seq_fwd_kernel / lstm_seq_bwd_kernel run the recurrence above for a single uni-directional layer in which every
+// row has length T, from an initial state (h0, c0), in bf16 or fp16 only.  The split into CTAs of u units, the grid
+// barrier, the cell code and the stores are those of lstm_fwd_kernel / lstm_bwd_kernel; what differs:
+//   - forward, step 0 stages h0 where the other steps stage y_{t-1}, and c starts from c0.  h_n = y[T-1] and
+//     c_n = cs[T-1], so neither has a store of its own;
+//   - backward, at t = T-1 the recurrent dh is dh_n and the carried dc is dc_n (either null: 0); c_{-1} is c0, and the
+//     carried dc after t = 0 is written to dc0 (fp32).  dh0 = dgates_0 W_hh is a GEMM in torch;
+//   - the step product runs on mma.sync m16n8k16 with fp32 accumulation (lstm_mma_dots): batch rows on the M side (a
+//     missing row is a zero fragment), the CTA's weight rows on the n side (forward: its 4u gate rows of W_hh;
+//     backward: its u columns), K = H (forward) or 4H (backward).  Rows of both operands lie lstm_seq_ld(K) elements
+//     apart in shared memory, zero from K on: that pads K to a multiple of 16 and makes the row stride an odd multiple of
+//     16 bytes, so the eight rows a fragment load touches fall in distinct banks.  Weight rows are not padded: a weight
+//     row past the CTA's last is a zero fragment too.
+//   - a warp task is one (16 batch rows, 8 weight rows, 1 / ksplit of the k steps); its k steps alternate between two
+//     accumulators, added at the end.  With ksplit > 1 the partial sums are added in split order after a block barrier,
+//     so, as everywhere in this file, every sum has a fixed order whichever warp runs it and no atomics touch data.
+// lstm_seq_ksplit is mirrored by ops/fused_lstm.py, which sizes the shared memory from it.
+
+template <typename S>
+struct LstmSeqFwdArgs {
+    const S* gx;
+    const S* whh;
+    const S* h0;
+    const float* c0;
+    S* y;
+    float* gates;
+    float* cs;
+    unsigned long long* bar;
+    int T, N, H, u, rows, ksplit;
+};
+
+template <typename S>
+struct LstmSeqBwdArgs {
+    const S* dy;
+    const float* gates;
+    const float* cs;
+    const S* whh;
+    const float* c0;
+    const S* dhn;                   // null: 0
+    const float* dcn;               // null: 0
+    S* dg;
+    float* dc0;
+    unsigned long long* bar;
+    int T, N, H, u, rows, ksplit;
+};
+
+__host__ __device__ __forceinline__ int lstm_seq_ld(int K) { return ((K + 15) & ~15) + 8; }
+
+// K splits of a step product over `rows` batch rows and R weight rows: enough to give every warp a task, at most one
+// per k step.
+__host__ __device__ __forceinline__ int lstm_seq_ksplit(int rows, int R, int K) {
+    const int tiles = ((rows + 15) >> 4) * ((R + 7) >> 3);
+    return max(1, min(kLstmWarps / tiles, (K + 15) >> 4));
+}
+
+__device__ __forceinline__ uint32_t lstm_u32(const void* p) { return *reinterpret_cast<const uint32_t*>(p); }
+
+// sP[(ks nc + j) R + r] = the ks-th split of sum_k sV[j ld + k] sW[r ld + k], j < nc, r < R, over k < 16 KS (zero
+// past K).  Fragment layout as the PTX ISA's m16n8k16 row.col: lane (g, t) = (lane / 4, lane % 4) loads A rows g and
+// g + 8 and B row g, at k = 2t and 2t + 8.
+template <typename S>
+__device__ __forceinline__ void lstm_mma_dots(const S* __restrict__ sW, const S* __restrict__ sV,
+                                              float* __restrict__ sP, int R, int ld, int KS, int nc, int ksplit) {
+    const int lane = lane_id(), warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    const int NT = (R + 7) >> 3, tasks = ((nc + 15) >> 4) * NT * ksplit;
+    for (int task = warp; task < tasks; task += kLstmWarps) {
+        const int ks = task % ksplit, tile = task / ksplit, mt = tile / NT, nt = tile - mt * NT;
+        const int j0 = mt * 16 + g, j1 = j0 + 8, r = nt * 8 + g;
+        const bool ok0 = j0 < nc, ok1 = j1 < nc, okw = r < R;
+        const S* a0 = sV + (size_t)(ok0 ? j0 : 0) * ld + 2 * t;
+        const S* a1 = sV + (size_t)(ok1 ? j1 : 0) * ld + 2 * t;
+        const S* b = sW + (size_t)(okw ? r : 0) * ld + 2 * t;
+        const int k_lo = ks * KS / ksplit, k_hi = (ks + 1) * KS / ksplit;
+        float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+        auto step = [&](float (&d)[4], int kk) {
+            const int k = kk * 16;
+            const uint32_t fa[4] = {ok0 ? lstm_u32(a0 + k) : 0u, ok1 ? lstm_u32(a1 + k) : 0u,
+                                    ok0 ? lstm_u32(a0 + k + 8) : 0u, ok1 ? lstm_u32(a1 + k + 8) : 0u};
+            const uint32_t fb[2] = {okw ? lstm_u32(b + k) : 0u, okw ? lstm_u32(b + k + 8) : 0u};
+            mma_m16n8k16<S>(d, fa, fb);
+        };
+        int kk = k_lo;
+#pragma unroll 2
+        for (; kk + 1 < k_hi; kk += 2) {
+            step(acc[0], kk);
+            step(acc[1], kk + 1);
+        }
+        if (kk < k_hi) step(acc[0], kk);
+        float* P = sP + (size_t)ks * nc * R;
+        const int rc = nt * 8 + 2 * t;                          // C fragment: rows g, g + 8; columns 2t, 2t + 1
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int j = h ? j1 : j0;
+            if (!(h ? ok1 : ok0)) continue;
+            if (rc < R) P[j * R + rc] = acc[0][2 * h] + acc[1][2 * h];
+            if (rc + 1 < R) P[j * R + rc + 1] = acc[0][2 * h + 1] + acc[1][2 * h + 1];
+        }
+    }
+}
+
+// out[r N + n] = sum_k sW[r ld + k] V[n K + k] for r < R and all N rows of V (global [N, K], possibly written in this
+// launch), `rows` at a time through sV (whose rows are zero from K to ld, as are sW's).
+template <typename S>
+__device__ __forceinline__ void lstm_seq_product(const S* __restrict__ sW, S* __restrict__ sV, float* __restrict__ sP,
+                                                 float* __restrict__ out, const S* V, int R, int K, int N, int rows,
+                                                 int ksplit) {
+    using Vec = typename Elem<S>::V;
+    const int ld = lstm_seq_ld(K), K4 = K >> 2, KS = (K + 15) >> 4;
+    for (int n0 = 0; n0 < N; n0 += rows) {
+        const int nc = min(rows, N - n0);
+        const Vec* src = reinterpret_cast<const Vec*>(V + (size_t)n0 * K);
+        for (int i = threadIdx.x; i < nc * K4; i += kLstmThreads) {
+            const int j = i / K4, k = i - j * K4;
+            reinterpret_cast<Vec*>(sV + (size_t)j * ld)[k] = __ldcg(src + i);
+        }
+        __syncthreads();
+        lstm_mma_dots(sW, sV, sP, R, ld, KS, nc, ksplit);
+        __syncthreads();
+        for (int i = threadIdx.x; i < R * nc; i += kLstmThreads) {
+            const int r = i / nc, j = i - r * nc;
+            float a = sP[j * R + r];
+            for (int ks = 1; ks < ksplit; ++ks) a += sP[((size_t)ks * nc + j) * R + r];
+            out[r * N + n0 + j] = a;
+        }
+    }
+    __syncthreads();
+}
+
+// Zero columns [K, ld) of `nrows` shared-memory rows.
+template <typename S>
+__device__ __forceinline__ void lstm_seq_zero_tail(S* s, int nrows, int K) {
+    const int ld = lstm_seq_ld(K), w = ld - K;
+    for (int i = threadIdx.x; i < nrows * w; i += kLstmThreads) {
+        const int r = i / w;
+        s[(size_t)r * ld + K + (i - r * w)] = Elem<S>::narrow1(0.f);
+    }
+}
+
+// Shared memory: W [4u][ld] and h_{t-1} rows [rows][ld] of S, ld = lstm_seq_ld(H) | partial sums [ksplit][rows][4u],
+// gate sums [4u][N] and c [u][N] of float.  ld % 8 == 0 keeps every section 16-byte aligned.
+template <typename S>
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_fwd_kernel(const LstmSeqFwdArgs<S> p) {
+    using El = Elem<S>;
+    using Vec = typename El::V;
+    extern __shared__ float4 lstm_smem[];
+    const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2, ld = lstm_seq_ld(H);
+    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    S* sW = reinterpret_cast<S*>(lstm_smem);
+    S* sV = sW + (size_t)R * ld;
+    float* sP = reinterpret_cast<float*>(sV + (size_t)p.rows * ld);
+    float* sG = sP + (size_t)p.ksplit * p.rows * R;
+    float* sC = sG + R * N;
+    for (int i = threadIdx.x; i < R * H4; i += kLstmThreads) {      // local row q u + j = W_hh row q H + u0 + j
+        const int lr = i / H4, k = i - lr * H4, q = lr / u, j = lr - q * u;
+        Vec v = El::zero();
+        if (j < nu) v = __ldg(reinterpret_cast<const Vec*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
+        reinterpret_cast<Vec*>(sW + (size_t)lr * ld)[k] = v;
+    }
+    lstm_seq_zero_tail(sW, R, H);
+    lstm_seq_zero_tail(sV, p.rows, H);
+    for (int i = threadIdx.x; i < u * N; i += kLstmThreads) {
+        const int j = i / N, n = i - j * N;
+        sC[i] = j < nu ? __ldg(p.c0 + (size_t)n * H + u0 + j) : 0.f;
+    }
+    for (int s = 0; s < p.T; ++s) {
+        const S* hp = s == 0 ? p.h0 : p.y + (size_t)(s - 1) * N * H;
+        lstm_seq_product(sW, sV, sP, sG, hp, R, H, N, p.rows, p.ksplit);
+        for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
+            const int j = i / N, n = i - j * N, unit = u0 + j;
+            const size_t row = (size_t)s * N + n;
+            const S* gx = p.gx + row * 4 * H + unit;
+            float* gs = p.gates + row * 4 * H + unit;
+            const size_t o = row * H + unit;
+            const float gi = lstm_sigmoid(sG[(0 * u + j) * N + n] + El::ld(gx));
+            const float gf = lstm_sigmoid(sG[(1 * u + j) * N + n] + El::ld(gx + H));
+            const float gg = tanhf(sG[(2 * u + j) * N + n] + El::ld(gx + 2 * H));
+            const float go = lstm_sigmoid(sG[(3 * u + j) * N + n] + El::ld(gx + 3 * H));
+            const float c = gf * sC[j * N + n] + gi * gg;
+            sC[j * N + n] = c;
+            gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
+            p.cs[o] = c;
+            p.y[o] = El::narrow1(go * tanhf(c));
+        }
+        if (s + 1 < p.T) grid_sync(p.bar);
+    }
+}
+
+// Shared memory: W^T [u][ld] and dgates_{t+1} rows [rows][ld] of S, ld = lstm_seq_ld(4H) | partial sums
+// [ksplit][rows][u], dh_rec [u][N] and carried dc [u][N] of float.
+template <typename S>
+__global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_bwd_kernel(const LstmSeqBwdArgs<S> p) {
+    using El = Elem<S>;
+    extern __shared__ float4 lstm_smem[];
+    const int H = p.H, N = p.N, u = p.u, G = 4 * H, ld = lstm_seq_ld(G);
+    const int u0 = blockIdx.x * u, nu = min(u, H - u0);
+    S* sW = reinterpret_cast<S*>(lstm_smem);
+    S* sV = sW + (size_t)u * ld;
+    float* sP = reinterpret_cast<float*>(sV + (size_t)p.rows * ld);
+    float* sD = sP + (size_t)p.ksplit * p.rows * u;
+    float* sDC = sD + u * N;
+    for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
+        const int k = i / u, j = i - k * u;
+        sW[(size_t)j * ld + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : El::narrow1(0.f);
+    }
+    lstm_seq_zero_tail(sW, u, G);
+    lstm_seq_zero_tail(sV, p.rows, G);
+    for (int i = threadIdx.x; i < u * N; i += kLstmThreads) {
+        const int j = i / N, n = i - j * N;
+        const size_t o = (size_t)n * H + u0 + j;
+        sD[i] = j < nu && p.dhn ? El::ld(p.dhn + o) : 0.f;
+        sDC[i] = j < nu && p.dcn ? __ldg(p.dcn + o) : 0.f;
+    }
+    __syncthreads();
+    for (int s = p.T - 1; s >= 0; --s) {
+        if (s < p.T - 1) lstm_seq_product(sW, sV, sP, sD, p.dg + (size_t)(s + 1) * N * G, u, G, N, p.rows, p.ksplit);
+        for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
+            const int j = i / N, n = i - j * N, unit = u0 + j;
+            const size_t row = (size_t)s * N + n;
+            const size_t o = row * H + unit;
+            S* dg = p.dg + row * G + unit;
+            const float* gs = p.gates + row * G + unit;
+            const float gi = __ldg(gs), gf = __ldg(gs + H), gg = __ldg(gs + 2 * H), go = __ldg(gs + 3 * H);
+            const float tc = tanhf(__ldg(p.cs + o));
+            const float cp = s > 0 ? __ldg(p.cs + o - (size_t)N * H) : __ldg(p.c0 + (size_t)n * H + unit);
+            const float dh = El::ld(p.dy + o) + sD[j * N + n];
+            const float dc = dh * go * (1.f - tc * tc) + sDC[j * N + n];
+            dg[0] = El::narrow1(dc * gg * gi * (1.f - gi));
+            dg[H] = El::narrow1(dc * cp * gf * (1.f - gf));
+            dg[2 * H] = El::narrow1(dc * gi * (1.f - gg * gg));
+            dg[3 * H] = El::narrow1(dh * tc * go * (1.f - go));
+            sDC[j * N + n] = dc * gf;
+            if (s == 0) p.dc0[(size_t)n * H + unit] = dc * gf;
+        }
+        if (s > 0) grid_sync(p.bar);
+    }
+}
+
+static size_t lstm_seq_fwd_smem(int H, int N, int u, int rows, int elem) {
+    const int R = 4 * u;
+    return (size_t)elem * (R + rows) * lstm_seq_ld(H) +
+           sizeof(float) * ((size_t)lstm_seq_ksplit(rows, R, H) * rows * R + (size_t)R * N + (size_t)u * N);
+}
+
+static size_t lstm_seq_bwd_smem(int H, int N, int u, int rows, int elem) {
+    return (size_t)elem * (u + rows) * lstm_seq_ld(4 * H) +
+           sizeof(float) * ((size_t)lstm_seq_ksplit(rows, u, 4 * H) * rows * u + (size_t)2 * u * N);
+}
+
+// The tensor-core step has no fp32 form: fp32 is an invalid dtype here.
+template <class F>
+static cudaError_t with_dtype16(Dtype dtype, F&& f) {
+    switch (dtype) {
+        case Dtype::kBF16: return f(__nv_bfloat16{});
+        case Dtype::kF16: return f(__half{});
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+cudaError_t launch_lstm_seq_forward(const void* gx, const void* whh, const void* h0, const float* c0, void* y,
+                                    float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u,
+                                    int rows, cudaStream_t stream, Dtype dtype) {
+    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
+    return with_dtype16(dtype, [&](auto e) {
+        using S = decltype(e);
+        const LstmSeqFwdArgs<S> p{static_cast<const S*>(gx), static_cast<const S*>(whh), static_cast<const S*>(h0), c0,
+                                  static_cast<S*>(y), gates, cs, bar, T, N, H, u, rows,
+                                  lstm_seq_ksplit(rows, 4 * u, H)};
+        return lstm_launch(lstm_seq_fwd_kernel<S>, p, (H + u - 1) / u, lstm_seq_fwd_smem(H, N, u, rows, sizeof(S)),
+                           stream);
+    });
+}
+
+cudaError_t launch_lstm_seq_backward(const void* dy, const float* gates, const float* cs, const void* whh,
+                                     const float* c0, const void* dhn, const float* dcn, void* dg, float* dc0,
+                                     unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
+                                     Dtype dtype) {
+    if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
+    return with_dtype16(dtype, [&](auto e) {
+        using S = decltype(e);
+        const LstmSeqBwdArgs<S> p{static_cast<const S*>(dy), gates, cs, static_cast<const S*>(whh), c0,
+                                  static_cast<const S*>(dhn), dcn, static_cast<S*>(dg), dc0, bar, T, N, H, u, rows,
+                                  lstm_seq_ksplit(rows, u, 4 * H)};
+        return lstm_launch(lstm_seq_bwd_kernel<S>, p, (H + u - 1) / u, lstm_seq_bwd_smem(H, N, u, rows, sizeof(S)),
+                           stream);
     });
 }
 

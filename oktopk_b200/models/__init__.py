@@ -27,7 +27,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``) and ``fuse_attn=True`` ``net.fuse_attn``; for
     ``lstman4``,
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
-    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``)."""
+    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``); for ``lstm`` (PTB),
+    ``fuse_lstm=True`` turns on ``net.fuse_lstm`` and ``fuse_xent=True`` ``net.fuse_xent``."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
@@ -55,7 +56,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
         net.fuse_lstm = fuse_lstm
         ext = {"labels": AN4_LABELS}
     elif d == "lstm":
-        net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20))
+        net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20),
+                      fuse_lstm=bool(kwargs.get("fuse_lstm", False)), fuse_xent=bool(kwargs.get("fuse_xent", False)))
     elif d in ("bert", "bert_base"):
         cfg = kwargs.get("config")
         if isinstance(cfg, str):

@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops.fused_lstm import lstm_layer, stock_layer
+from ..ops.fused_lstm import lstm_layer, lstm_stack, stock_layer
 
 AN4_LABELS = "_'ABCDEFGHIJKLMNOPQRSTUVWXYZ "     # 29 symbols, index 0 = CTC blank
 
@@ -197,11 +197,19 @@ def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool 
 
 
 class PTBLSTM(nn.Module):
-    """2-layer 1500-hidden word-level LSTM language model (``VGG/models/lstm.py:5-40``), vocab 10k."""
+    """2-layer 1500-hidden word-level LSTM language model (``VGG/models/lstm.py:5-40``), vocab 10k.
+
+    ``fuse_lstm=True`` (or ``net.fuse_lstm = True`` at any time) runs the stacked ``nn.LSTM`` through
+    ``ops/fused_lstm.lstm_stack``: under bf16 / fp16 CUDA autocast, on the 16-bit stacked-layer kernels with the carried
+    state in and out; anywhere else (fp32 included: H = 1500 has no fp32 kernel) exactly the stock layer.  The returned
+    c_n is then fp32.  ``fuse_xent=True`` (``net.fuse_xent``) asks the trainer to compute the loss with the fused softmax
+    cross-entropy (``ops/fused_xent``).  Parameters, buffers and ``state_dict`` keys are the same either way."""
 
     def __init__(self, vocab_size: int = 10000, embedding_dim: int = 1500, num_steps: int = 35, batch_size: int = 20,
-                 num_layers: int = 2, dp_keep_prob: float = 0.35):
+                 num_layers: int = 2, dp_keep_prob: float = 0.35, fuse_lstm: bool = False, fuse_xent: bool = False):
         super().__init__()
+        self.fuse_lstm = fuse_lstm
+        self.fuse_xent = fuse_xent
         self.embedding_dim, self.num_layers = embedding_dim, num_layers
         self.dropout = nn.Dropout(1 - dp_keep_prob)
         self.word_embeddings = nn.Embedding(vocab_size, embedding_dim)
@@ -217,7 +225,10 @@ class PTBLSTM(nn.Module):
 
     def forward(self, inputs: torch.Tensor, hidden):
         emb = self.dropout(self.word_embeddings(inputs))
-        out, hidden = self.lstm(emb, hidden)
+        if self.fuse_lstm:
+            out, hidden = lstm_stack(emb, hidden, self.lstm, self.lstm.dropout, self.training)
+        else:
+            out, hidden = self.lstm(emb, hidden)
         out = self.dropout(out)
         logits = self.sm_fc(out.view(-1, self.embedding_dim))
         return logits.view(inputs.size(0), inputs.size(1), -1), hidden

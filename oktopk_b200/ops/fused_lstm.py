@@ -35,6 +35,10 @@ and the gates' gradients are 16-bit; the saved gates and c, the cell state and e
 dgates_t is rounded to nearest even (an fp16 overflow gives inf, for loss scaling to see) and it is the rounded value
 that the next step reads.  y comes back in the autocast type, as ``nn.LSTM``'s does, the parameter gradients in fp32.
 This differs from cuDNN's 16-bit RNN, which also keeps c in 16 bits.
+
+``lstm_stack(x, hx, rnn, dropout_p, training)`` runs a multi-layer ``nn.LSTM`` from a carried state (the PTB language
+model) under bf16 / fp16 autocast on a second pair of kernels, whose step product runs on the tensor cores; see its
+docstring.
 """
 from __future__ import annotations
 
@@ -226,3 +230,191 @@ def lstm_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, dev_lengt
             w_hh = w_hh.clone()
         ps[i] = w_hh
     return _LstmLayer.apply(x.contiguous(), dev_lengths.contiguous(), geom, dt, *ps)
+
+
+# ---- stacked layers from a carried state (the PTB language model) -----------------------------------------------------
+
+LSTM_WARPS = LSTM_THREADS // 32
+
+
+class LstmSeqGeometry(NamedTuple):
+    units: int              # hidden units per CTA (u)
+    grid: int               # CTAs: ceil(H / u), one per SM
+    fwd_rows: int           # rows of h_{t-1} staged in shared memory at a time by the forward kernel
+    bwd_rows: int           # rows of dgates_{t+1} staged at a time by the backward kernel
+    fwd_smem: int           # dynamic shared memory per CTA, bytes
+    bwd_smem: int
+
+
+def _seq_ld(K: int) -> int:
+    """csrc/lstm.cu lstm_seq_ld: the shared-memory row stride of a K-element operand row."""
+    return -(-K // 16) * 16 + 8
+
+
+def _seq_ksplit(rows: int, R: int, K: int) -> int:
+    """csrc/lstm.cu lstm_seq_ksplit."""
+    tiles = -(-rows // 16) * -(-R // 8)
+    return max(1, min(LSTM_WARPS // tiles, -(-K // 16)))
+
+
+def _seq_fwd_smem(H: int, N: int, u: int, rows: int) -> int:
+    R = 4 * u
+    return 2 * (R + rows) * _seq_ld(H) + 4 * (_seq_ksplit(rows, R, H) * rows * R + R * N + u * N)
+
+
+def _seq_bwd_smem(H: int, N: int, u: int, rows: int) -> int:
+    return 2 * (u + rows) * _seq_ld(4 * H) + 4 * (_seq_ksplit(rows, u, 4 * H) * rows * u + 2 * u * N)
+
+
+def lstm_seq_geometry(H: int, N: int, sms: int, smem_per_block: int) -> Optional[LstmSeqGeometry]:
+    """How the 16-bit stacked-layer kernels (``lstm_seq_forward`` / ``lstm_seq_backward``) split a layer of H units at
+    batch N over ``sms`` SMs with ``smem_per_block`` bytes of opt-in shared memory per CTA, or None when they cannot.
+    As ``lstm_geometry``, each CTA owns u = ceil(H / sms) units and keeps its slice of W_hh (4u rows forward, u columns
+    backward) in shared memory, here with each row padded to ``_seq_ld`` elements for the tensor-core fragments, next to
+    as many staged rows of the step's operand as fit (at least one), the K-split partial sums of the step product, and
+    the fp32 gate sums and cell state (forward) or dh sums and carried dc (backward).  H % 4 == 0, 1 <= N <= MAX_BATCH.
+    On an H100 (132 SMs, 232 448 B): H = 1500, N = 20 is u = 12 on 125 CTAs with all 20 rows of h_{t-1} staged forward
+    (214 272 B) and 6 rows of dgates_{t+1} at a time backward (220 512 B)."""
+    if H <= 0 or H % 4 or not 1 <= N <= MAX_BATCH or sms <= 0:
+        return None
+    u = -(-H // sms)
+    rows = []
+    for smem in (_seq_fwd_smem, _seq_bwd_smem):
+        r = next((r for r in range(N, 0, -1) if smem(H, N, u, r) <= smem_per_block), 0)
+        if r == 0:
+            return None
+        rows.append(r)
+    return LstmSeqGeometry(u, -(-H // u), rows[0], rows[1], _seq_fwd_smem(H, N, u, rows[0]),
+                           _seq_bwd_smem(H, N, u, rows[1]))
+
+
+def _stack_params(rnn: nn.LSTM, layer: int) -> Tuple[torch.Tensor, ...]:
+    return tuple(getattr(rnn, "%s_l%d" % (n, layer)) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
+
+
+def _stack_ok(x: torch.Tensor, hx, rnn: nn.Module) -> Optional[Tuple[LstmSeqGeometry, torch.dtype]]:
+    """The geometry and the kernels' storage type when ``lstm_stack`` runs the native path, else None."""
+    if not (isinstance(rnn, nn.LSTM) and rnn.num_layers >= 1 and not rnn.bidirectional and rnn.bias
+            and rnn.proj_size == 0 and not rnn.batch_first):
+        return None
+    if not (x.is_cuda and x.dim() == 3 and x.size(2) == rnn.input_size and x.size(0) > 0):
+        return None
+    if not torch.is_autocast_enabled("cuda"):
+        return None
+    dt = torch.get_autocast_dtype("cuda")
+    if dt not in (torch.bfloat16, torch.float16) or x.dtype not in (torch.float32, dt) or not ext.available():
+        return None
+    if any(p.dtype != torch.float32 or p.device != x.device for p in rnn.parameters()):
+        return None
+    L, N, H = rnn.num_layers, x.size(1), rnn.hidden_size
+    if hx is not None:
+        if not (isinstance(hx, (tuple, list)) and len(hx) == 2):
+            return None
+        for h in hx:
+            if not (isinstance(h, torch.Tensor) and tuple(h.shape) == (L, N, H) and h.device == x.device
+                    and h.dtype in (torch.float32, dt)):
+                return None
+    p = torch.cuda.get_device_properties(x.device)
+    geom = lstm_seq_geometry(H, N, p.multi_processor_count, p.shared_memory_per_block_optin)
+    return None if geom is None else (geom, dt)
+
+
+class _LstmSeqLayer(torch.autograd.Function):
+    """One layer from (h0, c0) on the stacked-layer kernels: returns y [T, N, H] and h_n (both of type ``dt``) and c_n
+    (fp32).  x, h0 and the parameters are cast to ``dt`` here, once per forward, and both passes run with autocast off.
+    ``h0`` of the input's type or ``dt``, ``c0`` fp32 or ``dt``; their gradients come back in their types."""
+
+    @staticmethod
+    def forward(ctx, x, h0, c0, geom, dt, w_ih, w_hh, b_ih, b_hh):
+        C = ext.require()
+        ctx.set_materialize_grads(False)
+        T, N, I = x.shape
+        H = w_hh.size(1)
+        with torch.autocast(x.device.type, enabled=False):
+            xs = x.to(dt).contiguous()
+            w_ih_s, w_hh_s = w_ih.to(dt), w_hh.to(dt).contiguous()
+            h0s, c0f = h0.to(dt).contiguous(), c0.float().contiguous()
+            gx = torch.addmm((b_ih + b_hh).to(dt), xs.view(T * N, I), w_ih_s.t())      # (T N) x 4H
+        y = torch.empty(T, N, H, device=x.device, dtype=dt)
+        gates = torch.empty(T, N, 4 * H, device=x.device, dtype=torch.float32)
+        cs = torch.empty(T, N, H, device=x.device, dtype=torch.float32)
+        bar = torch.zeros(1, dtype=torch.int64, device=x.device)
+        C.lstm_seq_forward(gx.data_ptr(), w_hh_s.data_ptr(), h0s.data_ptr(), c0f.data_ptr(), y.data_ptr(),
+                           gates.data_ptr(), cs.data_ptr(), bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows,
+                           torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt])
+        ctx.save_for_backward(xs, h0s, c0f, y, gates, cs, w_ih_s, w_hh_s)
+        ctx.geom = geom
+        ctx.dtypes = (x.dtype, h0.dtype, c0.dtype)
+        return y, y[T - 1].clone(), cs[T - 1].clone()
+
+    @staticmethod
+    def backward(ctx, dy, dhn, dcn):
+        C = ext.require()
+        x, h0, c0, y, gates, cs, w_ih, w_hh = ctx.saved_tensors
+        T, N, I = x.shape
+        H = w_hh.size(1)
+        dt = y.dtype
+        dy = torch.zeros_like(y) if dy is None else dy.to(dt).contiguous()
+        dhn = None if dhn is None else dhn.to(dt).contiguous()
+        dcn = None if dcn is None else dcn.float().contiguous()
+        dg = torch.empty(T, N, 4 * H, device=x.device, dtype=dt)
+        dc0 = torch.empty(N, H, device=x.device, dtype=torch.float32)
+        bar = torch.zeros(1, dtype=torch.int64, device=x.device)
+        C.lstm_seq_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), w_hh.data_ptr(), c0.data_ptr(),
+                            0 if dhn is None else dhn.data_ptr(), 0 if dcn is None else dcn.data_ptr(), dg.data_ptr(),
+                            dc0.data_ptr(), bar.data_ptr(), T, N, H, ctx.geom.units, ctx.geom.bwd_rows,
+                            torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt])
+        need = ctx.needs_input_grad
+        x_dt, h0_dt, c0_dt = ctx.dtypes
+        g2 = dg.view(T * N, 4 * H)
+        with torch.autocast(x.device.type, enabled=False):      # GEMMs in dt; the parameters' gradients come back fp32
+            dx = (g2 @ w_ih).view(T, N, I).to(x_dt) if need[0] else None
+            dh0 = (dg[0] @ w_hh).to(h0_dt) if need[1] else None
+            dw_ih = (g2.t() @ x.view(T * N, I)).float() if need[5] else None
+            if need[6]:                                         # h_{t-1}: h0, then y[:-1]
+                hp = torch.cat([h0.unsqueeze(0), y[:-1]]).view(T * N, H)
+                dw_hh = (g2.t() @ hp).float()
+            else:
+                dw_hh = None
+            db = g2.sum(0, dtype=torch.float32) if need[7] or need[8] else None
+        db_ih = db if need[7] else None
+        db_hh = (db.clone() if need[7] else db) if need[8] else None             # two tensors, never one aliased
+        return dx, dh0, dc0.to(c0_dt) if need[2] else None, None, None, dw_ih, dw_hh, db_ih, db_hh
+
+
+def lstm_stack(x: torch.Tensor, hx, rnn: nn.Module, dropout_p: float, training: bool):
+    """``rnn(x, hx)`` for a uni-directional, multi-layer ``nn.LSTM`` over the time-major ``x`` (T x N x I): returns
+    ``(y, (h_n, c_n))`` with h_n and c_n [L, N, H], as ``nn.LSTM`` does.  ``hx`` = (h0, c0), each [L, N, H], or None
+    (zeros).
+
+    Under bf16 / fp16 CUDA autocast its layers run one after another on the stacked-layer kernels (``lstm_seq_forward``
+    / ``lstm_seq_backward``): each layer from its own (h0, c0), every row of length T, the step product on the tensor
+    cores, W_hh held in shared memory in the autocast type (at H = 1500 that needs 16 bits: the fp32 slice, 288 KB per
+    CTA, does not fit).  Between layers, in training, ``F.dropout(p=dropout_p)``, where ``nn.LSTM`` places its dropout
+    (cuDNN draws its own masks, so the stock and fused layers see different ones).  y and h_n come back in the autocast
+    type and c_n in fp32: the kernels keep the cell state in fp32, where cuDNN's 16-bit RNN keeps it in 16 bits.  The
+    parameter gradients are fp32; h0 and c0 may be fp32 or of the autocast type, and their gradients have their types.
+    Numerics otherwise as the module docstring's 16-bit layer: W_hh, gx, y, dy and dgates 16-bit, rounded to nearest
+    even (an fp16 overflow is inf), everything else fp32, bitwise reproducible.
+
+    Needs the native extension, fp32 parameters on x's device, bias, ``proj_size == 0``, ``batch_first=False``, x of
+    fp32 or the autocast type, T >= 1, hx of the right shape, and an (H, N) that ``lstm_seq_geometry`` accepts on the
+    device.  Anything else -- autocast off (fp32), the CPU, fp64, a bidirectional ``rnn``, a layer too large -- returns
+    exactly ``rnn(x, hx)``."""
+    ok = _stack_ok(x, hx, rnn)
+    if ok is None:
+        return rnn(x, hx)
+    geom, dt = ok
+    L, N, H = rnn.num_layers, x.size(1), rnn.hidden_size
+    if hx is None:
+        z = torch.zeros(L, N, H, device=x.device, dtype=dt)
+        hx = (z, z.float())
+    h0, c0 = hx
+    hs, cs = [], []
+    for layer in range(L):
+        if layer > 0 and training and dropout_p > 0:
+            x = nn.functional.dropout(x, dropout_p, True)
+        x, h, c = _LstmSeqLayer.apply(x.contiguous(), h0[layer], c0[layer], geom, dt, *_stack_params(rnn, layer))
+        hs.append(h)
+        cs.append(c)
+    return x, (torch.stack(hs), torch.stack(cs))

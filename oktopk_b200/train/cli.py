@@ -90,6 +90,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-lstm", action="store_true",
                    help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
                         "and pass, instead of packed sequences through cuDNN (default: stock)")
+    p.add_argument("--fused-lstm-lm", action="store_true",
+                   help="lstm (PTB), with --bf16 or --fp16: the stacked LSTM runs on the 16-bit stacked-layer fused "
+                        "recurrence kernels, the hidden state carried in and out (default: stock cuDNN layer)")
     p.add_argument("--fused-lstm-autocast", action="store_true",
                    help="with --fused-lstm and --bf16 or --fp16: the LSTM layers take the 16-bit fused recurrence kernels "
                         "(default: stock layers under autocast)")
@@ -140,7 +143,7 @@ def model_args(args: argparse.Namespace):
         model_kwargs["mlm_capacity"] = args.mlm_capacity
     if args.fused_attn:
         model_kwargs["fuse_attn"] = True
-    if args.fused_lstm:
+    if args.fused_lstm or args.fused_lstm_lm:
         model_kwargs["fuse_lstm"] = True
     if args.fused_lstm_autocast:
         model_kwargs["fuse_lstm_autocast"] = True
@@ -161,12 +164,14 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln``, ``--fused-xent``, ``--sparse-mlm``, ``--mlm-capacity`` and ``--fused-attn`` are for BERT only
-    (``--dnn bert_base`` / ``bert``, or a ``--module models.bertN.depth=M``); ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
+    """``--fused-ln``, ``--sparse-mlm``, ``--mlm-capacity`` and ``--fused-attn`` are for BERT only (``--dnn bert_base``
+    / ``bert``, or a ``--module models.bertN.depth=M``), ``--fused-xent`` for BERT and the PTB model (``--dnn lstm``);
+    ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
     dnn = model_args(args)[0]
-    for flag, on in (("--fused-ln", args.fused_ln), ("--fused-xent", args.fused_xent),
-                     ("--sparse-mlm", args.sparse_mlm), ("--mlm-capacity", args.mlm_capacity is not None),
-                     ("--fused-attn", args.fused_attn)):
+    if args.fused_xent and dnn not in ("bert", "bert_base", "lstm"):
+        parser.error("--fused-xent applies to BERT (bert_base, bert) and lstm, not %s" % dnn)
+    for flag, on in (("--fused-ln", args.fused_ln), ("--sparse-mlm", args.sparse_mlm),
+                     ("--mlm-capacity", args.mlm_capacity is not None), ("--fused-attn", args.fused_attn)):
         if on and dnn not in ("bert", "bert_base"):
             parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
     if args.mlm_capacity is not None:
@@ -179,9 +184,14 @@ def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
     """``--fused-lstm`` and ``--bidirectional`` are for the AN4 DeepSpeech model (``--dnn lstman4``) only;
     ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
-    needs ``--fused-lstm`` and ``--bidirectional``."""
+    needs ``--fused-lstm`` and ``--bidirectional``.  ``--fused-lstm-lm`` is for the PTB model (``--dnn lstm``) and
+    needs ``--bf16`` or ``--fp16``."""
     if args.fused_lstm and model_args(args)[0] != "lstman4":
         parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
+    if args.fused_lstm_lm and model_args(args)[0] != "lstm":
+        parser.error("--fused-lstm-lm applies to lstm, not %s" % model_args(args)[0])
+    if args.fused_lstm_lm and not (args.bf16 or args.fp16):
+        parser.error("--fused-lstm-lm needs --bf16 or --fp16")
     if args.fused_lstm_autocast and not args.fused_lstm:
         parser.error("--fused-lstm-autocast needs --fused-lstm")
     if args.fused_lstm_autocast and not (args.bf16 or args.fp16):

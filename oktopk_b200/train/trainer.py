@@ -23,6 +23,7 @@ from .. import compression as _comp
 from ..config import LossScale, OkTopkConfig, preset as _preset
 from ..models import create_net
 from ..models.bert import BertPreTrainingHeads
+from ..ops.fused_xent import softmax_cross_entropy
 from ..optimizer import BertAdam, DistributedOptimizer, broadcast_parameters
 from ..parallel.world import World, world as _world
 from ..utils.logging import get_logger
@@ -206,6 +207,8 @@ class Trainer:
                 self.hidden = self.net.init_hidden(x.size(1), self.device)
             self.hidden = tuple(h.detach() for h in self.hidden)
             out, self.hidden = self.net(x, self.hidden)
+            if getattr(self.net, "fuse_xent", False):
+                return softmax_cross_entropy(out.view(-1, out.size(-1)), y.view(-1)), None
             return self.criterion(out.view(-1, out.size(-1)), y.view(-1)), None
         x, y = batch
         if self.channels_last and x.dim() == 4:
