@@ -99,6 +99,10 @@ class OkTopkConfig:
     early_pack: bool = True
     early_pack_frac: float = 0.85
     early_pack_ctas: int = 32
+    # with a fused SGD update, each early-pack segment is followed by the zero-gradient update of its ranges (old values
+    # stashed, 8 B per element of the bucket), so that after the call only the elements it wrote are recomputed
+    # (csrc/optim.cu sgd_ahead_kernel).  OKTOPK_SGD_AHEAD=0 in the environment turns it off.
+    sgd_ahead: bool = True
     gselect_mode: str = "auto"          # global selection over the reduced region: 'list' | 'scan' | 'auto' (density <= 0.5 % -> list)
     peer_timeout_s: float = 60.0        # bound of every cross-GPU flag wait inside the kernels (0 = wait forever)
 

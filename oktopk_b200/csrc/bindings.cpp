@@ -505,6 +505,47 @@ static void fused_sgd(uint64_t p, uint64_t g, uint64_t mom, int n, double moment
                         S_(stream)),
        "fused_sgd");
 }
+// [(lo, hi), ...] element ranges of an n-element (bucket, param group) slice, at multiples of 4 and inside its whole
+// float4 vectors -> a table of vector ranges
+static SgdRanges sgd_ranges(const std::vector<std::pair<long long, long long>>& rs, int n, const char* what) {
+    if ((int)rs.size() > kPackRangeMax)
+        throw std::runtime_error(std::string(what) + ": more than " + std::to_string(kPackRangeMax) + " ranges");
+    SgdRanges r;
+    std::memset(&r, 0, sizeof(r));
+    r.nr = (int)rs.size();
+    for (int q = 0; q < r.nr; ++q) {
+        const long long lo = rs[q].first, hi = rs[q].second;
+        if (lo < 0 || hi < lo || lo % 4 || hi % 4 || hi > 4LL * (n / 4))
+            throw std::runtime_error(std::string(what) + ": ranges must lie at multiples of 4 inside the slice's whole "
+                                     "float4 vectors");
+        r.lo[q] = (int)(lo / 4);
+        r.hi[q] = (int)(hi / 4);
+    }
+    return r;
+}
+static void sgd_ahead(uint64_t p, uint64_t mom, uint64_t sp, uint64_t sm, int n,
+                      const std::vector<std::pair<long long, long long>>& ranges, double momentum, double dampening,
+                      double wd, int nesterov, int max_ctas, uint64_t stream, uint64_t scal_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("sgd_ahead: scal_ptr must point at the group's device scalars");
+    if (momentum != 0.0 && (mom == 0 || sm == 0)) throw std::runtime_error("sgd_ahead: momentum needs mom and sm");
+    const SgdHyper h{(float)momentum, (float)dampening, (float)wd, nesterov, 0};
+    ck(launch_sgd_ahead(P_<float>(p), P_<float>(mom), P_<float>(sp), P_<float>(sm), sgd_ranges(ranges, n, "sgd_ahead"),
+                        h, max_ctas, P_<float>(scal_ptr), S_(stream)),
+       "sgd_ahead");
+}
+static void fused_sgd_tail(uint64_t p, uint64_t g, uint64_t mom, uint64_t sp, uint64_t sm, int n,
+                           const std::vector<std::pair<long long, long long>>& ahead,
+                           const std::vector<std::pair<long long, long long>>& dense, double momentum, double dampening,
+                           double wd, int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr,
+                           uint64_t fault_ptr, uint64_t skip_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("fused_sgd_tail: scal_ptr must point at the group's device scalars");
+    if (momentum != 0.0 && (mom == 0 || sm == 0)) throw std::runtime_error("fused_sgd_tail: momentum needs mom and sm");
+    const SgdHyper h{(float)momentum, (float)dampening, (float)wd, nesterov, first};
+    ck(launch_fused_sgd_tail(P_<float>(p), P_<float>(g), P_<float>(mom), P_<const float>(sp), P_<const float>(sm), n,
+                             sgd_ranges(ahead, n, "fused_sgd_tail"), sgd_ranges(dense, n, "fused_sgd_tail"), h,
+                             zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
+       "fused_sgd_tail");
+}
 static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double b1, double b2, double eps,
                             double wd, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
                             uint64_t skip_ptr) {
@@ -818,6 +859,13 @@ PYBIND11_MODULE(_C, m) {
     m.def("fused_sgd", &fused_sgd, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("n"), py::arg("momentum"),
           py::arg("dampening"), py::arg("wd"), py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"),
           py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
+    m.def("sgd_ahead", &sgd_ahead, py::arg("p"), py::arg("mom"), py::arg("sp"), py::arg("sm"), py::arg("n"),
+          py::arg("ranges"), py::arg("momentum"), py::arg("dampening"), py::arg("wd"), py::arg("nesterov"),
+          py::arg("max_ctas"), py::arg("stream"), py::arg("scal_ptr"));
+    m.def("fused_sgd_tail", &fused_sgd_tail, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("sp"), py::arg("sm"),
+          py::arg("n"), py::arg("ahead"), py::arg("dense"), py::arg("momentum"), py::arg("dampening"), py::arg("wd"),
+          py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"), py::arg("stream"), py::arg("scal_ptr"),
+          py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
     m.def("fused_bert_adam", &fused_bert_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"), py::arg("stream"),
           py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);

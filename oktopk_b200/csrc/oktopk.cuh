@@ -295,6 +295,27 @@ cudaError_t launch_kth_abs(const float* x, int n, int k, OktState* st, float* ou
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
                              const int* skip, cudaStream_t stream);
+// Early SGD update (sgd_ahead_kernel / fused_sgd_tail_kernel in optim.cu).  SgdRanges: float4 vector ranges [lo, hi) of a
+// (bucket, param group) slice, in slice order, at most kPackRangeMax of them; SgdHyper: torch.optim.SGD's group options.
+struct SgdRanges {
+    int nr;
+    int lo[kPackRangeMax];
+    int hi[kPackRangeMax];
+};
+struct SgdHyper {
+    float momentum, dampening, wd;
+    int nesterov, first;
+};
+// the zero-gradient update over `r` in place, old p / m to the stash sp / sm (sm: only with momentum), on at most
+// max_ctas CTAs; never on a first step
+cudaError_t launch_sgd_ahead(float* p, float* mom, float* sp, float* sm, const SgdRanges& r, const SgdHyper& h,
+                             int max_ctas, const float* scal, cudaStream_t stream);
+// the rest of a step whose `ahead` ranges had launch_sgd_ahead: there, every vector with a written gradient is
+// recomputed from the stash (fault or skip: every vector is restored from it); `dense` and the scalar tail of the
+// n-element slice take fused_sgd's update
+cudaError_t launch_fused_sgd_tail(float* p, float* g, float* mom, const float* sp, const float* sm, int n,
+                                  const SgdRanges& ahead, const SgdRanges& dense, const SgdHyper& h, int zero_grad,
+                                  const float* scal, const int* fault, const int* skip, cudaStream_t stream);
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
                                    float weight_decay, int zero_grad, const float* scal, const int* fault,
                                    const int* skip, cudaStream_t stream);

@@ -74,24 +74,154 @@ __device__ __forceinline__ void update_pass(float* __restrict__ p, float* __rest
         }
 }
 
+// torch.optim.SGD on one element, the one definition fused_sgd_kernel, sgd_ahead_kernel and fused_sgd_tail_kernel share.
+// Every rounding spelled out, so that where nvcc contracts into an fma cannot change the result.
+__device__ __forceinline__ void sgd_update(const SgdHyper& h, float lr, float& pw, float gw, float& mw) {
+    const float damp = h.first ? 0.f : h.dampening;    // torch: the first step copies d_p into the buffer
+    float d = __fmaf_rn(h.wd, pw, gw);
+    if (h.momentum != 0.f) {
+        mw = h.first ? d : __fmaf_rn(1.f - damp, d, __fmul_rn(h.momentum, mw));
+        d = h.nesterov ? __fmaf_rn(h.momentum, mw, d) : mw;
+    }
+    pw = __fmaf_rn(-lr, d, pw);
+}
+
+__device__ __forceinline__ void sgd_update4(const SgdHyper& h, float lr, float4& pw, const float4& gw, float4& mw) {
+    sgd_update(h, lr, pw.x, gw.x, mw.x); sgd_update(h, lr, pw.y, gw.y, mw.y);
+    sgd_update(h, lr, pw.z, gw.z, mw.z); sgd_update(h, lr, pw.w, gw.w, mw.w);
+}
+
 // scal -> {lr}
 __global__ void __launch_bounds__(kOptThreads) fused_sgd_kernel(float* __restrict__ p, float* __restrict__ g,
-                                                                 float* __restrict__ mom, int n, float momentum,
-                                                                 float dampening, float wd, int nesterov, int first,
+                                                                 float* __restrict__ mom, int n, const SgdHyper h,
                                                                  int zero_grad, const float* __restrict__ scal,
                                                                  const int* __restrict__ fault,
                                                                  const int* __restrict__ skip) {
-    const float damp = first ? 0.f : dampening;       // torch: the first step copies d_p into the buffer
-    // every rounding spelled out, so that where nvcc contracts into an fma cannot change the result
-    update_pass<1, 1>(p, g, mom, nullptr, n, momentum != 0.f && !first, momentum != 0.f, zero_grad, scal, fault, skip,
-                      [=](const float* s, float& pw, float gw, float& mw, float&) {
-                          float d = __fmaf_rn(wd, pw, gw);
-                          if (momentum != 0.f) {
-                              mw = first ? d : __fmaf_rn(1.f - damp, d, __fmul_rn(momentum, mw));
-                              d = nesterov ? __fmaf_rn(momentum, mw, d) : mw;
-                          }
-                          pw = __fmaf_rn(-s[0], d, pw);
-                      });
+    update_pass<1, 1>(p, g, mom, nullptr, n, h.momentum != 0.f && !h.first, h.momentum != 0.f, zero_grad, scal, fault,
+                      skip, [=](const float* s, float& pw, float gw, float& mw, float&) { sgd_update(h, s[0], pw, gw, mw); });
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Early SGD update.  On a sparse step the reduced gradient is zero on all but ~k of the n elements, and there the update
+// depends only on p, m and lr.  Once autograd has produced a parameter's gradient nothing in the step reads its weights
+// again, so the zero-gradient update can run during backward, beside the bucket's early-pack segment: sgd_ahead_kernel
+// stashes the old p and m and applies it in place.  After the Ok-Topk call fused_sgd_tail_kernel recomputes, from the
+// stash, every vector of those ranges whose gradient the call wrote (any bit set: a -0 counts too), so that each element
+// ends up with exactly fused_sgd_kernel's result, and runs fused_sgd_kernel's update over the ranges the ahead pass did
+// not cover.
+// ------------------------------------------------------------------------------------------------------------
+constexpr int kAheadUnroll = 4;       // float4 vectors in flight per thread: the pass runs on a capped grid
+
+__device__ __forceinline__ void st_evict_f4(float4* p, const float4& v) {
+    asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+// Loads and stores are evict-first: backward's activations keep L2.
+__global__ void __launch_bounds__(kOptThreads) sgd_ahead_kernel(float* __restrict__ p, float* __restrict__ mom,
+                                                                 float* __restrict__ sp, float* __restrict__ sm,
+                                                                 const SgdRanges r, const SgdHyper h,
+                                                                 const float* __restrict__ scal) {
+    const float lr = scal[0];
+    const bool use_m = h.momentum != 0.f;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    float4* m4 = reinterpret_cast<float4*>(mom);
+    float4* sp4 = reinterpret_cast<float4*>(sp);
+    float4* sm4 = reinterpret_cast<float4*>(sm);
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int stride = gridDim.x * kOptThreads;
+    for (int q = 0; q < r.nr; ++q) {
+        const int hi = r.hi[q];
+        for (int i0 = r.lo[q] + blockIdx.x * kOptThreads + threadIdx.x; i0 < hi; i0 += kAheadUnroll * stride) {
+            float4 pw[kAheadUnroll], mw[kAheadUnroll];
+#pragma unroll
+            for (int u = 0; u < kAheadUnroll; ++u) {
+                const int i = i0 + u * stride;
+                pw[u] = mw[u] = zero;
+                if (i < hi) {
+                    pw[u] = ld_stream_f4(p4 + i);
+                    if (use_m) mw[u] = ld_stream_f4(m4 + i);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < kAheadUnroll; ++u) {
+                const int i = i0 + u * stride;
+                if (i >= hi) continue;
+                st_evict_f4(sp4 + i, pw[u]);
+                if (use_m) st_evict_f4(sm4 + i, mw[u]);
+                sgd_update4(h, lr, pw[u], zero, mw[u]);
+                st_evict_f4(p4 + i, pw[u]);
+                if (use_m) st_evict_f4(m4 + i, mw[u]);
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ bool any_bits(const float4& v) {
+    return (__float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z) | __float_as_uint(v.w)) != 0u;
+}
+
+// scal -> {lr}.  A vector is zeroed in g under fused_sgd_kernel's rule (a lane != 0), so the bucket ends up the same too.
+__global__ void __launch_bounds__(kOptThreads) fused_sgd_tail_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                                      float* __restrict__ mom,
+                                                                      const float* __restrict__ sp,
+                                                                      const float* __restrict__ sm, int n,
+                                                                      const SgdRanges ahead, const SgdRanges dense,
+                                                                      const SgdHyper h, int zero_grad,
+                                                                      const float* __restrict__ scal,
+                                                                      const int* __restrict__ fault,
+                                                                      const int* __restrict__ skip) {
+    const bool use_m = h.momentum != 0.f;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    float4* g4 = reinterpret_cast<float4*>(g);
+    float4* m4 = reinterpret_cast<float4*>(mom);
+    const float4* sp4 = reinterpret_cast<const float4*>(sp);
+    const float4* sm4 = reinterpret_cast<const float4*>(sm);
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int first = blockIdx.x * kOptThreads + threadIdx.x, stride = gridDim.x * kOptThreads;
+    const bool faulted = fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0;
+    if (faulted || verdict_set(skip)) {
+        // the step is not applied: p and m get their old values back; after a fault the gradient is left as it is
+        // (fused_sgd_kernel returns at once), after a skip it is cleared as fused_sgd_kernel clears it
+        for (int q = 0; q < ahead.nr; ++q)
+            for (int i = ahead.lo[q] + first; i < ahead.hi[q]; i += stride) {
+                p4[i] = sp4[i];
+                if (use_m) m4[i] = sm4[i];
+            }
+        if (faulted) return;
+        update_pass<1, 1>(p, g, mom, nullptr, n, false, false, zero_grad, scal, nullptr, skip,
+                          [](const float*, float&, float, float&, float&) {});
+        return;
+    }
+    const float lr = scal[0];
+    for (int q = 0; q < ahead.nr; ++q)
+        for (int i = ahead.lo[q] + first; i < ahead.hi[q]; i += stride) {
+            const float4 gw = ld_stream_f4(g4 + i);
+            if (!any_bits(gw)) continue;                // the ahead pass's result stands
+            float4 pw = sp4[i], mw = zero;
+            if (use_m) mw = sm4[i];
+            sgd_update4(h, lr, pw, gw, mw);
+            p4[i] = pw;
+            if (use_m) m4[i] = mw;
+            if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
+        }
+    for (int q = 0; q < dense.nr; ++q)
+        for (int i = dense.lo[q] + first; i < dense.hi[q]; i += stride) {
+            float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = zero;
+            if (use_m && !h.first) mw = m4[i];
+            sgd_update4(h, lr, pw, gw, mw);
+            p4[i] = pw;
+            if (use_m) m4[i] = mw;
+            if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
+        }
+    if (blockIdx.x == 0)
+        for (int i = (n >> 2) * 4 + threadIdx.x; i < n; i += kOptThreads) {
+            float pw = p[i], gw = g[i], mw = 0.f;
+            if (use_m && !h.first) mw = mom[i];
+            sgd_update(h, lr, pw, gw, mw);
+            p[i] = pw;
+            if (use_m) mom[i] = mw;
+            if (zero_grad) g[i] = 0.f;
+        }
 }
 
 // scal -> {scheduled lr}
@@ -185,8 +315,28 @@ static inline int opt_grid(int n) {
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
                              const int* skip, cudaStream_t stream) {
-    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, momentum, dampening, weight_decay, nesterov,
-                                                             first_step, zero_grad, scal, fault, skip);
+    const SgdHyper h{momentum, dampening, weight_decay, nesterov, first_step};
+    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, h, zero_grad, scal, fault, skip);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_sgd_ahead(float* p, float* mom, float* sp, float* sm, const SgdRanges& r, const SgdHyper& h,
+                             int max_ctas, const float* scal, cudaStream_t stream) {
+    if (h.first) return cudaErrorInvalidValue;
+    long long vecs = 0;
+    for (int q = 0; q < r.nr; ++q) vecs += r.hi[q] - r.lo[q];
+    if (vecs <= 0) return cudaSuccess;
+    long long grid = (vecs + kOptThreads * kAheadUnroll - 1) / (kOptThreads * kAheadUnroll);
+    grid = std::min<long long>(grid, std::max(max_ctas, 1));
+    sgd_ahead_kernel<<<(int)grid, kOptThreads, 0, stream>>>(p, mom, sp, sm, r, h, scal);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fused_sgd_tail(float* p, float* g, float* mom, const float* sp, const float* sm, int n,
+                                  const SgdRanges& ahead, const SgdRanges& dense, const SgdHyper& h, int zero_grad,
+                                  const float* scal, const int* fault, const int* skip, cudaStream_t stream) {
+    fused_sgd_tail_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, sp, sm, n, ahead, dense, h, zero_grad,
+                                                                  scal, fault, skip);
     return cudaGetLastError();
 }
 

@@ -23,6 +23,7 @@ What is different by design (GPU-first):
 from __future__ import annotations
 
 import math
+import os
 import warnings
 from typing import Dict, Iterable, List, Optional
 
@@ -35,6 +36,13 @@ from .parallel.allreducer import AllReducer
 from .parallel.buckets import Bucket, attach, build_buckets
 from .parallel.early_pack import PackPlanner
 from .parallel.world import World, world as _world
+
+
+# CTA cap of the early SGD update (sgd_ahead_kernel).  It streams 24 B per element beside backward and must finish before
+# backward does, or the update after the call waits for it; every CTA beyond that takes HBM bandwidth from backward.
+# VGG-16, 16 images, H100 SXM at 700 W, ms/step against the update off: 8 CTAs +13.6 %, 12 -0.3 %, 16 -3.0 %, 20 -4.4 %,
+# 24 -4.2 %, 32 -0.5 % (ROADMAP 2b).  24 keeps a margin from the cliff below.
+SGD_AHEAD_CTAS = 24
 
 
 # ====================================================================================== loss scaling
@@ -187,6 +195,21 @@ class _BucketedComm:
             # high priority: a bucket's (SM-partitioned) communication kernel should get its SMs as soon as backward
             # kernels retire CTAs, not after the whole backward queue
             self._comm_stream = torch.cuda.Stream(priority=-1)
+        # Early SGD update (csrc/optim.cu sgd_ahead_kernel): beside each early-pack segment, the zero-gradient update of
+        # its ranges runs on a side stream, forked from the segment's event; the tail after the call recomputes, from the
+        # stash of old values, only the elements the call wrote.  The stash is the bucket's length, allocated here.
+        self._ahead_stash: Dict[int, tuple] = {}
+        self._ahead_stream = None
+        self._ahead_ctas = SGD_AHEAD_CTAS
+        if (self._packs and self._update is _SGDUpdate and self._cfg.sgd_ahead
+                and os.environ.get("OKTOPK_SGD_AHEAD", "1") != "0"):
+            self._ahead_stream = torch.cuda.Stream()
+            for b in self._buckets:
+                if b.index in self._packs:
+                    mom = any(self.param_groups[gi].get("momentum", 0.0) != 0 for gi, _, _ in b.group_slices)
+                    self._ahead_stash[b.index] = (torch.empty_like(b.grad), torch.empty_like(b.grad) if mom else None)
+        for b in self._buckets:
+            b.ahead = None                        # this step: None undecided, else whether its segments update early
         allreducer.add_resync_hook(self._resync_replicas)
         if loss_scale is not None:
             allreducer.enable_loss_scaling()
@@ -295,11 +318,37 @@ class _BucketedComm:
             ptrs.append(g.data_ptr())
             offs.append(o)
             lens.append(g.numel())
+        if b.ahead is None:
+            # the step's momentum buffers exist (not its first step) and the device lr is this step's (eager steps push
+            # it here, ahead of step(); graph replays push it before the replay)
+            b.ahead = b.index in self._ahead_stash and self._update.keys[0] in self._flat_state.get(b.index, {})
+            if b.ahead:
+                self._maybe_refresh_lr()
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
         self._comm_stream.wait_event(ev)
         with torch.cuda.stream(self._comm_stream):
             self._allreducer.pack_segment(b.name, ranges, (ptrs, offs, lens), stream=self._comm_stream)
+        if b.ahead:
+            self._sgd_ahead(b, ranges, ev)
+
+    def _sgd_ahead(self, b: Bucket, ranges, ev) -> None:
+        """The zero-gradient SGD update of bucket ``b``'s ``ranges`` (those of the segment just enqueued), per param group,
+        behind ``ev`` on the side stream; ``synchronize()`` joins it."""
+        s_ = self._ahead_stream
+        if s_ is not self._comm_stream:
+            s_.wait_event(ev)
+        sp, sm = self._ahead_stash[b.index]
+        fs = self._flat_state[b.index]
+        C = ext.require()
+        for gi, s, e in b.group_slices:
+            rs = _clip_ranges(ranges, s, e)
+            if not rs:
+                continue
+            m, damp, wd, nest = _SGDUpdate.hyper(self, self.param_groups[gi])
+            C.sgd_ahead(b.flat_param.data_ptr() + 4 * s, fs["momentum_buffer"].data_ptr() + 4 * s, sp.data_ptr() + 4 * s,
+                        sm.data_ptr() + 4 * s if sm is not None else 0, e - s, rs, m, damp, wd, int(nest),
+                        int(self._ahead_ctas), s_.cuda_stream, self._lr_ptr(gi))
 
     def _launch_ready(self) -> None:
         # strictly in bucket order on every rank: the fused kernels spin on peers' flags, so two
@@ -450,6 +499,8 @@ class _BucketedComm:
             cur = torch.cuda.current_stream()
             for b in self._buckets:
                 cur.wait_event(b.event)
+            if any(b.ahead for b in self._buckets):
+                cur.wait_stream(self._ahead_stream)
         for b in self._buckets:                   # the reductions' reads of the gradient tensors are ordered before
             b.held = None                         # anything the current stream does next: their memory may be reused
         self._synced = True
@@ -461,6 +512,7 @@ class _BucketedComm:
             if b.index in self._packs:
                 self._packs[b.index].reset()
                 b.packing = None
+            b.ahead = None
         self._next_launch = 0
         self._synced = False
         self._allreducer.poll_faults()           # pinned host flag, no sync: a timed-out peer wait surfaces at once
@@ -561,6 +613,10 @@ class _BucketedComm:
         # after a landing step the next landing copy overwrites the whole bucket: it need not be cleared
         zero_grad = 0 if self._land and not self._direct else 1
         skip_ptr = self._ls.found_ptr if self._ls is not None else 0
+        if b.ahead and on_gpu:
+            self._sgd_tail(b, fs, zero_grad, skip_ptr)
+            b.dirty = False
+            return
         for gi, s, e in b.group_slices:
             def launch(fn, *hyper):
                 fn(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
@@ -572,6 +628,23 @@ class _BucketedComm:
             if not on_gpu:
                 b.grad[s:e].zero_()
         b.dirty = False
+
+    def _sgd_tail(self, b: Bucket, fs: Dict[str, torch.Tensor], zero_grad: int, skip_ptr: int) -> None:
+        """The update of a bucket whose segments' ranges had ``_sgd_ahead``: one ``fused_sgd_tail`` per param group, which
+        recomputes the elements the call wrote in those ranges and updates ``PackPlanner.rest()`` in full."""
+        planner = self._packs[b.index]
+        ahead = [r for seg in planner.segments for r in seg]
+        rest = planner.rest()
+        sp, sm = self._ahead_stash[b.index]
+        C = ext.require()
+        for gi, s, e in b.group_slices:
+            m, damp, wd, nest = _SGDUpdate.hyper(self, self.param_groups[gi])
+            C.fused_sgd_tail(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
+                             fs["momentum_buffer"].data_ptr() + 4 * s, sp.data_ptr() + 4 * s,
+                             sm.data_ptr() + 4 * s if sm is not None else 0, e - s, _clip_ranges(ahead, s, e),
+                             _clip_ranges(rest, s, e), m, damp, wd, int(nest), 0, zero_grad,
+                             torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
+                             self._allreducer.fault_ptr(b.name), skip_ptr)
 
     def _adopt_state(self, counter: Optional[int] = None) -> None:
         """Move per-parameter state (from ``load_state_dict`` or the wrapped optimizer) into the flat buffers.  A bucket
@@ -614,6 +687,18 @@ class _BucketedComm:
                         self.state[p][k] = v
 
 
+def _clip_ranges(ranges, s: int, e: int):
+    """Bucket element ranges -> their parts inside the param-group slice [s, e), relative to s and clipped to the slice's
+    whole float4 vectors (its scalar tail is the tail kernel's, densely)."""
+    top = 4 * ((e - s) // 4)
+    out = []
+    for lo, hi in ranges:
+        lo, hi = max(lo - s, 0), min(hi - s, top)
+        if lo < hi:
+            out.append((lo, hi))
+    return out
+
+
 # ====================================================================================== fused update families
 # What a fused flat-bucket update needs to know about one optimizer: the per-parameter state it keeps in flat buffers
 # (``keys``), its device scalars per param group (``scalars``, ``n_scalars`` of them) and its update of one (bucket,
@@ -629,11 +714,15 @@ class _SGDUpdate:
         return (float(g["lr"]),)
 
     @staticmethod
+    def hyper(opt, g):
+        """(momentum, dampening, weight_decay, nesterov) of param group ``g``."""
+        m = 0.0 if opt.momentum_correction else g.get("momentum", 0.0)   # momentum correction: applied before the call
+        return m, g.get("dampening", 0.0), g.get("weight_decay", 0.0), bool(g.get("nesterov", False))
+
+    @staticmethod
     def update(opt, b, g, s, e, fs, first, launch):
-        lr, m, damp, wd, nest = g["lr"], g.get("momentum", 0.0), g.get("dampening", 0.0), \
-            g.get("weight_decay", 0.0), bool(g.get("nesterov", False))
-        if opt.momentum_correction:
-            m = 0.0                                # momentum already applied before communication
+        lr = g["lr"]
+        m, damp, wd, nest = _SGDUpdate.hyper(opt, g)
         if launch is not None:
             launch(ext.require().fused_sgd, m, damp, wd, int(nest), int(first))
             return

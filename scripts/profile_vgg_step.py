@@ -1,16 +1,19 @@
 #!/usr/bin/env python
 """Kernel-by-kernel timeline of one VGG-16 training step (``bench.py``'s flagship configuration), from ``torch.profiler``.
 
-    python scripts/profile_vgg_step.py [--steps 20] [--warmup 20] [--out profiles/vgg_step]
+    python scripts/profile_vgg_step.py [--steps 20] [--warmup 20] [--out profiles/vgg_step] [--no-sgd-ahead]
 
 Builds the workload as ``bench.py`` does (16 images, fp32, Ok-Topk at density 0.001, the preset's untimed dense warm-up,
 whole-step CUDA graphs), replays ``--steps`` threshold-reuse sparse steps under the profiler and splits the trace into
-steps at each ``fused_sgd_kernel``.  It writes ``<out>/vgg_step.md`` and ``.json``:
+steps at each SGD update (``fused_sgd_kernel``, or ``fused_sgd_tail_kernel`` after the early SGD update; ``--no-sgd-ahead``
+turns that off).  It writes ``<out>/vgg_step.md`` and ``.json``:
 
 * every kernel of the median-length step with its grid, block, duration and start offset within the step;
 * per step: the step span, the Ok-Topk call and the *backward tail* -- the time from the end of layer 9's convolution
   backward (the last of layers 9 - 13's weight gradients; the start of layer 8's batch-norm backward) to the start of
   the Ok-Topk call, i.e. how long the bucket's big gradients sit finished while backward runs layers 8 -> 1;
+* per step: the update kernel's and the early SGD update's (``sgd_ahead_kernel``) durations, and the backward span from
+  the start of layer 13's batch-norm backward to the end of layer 1's;
 * the grid sizes of the kernels in that tail.
 """
 from __future__ import annotations
@@ -33,11 +36,11 @@ N_CONV = 13          # VGG-16's convolution + batch-norm layers
 
 
 def split_steps(kernels):
-    """Kernel events sorted by start time -> lists of one step each (a step ends with its fused_sgd_kernel)."""
+    """Kernel events sorted by start time -> lists of one step each (a step ends with its SGD update kernel)."""
     steps, cur = [], []
     for k in kernels:
         cur.append(k)
-        if "fused_sgd_kernel" in k["name"]:
+        if "fused_sgd_kernel" in k["name"] or "fused_sgd_tail_kernel" in k["name"]:
             steps.append(cur)
             cur = []
     return steps
@@ -48,6 +51,12 @@ def analyse(step):
     okt = [k for k in step if "oktopk_fused_kernel" in k["name"]]
     bn_bwd = [k for k in step if "bn_bwd" in k["name"]]
     out = {"span_us": step[-1]["ts"] + step[-1]["dur"] - t0, "kernels": len(step)}
+    out["update_us"] = step[-1]["dur"]
+    ahead = [k for k in step if "sgd_ahead_kernel" in k["name"]]
+    if ahead:
+        out["ahead_us"] = sum(k["dur"] for k in ahead)
+    if bn_bwd:
+        out["backward_us"] = bn_bwd[-1]["ts"] + bn_bwd[-1]["dur"] - bn_bwd[0]["ts"]
     if okt:
         out["oktopk_us"] = okt[0]["dur"]
         out["oktopk_start_us"] = okt[0]["ts"] - t0
@@ -67,6 +76,7 @@ def main(argv=None) -> int:
     p.add_argument("--steps", type=int, default=20)
     p.add_argument("--warmup", type=int, default=20)
     p.add_argument("--out", default=os.path.join("profiles", "vgg_step"))
+    p.add_argument("--no-sgd-ahead", action="store_true", help="OkTopkConfig.sgd_ahead=False")
     a = p.parse_args(argv)
 
     import torch
@@ -79,7 +89,7 @@ def main(argv=None) -> int:
     w = okt.init()
     ext.require()
     dnn, dataset, bs, lr, preset = bench.MODELS["vgg16"]
-    cfg = okt.preset(preset, density=0.001)
+    cfg = okt.preset(preset, density=0.001, sgd_ahead=not a.no_sgd_ahead)
     tr = Trainer(dnn=dnn, dataset=dataset, batch_size=bs, lr=lr, compressor="oktopk", density=0.001,
                  compression=True, cfg=cfg, world=w, seq_len=128, t_total=100000, warmup=0.1, cuda_graph=True)
     tr.adjust_learning_rate = lambda: lr
@@ -125,7 +135,8 @@ def main(argv=None) -> int:
 
     props = torch.cuda.get_device_properties(0)
     summ = {k: statistics.median(i[k] for _, i in reuse if k in i)
-            for k in ("span_us", "oktopk_us", "oktopk_start_us", "tail_start_us", "tail_us", "tail_busy_us")
+            for k in ("span_us", "oktopk_us", "oktopk_start_us", "tail_start_us", "tail_us", "tail_busy_us", "update_us",
+                      "ahead_us", "backward_us")
             if any(k in i for _, i in reuse)}
     summ["steps"] = len(reuse)
     t0 = rep[0]["ts"]
