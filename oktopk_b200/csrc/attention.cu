@@ -62,19 +62,11 @@ constexpr float kAttScale = 0.125f;             // 1 / sqrt(64)
 // from_c:  the A operand of k chunk kc taken from a warp's 16 x 8N fp32 accumulator (P or dS)
 template <typename T> struct AttnMma;
 
-template <> struct AttnMma<float> {             // 3xTF32, m16n8k8
+template <> struct AttnMma<float> {             // 3xTF32, m16n8k8 (elem.cuh)
     static constexpr int kK = 8;
     struct A { uint32_t h[4], l[4]; };
     struct B { uint32_t h[2], l[2]; };
-    static __device__ __forceinline__ uint32_t tf32(float x) {   // round to nearest; the low 13 bits cleared, so
-        uint32_t r;                                              // that x - tf32(x) is the exact remainder
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-        return r & 0xffffe000u;
-    }
-    static __device__ __forceinline__ void split(float x, uint32_t& h, uint32_t& l) {
-        h = tf32(x);
-        l = tf32(x - __uint_as_float(h));
-    }
+    static __device__ __forceinline__ void split(float x, uint32_t& h, uint32_t& l) { tf32_split(x, h, l); }
     // slot order a0 (g, t) a1 (g+8, t) a2 (g, t+4) a3 (g+8, t+4); slot t is column 2t, slot t + 4 column 2t + 1
     static __device__ __forceinline__ A make_a(float g0, float g1, float g8a, float g8b) {
         A a;
@@ -109,21 +101,10 @@ template <> struct AttnMma<float> {             // 3xTF32, m16n8k8
     static __device__ __forceinline__ A from_c(const float (&c)[N][4], int kc) {
         return make_a(c[kc][0], c[kc][1], c[kc][2], c[kc][3]);
     }
-    static __device__ __forceinline__ void mma1(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-        asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-    }
-    // The tensor cores truncate as they accumulate.  Chained through one accumulator over a 64-long sum that bias adds
-    // up (24 truncations, ~1e-5 relative at S = 512); so each k8 step sums into a fresh zero accumulator and is added
-    // to d with a rounded fp32 add.
+    // Chained through one accumulator, a 64-long sum's truncations bias it (24 of them, ~1e-5 relative at S = 512);
+    // the elem.cuh product adds each k8 step to d with a rounded fp32 add instead.
     static __device__ __forceinline__ void mma(float (&d)[4], const A& a, const B& b) {
-        float t[4] = {0.f, 0.f, 0.f, 0.f};
-        mma1(t, a.l, b.h);                      // the small terms first
-        mma1(t, a.h, b.l);
-        mma1(t, a.h, b.h);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) d[i] += t[i];
+        mma_m16n8k8_3xtf32(d, a.h, a.l, b.h, b.l);
     }
 };
 

@@ -739,30 +739,30 @@ static void lstm_backward(uint64_t dy, uint64_t gates, uint64_t cs, uint64_t whh
                             H, u, rows, S_(stream), dt),
        "lstm_backward");
 }
-// One layer of a stacked LSTM from an initial state (csrc/lstm.cu lstm_seq_*), bf16 / fp16 only: gx [T, N, 4H], whh
-// [4H, H], y [T, N, H], h0 [N, H] of type dtype; c0 [N, H], gates, cs fp32; bar one zeroed int64.  Backward: dy
-// [T, N, H] and dhn [N, H] (or 0) of type dtype, dcn [N, H] fp32 (or 0); writes dg [T, N, 4H] (dtype) and dc0 [N, H]
-// (fp32).
+// One layer of a stacked LSTM from an initial state (csrc/lstm.cu lstm_seq_*): gx [T, N, 4H], whh [4H, H], y [T, N, H],
+// h0 [N, H] of type dtype; c0 [N, H], gates, cs fp32; bar one zeroed int64.  Backward: dy [T, N, H] and dhn [N, H] (or
+// 0) of type dtype, dcn [N, H] fp32 (or 0); writes dg [T, N, 4H] (dtype) and dc0 [N, H] (fp32).  fp32 takes the split
+// of ops/fused_lstm.lstm_seq_f32_geometry: r_on weight rows on chip, kc-column chunks; its backward whh is W_hh^T
+// [H, 4H] and every operand read in vectors (whh, h0, y, dg) is 16-byte aligned.
 static void lstm_seq_forward(uint64_t gx, uint64_t whh, uint64_t h0, uint64_t c0, uint64_t y, uint64_t gates,
                              uint64_t cs, uint64_t bar, int T, int N, int H, int u, int rows, uint64_t stream,
-                             int dtype) {
+                             int dtype, int r_on, int kc) {
     const Dtype dt = dtype_arg(dtype, "lstm_seq_forward");
-    if (dt == Dtype::kF32) throw std::runtime_error("lstm_seq_forward: bf16 or fp16 only");
     lstm_check("lstm_seq_forward", T, N, H, u, rows, dt, {gx, whh, h0, c0, y, gates, cs, bar}, {whh, h0, y}, bar);
     ck(launch_lstm_seq_forward(P_<const void>(gx), P_<const void>(whh), P_<const void>(h0), P_<const float>(c0),
                                P_<void>(y), P_<float>(gates), P_<float>(cs), P_<unsigned long long>(bar), T, N, H, u,
-                               rows, S_(stream), dt),
+                               rows, r_on, kc, S_(stream), dt),
        "lstm_seq_forward");
 }
 static void lstm_seq_backward(uint64_t dy, uint64_t gates, uint64_t cs, uint64_t whh, uint64_t c0, uint64_t dhn,
                               uint64_t dcn, uint64_t dg, uint64_t dc0, uint64_t bar, int T, int N, int H, int u, int rows,
-                              uint64_t stream, int dtype) {
+                              uint64_t stream, int dtype, int r_on, int kc) {
     const Dtype dt = dtype_arg(dtype, "lstm_seq_backward");
-    if (dt == Dtype::kF32) throw std::runtime_error("lstm_seq_backward: bf16 or fp16 only");
-    lstm_check("lstm_seq_backward", T, N, H, u, rows, dt, {dy, gates, cs, whh, c0, dg, dc0, bar}, {dg}, bar);
+    lstm_check("lstm_seq_backward", T, N, H, u, rows, dt, {dy, gates, cs, whh, c0, dg, dc0, bar},
+               dt == Dtype::kF32 ? std::initializer_list<uint64_t>{whh, dg} : std::initializer_list<uint64_t>{dg}, bar);
     ck(launch_lstm_seq_backward(P_<const void>(dy), P_<const float>(gates), P_<const float>(cs), P_<const void>(whh),
                                 P_<const float>(c0), P_<const void>(dhn), P_<const float>(dcn), P_<void>(dg),
-                                P_<float>(dc0), P_<unsigned long long>(bar), T, N, H, u, rows, S_(stream), dt),
+                                P_<float>(dc0), P_<unsigned long long>(bar), T, N, H, u, rows, r_on, kc, S_(stream), dt),
        "lstm_seq_backward");
 }
 static void maxpool2_fwd(uint64_t x, uint64_t y, uint64_t arg, int N, int H, int W, int C, uint64_t stream) {
@@ -933,10 +933,11 @@ PYBIND11_MODULE(_C, m) {
           py::arg("stream"), py::arg("dtype") = 0, py::arg("whh_rev") = 0);
     m.def("lstm_seq_forward", &lstm_seq_forward, py::arg("gx"), py::arg("whh"), py::arg("h0"), py::arg("c0"),
           py::arg("y"), py::arg("gates"), py::arg("cs"), py::arg("bar"), py::arg("T"), py::arg("N"), py::arg("H"),
-          py::arg("u"), py::arg("rows"), py::arg("stream"), py::arg("dtype"));
+          py::arg("u"), py::arg("rows"), py::arg("stream"), py::arg("dtype"), py::arg("r_on") = 0, py::arg("kc") = 0);
     m.def("lstm_seq_backward", &lstm_seq_backward, py::arg("dy"), py::arg("gates"), py::arg("cs"), py::arg("whh"),
           py::arg("c0"), py::arg("dhn"), py::arg("dcn"), py::arg("dg"), py::arg("dc0"), py::arg("bar"), py::arg("T"),
-          py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"), py::arg("stream"), py::arg("dtype"));
+          py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"), py::arg("stream"), py::arg("dtype"),
+          py::arg("r_on") = 0, py::arg("kc") = 0);
     m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;

@@ -121,6 +121,41 @@ template <> __device__ __forceinline__ void mma_m16n8k16<__half>(float (&d)[4], 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
+// 3xTF32 for fp32 products on the tensor cores (attention, the stacked-layer LSTM): each operand is split into a TF32
+// high part and a TF32 remainder, and a.b ~ ah.bh + ah.bl + al.bh, which keeps about fp32 accuracy (the dropped al.bl
+// is below 2^-22 relative) at three tensor-core products.
+//
+// tf32(x): x rounded to nearest, the low 13 bits cleared, so that x - tf32(x) is the exact remainder.
+__device__ __forceinline__ uint32_t tf32_hi(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r & 0xffffe000u;
+}
+__device__ __forceinline__ void tf32_split(float x, uint32_t& h, uint32_t& l) {
+    h = tf32_hi(x);
+    l = tf32_hi(x - __uint_as_float(h));
+}
+
+// d += a b, mma.sync m16n8k8 (row.col) in TF32 with fp32 accumulation; fragments in the PTX ISA's register layout:
+// a0 (g, t), a1 (g + 8, t), a2 (g, t + 4), a3 (g + 8, t + 4); b0 (k = t, n = g), b1 (k = t + 4, n = g).
+__device__ __forceinline__ void mma_m16n8k8_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// d += (ah + al)(bh + bl) in 3xTF32 over one k8 step.  The tensor cores truncate as they accumulate, so the three
+// products go into a fresh zero accumulator, the small terms first, and that is added to d with a rounded fp32 add.
+__device__ __forceinline__ void mma_m16n8k8_3xtf32(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                                   const uint32_t (&bh)[2], const uint32_t (&bl)[2]) {
+    float t[4] = {0.f, 0.f, 0.f, 0.f};
+    mma_m16n8k8_tf32(t, al, bh);
+    mma_m16n8k8_tf32(t, ah, bl);
+    mma_m16n8k8_tf32(t, ah, bh);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) d[i] += t[i];
+}
+
 // f(T{}) with T the storage type of `dtype`: a launcher calls its templated body through it once, whatever the type.
 template <class F>
 cudaError_t with_dtype(Dtype dtype, F&& f) {

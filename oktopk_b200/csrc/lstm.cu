@@ -53,6 +53,7 @@ namespace okt {
 constexpr int kLstmThreads = 512;                // ops/fused_lstm.py LSTM_THREADS
 constexpr int kLstmWarps = kLstmThreads / 32;
 constexpr int kLstmNB = 4;                       // batch rows of one warp task in lstm_dots
+constexpr int kMaxLstmBatch = 64;                // ops/fused_lstm.py MAX_BATCH: the fp32 stacked-layer step's M tiles
 
 // whh[1] is null for a one-direction layer; g = ceil(H / u) CTAs per direction.
 template <typename S>
@@ -376,7 +377,8 @@ cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float
 // ---- One layer of a stacked language-model LSTM (PTB): carried state, step product on the tensor cores ----------------
 //
 // lstm_seq_fwd_kernel / lstm_seq_bwd_kernel run the recurrence above for a single uni-directional layer in which every
-// row has length T, from an initial state (h0, c0), in bf16 or fp16 only.  The split into CTAs of u units, the grid
+// row has length T, from an initial state (h0, c0), in bf16 or fp16 (below) and in fp32 (the fp32 section further down:
+// same kernels, another prologue and step product).  The split into CTAs of u units, the grid
 // barrier, the cell code and the stores are those of lstm_fwd_kernel / lstm_bwd_kernel; what differs:
 //   - forward, step 0 stages h0 where the other steps stage y_{t-1}, and c starts from c0.  h_n = y[T-1] and
 //     c_n = cs[T-1], so neither has a store of its own;
@@ -404,6 +406,7 @@ struct LstmSeqFwdArgs {
     float* cs;
     unsigned long long* bar;
     int T, N, H, u, rows, ksplit;
+    int r_on, kc;                   // fp32 only: weight rows in shared memory, staged chunk width (lstm_f32_product)
 };
 
 template <typename S>
@@ -419,6 +422,7 @@ struct LstmSeqBwdArgs {
     float* dc0;
     unsigned long long* bar;
     int T, N, H, u, rows, ksplit;
+    int r_on, kc;                   // fp32 only, as LstmSeqFwdArgs
 };
 
 __host__ __device__ __forceinline__ int lstm_seq_ld(int K) { return ((K + 15) & ~15) + 8; }
@@ -513,35 +517,199 @@ __device__ __forceinline__ void lstm_seq_zero_tail(S* s, int nrows, int K) {
     }
 }
 
+// ---- fp32: W_hh split between shared memory and L2, 3xTF32 step product ---------------------------------------------
+//
+// The fp32 slice of W_hh at H = 1500 (288 KB per CTA at u = 12) does not fit in shared memory, but all of W_hh (36 MB)
+// fits in L2.  So the CTA keeps its first r_on weight rows in shared memory, loaded once, and reads the others from
+// global memory at every step with an L2 evict_last policy; nothing else runs during the launch to evict them.  The
+// step operand (all N batch rows) is staged kc columns at a time, double-buffered with cp.async, which leaves most of
+// shared memory to the weights.  The product runs in 3xTF32 on mma.sync m16n8k8 (elem.cuh), batch rows on the M side,
+// weight rows on the n side.  Rows of W in shared memory lie lstm_f32_ld(K) floats apart and staged rows kc + 4 apart,
+// both = 4 (mod 8): the eight rows a fragment load touches (g = 0..7, column t) then fall in distinct banks.
+// Backward, the weight rows are the CTA's u columns of W_hh, which the fp32 launch reads as rows of W_hh^T [H][4H], so
+// that a streamed row is contiguous.  lstm_f32_ld and lstm_f32_ksplit are mirrored by ops/fused_lstm.py.
+
+__host__ __device__ __forceinline__ int lstm_f32_ld(int K) { return ((K + 7) & ~7) + 4; }
+
+// One task per warp: 8 weight rows and 1 / ksplit of each chunk's k8 steps, for every batch row.
+__host__ __device__ __forceinline__ int lstm_f32_ksplit(int R) { return max(1, kLstmWarps / ((R + 7) >> 3)); }
+
+__device__ __forceinline__ void lstm_cp_async16(void* dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src)
+                 : "memory");
+}
+__device__ __forceinline__ void lstm_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void lstm_cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+__device__ __forceinline__ uint64_t lstm_evict_last_policy() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+// A weight, read-only for the whole launch: through the non-coherent path, kept in L2.
+__device__ __forceinline__ float lstm_ldg_last(const float* p, uint64_t pol) {
+    float v;
+    asm("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+    return v;
+}
+
+// Zero columns [K, ld) of `nrows` fp32 shared-memory rows `ld` apart.
+__device__ __forceinline__ void lstm_f32_zero_tail(float* s, int nrows, int K, int ld) {
+    const int w = ld - K;
+    for (int i = threadIdx.x; i < nrows * w; i += kLstmThreads) {
+        const int r = i / w;
+        s[(size_t)r * ld + K + (i - r * w)] = 0.f;
+    }
+}
+
+// out[r N + n] = sum_k W_r[k] V[n K + k] for r < R and n < N; V is global [N, K], possibly written in this launch.
+// W_r is row r of sW (lstm_f32_ld(K) apart, zero from K on) for r < r_on, else the global row grow(r) (null: a zero
+// row).  V goes through sV [2][N][kc + 4] one kc-column chunk at a time, the next chunk's cp.async under this one's
+// products; zero columns pad the last chunk to a whole k8 step.  Warp w < NT ksplit (NT = ceil(R / 8)) takes weight
+// rows [8 nt, 8 nt + 8), nt = w / ksplit, and the (w % ksplit)-th part of every chunk's k8 steps, for all batch rows
+// (16 per M tile, rows past N zero fragments): so each streamed weight element is loaded once per step.  Its sums stay
+// in registers across the chunks, go to sP [ksplit][N][R] at the end, and are added in split order: fixed whichever warp
+// runs what, and no atomics.
+template <class RowPtr>
+__device__ __forceinline__ void lstm_f32_product(const float* __restrict__ sW, float* __restrict__ sV,
+                                                 float* __restrict__ sP, float* __restrict__ out, const float* V, int R,
+                                                 int r_on, int K, int N, int kc, int ksplit, RowPtr grow,
+                                                 uint64_t pol) {
+    constexpr int kMT = (kMaxLstmBatch + 15) / 16, kPf = 8;        // M tiles at most; k8 steps of weights in flight
+    const int lane = lane_id(), warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    const int ldw = lstm_f32_ld(K), ldv = kc + 4, K4 = K >> 2, nch = (K + kc - 1) / kc, MT = (N + 15) >> 4;
+    const int nt = warp / ksplit, ks = warp - nt * ksplit, r = nt * 8 + g;
+    const bool active = r - g < R, on = r < r_on;
+    const float* wg = active && !on && r < R ? grow(r) : nullptr;
+    const float* ws = sW + (size_t)(on ? r : 0) * ldw;
+    float acc[kMT][4];
+#pragma unroll
+    for (int m = 0; m < kMT; ++m) acc[m][0] = acc[m][1] = acc[m][2] = acc[m][3] = 0.f;
+    auto stage = [&](int c) {
+        float* d = sV + (size_t)(c & 1) * N * ldv;
+        const int k0 = c * kc, w4 = min(kc >> 2, K4 - (k0 >> 2)), pad = ((4 * w4 + 7) & ~7) - 4 * w4;
+        for (int i = threadIdx.x; i < N * w4; i += kLstmThreads) {
+            const int n = i / w4, k = i - n * w4;
+            lstm_cp_async16(d + (size_t)n * ldv + 4 * k, V + (size_t)n * K + k0 + 4 * k);
+        }
+        lstm_cp_async_commit();
+        for (int i = threadIdx.x; i < N * pad; i += kLstmThreads) d[(size_t)(i / pad) * ldv + 4 * w4 + i % pad] = 0.f;
+    };
+    stage(0);
+    for (int c = 0; c < nch; ++c) {
+        lstm_cp_async_wait_all();
+        __syncthreads();                // chunk c landed, and every warp is done with chunk c - 1's buffer
+        if (c + 1 < nch) stage(c + 1);
+        if (!active) continue;
+        const float* v = sV + (size_t)(c & 1) * N * ldv;
+        const int k0 = c * kc, S = (min(kc, K - k0) + 7) >> 3;
+        const int s_hi = (ks + 1) * S / ksplit;
+        for (int s0 = ks * S / ksplit; s0 < s_hi; s0 += kPf) {
+            float b[kPf][2];
+#pragma unroll
+            for (int i = 0; i < kPf; ++i) {             // fragment b0 (k = t), b1 (k = t + 4) of weight row r
+                const int k = k0 + 8 * (s0 + i) + t;
+                const bool in = s0 + i < s_hi;
+                if (on) {
+                    b[i][0] = in ? ws[k] : 0.f;
+                    b[i][1] = in ? ws[k + 4] : 0.f;
+                } else {
+                    b[i][0] = wg && in && k < K ? lstm_ldg_last(wg + k, pol) : 0.f;
+                    b[i][1] = wg && in && k + 4 < K ? lstm_ldg_last(wg + k + 4, pol) : 0.f;
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < kPf; ++i) {
+                if (s0 + i >= s_hi) break;
+                uint32_t bh[2], bl[2];
+                tf32_split(b[i][0], bh[0], bl[0]);
+                tf32_split(b[i][1], bh[1], bl[1]);
+                const int kl = 8 * (s0 + i) + t;
+#pragma unroll
+                for (int m = 0; m < kMT; ++m) {
+                    if (m >= MT) break;
+                    const int j0 = 16 * m + g, j1 = j0 + 8;
+                    const float* v0 = v + (size_t)(j0 < N ? j0 : 0) * ldv + kl;
+                    const float* v1 = v + (size_t)(j1 < N ? j1 : 0) * ldv + kl;
+                    const float a[4] = {j0 < N ? v0[0] : 0.f, j1 < N ? v1[0] : 0.f, j0 < N ? v0[4] : 0.f,
+                                        j1 < N ? v1[4] : 0.f};
+                    uint32_t ah[4], al[4];
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) tf32_split(a[q], ah[q], al[q]);
+                    mma_m16n8k8_3xtf32(acc[m], ah, al, bh, bl);
+                }
+            }
+        }
+    }
+    if (active) {
+        float* P = sP + (size_t)ks * N * R;
+        const int rc = nt * 8 + 2 * t;                              // C fragment: rows g, g + 8; columns 2t, 2t + 1
+#pragma unroll
+        for (int m = 0; m < kMT; ++m) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int j = 16 * m + g + 8 * h;
+                if (j >= N) continue;
+                if (rc < R) P[j * R + rc] = acc[m][2 * h];
+                if (rc + 1 < R) P[j * R + rc + 1] = acc[m][2 * h + 1];
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < R * N; i += kLstmThreads) {
+        const int rr = i / N, n = i - rr * N;
+        float a = sP[n * R + rr];
+        for (int k = 1; k < ksplit; ++k) a += sP[((size_t)k * N + n) * R + rr];
+        out[i] = a;
+    }
+    __syncthreads();
+}
+
 // Shared memory: W [4u][ld] and h_{t-1} rows [rows][ld] of S, ld = lstm_seq_ld(H) | partial sums [ksplit][rows][4u],
 // gate sums [4u][N] and c [u][N] of float.  ld % 8 == 0 keeps every section 16-byte aligned.
+// fp32: W [r_on][lstm_f32_ld(H)] | two h_{t-1} chunks [2][N][kc + 4] | partial sums [ksplit][N][4u] | gate sums, c.
 template <typename S>
 __global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_fwd_kernel(const LstmSeqFwdArgs<S> p) {
     using El = Elem<S>;
     using Vec = typename El::V;
+    constexpr bool kF32 = std::is_same<S, float>::value;
     extern __shared__ float4 lstm_smem[];
-    const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2, ld = lstm_seq_ld(H);
+    const int H = p.H, N = p.N, u = p.u, R = 4 * u, H4 = H >> 2;
+    const int ld = kF32 ? lstm_f32_ld(H) : lstm_seq_ld(H), won = kF32 ? p.r_on : R;    // rows of W in shared memory
     const int u0 = blockIdx.x * u, nu = min(u, H - u0);
     S* sW = reinterpret_cast<S*>(lstm_smem);
-    S* sV = sW + (size_t)R * ld;
-    float* sP = reinterpret_cast<float*>(sV + (size_t)p.rows * ld);
-    float* sG = sP + (size_t)p.ksplit * p.rows * R;
+    S* sV = sW + (size_t)won * ld;
+    float* sP = reinterpret_cast<float*>(sV + (kF32 ? (size_t)2 * N * (p.kc + 4) : (size_t)p.rows * ld));
+    float* sG = sP + (size_t)p.ksplit * (kF32 ? N : p.rows) * R;
     float* sC = sG + R * N;
-    for (int i = threadIdx.x; i < R * H4; i += kLstmThreads) {      // local row q u + j = W_hh row q H + u0 + j
+    for (int i = threadIdx.x; i < won * H4; i += kLstmThreads) {    // local row q u + j = W_hh row q H + u0 + j
         const int lr = i / H4, k = i - lr * H4, q = lr / u, j = lr - q * u;
         Vec v = El::zero();
         if (j < nu) v = __ldg(reinterpret_cast<const Vec*>(p.whh + (size_t)(q * H + u0 + j) * H) + k);
         reinterpret_cast<Vec*>(sW + (size_t)lr * ld)[k] = v;
     }
-    lstm_seq_zero_tail(sW, R, H);
-    lstm_seq_zero_tail(sV, p.rows, H);
+    uint64_t pol = 0;
+    if constexpr (kF32) {
+        lstm_f32_zero_tail(sW, won, H, ld);
+        pol = lstm_evict_last_policy();
+    } else {
+        lstm_seq_zero_tail(sW, R, H);
+        lstm_seq_zero_tail(sV, p.rows, H);
+    }
+    auto grow = [&](int lr) -> const float* {                       // fp32: streamed local row lr, as above
+        const int q = lr / u, j = lr - q * u;
+        return j < nu ? reinterpret_cast<const float*>(p.whh) + (size_t)(q * H + u0 + j) * H : nullptr;
+    };
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) {
         const int j = i / N, n = i - j * N;
         sC[i] = j < nu ? __ldg(p.c0 + (size_t)n * H + u0 + j) : 0.f;
     }
     for (int s = 0; s < p.T; ++s) {
         const S* hp = s == 0 ? p.h0 : p.y + (size_t)(s - 1) * N * H;
-        lstm_seq_product(sW, sV, sP, sG, hp, R, H, N, p.rows, p.ksplit);
+        if constexpr (kF32)
+            lstm_f32_product(sW, sV, sP, sG, hp, R, won, H, N, p.kc, p.ksplit, grow, pol);
+        else
+            lstm_seq_product(sW, sV, sP, sG, hp, R, H, N, p.rows, p.ksplit);
         for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
             const int j = i / N, n = i - j * N, unit = u0 + j;
             const size_t row = (size_t)s * N + n;
@@ -567,20 +735,37 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_fwd_kernel(const Lst
 template <typename S>
 __global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_bwd_kernel(const LstmSeqBwdArgs<S> p) {
     using El = Elem<S>;
+    constexpr bool kF32 = std::is_same<S, float>::value;
     extern __shared__ float4 lstm_smem[];
-    const int H = p.H, N = p.N, u = p.u, G = 4 * H, ld = lstm_seq_ld(G);
+    const int H = p.H, N = p.N, u = p.u, G = 4 * H;
+    const int ld = kF32 ? lstm_f32_ld(G) : lstm_seq_ld(G), won = kF32 ? p.r_on : u;     // rows of W^T in shared memory
     const int u0 = blockIdx.x * u, nu = min(u, H - u0);
     S* sW = reinterpret_cast<S*>(lstm_smem);
-    S* sV = sW + (size_t)u * ld;
-    float* sP = reinterpret_cast<float*>(sV + (size_t)p.rows * ld);
-    float* sD = sP + (size_t)p.ksplit * p.rows * u;
+    S* sV = sW + (size_t)won * ld;
+    float* sP = reinterpret_cast<float*>(sV + (kF32 ? (size_t)2 * N * (p.kc + 4) : (size_t)p.rows * ld));
+    float* sD = sP + (size_t)p.ksplit * (kF32 ? N : p.rows) * u;
     float* sDC = sD + u * N;
-    for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {       // sW[j][k] = W_hh[k][u0 + j]
-        const int k = i / u, j = i - k * u;
-        sW[(size_t)j * ld + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : El::narrow1(0.f);
+    uint64_t pol = 0;
+    if constexpr (kF32) {                                           // whh is W_hh^T: sW[j][k] = W_hh^T[u0 + j][k]
+        const int G4 = G >> 2;
+        for (int i = threadIdx.x; i < won * G4; i += kLstmThreads) {
+            const int j = i / G4, k = i - j * G4;
+            reinterpret_cast<float4*>(sW + (size_t)j * ld)[k] =
+                j < nu ? __ldg(reinterpret_cast<const float4*>(p.whh + (size_t)(u0 + j) * G) + k) : El::zero();
+        }
+        lstm_f32_zero_tail(sW, won, G, ld);
+        pol = lstm_evict_last_policy();
+    } else {
+        for (int i = threadIdx.x; i < u * G; i += kLstmThreads) {   // sW[j][k] = W_hh[k][u0 + j]
+            const int k = i / u, j = i - k * u;
+            sW[(size_t)j * ld + k] = j < nu ? __ldg(p.whh + (size_t)k * H + u0 + j) : El::narrow1(0.f);
+        }
+        lstm_seq_zero_tail(sW, u, G);
+        lstm_seq_zero_tail(sV, p.rows, G);
     }
-    lstm_seq_zero_tail(sW, u, G);
-    lstm_seq_zero_tail(sV, p.rows, G);
+    auto grow = [&](int j) -> const float* {                        // fp32: streamed row j of W_hh^T's slice
+        return j < nu ? reinterpret_cast<const float*>(p.whh) + (size_t)(u0 + j) * G : nullptr;
+    };
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) {
         const int j = i / N, n = i - j * N;
         const size_t o = (size_t)n * H + u0 + j;
@@ -589,7 +774,13 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_seq_bwd_kernel(const Lst
     }
     __syncthreads();
     for (int s = p.T - 1; s >= 0; --s) {
-        if (s < p.T - 1) lstm_seq_product(sW, sV, sP, sD, p.dg + (size_t)(s + 1) * N * G, u, G, N, p.rows, p.ksplit);
+        if (s < p.T - 1) {
+            const S* dgn = p.dg + (size_t)(s + 1) * N * G;
+            if constexpr (kF32)
+                lstm_f32_product(sW, sV, sP, sD, dgn, u, won, G, N, p.kc, p.ksplit, grow, pol);
+            else
+                lstm_seq_product(sW, sV, sP, sD, dgn, u, G, N, p.rows, p.ksplit);
+        }
         for (int i = threadIdx.x; i < nu * N; i += kLstmThreads) {
             const int j = i / N, n = i - j * N, unit = u0 + j;
             const size_t row = (size_t)s * N + n;
@@ -623,42 +814,53 @@ static size_t lstm_seq_bwd_smem(int H, int N, int u, int rows, int elem) {
            sizeof(float) * ((size_t)lstm_seq_ksplit(rows, u, 4 * H) * rows * u + (size_t)2 * u * N);
 }
 
-// The tensor-core step has no fp32 form: fp32 is an invalid dtype here.
-template <class F>
-static cudaError_t with_dtype16(Dtype dtype, F&& f) {
-    switch (dtype) {
-        case Dtype::kBF16: return f(__nv_bfloat16{});
-        case Dtype::kF16: return f(__half{});
-        default: return cudaErrorInvalidValue;
-    }
+// fp32: r_on weight rows in shared memory, two staged chunks of kc columns of the N batch rows.
+static size_t lstm_f32_fwd_smem(int H, int N, int u, int r_on, int kc) {
+    const int R = 4 * u;
+    return sizeof(float) * ((size_t)r_on * lstm_f32_ld(H) + (size_t)2 * N * (kc + 4) +
+                            (size_t)lstm_f32_ksplit(R) * N * R + (size_t)R * N + (size_t)u * N);
+}
+
+static size_t lstm_f32_bwd_smem(int H, int N, int u, int r_on, int kc) {
+    return sizeof(float) * ((size_t)r_on * lstm_f32_ld(4 * H) + (size_t)2 * N * (kc + 4) +
+                            (size_t)lstm_f32_ksplit(u) * N * u + (size_t)2 * u * N);
+}
+
+// The fp32 split: R weight rows per CTA, at most 8 per warp; r_on of them on chip; chunks of whole k8 steps.
+static bool lstm_f32_ok(int N, int R, int r_on, int kc) {
+    return N <= kMaxLstmBatch && R <= 8 * kLstmWarps && r_on >= 0 && r_on <= R && kc > 0 && kc % 8 == 0;
 }
 
 cudaError_t launch_lstm_seq_forward(const void* gx, const void* whh, const void* h0, const float* c0, void* y,
                                     float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u,
-                                    int rows, cudaStream_t stream, Dtype dtype) {
+                                    int rows, int r_on, int kc, cudaStream_t stream, Dtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    return with_dtype16(dtype, [&](auto e) {
+    if (dtype == Dtype::kF32 && !lstm_f32_ok(N, 4 * u, r_on, kc)) return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
         using S = decltype(e);
+        constexpr bool kF32 = std::is_same<S, float>::value;
         const LstmSeqFwdArgs<S> p{static_cast<const S*>(gx), static_cast<const S*>(whh), static_cast<const S*>(h0), c0,
                                   static_cast<S*>(y), gates, cs, bar, T, N, H, u, rows,
-                                  lstm_seq_ksplit(rows, 4 * u, H)};
-        return lstm_launch(lstm_seq_fwd_kernel<S>, p, (H + u - 1) / u, lstm_seq_fwd_smem(H, N, u, rows, sizeof(S)),
-                           stream);
+                                  kF32 ? lstm_f32_ksplit(4 * u) : lstm_seq_ksplit(rows, 4 * u, H), r_on, kc};
+        const size_t smem = kF32 ? lstm_f32_fwd_smem(H, N, u, r_on, kc) : lstm_seq_fwd_smem(H, N, u, rows, sizeof(S));
+        return lstm_launch(lstm_seq_fwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
     });
 }
 
 cudaError_t launch_lstm_seq_backward(const void* dy, const float* gates, const float* cs, const void* whh,
                                      const float* c0, const void* dhn, const float* dcn, void* dg, float* dc0,
-                                     unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
-                                     Dtype dtype) {
+                                     unsigned long long* bar, int T, int N, int H, int u, int rows, int r_on, int kc,
+                                     cudaStream_t stream, Dtype dtype) {
     if (!lstm_shape_ok(T, N, H, u, rows)) return cudaErrorInvalidValue;
-    return with_dtype16(dtype, [&](auto e) {
+    if (dtype == Dtype::kF32 && !lstm_f32_ok(N, u, r_on, kc)) return cudaErrorInvalidValue;
+    return with_dtype(dtype, [&](auto e) {
         using S = decltype(e);
+        constexpr bool kF32 = std::is_same<S, float>::value;
         const LstmSeqBwdArgs<S> p{static_cast<const S*>(dy), gates, cs, static_cast<const S*>(whh), c0,
                                   static_cast<const S*>(dhn), dcn, static_cast<S*>(dg), dc0, bar, T, N, H, u, rows,
-                                  lstm_seq_ksplit(rows, u, 4 * H)};
-        return lstm_launch(lstm_seq_bwd_kernel<S>, p, (H + u - 1) / u, lstm_seq_bwd_smem(H, N, u, rows, sizeof(S)),
-                           stream);
+                                  kF32 ? lstm_f32_ksplit(u) : lstm_seq_ksplit(rows, u, 4 * H), r_on, kc};
+        const size_t smem = kF32 ? lstm_f32_bwd_smem(H, N, u, r_on, kc) : lstm_seq_bwd_smem(H, N, u, rows, sizeof(S));
+        return lstm_launch(lstm_seq_bwd_kernel<S>, p, (H + u - 1) / u, smem, stream);
     });
 }
 

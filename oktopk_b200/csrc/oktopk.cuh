@@ -438,16 +438,20 @@ cudaError_t launch_lstm_forward(const void* gx, const void* whh, const void* whh
 cudaError_t launch_lstm_backward(const void* dy, const float* gates, const float* cs, const void* whh,
                                  const void* whh_rev, const int* len, void* dg, unsigned long long* bar, int T, int N,
                                  int H, int u, int rows, cudaStream_t stream, Dtype dtype);
-// one layer of a stacked LSTM from an initial state, every row of length T, bf16 / fp16 only (fp32 is invalid), the
-// step product on the tensor cores (csrc/lstm.cu).  gx, whh, y, dy, dg as above; h0 and dhn [N, H] of type `dtype`, c0,
-// dcn and dc0 [N, H] fp32; dhn and dcn may be null (zero).  whh, h0, y and dg 8-byte aligned, H % 4 == 0.
+// one layer of a stacked LSTM from an initial state, every row of length T, the step product on the tensor cores
+// (csrc/lstm.cu).  gx, whh, y, dy, dg as above; h0 and dhn [N, H] of type `dtype`, c0, dcn and dc0 [N, H] fp32; dhn and
+// dcn may be null (zero).  whh, h0, y and dg aligned to four elements, H % 4 == 0.  bf16 / fp16 stage `rows` batch rows
+// at a time and keep all of the CTA's W_hh slice on chip (r_on and kc are ignored).  fp32 (N <= 64): the CTA keeps its
+// first r_on weight rows on chip (forward: of its 4u gate rows, at most 128; backward: of its u columns) and streams
+// the rest from L2 every step, staging all N rows kc columns at a time (kc % 8 == 0); `rows` is only checked; the
+// backward pass's whh is W_hh^T [H, 4H].
 cudaError_t launch_lstm_seq_forward(const void* gx, const void* whh, const void* h0, const float* c0, void* y,
                                     float* gates, float* cs, unsigned long long* bar, int T, int N, int H, int u,
-                                    int rows, cudaStream_t stream, Dtype dtype);
+                                    int rows, int r_on, int kc, cudaStream_t stream, Dtype dtype);
 cudaError_t launch_lstm_seq_backward(const void* dy, const float* gates, const float* cs, const void* whh,
                                      const float* c0, const void* dhn, const float* dcn, void* dg, float* dc0,
-                                     unsigned long long* bar, int T, int N, int H, int u, int rows, cudaStream_t stream,
-                                     Dtype dtype);
+                                     unsigned long long* bar, int T, int N, int H, int u, int rows, int r_on, int kc,
+                                     cudaStream_t stream, Dtype dtype);
 // fused self-attention, head dim 64 (csrc/attention.cu): qkv and dqkv [B, S, 3 H 64], out and dout [B, S, H 64], all of
 // type `dtype` (a Dtype), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
 // fp32 (lse written by the forward pass, delta scratch of the backward pass).  keep_thr >= 2^32 turns the dropout off

@@ -28,7 +28,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ``lstman4``,
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
     ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``); for ``lstm`` (PTB),
-    ``fuse_lstm=True`` turns on ``net.fuse_lstm`` and ``fuse_xent=True`` ``net.fuse_xent``."""
+    ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_fp32=True`` ``net.fuse_lstm_fp32`` and ``fuse_xent=True``
+    ``net.fuse_xent``."""
     ext = None
     d = dnn.lower()
     if d.startswith("vgg"):
@@ -57,7 +58,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
         ext = {"labels": AN4_LABELS}
     elif d == "lstm":
         net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20),
-                      fuse_lstm=bool(kwargs.get("fuse_lstm", False)), fuse_xent=bool(kwargs.get("fuse_xent", False)))
+                      fuse_lstm=bool(kwargs.get("fuse_lstm", False)), fuse_xent=bool(kwargs.get("fuse_xent", False)),
+                      fuse_lstm_fp32=bool(kwargs.get("fuse_lstm_fp32", False)))
     elif d in ("bert", "bert_base"):
         cfg = kwargs.get("config")
         if isinstance(cfg, str):

@@ -201,14 +201,17 @@ class PTBLSTM(nn.Module):
 
     ``fuse_lstm=True`` (or ``net.fuse_lstm = True`` at any time) runs the stacked ``nn.LSTM`` through
     ``ops/fused_lstm.lstm_stack``: under bf16 / fp16 CUDA autocast, on the 16-bit stacked-layer kernels with the carried
-    state in and out; anywhere else (fp32 included: H = 1500 has no fp32 kernel) exactly the stock layer.  The returned
-    c_n is then fp32.  ``fuse_xent=True`` (``net.fuse_xent``) asks the trainer to compute the loss with the fused softmax
+    state in and out; anywhere else exactly the stock layer, unless ``fuse_lstm_fp32=True`` (``net.fuse_lstm_fp32``) is
+    set as well, which runs fp32 on CUDA on the fp32 forms of the kernels (W_hh partly streamed from L2, the step in
+    3xTF32).  The returned c_n is fp32 either way.  ``fuse_lstm_fp32`` alone is the stock layer.  ``fuse_xent=True`` (``net.fuse_xent``) asks the trainer to compute the loss with the fused softmax
     cross-entropy (``ops/fused_xent``).  Parameters, buffers and ``state_dict`` keys are the same either way."""
 
     def __init__(self, vocab_size: int = 10000, embedding_dim: int = 1500, num_steps: int = 35, batch_size: int = 20,
-                 num_layers: int = 2, dp_keep_prob: float = 0.35, fuse_lstm: bool = False, fuse_xent: bool = False):
+                 num_layers: int = 2, dp_keep_prob: float = 0.35, fuse_lstm: bool = False, fuse_xent: bool = False,
+                 fuse_lstm_fp32: bool = False):
         super().__init__()
         self.fuse_lstm = fuse_lstm
+        self.fuse_lstm_fp32 = fuse_lstm_fp32
         self.fuse_xent = fuse_xent
         self.embedding_dim, self.num_layers = embedding_dim, num_layers
         self.dropout = nn.Dropout(1 - dp_keep_prob)
@@ -226,7 +229,7 @@ class PTBLSTM(nn.Module):
     def forward(self, inputs: torch.Tensor, hidden):
         emb = self.dropout(self.word_embeddings(inputs))
         if self.fuse_lstm:
-            out, hidden = lstm_stack(emb, hidden, self.lstm, self.lstm.dropout, self.training)
+            out, hidden = lstm_stack(emb, hidden, self.lstm, self.lstm.dropout, self.training, self.fuse_lstm_fp32)
         else:
             out, hidden = self.lstm(emb, hidden)
         out = self.dropout(out)

@@ -37,8 +37,8 @@ that the next step reads.  y comes back in the autocast type, as ``nn.LSTM``'s d
 This differs from cuDNN's 16-bit RNN, which also keeps c in 16 bits.
 
 ``lstm_stack(x, hx, rnn, dropout_p, training)`` runs a multi-layer ``nn.LSTM`` from a carried state (the PTB language
-model) under bf16 / fp16 autocast on a second pair of kernels, whose step product runs on the tensor cores; see its
-docstring.
+model) under bf16 / fp16 autocast on a second pair of kernels, whose step product runs on the tensor cores, and with
+``fp32=True`` in fp32 on the fp32 forms of the same kernels; see its docstring.
 """
 from __future__ import annotations
 
@@ -288,21 +288,94 @@ def lstm_seq_geometry(H: int, N: int, sms: int, smem_per_block: int) -> Optional
                            _seq_bwd_smem(H, N, u, rows[1]))
 
 
+# fp32: the CTA's W_hh slice (288 KB at H = 1500) does not fit in shared memory.  The first r_on of its weight rows stay
+# on chip and the others are read from L2 at every step; the step operand is staged F32_CHUNK columns at a time.
+F32_CHUNK = 256             # columns of h_{t-1} / dgates_{t+1} per staged chunk (a multiple of 8)
+F32_MAX_ROWS = 8 * LSTM_WARPS       # weight rows per CTA the fp32 step takes: 8 per warp
+
+
+class LstmSeqF32Geometry(NamedTuple):
+    units: int              # hidden units per CTA (u)
+    grid: int               # CTAs: ceil(H / u), one per SM
+    fwd_r_on: int           # of the CTA's 4u gate rows of W_hh, how many are held in shared memory
+    fwd_kc: int             # columns of h_{t-1} staged at a time
+    bwd_r_on: int           # of its u columns of W_hh (rows of W_hh^T), how many are held in shared memory
+    bwd_kc: int             # columns of dgates_{t+1} staged at a time
+    fwd_smem: int           # dynamic shared memory per CTA, bytes
+    bwd_smem: int
+    fwd_l2_bytes: int       # weight bytes all CTAs together read from L2 at each step
+    bwd_l2_bytes: int
+
+
+def _f32_ld(K: int) -> int:
+    """csrc/lstm.cu lstm_f32_ld: the shared-memory row stride of a K-float weight row, = 4 (mod 8)."""
+    return -(-K // 8) * 8 + 4
+
+
+def _f32_ksplit(R: int) -> int:
+    """csrc/lstm.cu lstm_f32_ksplit."""
+    return max(1, LSTM_WARPS // -(-R // 8))
+
+
+def _f32_fixed_smem(N: int, R: int, kc: int, cell: int) -> int:
+    """Everything but the on-chip weight rows: two staged chunks, the K-split partial sums and ``cell`` fp32 values
+    (gate sums and c forward, dh sums and carried dc backward)."""
+    return 4 * (2 * N * (kc + 4) + _f32_ksplit(R) * N * R + cell)
+
+
+def lstm_seq_f32_geometry(H: int, N: int, sms: int, smem_per_block: int) -> Optional[LstmSeqF32Geometry]:
+    """How the fp32 stacked-layer kernels split a layer of H units at batch N over ``sms`` SMs with ``smem_per_block``
+    bytes of opt-in shared memory per CTA, or None when they cannot.  Each CTA owns u = ceil(H / sms) units, as in
+    ``lstm_seq_geometry``.  Forward its weight rows are its 4u gate rows of W_hh (K = H columns), backward its u columns
+    (K = 4H); it stages the step operand's N rows ``min(F32_CHUNK, K rounded up to 8)`` columns at a time in two
+    buffers, and keeps as many weight rows in shared memory as fit next to them, ``_f32_ld(K)`` floats apart; the
+    remaining rows are read from L2 at every step.  H % 4 == 0, 1 <= N <= MAX_BATCH, 4u <= F32_MAX_ROWS.  On an H100
+    (132 SMs, 232 448 B): H = 1500, N = 20 is u = 12 on 125 CTAs, 29 of 48 rows on chip forward (229 008 B) and 7 of
+    12 backward (219 312 B), in 256-column chunks; the other rows are 14.25 MB forward and 15 MB backward per step."""
+    if H <= 0 or H % 4 or not 1 <= N <= MAX_BATCH or sms <= 0:
+        return None
+    u = -(-H // sms)
+    grid = -(-H // u)
+    if 4 * u > F32_MAX_ROWS:
+        return None
+    split = []
+    for R, K, cell in ((4 * u, H, 5 * u * N), (u, 4 * H, 2 * u * N)):
+        kc = min(F32_CHUNK, -(-K // 8) * 8)
+        fixed = _f32_fixed_smem(N, R, kc, cell)
+        r_on = min(R, (smem_per_block - fixed) // (4 * _f32_ld(K)))
+        if r_on < 0:
+            return None
+        split.append((r_on, kc, fixed + 4 * r_on * _f32_ld(K)))
+    (fr, fkc, fsm), (br, bkc, bsm) = split
+    fwd_l2 = bwd_l2 = 0
+    for b in range(grid):                   # the last CTA may own fewer units; its rows past them are not read
+        nu = min(u, H - b * u)
+        fwd_l2 += sum(1 for lr in range(fr, 4 * u) if lr % u < nu) * H * 4
+        bwd_l2 += max(0, nu - br) * 4 * H * 4
+    return LstmSeqF32Geometry(u, grid, fr, fkc, br, bkc, fsm, bsm, fwd_l2, bwd_l2)
+
+
 def _stack_params(rnn: nn.LSTM, layer: int) -> Tuple[torch.Tensor, ...]:
     return tuple(getattr(rnn, "%s_l%d" % (n, layer)) for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh"))
 
 
-def _stack_ok(x: torch.Tensor, hx, rnn: nn.Module) -> Optional[Tuple[LstmSeqGeometry, torch.dtype]]:
-    """The geometry and the kernels' storage type when ``lstm_stack`` runs the native path, else None."""
+def _stack_ok(x: torch.Tensor, hx, rnn: nn.Module, fp32: bool = False):
+    """The geometry (``LstmSeqGeometry``, or ``LstmSeqF32Geometry`` in fp32) and the kernels' storage type when
+    ``lstm_stack`` runs the native path, else None."""
     if not (isinstance(rnn, nn.LSTM) and rnn.num_layers >= 1 and not rnn.bidirectional and rnn.bias
             and rnn.proj_size == 0 and not rnn.batch_first):
         return None
     if not (x.is_cuda and x.dim() == 3 and x.size(2) == rnn.input_size and x.size(0) > 0):
         return None
-    if not torch.is_autocast_enabled("cuda"):
+    if torch.is_autocast_enabled("cuda"):
+        dt = torch.get_autocast_dtype("cuda")
+        if dt not in (torch.bfloat16, torch.float16):
+            return None
+    elif fp32:
+        dt = torch.float32
+    else:
         return None
-    dt = torch.get_autocast_dtype("cuda")
-    if dt not in (torch.bfloat16, torch.float16) or x.dtype not in (torch.float32, dt) or not ext.available():
+    if x.dtype not in (torch.float32, dt) or not ext.available():
         return None
     if any(p.dtype != torch.float32 or p.device != x.device for p in rnn.parameters()):
         return None
@@ -315,14 +388,17 @@ def _stack_ok(x: torch.Tensor, hx, rnn: nn.Module) -> Optional[Tuple[LstmSeqGeom
                     and h.dtype in (torch.float32, dt)):
                 return None
     p = torch.cuda.get_device_properties(x.device)
-    geom = lstm_seq_geometry(H, N, p.multi_processor_count, p.shared_memory_per_block_optin)
+    geometry = lstm_seq_f32_geometry if dt == torch.float32 else lstm_seq_geometry
+    geom = geometry(H, N, p.multi_processor_count, p.shared_memory_per_block_optin)
     return None if geom is None else (geom, dt)
 
 
 class _LstmSeqLayer(torch.autograd.Function):
     """One layer from (h0, c0) on the stacked-layer kernels: returns y [T, N, H] and h_n (both of type ``dt``) and c_n
     (fp32).  x, h0 and the parameters are cast to ``dt`` here, once per forward, and both passes run with autocast off.
-    ``h0`` of the input's type or ``dt``, ``c0`` fp32 or ``dt``; their gradients come back in their types."""
+    ``h0`` of the input's type or ``dt``, ``c0`` fp32 or ``dt``; their gradients come back in their types.  With
+    ``dt`` fp32 nothing is cast, ``geom`` is an ``LstmSeqF32Geometry``, and the backward kernel reads W_hh^T, a copy
+    made per backward pass."""
 
     @staticmethod
     def forward(ctx, x, h0, c0, geom, dt, w_ih, w_hh, b_ih, b_hh):
@@ -332,16 +408,17 @@ class _LstmSeqLayer(torch.autograd.Function):
         H = w_hh.size(1)
         with torch.autocast(x.device.type, enabled=False):
             xs = x.to(dt).contiguous()
-            w_ih_s, w_hh_s = w_ih.to(dt), w_hh.to(dt).contiguous()
-            h0s, c0f = h0.to(dt).contiguous(), c0.float().contiguous()
+            w_ih_s, w_hh_s = w_ih.to(dt), ext.dense16(w_hh.to(dt))
+            h0s, c0f = ext.dense16(h0.to(dt)), c0.float().contiguous()
             gx = torch.addmm((b_ih + b_hh).to(dt), xs.view(T * N, I), w_ih_s.t())      # (T N) x 4H
         y = torch.empty(T, N, H, device=x.device, dtype=dt)
         gates = torch.empty(T, N, 4 * H, device=x.device, dtype=torch.float32)
         cs = torch.empty(T, N, H, device=x.device, dtype=torch.float32)
         bar = torch.zeros(1, dtype=torch.int64, device=x.device)
+        split = (N, geom.fwd_r_on, geom.fwd_kc) if dt == torch.float32 else (geom.fwd_rows, 0, 0)
         C.lstm_seq_forward(gx.data_ptr(), w_hh_s.data_ptr(), h0s.data_ptr(), c0f.data_ptr(), y.data_ptr(),
-                           gates.data_ptr(), cs.data_ptr(), bar.data_ptr(), T, N, H, geom.units, geom.fwd_rows,
-                           torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt])
+                           gates.data_ptr(), cs.data_ptr(), bar.data_ptr(), T, N, H, geom.units, split[0],
+                           torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt], split[1], split[2])
         ctx.save_for_backward(xs, h0s, c0f, y, gates, cs, w_ih_s, w_hh_s)
         ctx.geom = geom
         ctx.dtypes = (x.dtype, h0.dtype, c0.dtype)
@@ -360,10 +437,16 @@ class _LstmSeqLayer(torch.autograd.Function):
         dg = torch.empty(T, N, 4 * H, device=x.device, dtype=dt)
         dc0 = torch.empty(N, H, device=x.device, dtype=torch.float32)
         bar = torch.zeros(1, dtype=torch.int64, device=x.device)
-        C.lstm_seq_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), w_hh.data_ptr(), c0.data_ptr(),
+        geom = ctx.geom
+        if dt == torch.float32:                                 # fp32 streams rows of W_hh^T from L2
+            whh, split = w_hh.t().contiguous(), (N, geom.bwd_r_on, geom.bwd_kc)
+        else:
+            whh, split = w_hh, (geom.bwd_rows, 0, 0)
+        C.lstm_seq_backward(dy.data_ptr(), gates.data_ptr(), cs.data_ptr(), whh.data_ptr(), c0.data_ptr(),
                             0 if dhn is None else dhn.data_ptr(), 0 if dcn is None else dcn.data_ptr(), dg.data_ptr(),
-                            dc0.data_ptr(), bar.data_ptr(), T, N, H, ctx.geom.units, ctx.geom.bwd_rows,
-                            torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt])
+                            dc0.data_ptr(), bar.data_ptr(), T, N, H, geom.units, split[0],
+                            torch.cuda.current_stream().cuda_stream, DTYPE_CODE[dt], split[1], split[2])
+        del whh
         need = ctx.needs_input_grad
         x_dt, h0_dt, c0_dt = ctx.dtypes
         g2 = dg.view(T * N, 4 * H)
@@ -382,7 +465,7 @@ class _LstmSeqLayer(torch.autograd.Function):
         return dx, dh0, dc0.to(c0_dt) if need[2] else None, None, None, dw_ih, dw_hh, db_ih, db_hh
 
 
-def lstm_stack(x: torch.Tensor, hx, rnn: nn.Module, dropout_p: float, training: bool):
+def lstm_stack(x: torch.Tensor, hx, rnn: nn.Module, dropout_p: float, training: bool, fp32: bool = False):
     """``rnn(x, hx)`` for a uni-directional, multi-layer ``nn.LSTM`` over the time-major ``x`` (T x N x I): returns
     ``(y, (h_n, c_n))`` with h_n and c_n [L, N, H], as ``nn.LSTM`` does.  ``hx`` = (h0, c0), each [L, N, H], or None
     (zeros).
@@ -397,11 +480,17 @@ def lstm_stack(x: torch.Tensor, hx, rnn: nn.Module, dropout_p: float, training: 
     Numerics otherwise as the module docstring's 16-bit layer: W_hh, gx, y, dy and dgates 16-bit, rounded to nearest
     even (an fp16 overflow is inf), everything else fp32, bitwise reproducible.
 
+    With ``fp32=True`` and autocast off, an fp32 ``x`` runs on the fp32 forms of the same kernels (``hx`` fp32 too):
+    y, h_n and c_n come back fp32.  The CTA keeps as many of its W_hh rows in shared memory as fit and reads the rest
+    from L2 at every step (``lstm_seq_f32_geometry``), and the step product runs in 3xTF32 on the tensor cores, about
+    fp32 accuracy, whatever ``torch.backends.cuda.matmul.allow_tf32`` says.  The input projection, dx, dh0, dW_ih and
+    dW_hh are torch GEMMs and follow that switch, as ``lstm_layer``'s do.  Under autocast ``fp32`` changes nothing.
+
     Needs the native extension, fp32 parameters on x's device, bias, ``proj_size == 0``, ``batch_first=False``, x of
-    fp32 or the autocast type, T >= 1, hx of the right shape, and an (H, N) that ``lstm_seq_geometry`` accepts on the
-    device.  Anything else -- autocast off (fp32), the CPU, fp64, a bidirectional ``rnn``, a layer too large -- returns
-    exactly ``rnn(x, hx)``."""
-    ok = _stack_ok(x, hx, rnn)
+    fp32 or the autocast type, T >= 1, hx of the right shape, and an (H, N) that ``lstm_seq_geometry`` (in fp32
+    ``lstm_seq_f32_geometry``) accepts on the device.  Anything else -- autocast off without ``fp32``, the CPU, fp64, a
+    bidirectional ``rnn``, a layer too large -- returns exactly ``rnn(x, hx)``."""
+    ok = _stack_ok(x, hx, rnn, fp32)
     if ok is None:
         return rnn(x, hx)
     geom, dt = ok

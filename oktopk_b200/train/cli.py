@@ -93,6 +93,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-lstm-lm", action="store_true",
                    help="lstm (PTB), with --bf16 or --fp16: the stacked LSTM runs on the 16-bit stacked-layer fused "
                         "recurrence kernels, the hidden state carried in and out (default: stock cuDNN layer)")
+    p.add_argument("--fused-lstm-lm-fp32", action="store_true",
+                   help="lstm (PTB), in fp32 (no --bf16 / --fp16): the stacked LSTM runs on the fp32 stacked-layer fused "
+                        "recurrence kernels, W_hh partly read from L2 every step, the step product in 3xTF32 "
+                        "(default: stock cuDNN layer)")
     p.add_argument("--fused-lstm-autocast", action="store_true",
                    help="with --fused-lstm and --bf16 or --fp16: the LSTM layers take the 16-bit fused recurrence kernels "
                         "(default: stock layers under autocast)")
@@ -143,8 +147,10 @@ def model_args(args: argparse.Namespace):
         model_kwargs["mlm_capacity"] = args.mlm_capacity
     if args.fused_attn:
         model_kwargs["fuse_attn"] = True
-    if args.fused_lstm or args.fused_lstm_lm:
+    if args.fused_lstm or args.fused_lstm_lm or args.fused_lstm_lm_fp32:
         model_kwargs["fuse_lstm"] = True
+    if args.fused_lstm_lm_fp32:
+        model_kwargs["fuse_lstm_fp32"] = True
     if args.fused_lstm_autocast:
         model_kwargs["fuse_lstm_autocast"] = True
     if args.bidirectional:
@@ -185,13 +191,17 @@ def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namesp
     """``--fused-lstm`` and ``--bidirectional`` are for the AN4 DeepSpeech model (``--dnn lstman4``) only;
     ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
     needs ``--fused-lstm`` and ``--bidirectional``.  ``--fused-lstm-lm`` is for the PTB model (``--dnn lstm``) and
-    needs ``--bf16`` or ``--fp16``."""
+    needs ``--bf16`` or ``--fp16``; ``--fused-lstm-lm-fp32`` is for the PTB model too, in fp32 only."""
     if args.fused_lstm and model_args(args)[0] != "lstman4":
         parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
     if args.fused_lstm_lm and model_args(args)[0] != "lstm":
         parser.error("--fused-lstm-lm applies to lstm, not %s" % model_args(args)[0])
     if args.fused_lstm_lm and not (args.bf16 or args.fp16):
         parser.error("--fused-lstm-lm needs --bf16 or --fp16")
+    if args.fused_lstm_lm_fp32 and model_args(args)[0] != "lstm":
+        parser.error("--fused-lstm-lm-fp32 applies to lstm, not %s" % model_args(args)[0])
+    if args.fused_lstm_lm_fp32 and (args.bf16 or args.fp16):
+        parser.error("--fused-lstm-lm-fp32 runs fp32: with --bf16 or --fp16 use --fused-lstm-lm")
     if args.fused_lstm_autocast and not args.fused_lstm:
         parser.error("--fused-lstm-autocast needs --fused-lstm")
     if args.fused_lstm_autocast and not (args.bf16 or args.fp16):
