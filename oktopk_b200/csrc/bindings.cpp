@@ -675,6 +675,33 @@ static void xent_backward(uint64_t x, uint64_t t, uint64_t lse, uint64_t g, uint
     ck(launch_xent_backward(P_<const void>(x), P_<const long long>(t), P_<const float>(lse), P_<const float>(g), P_<void>(dx),
                             R, V, ignore_index, dtype_arg(dtype, "xent_backward"), S_(stream)), "xent_backward");
 }
+// Softmax + CTC loss (csrc/ctc.cu) over x [T, N, C] (dtype codes as dtype_arg); targets [nt] int64 (targets64 = 1) or
+// int32, 0 when nt = 0; tn / ln [N] int32; ws ctc_workspace_floats(T, N, nt) floats, ab ctc_ab_floats(T, N, nt); loss
+// and g one float each.
+static void ctc_check(const char* what, int T, int N, int C, long long nt, uint64_t x, uint64_t t, int t64, int dtype,
+                      std::initializer_list<uint64_t> ptrs) {
+    if (!ctc_supported(T, N, C, nt))
+        throw std::runtime_error(std::string(what) + ": needs T, N > 0, 0 < C <= 128 and at most 2047 targets");
+    for (uint64_t p : ptrs)
+        if (p == 0) throw std::runtime_error(std::string(what) + ": null pointer");
+    if (nt > 0 && t == 0) throw std::runtime_error(std::string(what) + ": null targets");
+    if (t & (t64 ? 7 : 3)) throw std::runtime_error(std::string(what) + ": misaligned targets");
+    if (x & (dtype == 0 ? 3 : 1)) throw std::runtime_error(std::string(what) + ": misaligned logits");
+}
+static void ctc_forward(uint64_t x, uint64_t t, int t64, uint64_t tn, uint64_t ln, uint64_t ws, uint64_t loss, int T, int N,
+                        int C, long long nt, int dtype, uint64_t stream) {
+    ctc_check("ctc_forward", T, N, C, nt, x, t, t64, dtype, {x, tn, ln, ws, loss});
+    ck(launch_ctc_forward(P_<const void>(x), P_<const void>(t), t64, P_<const int>(tn), P_<const int>(ln), P_<float>(ws),
+                          P_<float>(loss), T, N, C, nt, dtype_arg(dtype, "ctc_forward"), S_(stream)), "ctc_forward");
+}
+static void ctc_backward(uint64_t x, uint64_t t, int t64, uint64_t tn, uint64_t ln, uint64_t ws, uint64_t ab, uint64_t g,
+                         uint64_t dx, int T, int N, int C, long long nt, int dtype, uint64_t stream) {
+    ctc_check("ctc_backward", T, N, C, nt, x, t, t64, dtype, {x, tn, ln, ws, ab, g, dx});
+    if (dx & (dtype == 0 ? 3 : 1)) throw std::runtime_error("ctc_backward: misaligned gradient");
+    ck(launch_ctc_backward(P_<const void>(x), P_<const void>(t), t64, P_<const int>(tn), P_<const int>(ln),
+                           P_<const float>(ws), P_<float>(ab), P_<const float>(g), P_<void>(dx), T, N, C, nt, dtype_arg(dtype, "ctc_backward"), S_(stream)),
+       "ctc_backward");
+}
 // Fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels [R] int64, rows [M] int32, tgt [M]
 // int64, slot [R] int32, count one int64, overflow one int64 or 0; x / dx [R, H] and out / dout [M, H] of type dtype.
 static void mlm_select(uint64_t labels, uint64_t rows, uint64_t tgt, uint64_t slot, uint64_t count, uint64_t overflow,
@@ -919,6 +946,15 @@ PYBIND11_MODULE(_C, m) {
           py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
     m.def("xent_backward", &xent_backward, py::arg("x"), py::arg("t"), py::arg("lse"), py::arg("g"), py::arg("dx"),
           py::arg("R"), py::arg("V"), py::arg("ignore_index"), py::arg("dtype"), py::arg("stream"));
+    m.def("ctc_forward", &ctc_forward, py::arg("x"), py::arg("t"), py::arg("t64"), py::arg("tn"), py::arg("ln"),
+          py::arg("ws"), py::arg("loss"), py::arg("T"), py::arg("N"), py::arg("C"), py::arg("nt"), py::arg("dtype"),
+          py::arg("stream"));
+    m.def("ctc_backward", &ctc_backward, py::arg("x"), py::arg("t"), py::arg("t64"), py::arg("tn"), py::arg("ln"),
+          py::arg("ws"), py::arg("ab"), py::arg("g"), py::arg("dx"), py::arg("T"), py::arg("N"), py::arg("C"), py::arg("nt"),
+          py::arg("dtype"), py::arg("stream"));
+    m.def("ctc_supported", &ctc_supported);
+    m.def("ctc_workspace_floats", &ctc_workspace_floats);
+    m.def("ctc_ab_floats", &ctc_ab_floats);
     m.def("mlm_select", &mlm_select, py::arg("labels"), py::arg("rows"), py::arg("tgt"), py::arg("slot"), py::arg("count"),
           py::arg("overflow"), py::arg("R"), py::arg("M"), py::arg("ignore_index"), py::arg("stream"));
     m.def("mlm_gather", &mlm_gather, py::arg("x"), py::arg("rows"), py::arg("out"), py::arg("M"), py::arg("H"),

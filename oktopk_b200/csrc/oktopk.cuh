@@ -417,6 +417,18 @@ cudaError_t launch_xent_forward(const void* x, const long long* t, float* lse, f
                                 long long V, long long ignore_index, Dtype dtype, cudaStream_t stream);
 cudaError_t launch_xent_backward(const void* x, const long long* t, const float* lse, const float* g, void* dx, int R,
                                  long long V, long long ignore_index, Dtype dtype, cudaStream_t stream);
+// fused softmax + CTC loss, blank 0, summed, zero_infinity (csrc/ctc.cu): x and dx [T, N, C] of type `dtype` (a Dtype);
+// targets [nt] int64 (targets64 = 1) or int32; tn, ln [N] int32 input / target lengths; ws ctc_workspace_floats(T, N, nt)
+// fp32, written by the forward pass and read by the backward pass; ab ctc_ab_floats(T, N, nt) fp32 scratch of the
+// backward pass; loss and g one fp32 each.  Needs ctc_supported(T, N, C, nt).  Two launches forward, one backward.
+bool ctc_supported(int T, int N, int C, long long nt);
+long long ctc_workspace_floats(int T, int N, long long nt);
+long long ctc_ab_floats(int T, int N, long long nt);
+cudaError_t launch_ctc_forward(const void* x, const void* targets, int targets64, const int* tn, const int* ln, float* ws,
+                               float* loss, int T, int N, int C, long long nt, Dtype dtype, cudaStream_t stream);
+cudaError_t launch_ctc_backward(const void* x, const void* targets, int targets64, const int* tn, const int* ln,
+                                const float* ws, float* ab, const float* g, void* dx, int T, int N, int C, long long nt,
+                                Dtype dtype, cudaStream_t stream);
 // fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels and tgt int64, rows [M] and slot
 // [R] int32, count one int64, overflow one int64 that accumulates max(count - M, 0) (or null); x [R, H] and out [M, H],
 // dout [M, H] and dx [R, H] of type `dtype` (a Dtype).  One launch each.

@@ -27,7 +27,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``) and ``fuse_attn=True`` ``net.fuse_attn``; for
     ``lstman4``,
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
-    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``); for ``lstm`` (PTB),
+    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``) and ``fuse_ctc=True``
+    ``net.fuse_ctc``; for ``lstm`` (PTB),
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_fp32=True`` ``net.fuse_lstm_fp32`` and ``fuse_xent=True``
     ``net.fuse_xent``."""
     ext = None
@@ -53,8 +54,10 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     elif d == "lstman4":
         kw = dict(kwargs)
         fuse_lstm = bool(kw.pop("fuse_lstm", False))
+        fuse_ctc = bool(kw.pop("fuse_ctc", False))
         net = lstman4(**kw)
         net.fuse_lstm = fuse_lstm
+        net.fuse_ctc = fuse_ctc
         ext = {"labels": AN4_LABELS}
     elif d == "lstm":
         net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20),

@@ -13,7 +13,8 @@ recurrence kernels of ``ops/fused_lstm.py`` instead of packing the sequences for
 ``fuse_lstm_autocast=True`` (``net.fuse_lstm_autocast``) is set as well, which runs the 16-bit forms of the kernels.
 The bidirectional network (``bidirectional=True``) keeps stock layers under ``fuse_lstm`` unless
 ``fuse_lstm_bidirectional=True`` (``net.fuse_lstm_bidirectional``) is set as well, which runs both directions of each
-layer in one launch of the kernels.
+layer in one launch of the kernels.  ``fuse_ctc=True`` (``net.fuse_ctc``, a plain attribute) asks the trainer to compute
+the CTC loss with the fused softmax + CTC kernels (``ops/fused_ctc``); it does not change the network.
 """
 from __future__ import annotations
 
@@ -107,7 +108,7 @@ class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
                  window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-                 fuse_lstm_bidirectional: bool = False):
+                 fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -132,6 +133,7 @@ class DeepSpeech(nn.Module):
         self.fuse_lstm = fuse_lstm
         self.fuse_lstm_autocast = fuse_lstm_autocast
         self.fuse_lstm_bidirectional = fuse_lstm_bidirectional
+        self.fuse_ctc = fuse_ctc
 
     @property
     def fuse_lstm(self) -> bool:
@@ -189,11 +191,11 @@ class DeepSpeech(nn.Module):
 
 def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
             fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-            fuse_lstm_bidirectional: bool = False) -> DeepSpeech:
+            fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
     return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
                       fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast,
-                      fuse_lstm_bidirectional=fuse_lstm_bidirectional)
+                      fuse_lstm_bidirectional=fuse_lstm_bidirectional, fuse_ctc=fuse_ctc)
 
 
 class PTBLSTM(nn.Module):

@@ -100,6 +100,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-lstm-autocast", action="store_true",
                    help="with --fused-lstm and --bf16 or --fp16: the LSTM layers take the 16-bit fused recurrence kernels "
                         "(default: stock layers under autocast)")
+    p.add_argument("--fused-ctc", action="store_true",
+                   help="lstman4: the CTC loss runs on the fused softmax + CTC kernels, the lengths read on the device "
+                        "and the backward deterministic (default: stock log_softmax + nn.CTCLoss)")
     p.add_argument("--bidirectional", action="store_true",
                    help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
                         "(default: uni-directional)")
@@ -157,6 +160,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["bidirectional"] = True
     if args.fused_lstm_bidirectional:
         model_kwargs["fuse_lstm_bidirectional"] = True
+    if args.fused_ctc:
+        model_kwargs["fuse_ctc"] = True
     return dnn, model_kwargs
 
 
@@ -191,7 +196,8 @@ def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namesp
     """``--fused-lstm`` and ``--bidirectional`` are for the AN4 DeepSpeech model (``--dnn lstman4``) only;
     ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
     needs ``--fused-lstm`` and ``--bidirectional``.  ``--fused-lstm-lm`` is for the PTB model (``--dnn lstm``) and
-    needs ``--bf16`` or ``--fp16``; ``--fused-lstm-lm-fp32`` is for the PTB model too, in fp32 only."""
+    needs ``--bf16`` or ``--fp16``; ``--fused-lstm-lm-fp32`` is for the PTB model too, in fp32 only.  ``--fused-ctc`` is
+    for ``lstman4`` only."""
     if args.fused_lstm and model_args(args)[0] != "lstman4":
         parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
     if args.fused_lstm_lm and model_args(args)[0] != "lstm":
@@ -212,6 +218,8 @@ def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namesp
         parser.error("--fused-lstm-bidirectional needs --fused-lstm")
     if args.fused_lstm_bidirectional and not args.bidirectional:
         parser.error("--fused-lstm-bidirectional needs --bidirectional")
+    if args.fused_ctc and model_args(args)[0] != "lstman4":
+        parser.error("--fused-ctc applies to lstman4, not %s" % model_args(args)[0])
 
 
 def main(argv=None) -> int:

@@ -23,6 +23,7 @@ from .. import compression as _comp
 from ..config import LossScale, OkTopkConfig, preset as _preset
 from ..models import create_net
 from ..models.bert import BertPreTrainingHeads
+from ..ops.fused_ctc import ctc_loss
 from ..ops.fused_xent import softmax_cross_entropy
 from ..optimizer import BertAdam, DistributedOptimizer, broadcast_parameters
 from ..parallel.world import World, world as _world
@@ -194,6 +195,8 @@ class Trainer:
             inputs, targets, in_pct, tsizes = batch
             lengths = (in_pct * inputs.size(3)).int()
             out, out_lens = self.net(inputs, lengths)
+            if getattr(self.net, "fuse_ctc", False):
+                return ctc_loss(out.transpose(0, 1), targets, out_lens, tsizes) / inputs.size(0), None
             logp = F.log_softmax(out.transpose(0, 1), dim=-1)          # T x N x C
             # int64 device targets => torch's native CTC kernels (int32 host targets would route to cuDNN's CTC, which
             # has no zero_infinity handling and produced NaN gradients on synthetic utterances)
