@@ -36,15 +36,20 @@
 // and rounded once to x's type, to nearest even, an fp16 gradient past 65504 becoming inf.  g (the loss's incoming
 // gradient, which carries a loss scale) is read from device memory.  No atomics: results are bitwise reproducible.
 //
-// Edge cases (per utterance; the others are unaffected):
+// Edge cases (per utterance, the others unaffected, except after a bad target length):
 //   - Ln = 0: the all-blank alignment, ctc = -sum_t log softmax(x)[t, 0].
 //   - Infeasible (Ln plus its repeated neighbours > Tn): ctc = +inf; zero_infinity makes its loss and gradient 0.
 //   - Tn = 0: ctc = 0 if Ln = 0, else +inf (then 0), and no gradient, as torch.
-//   - A label outside [0, C), a negative length, Tn > T or sum Ln > nt: ctc = NaN and a NaN gradient on frames
-//     t < Tn (every frame when Tn itself is out of range).  Torch device-asserts or raises instead.
+//   - A label outside [0, C) or Tn outside [0, T]: ctc = NaN and a NaN gradient on frames t < Tn (every frame when Tn
+//     itself is out of range).
+//   - A negative Ln at utterance m, or one that takes sum_{n<=m} Ln past nt: the target offsets of m and of every later
+//     utterance are undefined, so all of them are NaN as above; the utterances before m are unaffected.  Torch
+//     device-asserts or raises on these and on the previous case instead.
 //   - Frames t >= Tn are never read; their gradient is exactly 0 even if they hold inf or NaN (stock log_softmax's
 //     backward makes it NaN there).
-//   - An inf or NaN within an utterance's frames makes its loss and gradient NaN (not zeroed: only +inf is).
+//   - A -inf logit within an utterance's frames: the frame's log-sum-exp skips it, so the loss stays finite, as torch's;
+//     the gradient is NaN in every class of each frame holding one, as torch's is.  A NaN or +inf logit there makes
+//     the loss and gradient NaN (not zeroed: only a +inf ctc is).
 #include "common.cuh"
 #include "elem.cuh"
 #include "oktopk.cuh"

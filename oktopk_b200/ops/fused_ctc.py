@@ -19,9 +19,12 @@ kernels); targets int32 or int64.  The loss is a 0-d fp32 tensor.  The logits' g
 inf, so a loss-scaled overflow reaches the scaler's check).  ``g`` is read on the device.
 
 Edge cases, per utterance: ``Ln = 0`` is the all-blank alignment; an infeasible utterance (or ``Tn = 0`` with
-``Ln > 0``) contributes exactly 0 to the loss and the gradient; a label outside ``[0, C)`` (or device lengths that do not
-fit the shapes) makes that utterance's loss and gradient NaN, where torch device-asserts.  Frames ``t >= Tn`` are never
-read: their gradient is exactly 0 even if they hold inf or NaN.
+``Ln > 0``) contributes exactly 0 to the loss and the gradient; a label outside ``[0, C)`` or a device input length
+outside ``[0, T]`` makes that utterance's loss and gradient NaN, where torch device-asserts.  A negative target length,
+or one that takes the running sum of target lengths past ``targets.numel()``, leaves the target offsets undefined from
+that utterance on: it and every later utterance are NaN, the earlier ones unaffected.  Frames ``t >= Tn`` are never
+read: their gradient is exactly 0 even if they hold inf or NaN.  A ``-inf`` logit leaves the loss finite (as torch's)
+and makes the gradient of its frame NaN in every class (as torch's).
 
 Falls back to exactly the stock expression above wherever the fast path does not apply: CPU logits, no native
 extension, logits not 3-D or not fp32 / bf16 / fp16, ``C`` outside ``[1, 128]``, more than 2047 targets in the batch,

@@ -1,7 +1,9 @@
 """The fused softmax + CTC loss (``csrc/ctc.cu``, ``ops/fused_ctc.py``) on the GPU: loss and logits' gradient against
-``F.ctc_loss`` in float64 on the CPU, no worse than the stock fp32 op on the GPU; the edge cases of the kernels' header
-(zero_infinity, frames past Tn, a bad label, Ln = 0, Tn = 0); the loss scale and an fp16 overflow; determinism; no host
-synchronisation and CUDA-graph replay; launch counts; the whole DeepSpeech model; and Trainer steps against stock."""
+``F.ctc_loss`` in float64 on the CPU, no worse than the stock fp32 op on the GPU, with int32 and int64 targets, C from 1
+to 128, Ln on either side of every warp boundary up to 2047, batches past 32 utterances and blank labels; a single
+alignment against its closed form; the edge cases of the kernels' header (zero_infinity, frames past Tn, a bad label or
+length, Ln = 0, Tn = 0, a -inf logit); the loss scale and an fp16 overflow; determinism; no host synchronisation and
+CUDA-graph replay; launch counts; the whole DeepSpeech model; and Trainer steps against stock."""
 import copy
 
 import pytest
@@ -40,26 +42,49 @@ def _need(labels):
     return len(labels) + sum(1 for a, b in zip(labels, labels[1:]) if a == b)
 
 
-def _batch(N, T, seed, infeasible=False):
-    """Logits [T, N, C] and a batch with mixed Tn (the first utterance full length), Ln from 0 up to feasibility, runs
-    of repeated labels, and with `infeasible` one utterance that cannot be aligned."""
+def _path(labels):
+    """The one alignment of `labels` in _need(labels) frames: each label once, a blank between equal neighbours."""
+    out = []
+    for j, c in enumerate(labels):
+        if j and c == labels[j - 1]:
+            out.append(0)
+        out.append(c)
+    return out
+
+
+def _labels(L, g, nc=C, distinct=False):
+    """L random labels in [1, nc), with equal neighbours unless `distinct`."""
+    lab = torch.randint(1, nc, (L,), generator=g).tolist() if nc > 1 else []
+    for j in range(1, L if distinct else 0):
+        if lab[j] == lab[j - 1]:
+            lab[j] = lab[j] % (nc - 1) + 1
+    return lab
+
+
+def _batch(N, T, seed, infeasible=False, nc=C, labels=None, tn=None, targets=torch.int64):
+    """Logits [T, N, nc] and a batch: by default mixed Tn (the first utterance full length), Ln from 0 up to
+    feasibility, runs of repeated labels, and with `infeasible` one utterance that cannot be aligned.  `labels` (one
+    list per utterance; Tn defaults to T) and `tn` replace the drawn ones; `targets` is the targets' dtype."""
     g = torch.Generator().manual_seed(seed)
-    x = torch.randn(T, N, C, generator=g) * 2
-    tn = [T] + [int(torch.randint(1, T + 1, (1,), generator=g)) for _ in range(N - 1)]
-    tgts, lns = [], []
-    for n in range(N):
-        cap = tn[n]
-        L = int(torch.randint(0, cap + 1, (1,), generator=g)) if n else min(cap, 33)
-        lab = torch.randint(1, C, (L,), generator=g).tolist()
-        if L >= 4:
-            lab[1] = lab[2] = lab[3] = lab[0]                  # a run of repeats
-        while lab and _need(lab) > cap:
-            lab.pop()
-        if infeasible and n == N - 1:                        # cap repeats need 2 cap - 1 > cap frames
-            lab = [7] * cap if cap >= 2 else [3, 4]
-        tgts += lab
-        lns.append(len(lab))
-    return x, torch.tensor(tgts, dtype=torch.int64), torch.tensor(tn, dtype=torch.int32), torch.tensor(lns, dtype=torch.int32)
+    x = torch.randn(T, N, nc, generator=g) * 2
+    if tn is None:
+        tn = [T] * N if labels is not None else [T] + [int(torch.randint(1, T + 1, (1,), generator=g)) for _ in range(N - 1)]
+    if labels is None:
+        labels = []
+        for n in range(N):
+            cap = tn[n]
+            L = int(torch.randint(0, cap + 1, (1,), generator=g)) if n else min(cap, 33)
+            lab = _labels(L, g, nc)
+            if L >= 4:
+                lab[1] = lab[2] = lab[3] = lab[0]              # a run of repeats
+            while lab and _need(lab) > cap:
+                lab.pop()
+            if infeasible and n == N - 1:                    # cap repeats need 2 cap - 1 > cap frames
+                lab = [7] * cap if cap >= 2 else [3, 4]
+            labels.append(lab)
+    tgts = [c for lab in labels for c in lab]
+    return (x, torch.tensor(tgts, dtype=targets), torch.tensor(tn, dtype=torch.int32),
+            torch.tensor([len(lab) for lab in labels], dtype=torch.int32))
 
 
 def _fused(x, targets, tn, ln, g=1.0):
@@ -89,27 +114,216 @@ def _stock_gpu(x, targets, tn, ln):
     return loss.detach(), dx
 
 
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("N,T", [(1, 1), (2, 2), (2, 48), (5, 48), (1, 198), (2, 198), (5, 198), (2, 400), (5, 400)])
-def test_loss_and_gradient_against_float64(N, T, dtype):
-    x, targets, tn, ln = _batch(N, T, seed=N * 1000 + T, infeasible=T >= 2 and N >= 2)
-    x = x.to(dtype)                                           # the reference sees the same (widened) values
+DTYPES = [torch.float32, torch.bfloat16, torch.float16]
+TARGETS = [torch.int32, torch.int64]
+RND = {torch.float32: 0.0, torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}   # dx's rounding to x's type
+
+
+def _fused_fast(x, targets, tn, ln):
+    """_fused, asserting that the kernels ran: two launches forward, one backward."""
     n0 = _launches()
     lf, df = _fused(x.cuda(), targets.cuda(), tn, ln)
     n1 = _launches()
     assert (n1[0] - n0[0], n1[1] - n0[1]) == (2, 1)
-    assert df.dtype == dtype
-    lr, dr = _ref(x, targets, tn, ln)
+    assert df.dtype == x.dtype
+    return lf, df
+
+
+def _ref_alpha(x, targets, tn, ln):
+    """The summed loss of feasible utterances by the plain α recursion in float64 on the CPU, without torch's CTC, and
+    its gradient by autograd (-1e300 stands for log 0, so that no gradient is NaN)."""
+    xi = x.detach().double().cpu().requires_grad_(True)
+    lp = F.log_softmax(xi, -1)
+    loss, off = 0.0, 0
+    for n in range(x.shape[1]):
+        lab = targets[off:off + int(ln[n])].tolist()
+        off += len(lab)
+        ext = [0] + [v for c in lab for v in (c, 0)]
+        skip = torch.tensor([s >= 3 and s % 2 == 1 and ext[s] != ext[s - 2] for s in range(len(ext))])
+        neg = torch.full((len(ext),), -1e300, dtype=torch.float64)
+        a = torch.cat([torch.zeros(1, dtype=torch.float64), neg[1:]])       # before t = 0: the start state
+        for t in range(int(tn[n])):
+            a1 = torch.cat([neg[:1], a[:-1]])
+            a2 = torch.where(skip, torch.cat([neg[:2], a[:-2]]), neg)
+            a = torch.logsumexp(torch.stack([a, a1, a2]), 0) + lp[t, n, ext]
+        loss = loss - torch.logsumexp(a[-2:], 0)
+    (dx,) = torch.autograd.grad(loss, xi)
+    return loss.detach(), dx
+
+
+def _check_against_float64(x, targets, tn, ln, nan_frames=(), ref=_ref):
+    """The fused loss and dx of x (on the host, in its own dtype) against float64 on the CPU (`ref`): the error is at
+    most twice stock fp32 GPU's, plus dx's rounding to x's type and a 1e-5 floor.  On `nan_frames`, (t, n) pairs, dx is
+    NaN in every class, as float64's is; frames past Tn get exactly 0.  Returns the fused loss and dx."""
+    lf, df = _fused_fast(x, targets, tn, ln)
+    lr, dr = ref(x, targets, tn, ln)
     ls, ds = _stock_gpu(x, targets, tn, ln)
     el, es_l = abs(lf.double().cpu() - lr).item(), abs(ls.double().cpu() - lr).item()
     assert el <= 2 * es_l + 1e-5 * max(1.0, abs(lr.item())), (el, es_l, lr.item())
-    ef = (df.cpu().double() - dr).abs()
-    es = (ds.cpu().double() - dr).abs().max().item()
-    rnd = {torch.float32: 0.0, torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}[dtype]
-    tol = rnd * dr.abs() + 2 * es + 1e-5
+    df64, ds = df.cpu().double(), ds.cpu().double()
+    keep = torch.ones(x.shape[:2], dtype=torch.bool)
+    for t, n in nan_frames:
+        assert torch.isnan(df64[t, n]).all() and torch.isnan(dr[t, n]).all(), (t, n)
+        keep[t, n] = False
+    ef = (df64 - dr).abs()[keep]
+    es = (ds - dr).abs()[keep].max().item()
+    tol = RND[x.dtype] * dr.abs()[keep] + 2 * es + 1e-5
     assert bool((ef <= tol).all()), (ef.max().item(), es)
-    for n in range(N):                                        # frames past Tn: exactly 0
+    for n in range(x.shape[1]):                               # frames past Tn: exactly 0
         assert torch.all(df[int(tn[n]):, n] == 0)
+    return lf, df
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("N,T", [(1, 1), (2, 2), (2, 48), (5, 48), (1, 198), (2, 198), (5, 198), (2, 400), (5, 400)])
+def test_loss_and_gradient_against_float64(N, T, dtype, targets):
+    x, tg, tn, ln = _batch(N, T, seed=N * 1000 + T, infeasible=T >= 2 and N >= 2, targets=targets)
+    _check_against_float64(x.to(dtype), tg, tn, ln)           # the reference sees the same (widened) values
+
+
+def _multiwarp_batch(seed, targets=torch.int64):
+    """Utterances of 1023, 64, 0 and 500 labels (S = 2047, 129, 1, 1001: 16, 2, 1 and 8 warps), T = 1200."""
+    g = torch.Generator().manual_seed(seed)
+    labels = [_labels(L, g) for L in (1023, 64, 0, 500)]
+    return _batch(4, 1200, seed, labels=labels, tn=[1200, 300, 50, 1100], targets=targets)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("case", ["mixed", "multiwarp"])
+def test_int32_and_int64_targets_are_bitwise_equal(case, dtype):
+    out = []
+    for targets in TARGETS:
+        x, tg, tn, ln = _batch(5, 198, seed=16, targets=targets) if case == "mixed" else _multiwarp_batch(23, targets)
+        out.append(_fused_fast(x.to(dtype), tg, tn, ln))
+    assert torch.equal(out[0][0], out[1][0]) and torch.equal(out[0][1], out[1][1])
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("nc", [1, 2, 31, 32, 33, 64, 127, 128])
+def test_class_counts_against_float64(nc, dtype):
+    """C from 1 to kCtcMaxC, the labels reaching the top classes (96..127 at C = 128: the last 32-wide column of the
+    backward's per-class rows).  C = 1 holds only the blank, so Ln = 0."""
+    g = torch.Generator().manual_seed(100 + nc)
+    top = list(range(max(1, nc - 32), nc))
+    labels = [top[::-1], _labels(20, g, nc), [], top[-5:] + [1] + top[:5]] if nc > 1 else [[], [], [], []]
+    x, tg, tn, ln = _batch(4, 70, seed=nc, nc=nc, labels=labels, tn=[70, 50, 30, 45])
+    _check_against_float64(x.to(dtype), tg, tn, ln)
+
+
+# Ln around the α / β warp boundaries: S = 2 Ln + 1 states, 128 per warp, so Ln = 63 / 64 is one warp / two, 127 / 128
+# two / three, 191 / 192 two / four ... and 2047 = kCtcMaxTargets all 32 warps (S = 4095).
+LN_EDGES = [63, 64, 127, 128, 191, 192, 1023, 1024, 2047]
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("Ln,dtype", [(L, dt) for L in LN_EDGES for dt in (DTYPES if L in (63, 64, 2047) else DTYPES[:1])])
+def test_warp_boundaries_against_float64(Ln, dtype, targets):
+    """One utterance of Ln labels.  At Ln = 2047 the labels have no equal neighbours, so that T = 2100 is feasible."""
+    g = torch.Generator().manual_seed(Ln)
+    lab = _labels(Ln, g, distinct=Ln == 2047)
+    T = 2100 if Ln == 2047 else _need(lab) + 60
+    x, tg, tn, ln = _batch(1, T, seed=Ln, labels=[lab], targets=targets)
+    _check_against_float64(x.to(dtype), tg, tn, ln)
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_warp_boundaries_in_a_mixed_batch(dtype, targets):
+    """Single- and multi-warp utterances side by side, each at its own target and α offset, Tn from need to need + 60."""
+    g = torch.Generator().manual_seed(24)
+    labels = [_labels(L, g) for L in (63, 1023, 0, 128, 192, 64, 127)]
+    tn = [min(1200, _need(lab) + 10 * n) for n, lab in enumerate(labels)]
+    x, tg, tn, ln = _batch(7, 1200, seed=24, labels=labels, tn=tn, targets=targets)
+    _check_against_float64(x.to(dtype), tg, tn, ln)
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("Ln,pair,equal", [(128, 63, True), (128, 63, False), (1100, 1023, True), (1100, 1023, False),
+                                           (2047, None, None)])
+def test_exactly_one_alignment(Ln, pair, equal, dtype, targets):
+    """Tn = need: one alignment, so the posterior is one-hot along it, dx = softmax(x) - onehot(path) and the loss is
+    -sum log softmax along the path, in float64 without torch's CTC.  Labels `pair` and `pair` + 1 sit in states 2 pair
+    + 1 and 2 pair + 3 on either side of a warp boundary; equal, the α skip into the second and the β skip out of the
+    first must be off.  Tn = need - 1 is infeasible: loss and dx exactly 0."""
+    g = torch.Generator().manual_seed(Ln + 7 * bool(equal))
+    lab = _labels(Ln, g)
+    if pair is not None:
+        lab[pair + 1] = lab[pair] if equal else lab[pair] % (C - 1) + 1
+    path = _path(lab)
+    T = len(path)
+    assert T == _need(lab)
+    x, tg, tn, ln = _batch(1, T, seed=Ln, labels=[lab], targets=targets)
+    x = x.to(dtype)
+    lf, df = _fused_fast(x, tg, tn, ln)
+    lp = F.log_softmax(x[:, 0].double(), -1)
+    at = torch.arange(T)
+    lr = -lp[at, path].sum().item()
+    dr = lp.exp()
+    dr[at, path] -= 1
+    assert abs(lf.item() - lr) <= (1e-5 + T * 2.0 ** -24) * max(1.0, abs(lr)), (lf.item(), lr)
+    ef = (df[:, 0].cpu().double() - dr).abs()
+    assert bool((ef <= RND[dtype] * dr.abs() + 2e-6).all()), ef.max().item()
+    l0, d0 = _fused_fast(x[:-1], tg, tn - 1, ln)
+    assert l0.item() == 0 and torch.all(d0 == 0)
+
+
+@pytest.mark.parametrize("scale", [1, 8])
+def test_max_targets_deterministic_and_against_float64(scale):
+    """Ln = kCtcMaxTargets, T = 2100, fp32 logits, and x 8 (peaked): 2100 steps of the log-space recursion on all 32
+    warps, bitwise the same twice."""
+    g = torch.Generator().manual_seed(25)
+    x, tg, tn, ln = _batch(1, 2100, seed=25, labels=[_labels(2047, g, distinct=True)], targets=torch.int32)
+    x = x * scale
+    lf, df = _check_against_float64(x, tg, tn, ln)
+    l2, d2 = _fused_fast(x, tg, tn, ln)
+    assert torch.equal(lf, l2) and torch.equal(df, d2)
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("N,T", [(32, 40), (33, 40), (64, 40), (257, 14)])
+def test_large_batches_against_float64(N, T, targets):
+    """More than 32 utterances: the loss's reduction adds several per lane."""
+    x, tg, tn, ln = _batch(N, T, seed=N, targets=targets)
+    _check_against_float64(x, tg, tn, ln)
+
+
+def test_infeasible_utterance_past_32_leaves_the_others_unchanged():
+    x, targets, tn, ln = _batch(64, 40, seed=26)
+    labels = [lab.tolist() for lab in torch.split(targets, ln.tolist())]
+    keep = [n for n in range(64) if n != 40]
+    l63, d63 = _fused_fast(x[:, keep].contiguous(), torch.tensor([c for n in keep for c in labels[n]]), tn[keep],
+                           ln[keep])
+    labels[40] = [6] * (int(tn[40]) + 1)                     # more labels than frames
+    tb = torch.tensor([c for lab in labels for c in lab])
+    lnb = torch.tensor([len(lab) for lab in labels], dtype=torch.int32)
+    l64, d64 = _fused_fast(x, tb, tn, lnb)
+    assert torch.all(d64[:, 40] == 0)
+    assert torch.equal(d64[:, keep], d63)
+    assert l64.item() == pytest.approx(l63.item(), rel=1e-6)
+    assert _stock(x.double(), tb, tn, lnb, reduction="none")[40].item() == 0 and torch.isfinite(l64)
+
+
+@pytest.mark.parametrize("targets", TARGETS)
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_blank_label_in_targets_against_float64(dtype, targets):
+    """Label 0 among the targets, as torch accepts: class 0's posterior adds the blank states and those odd states.
+    The reference is the plain α recursion: torch's CPU CTC backward sets class 0's posterior at an utterance's last
+    frame, rather than adding to it, when the last label is 0.  Elsewhere the two references agree."""
+    g = torch.Generator().manual_seed(27)
+    lab = _labels(12, g)
+    lab[2] = lab[5] = lab[6] = 0
+    labels = [[3, 0, 5, 0, 0, 7, 0], [0], [0, 0, 0], lab]
+    x, tg, tn, ln = _batch(4, 40, seed=27, labels=labels, tn=[40, 10, 25, 33], targets=targets)
+    x = x.to(dtype)
+    la, da = _ref_alpha(x, tg, tn, ln)
+    lr, dr = _ref(x, tg, tn, ln)
+    assert la.item() == pytest.approx(lr.item(), rel=1e-12)
+    for n, lab in enumerate(labels):
+        last = int(tn[n]) - (lab[-1] == 0)
+        assert torch.allclose(da[:last, n], dr[:last, n], rtol=0, atol=1e-12), n
+    _check_against_float64(x, tg, tn, ln, ref=_ref_alpha)
 
 
 def test_zero_infinity_leaves_the_others_unchanged():
@@ -155,6 +369,45 @@ def test_label_out_of_range_is_nan_for_that_utterance():
     ref = _fused(x[:, [0, 2]].contiguous().cuda(), torch.tensor([1, 2, 3, 7, 8]).cuda(), torch.tensor([40, 20], dtype=torch.int32),
                  torch.tensor([3, 2], dtype=torch.int32))[1]
     assert torch.equal(dx[:, 0], ref[:, 0]) and torch.equal(dx[:, 2], ref[:, 1])
+
+
+@pytest.mark.parametrize("case", ["negative", "past_nt"])
+def test_bad_target_length_is_nan_from_that_utterance_on(case):
+    """A negative Ln at utterance m, or one that takes sum Ln past nt, leaves the target offsets of m and every later
+    utterance undefined: they are NaN on their frames t < Tn; the ones before m are unchanged."""
+    x, targets, tn, ln = _batch(5, 50, seed=28)
+    m = 2
+    bad = ln.clone()
+    bad[m] = -1 if case == "negative" else int(ln[m]) + targets.numel()
+    l0, d0 = _fused_fast(x, targets, tn, ln)
+    lb, db = _fused_fast(x, targets, tn, bad)
+    assert torch.isnan(lb)
+    assert torch.equal(db[:, :m], d0[:, :m])
+    for n in range(m, 5):
+        assert torch.isnan(db[:int(tn[n]), n]).all() and torch.all(db[int(tn[n]):, n] == 0), n
+
+
+def test_device_input_length_past_t_is_nan_for_that_utterance():
+    x, targets, tn, ln = _batch(3, 50, seed=29)
+    bad = tn.clone()
+    bad[1] = 53
+    l0, d0 = _fused_fast(x, targets, tn.cuda(), ln)
+    lb, db = _fused_fast(x, targets, bad.cuda(), ln)
+    assert torch.isnan(lb)
+    assert torch.isnan(db[:, 1]).all()
+    assert torch.equal(db[:, 0], d0[:, 0]) and torch.equal(db[:, 2], d0[:, 2])
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_minus_inf_logit_keeps_the_loss_and_makes_its_frames_nan(dtype):
+    """The frame's log-sum-exp skips a -inf logit, so the loss stays finite and equals float64; the gradient is NaN in
+    every class of exactly the frames that hold one, as float64 torch's is.  One -inf at a class of the utterance's
+    labels, one at another class."""
+    x, targets, tn, ln = _batch(3, 60, seed=30, labels=[[1, 2, 3, 4], [5, 6, 5, 7, 8], [9]], tn=[60, 45, 30])
+    x = x.to(dtype)
+    x[10, 1, 6] = x[20, 1, 11] = float("-inf")
+    lf, _ = _check_against_float64(x, targets, tn, ln, nan_frames=[(10, 1), (20, 1)])
+    assert torch.isfinite(lf)
 
 
 def test_empty_targets_and_zero_length_inputs():
@@ -321,8 +574,9 @@ def test_trainer_steps_follow_stock(precision):
         assert b == pytest.approx(a, rel=rel), losses
 
 
-@pytest.mark.parametrize("case", ["fp64", "wide_c", "many_targets", "padded_targets"])
+@pytest.mark.parametrize("case", ["fp64", "wide_c", "c129", "many_targets", "padded_targets", "at_limit"])
 def test_fallbacks_on_the_gpu_are_the_stock_expression(case):
+    """Past the gate's limits the op is the stock expression, bitwise; at them (C = 128, nt = 2047) the kernels run."""
     g = torch.Generator().manual_seed(19)
     T, N = 12, 3
     x = torch.randn(T, N, C, generator=g)
@@ -333,12 +587,23 @@ def test_fallbacks_on_the_gpu_are_the_stock_expression(case):
         x = x.double()
     elif case == "wide_c":
         x = torch.randn(T, N, 200, generator=g)
+    elif case == "c129":
+        x = torch.randn(T, N, 129, generator=g)
+        t[0] = 128
     elif case == "many_targets":                              # 2048 targets, though each utterance's are feasible
         ln = torch.tensor([4, 3, 2041], dtype=torch.int32)
         tn = torch.tensor([12, 9, 12], dtype=torch.int32)
         t = torch.randint(1, C, (2048,), generator=g)
+    elif case == "at_limit":                                  # C = 128 and 2047 targets, the last utterance infeasible
+        x = torch.randn(T, N, 128, generator=g)
+        ln = torch.tensor([4, 3, 2040], dtype=torch.int32)
+        tn = torch.tensor([12, 9, 12], dtype=torch.int32)
+        t = torch.randint(1, 128, (2047,), generator=g)
     else:
         t = torch.randint(1, C, (N, 4), generator=g)
+    if case == "at_limit":
+        _check_against_float64(x, t, tn, ln)
+        return
     x, t = x.cuda(), t.cuda()
     outs = []
     for fused in (True, False):
