@@ -622,6 +622,43 @@ static void ln_backward(uint64_t x, uint64_t a, uint64_t dy, uint64_t gamma, uin
                           P_<void>(da), P_<float>(partial), P_<float>(dgamma), P_<float>(dbeta), R, H, p_keep_thr,
                           (float)scale, dtype_arg(a_dtype, "ln_backward"), S_(stream)), "ln_backward");
 }
+// y = dropout(LayerNorm(word[ids] + pos[r % S] + typ[tt])) over R = B S tokens (csrc/embedding.cu): ids, tt int64 [R];
+// tables, gamma, beta, y, dy, de and the table gradients fp32; stats 2R floats ([mean; rstd]); ovf one int64 or 0;
+// partial ln_bwd_grid(R) * 2H floats.  p_keep_thr and seed as for ln_forward.
+static void emb_check(const char* what, int R, int S, int H, int np, int nv, int nt, long long p_keep_thr, uint64_t seed,
+                      std::initializer_list<uint64_t> vec_ptrs, std::initializer_list<uint64_t> ptrs) {
+    if (!emb_supported(R, S, H, np) || nv <= 0 || nt <= 0)
+        throw std::runtime_error(std::string(what) + ": needs 0 < R = B S <= 4096, S <= the position rows, nonempty "
+                                                     "tables and H in 128, 256, ..., 1024");
+    if (p_keep_thr < 0 || p_keep_thr > (1LL << 32)) throw std::runtime_error(std::string(what) + ": p_keep_thr out of range");
+    if (p_keep_thr < (1LL << 32) && seed == 0) throw std::runtime_error(std::string(what) + ": dropout needs the seed");
+    for (uint64_t p : vec_ptrs)
+        if (p == 0 || (p & 15)) throw std::runtime_error(std::string(what) + ": tensors must be non-null and 16-byte aligned");
+    for (uint64_t p : ptrs)
+        if (p == 0 || (p & 7)) throw std::runtime_error(std::string(what) + ": ids and statistics must be non-null and aligned");
+}
+static void emb_forward(uint64_t ids, uint64_t tt, uint64_t word, uint64_t pos, uint64_t typ, uint64_t gamma, uint64_t beta,
+                        uint64_t y, uint64_t stats, uint64_t ovf, uint64_t seed, int R, int S, int H, int nv, int np, int nt,
+                        long long p_keep_thr, double scale, double eps, uint64_t stream) {
+    emb_check("emb_forward", R, S, H, np, nv, nt, p_keep_thr, seed, {word, pos, typ, gamma, beta, y}, {ids, tt, stats});
+    if (ovf & 7) throw std::runtime_error("emb_forward: misaligned counter");
+    ck(launch_emb_forward(P_<const long long>(ids), P_<const long long>(tt), P_<const float>(word), P_<const float>(pos),
+                          P_<const float>(typ), P_<const float>(gamma), P_<const float>(beta), P_<float>(y),
+                          P_<float>(stats), P_<long long>(ovf), P_<const unsigned long long>(seed), R, S, H, nv, nt,
+                          p_keep_thr, (float)scale, (float)eps, S_(stream)), "emb_forward");
+}
+static void emb_backward(uint64_t ids, uint64_t tt, uint64_t word, uint64_t pos, uint64_t typ, uint64_t gamma,
+                         uint64_t stats, uint64_t dy, uint64_t seed, uint64_t de, uint64_t partial,
+                         uint64_t dgamma, uint64_t dbeta, uint64_t dword, uint64_t dpos, uint64_t dtyp, int R, int S, int H,
+                         int nv, int np, int nt, long long p_keep_thr, double scale, uint64_t stream) {
+    emb_check("emb_backward", R, S, H, np, nv, nt, p_keep_thr, seed,
+              {word, pos, typ, gamma, dy, de, partial, dgamma, dbeta, dword, dpos, dtyp}, {ids, tt, stats});
+    ck(launch_emb_backward(P_<const long long>(ids), P_<const long long>(tt), P_<const float>(word), P_<const float>(pos),
+                           P_<const float>(typ), P_<const float>(gamma), P_<const float>(stats), P_<const float>(dy),
+                           P_<const unsigned long long>(seed), P_<float>(de), P_<float>(partial),
+                           P_<float>(dgamma), P_<float>(dbeta), P_<float>(dword), P_<float>(dpos), P_<float>(dtyp), R, S, H,
+                           nv, np, nt, p_keep_thr, (float)scale, S_(stream)), "emb_backward");
+}
 // Fused self-attention, head dim 64 (csrc/attention.cu): qkv / dqkv [B, S, 3 H 64] and out / dout [B, S, H 64] of type
 // dtype (codes as dtype_arg), 16-byte aligned; mask [B, S] fp32 or 0; lse / delta [B, H, S] fp32.  p_keep_thr and seed as
 // for ln_forward; scale = 1 / (1 - p).
@@ -935,6 +972,15 @@ PYBIND11_MODULE(_C, m) {
           py::arg("stream"));
     m.def("ln_bwd_grid", &ln_bwd_grid);
     m.def("ln_supported_h", &ln_supported_h);
+    m.def("emb_forward", &emb_forward, py::arg("ids"), py::arg("tt"), py::arg("word"), py::arg("pos"), py::arg("typ"),
+          py::arg("gamma"), py::arg("beta"), py::arg("y"), py::arg("stats"), py::arg("ovf"), py::arg("seed"), py::arg("R"),
+          py::arg("S"), py::arg("H"), py::arg("nv"), py::arg("np"), py::arg("nt"), py::arg("p_keep_thr"), py::arg("scale"),
+          py::arg("eps"), py::arg("stream"));
+    m.def("emb_backward", &emb_backward, py::arg("ids"), py::arg("tt"), py::arg("word"), py::arg("pos"), py::arg("typ"),
+          py::arg("gamma"), py::arg("stats"), py::arg("dy"), py::arg("seed"), py::arg("de"), py::arg("partial"), py::arg("dgamma"), py::arg("dbeta"), py::arg("dword"), py::arg("dpos"), py::arg("dtyp"),
+          py::arg("R"), py::arg("S"), py::arg("H"), py::arg("nv"), py::arg("np"), py::arg("nt"), py::arg("p_keep_thr"),
+          py::arg("scale"), py::arg("stream"));
+    m.def("emb_supported", &emb_supported);
     m.def("attn_forward", &attn_forward, py::arg("qkv"), py::arg("mask"), py::arg("seed"), py::arg("out"), py::arg("lse"),
           py::arg("B"), py::arg("S"), py::arg("H"), py::arg("p_keep_thr"), py::arg("scale"), py::arg("dtype"),
           py::arg("stream"));

@@ -350,5 +350,42 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
     return c;
 }
 
+// ------------------------------------------------------------------------------------------
+// Dropout keep bits of the fused LayerNorm and embedding kernels: flat element i is kept iff word i % 4 of
+// Philox4x32-10(counter (i/4 low, i/4 high, 0, 0), key (seed low, seed high)) is below keep_thr = floor((1-p) 2^32);
+// keep_thr >= 2^32 (p = 0) keeps everything and never reads the seed.
+// ------------------------------------------------------------------------------------------
+constexpr long long kLnKeepAll = 1LL << 32;
+
+struct LnDrop {
+    bool on;
+    uint32_t thr, k0, k1;
+    float s;
+};
+
+__device__ __forceinline__ LnDrop ln_drop(const unsigned long long* seed, long long keep_thr, float scale) {
+    LnDrop d;
+    d.on = keep_thr < kLnKeepAll;
+    d.thr = (uint32_t)keep_thr;
+    const unsigned long long k = d.on ? __ldg(seed) : 0ull;
+    d.k0 = (uint32_t)k;
+    d.k1 = (uint32_t)(k >> 32);
+    d.s = scale;
+    return d;
+}
+
+// The keep bits of the four elements from flat index i (i % 4 == 0), element k in bit k.
+__device__ __forceinline__ uint32_t ln_keep(const LnDrop& d, unsigned long long i) {
+    if (!d.on) return 0xfu;
+    const unsigned long long q = i >> 2;
+    const uint4 r = philox4x32_10(make_uint4((uint32_t)q, (uint32_t)(q >> 32), 0u, 0u), d.k0, d.k1);
+    return (uint32_t)(r.x < d.thr) | ((uint32_t)(r.y < d.thr) << 1) | ((uint32_t)(r.z < d.thr) << 2) |
+           ((uint32_t)(r.w < d.thr) << 3);
+}
+
+// The multiplier at those four elements: s where kept, 0 where dropped.
+__device__ __forceinline__ float4 ln_mult(const LnDrop& d, uint32_t keep) {
+    return make_float4((keep & 1u) ? d.s : 0.f, (keep & 2u) ? d.s : 0.f, (keep & 4u) ? d.s : 0.f, (keep & 8u) ? d.s : 0.f);
+}
 
 }  // namespace okt

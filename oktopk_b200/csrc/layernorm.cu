@@ -41,38 +41,6 @@ constexpr int kLnWarps = 4;                    // rows in flight per CTA
 constexpr int kLnThreads = 32 * kLnWarps;
 constexpr int kLnFwdMaxBlocks = 8192;
 constexpr int kLnBwdMaxBlocks = 256;           // rows of the backward pass's column partials
-constexpr long long kLnKeepAll = 1LL << 32;
-
-struct LnDrop {
-    bool on;
-    uint32_t thr, k0, k1;
-    float s;
-};
-
-__device__ __forceinline__ LnDrop ln_drop(const unsigned long long* seed, long long keep_thr, float scale) {
-    LnDrop d;
-    d.on = keep_thr < kLnKeepAll;
-    d.thr = (uint32_t)keep_thr;
-    const unsigned long long k = d.on ? __ldg(seed) : 0ull;
-    d.k0 = (uint32_t)k;
-    d.k1 = (uint32_t)(k >> 32);
-    d.s = scale;
-    return d;
-}
-
-// The keep bits of the four elements from flat index i (i % 4 == 0), element k in bit k.
-__device__ __forceinline__ uint32_t ln_keep(const LnDrop& d, unsigned long long i) {
-    if (!d.on) return 0xfu;
-    const unsigned long long q = i >> 2;
-    const uint4 r = philox4x32_10(make_uint4((uint32_t)q, (uint32_t)(q >> 32), 0u, 0u), d.k0, d.k1);
-    return (uint32_t)(r.x < d.thr) | ((uint32_t)(r.y < d.thr) << 1) | ((uint32_t)(r.z < d.thr) << 2) |
-           ((uint32_t)(r.w < d.thr) << 3);
-}
-
-// The multiplier of a at those four elements: s where kept, 0 where dropped.
-__device__ __forceinline__ float4 ln_mult(const LnDrop& d, uint32_t keep) {
-    return make_float4((keep & 1u) ? d.s : 0.f, (keep & 2u) ? d.s : 0.f, (keep & 4u) ? d.s : 0.f, (keep & 8u) ? d.s : 0.f);
-}
 
 // z = x + a m for one lane's float4 column j of a row; the forward and backward passes share it, so z is bitwise the same
 template <typename T>
@@ -223,6 +191,11 @@ static int ln_rows_grid(int R, int cap) {
 
 int ln_bwd_grid(int R) { return ln_rows_grid(R, kLnBwdMaxBlocks); }
 
+cudaError_t launch_ln_dgb(const float* partial, int G, int H, float* dgamma, float* dbeta, cudaStream_t stream) {
+    ln_dgb_kernel<<<2 * H / 32, 32 * kLnDgbWarps, 0, stream>>>(partial, G, H, dgamma, dbeta);
+    return cudaGetLastError();
+}
+
 template <typename T>
 static cudaError_t ln_forward_t(const float* x, const void* a, float* y, const float* gamma, const float* beta, float* mean,
                                 float* rstd, const unsigned long long* seed, int R, int H, long long keep_thr, float scale,
@@ -256,8 +229,7 @@ static cudaError_t ln_backward_t(const float* x, const void* a, const float* dy,
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    ln_dgb_kernel<<<2 * H / 32, 32 * kLnDgbWarps, 0, stream>>>(partial, grid, H, dgamma, dbeta);
-    return cudaGetLastError();
+    return launch_ln_dgb(partial, grid, H, dgamma, dbeta, stream);
 }
 
 static bool ln_args_ok(int R, int H, long long keep_thr, const unsigned long long* seed) {

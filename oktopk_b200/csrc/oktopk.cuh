@@ -410,6 +410,23 @@ cudaError_t launch_ln_backward(const float* x, const void* a, const float* dy, c
                                const float* rstd, const unsigned long long* seed, float* dx, void* da, float* partial,
                                float* dgamma, float* dbeta, int R, int H, long long keep_thr, float scale, Dtype a_dtype,
                                cudaStream_t stream);
+// dgamma | dbeta = the sum of the G rows of partial [G, 2H], in a fixed order (the last launch of launch_ln_backward)
+cudaError_t launch_ln_dgb(const float* partial, int G, int H, float* dgamma, float* dbeta, cudaStream_t stream);
+// fused embedding sum + LayerNorm + dropout of BERT's input block (csrc/embedding.cu): ids and tt [R] int64, token r at
+// position r % S; word [nv, H], pos [np, H], typ [nt, H], gamma, beta, y, stats ([mean; rstd], 2R) and de [R, H] fp32;
+// ovf one int64 that counts ids outside [0, nv) and types outside [0, nt) (or null).  Needs emb_supported(R, S, H, np).
+// The backward pass takes partial of ln_bwd_grid(R) 2H floats and writes every element of dword, dpos and dtyp.  One
+// launch forward, three backward.
+bool emb_supported(int R, int S, int H, int np);
+cudaError_t launch_emb_forward(const long long* ids, const long long* tt, const float* word, const float* pos,
+                               const float* typ, const float* gamma, const float* beta, float* y, float* stats,
+                               long long* ovf, const unsigned long long* seed, int R, int S, int H, int nv, int nt,
+                               long long keep_thr, float scale, float eps, cudaStream_t stream);
+cudaError_t launch_emb_backward(const long long* ids, const long long* tt, const float* word, const float* pos,
+                                const float* typ, const float* gamma, const float* stats, const float* dy,
+                                const unsigned long long* seed, float* de, float* partial, float* dgamma,
+                                float* dbeta, float* dword, float* dpos, float* dtyp, int R, int S, int H, int nv, int np,
+                                int nt, long long keep_thr, float scale, cudaStream_t stream);
 // fused softmax cross-entropy, mean over the rows whose target is not ignore_index (csrc/xent.cu): x and dx [R, V] of
 // type `dtype` (a Dtype), 16-byte aligned; t [R] int64; lse [R + 1] fp32 (per-row log-sum-exp, then n);
 // rowloss [R] fp32 scratch; loss and g one fp32 each.  Two launches forward, one backward.

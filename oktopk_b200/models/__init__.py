@@ -24,7 +24,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
     ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``); for BERT,
     ``fuse_ln=True`` turns on ``net.fuse_ln``, ``fuse_xent=True`` ``net.fuse_xent`` and ``sparse_mlm=True``
-    ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``) and ``fuse_attn=True`` ``net.fuse_attn``; for
+    ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``), ``fuse_attn=True`` ``net.fuse_attn`` and
+    ``fuse_emb=True`` ``net.fuse_emb``; for
     ``lstman4``,
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
     ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``) and ``fuse_ctc=True``
@@ -76,7 +77,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
                                  fuse_xent=bool(kwargs.get("fuse_xent", False)),
                                  sparse_mlm=bool(kwargs.get("sparse_mlm", False)),
                                  mlm_capacity=float(kwargs.get("mlm_capacity", 0.25)),
-                                 fuse_attn=bool(kwargs.get("fuse_attn", False)))
+                                 fuse_attn=bool(kwargs.get("fuse_attn", False)),
+                                 fuse_emb=bool(kwargs.get("fuse_emb", False)))
     else:
         raise ValueError("unknown dnn %r (have %s)" % (dnn, DNNS))
     if d in FUSED_BN_RESNETS:

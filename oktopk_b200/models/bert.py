@@ -11,7 +11,8 @@ matmul -> softmax -> matmul on the full [B,12,S,S] score tensor), ``F.layer_norm
 ``fuse_ln=True`` the encoder's dropout + residual + LayerNorm sites on the fused kernels of ``ops/fused_ln.py``, and
 with ``fuse_xent=True`` the masked-LM loss on the fused softmax cross-entropy of ``ops/fused_xent.py``, and with
 ``sparse_mlm=True`` the masked-LM head on the labelled rows only, gathered by ``ops/mlm_gather.py``, and with
-``fuse_attn=True`` self-attention on the fused kernels of ``ops/fused_attn.py``.
+``fuse_attn=True`` self-attention on the fused kernels of ``ops/fused_attn.py``, and with ``fuse_emb=True`` the
+embedding sum + LayerNorm + dropout on the fused kernels of ``ops/fused_emb.py``.
 """
 from __future__ import annotations
 
@@ -60,6 +61,10 @@ def _act(name: str):
 
 
 class BertEmbeddings(nn.Module):
+    """``fuse_emb`` (default off) runs the whole block through the fused kernels of ``ops/fused_emb.py``, which count
+    ids and token types outside their tables in the non-persistent buffer ``id_overflow`` instead of faulting;
+    parameters and ``state_dict`` keys are the same either way."""
+
     def __init__(self, c: BertConfig):
         super().__init__()
         self.word_embeddings = nn.Embedding(c.vocab_size, c.hidden_size)
@@ -67,8 +72,13 @@ class BertEmbeddings(nn.Module):
         self.token_type_embeddings = nn.Embedding(c.type_vocab_size, c.hidden_size)
         self.LayerNorm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
         self.dropout = nn.Dropout(c.hidden_dropout_prob)
+        self.fuse_emb = False
+        self.register_buffer("id_overflow", torch.zeros(1, dtype=torch.int64), persistent=False)
 
     def forward(self, input_ids: torch.Tensor, token_type_ids: torch.Tensor) -> torch.Tensor:
+        if self.fuse_emb:
+            from ..ops.fused_emb import embedding_layer_norm
+            return embedding_layer_norm(input_ids, token_type_ids, self, self.dropout.p if self.training else 0.0)
         pos = torch.arange(input_ids.size(1), device=input_ids.device).unsqueeze(0)
         e = self.word_embeddings(input_ids) + self.position_embeddings(pos) + self.token_type_embeddings(token_type_ids)
         return self.dropout(self.LayerNorm(e))
@@ -243,11 +253,12 @@ class BertForPreTraining(nn.Module):
     ``fuse_xent=True`` (or ``net.fuse_xent``) sets ``PretrainingCriterion.fuse_xent``; ``sparse_mlm=True`` (or
     ``net.sparse_mlm``) runs the masked-LM head on the labelled rows only when labels are given, gathered into
     ``mlm_capacity`` (or ``net.mlm_capacity``) times B·S rows, rounded up to a multiple of 8 (``BertPreTrainingHeads``);
-    ``fuse_attn=True`` (or ``net.fuse_attn``) sets ``BertSelfAttention.fuse_attn`` on every encoder layer."""
+    ``fuse_attn=True`` (or ``net.fuse_attn``) sets ``BertSelfAttention.fuse_attn`` on every encoder layer;
+    ``fuse_emb=True`` (or ``net.fuse_emb``) sets ``BertEmbeddings.fuse_emb``."""
 
     def __init__(self, config: Optional[BertConfig] = None, depth: int = 4, recompute: bool = False,
                  fuse_ln: bool = False, fuse_xent: bool = False, sparse_mlm: bool = False, mlm_capacity: float = 0.25,
-                 fuse_attn: bool = False):
+                 fuse_attn: bool = False, fuse_emb: bool = False):
         super().__init__()
         self.config = config or BertConfig()
         self.recompute = recompute           # ``--recompute_step`` (BERT/runtime.py:546-557, modeling.py:414-431)
@@ -260,6 +271,16 @@ class BertForPreTraining(nn.Module):
         self.sparse_mlm = sparse_mlm
         self.mlm_capacity = mlm_capacity
         self.fuse_attn = fuse_attn
+        self.fuse_emb = fuse_emb
+
+    @property
+    def fuse_emb(self) -> bool:
+        """True when the embedding sum + LayerNorm + dropout runs through the fused kernels."""
+        return self.stages[0].embeddings.fuse_emb
+
+    @fuse_emb.setter
+    def fuse_emb(self, on: bool) -> None:
+        self.stages[0].embeddings.fuse_emb = bool(on)
 
     @property
     def fuse_attn(self) -> bool:

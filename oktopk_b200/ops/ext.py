@@ -19,7 +19,7 @@ _LAUNCHERS = {"oktopk_run": 1, "gather_run": 1, "gtopk_run": 1, "dense_run": 1, 
               "maxpool2_fwd": 1, "maxpool2_bwd": 1, "unscale_check": 1, "ln_forward": 1, "ln_backward": 2,
               "xent_forward": 2, "xent_backward": 1, "lstm_forward": 1, "lstm_backward": 1, "mlm_select": 1,
               "mlm_gather": 1, "mlm_scatter": 1, "attn_forward": 1, "attn_backward": 2, "lstm_seq_forward": 1,
-              "lstm_seq_backward": 1, "ctc_forward": 2, "ctc_backward": 1}
+              "lstm_seq_backward": 1, "ctc_forward": 2, "ctc_backward": 1, "emb_forward": 1, "emb_backward": 3}
 
 
 class _CountingModule:

@@ -87,6 +87,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="BERT: the self-attention of every encoder layer takes the fused attention kernels, which read "
                         "the packed QKV projection and regenerate the dropout mask (default: stock "
                         "scaled_dot_product_attention)")
+    p.add_argument("--fused-emb", action="store_true",
+                   help="BERT: the embedding sum + LayerNorm + dropout runs on the fused embedding kernels, one kernel "
+                        "forward and the table gradients without a sort (default: stock ops)")
     p.add_argument("--fused-lstm", action="store_true",
                    help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
                         "and pass, instead of packed sequences through cuDNN (default: stock)")
@@ -150,6 +153,8 @@ def model_args(args: argparse.Namespace):
         model_kwargs["mlm_capacity"] = args.mlm_capacity
     if args.fused_attn:
         model_kwargs["fuse_attn"] = True
+    if args.fused_emb:
+        model_kwargs["fuse_emb"] = True
     if args.fused_lstm or args.fused_lstm_lm or args.fused_lstm_lm_fp32:
         model_kwargs["fuse_lstm"] = True
     if args.fused_lstm_lm_fp32:
@@ -175,14 +180,15 @@ def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespac
 
 
 def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln``, ``--sparse-mlm``, ``--mlm-capacity`` and ``--fused-attn`` are for BERT only (``--dnn bert_base``
+    """``--fused-ln``, ``--sparse-mlm``, ``--mlm-capacity``, ``--fused-attn`` and ``--fused-emb`` are for BERT only (``--dnn bert_base``
     / ``bert``, or a ``--module models.bertN.depth=M``), ``--fused-xent`` for BERT and the PTB model (``--dnn lstm``);
     ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
     dnn = model_args(args)[0]
     if args.fused_xent and dnn not in ("bert", "bert_base", "lstm"):
         parser.error("--fused-xent applies to BERT (bert_base, bert) and lstm, not %s" % dnn)
     for flag, on in (("--fused-ln", args.fused_ln), ("--sparse-mlm", args.sparse_mlm),
-                     ("--mlm-capacity", args.mlm_capacity is not None), ("--fused-attn", args.fused_attn)):
+                     ("--mlm-capacity", args.mlm_capacity is not None), ("--fused-attn", args.fused_attn),
+                     ("--fused-emb", args.fused_emb)):
         if on and dnn not in ("bert", "bert_base"):
             parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
     if args.mlm_capacity is not None:
