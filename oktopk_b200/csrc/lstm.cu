@@ -15,11 +15,11 @@
 // gate sums, then its units' c_t and h_t; it writes y_t, the activated gates and c_t (for the backward pass) and crosses
 // the grid barrier, after which every CTA can read all of y_t.
 //
-// Backward (lstm_bwd_kernel), t from T-1 down to 0: the CTA keeps the 4H x u columns of W_hh of the same units, so that
-// dh_rec[j] = sum_k W_hh[k, j] dgates_{t+1}[k] is local.  At step t it stages dgates_{t+1} (N x 4H) and forms its u x N
-// dh_rec; with dy_t, the saved gates and c, and its carried dc it writes dgates_t for its units' 4 gate rows and crosses
-// the barrier.  For t >= len_b, dgates and the carried dc are exactly 0.  dx, dW_ih, dW_hh and the bias gradients are
-// GEMMs and sums over dgates in torch.
+// Backward (lstm_bwd_kernel), t from Tm-1 down to 0 (Tm: below): the CTA keeps the 4H x u columns of W_hh of the same
+// units, so that dh_rec[j] = sum_k W_hh[k, j] dgates_{t+1}[k] is local.  At step t it stages dgates_{t+1} (N x 4H)
+// and forms its u x N dh_rec; with dy_t, the saved gates and c, and its carried dc it writes dgates_t for its units' 4
+// gate rows and crosses the barrier.  For t >= len_b, dgates and the carried dc are exactly 0.  dx, dW_ih, dW_hh and the
+// bias gradients are GEMMs and sums over dgates in torch.
 //
 // The barrier is common.cuh's ticket grid_sync on a counter the caller zeroes: one per step, the only cross-CTA
 // dependency being the whole of y_t (dgates_t), which every CTA reads.  Operands written by other CTAs in this launch
@@ -34,6 +34,12 @@
 // element is widened on load and enters the same fmaf chain in the same order, so a 16-bit launch is the fp32 kernel run
 // on the widened operands, except where a y or dgates it stored (rounded to nearest even, not saturated: an fp16
 // overflow is inf) is read back at the next step.
+//
+// Bound: both passes walk only the Tm = min(max_n len_n, T) steps some row still needs (lstm_steps).  Every CTA reads the
+// same N lengths, so every CTA gets the same Tm and crosses the same number of barriers.  For t in [Tm, T) y (forward)
+// and dgates (backward) are written as exact zeros before the walk: no other CTA reads them, so they need no barrier.
+// The saved gates and c at those times are never read and stay unwritten.  So a launch over a T padded past the longest
+// utterance costs the recurrence nothing, and gives y and dgates on [0, Tm) bit for bit what a launch at T = Tm gives.
 //
 // Directions: a bidirectional layer runs both of its directions in one launch of dirs * g CTAs (g = ceil(H / u)).  CTA
 // b serves direction d = b / g with units [(b % g) u, ...) of that direction's own W_hh.  Every per-timestep tensor is
@@ -84,6 +90,13 @@ __device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + exp
 
 // The time that row n (length L) of a direction works on at step s (the file header's pi).
 __device__ __forceinline__ int lstm_time(int s, int L, bool rev) { return rev && s < L ? L - 1 - s : s; }
+
+// The header's Tm: the longest of the N lengths, at most T (and 0 if none is positive).
+__device__ __forceinline__ int lstm_steps(const int* __restrict__ len, int N, int T) {
+    int m = 0;
+    for (int n = 0; n < N; ++n) m = max(m, __ldg(len + n));
+    return min(m, T);
+}
 
 // Copy batch rows [n0, n0 + nrows) of the [T, N, K] tensor V (K % 4 == 0, Vec-aligned), which other CTAs wrote in this
 // launch, to shared memory: row n from time lstm_time(s, len_n, rev).  Forward that is one contiguous block; in
@@ -191,7 +204,12 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
         reinterpret_cast<Vec*>(sW)[i] = v;
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sC[i] = 0.f;
-    for (int s = 0; s < p.T; ++s) {
+    const int Tm = lstm_steps(p.len, N, p.T);
+    for (int i = threadIdx.x; i < (p.T - Tm) * nu * N; i += kLstmThreads) {       // y past every length: exact zeros
+        const int j = i % nu, r = i / nu;
+        y[((size_t)Tm * N + r) * H + u0 + j] = El::narrow1(0.f);
+    }
+    for (int s = 0; s < Tm; ++s) {
         if (s == 0) {
             for (int i = threadIdx.x; i < R * N; i += kLstmThreads) sG[i] = 0.f;
             __syncthreads();
@@ -221,7 +239,7 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_fwd_kernel(const LstmFwd
                 y[o] = El::narrow1(0.f);
             }
         }
-        if (s + 1 < p.T) grid_sync(bar, p.g);
+        if (s + 1 < Tm) grid_sync(bar, p.g);
     }
 }
 
@@ -249,8 +267,14 @@ __global__ void __launch_bounds__(kLstmThreads, 1) lstm_bwd_kernel(const LstmBwd
         sW[(size_t)j * G + k] = j < nu ? __ldg(whh + (size_t)k * H + u0 + j) : El::narrow1(0.f);
     }
     for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sDC[i] = 0.f;
-    for (int s = p.T - 1; s >= 0; --s) {
-        if (s == p.T - 1) {
+    const int Tm = lstm_steps(p.len, N, p.T);
+    for (int i = threadIdx.x; i < (p.T - Tm) * nu * N; i += kLstmThreads) {       // dgates past every length: zeros
+        const int j = i % nu, r = i / nu;
+        S* dg = dg0 + ((size_t)Tm * N + r) * G + u0 + j;
+        dg[0] = dg[H] = dg[2 * H] = dg[3 * H] = El::narrow1(0.f);
+    }
+    for (int s = Tm - 1; s >= 0; --s) {
+        if (s == Tm - 1) {
             for (int i = threadIdx.x; i < u * N; i += kLstmThreads) sD[i] = 0.f;
             __syncthreads();
         } else {

@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops.fused_lstm import lstm_layer, lstm_stack, stock_layer
+from ..ops.fused_lstm import lstm_layer, lstm_layer_device, lstm_stack, stock_layer
 
 AN4_LABELS = "_'ABCDEFGHIJKLMNOPQRSTUVWXYZ "     # 29 symbols, index 0 = CTC blank
 
@@ -76,10 +76,18 @@ class BatchRNN(nn.Module):
         self.batch_norm = _SeqBN(nn.BatchNorm1d(input_size)) if batch_norm else None
         self.rnn = rnn_type(input_size=input_size, hidden_size=hidden_size, bidirectional=bidirectional, bias=True)
 
-    def forward(self, x: torch.Tensor, lengths: torch.Tensor, dev_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``lengths``: host int tensor; ``dev_lengths``: optionally the same as int32 on the device (fused path)."""
+    def forward(self, x: torch.Tensor, lengths: Optional[torch.Tensor],
+                dev_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``lengths``: host int tensor; ``dev_lengths``: optionally the same as int32 on the device (fused path).
+        ``lengths=None``: the lengths are ``dev_lengths`` only and are never read on the host (``lstm_layer_device``);
+        the layer must then take the fused kernels, else ``RuntimeError``."""
+        if lengths is None and not self.fuse:
+            raise RuntimeError("device-only lengths need the fused LSTM layer (fuse_lstm)")
         if self.batch_norm is not None:
             x = self.batch_norm(x)
+        if lengths is None:
+            return lstm_layer_device(x, dev_lengths, self.rnn, autocast=self.fuse_autocast,
+                                     bidirectional=self.fuse_bidirectional)
         if self.fuse:
             return lstm_layer(x, lengths, self.rnn, dev_lengths, autocast=self.fuse_autocast,
                               bidirectional=self.fuse_bidirectional)
@@ -172,15 +180,47 @@ class DeepSpeech(nn.Module):
                 seq = (seq + 2 * m.padding[1] - m.dilation[1] * (m.kernel_size[1] - 1) - 1) // m.stride[1] + 1
         return seq.int()
 
-    def forward(self, x: torch.Tensor, lengths: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    def device_lengths_error(self, cuda: bool = True, autocast: bool = False) -> Optional[str]:
+        """Why ``forward(..., device_lengths=True)`` cannot run on a CUDA (``cuda``) input with bf16 / fp16 autocast on
+        (``autocast``) or off, or None: every LSTM layer must take the fused kernels, since the stock layers pack their
+        sequences with host lengths."""
+        if not cuda:
+            return "device lengths need a CUDA input"
+        if not self.fuse_lstm:
+            return "device lengths need fuse_lstm: the stock LSTM layers pack with host lengths"
+        if autocast and not self.fuse_lstm_autocast:
+            return "device lengths under autocast need fuse_lstm_autocast: the LSTM layers would be stock"
+        if self._bidirectional and not self.fuse_lstm_bidirectional:
+            return "device lengths with bidirectional layers need fuse_lstm_bidirectional: the layers would be stock"
+        return None
+
+    def forward(self, x: torch.Tensor, lengths: torch.Tensor,
+                device_lengths: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``lengths``: the input frames of each utterance.  ``device_lengths=True``: ``lengths`` is an int32 tensor on
+        ``x``'s device, each in [1, T], and is never read on the host: the conv masks, every LSTM layer
+        (``lstm_layer_device``) and the returned output lengths stay on the device, so the step can be captured in a CUDA
+        graph.  It raises ``RuntimeError`` where a layer would be stock (``device_lengths_error``).  Default: the
+        lengths are copied to the host once, as they always were."""
+        if device_lengths:
+            why = self.device_lengths_error(x.is_cuda, torch.is_autocast_enabled("cuda"))
+            if why is not None:
+                raise RuntimeError(why)
+            if lengths.dtype != torch.int32 or lengths.device != x.device:
+                raise RuntimeError("device lengths must be an int32 tensor on the input's device")
+            return self._forward(x, self.get_seq_lens(lengths), None)
         out_lens = self.get_seq_lens(lengths.cpu().int())
+        return self._forward(x, out_lens, out_lens)
+
+    def _forward(self, x: torch.Tensor, out_lens: torch.Tensor,
+                 host_lens: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``out_lens`` on the host (``host_lens`` the same tensor) or on the device only (``host_lens`` None)."""
         x = self.conv(x, out_lens)
         b, c, d, t = x.size()
         x = x.view(b, c * d, t).permute(2, 0, 1).contiguous()        # T x N x H
         # the fused layers read the lengths on the device: one copy for all of them
         dev_lens = out_lens.to(x.device) if x.is_cuda and any(m.fuse for m in self.rnns) else None
         for rnn in self.rnns:
-            x = rnn(x, out_lens, dev_lens)
+            x = rnn(x, host_lens, dev_lens)
         if self.lookahead is not None:
             x = self.lookahead(x)
         x = self.fc(x).transpose(0, 1)                                # N x T x classes

@@ -36,6 +36,9 @@ dgates_t is rounded to nearest even (an fp16 overflow gives inf, for loss scalin
 that the next step reads.  y comes back in the autocast type, as ``nn.LSTM``'s does, the parameter gradients in fp32.
 This differs from cuDNN's 16-bit RNN, which also keeps c in 16 bits.
 
+``lstm_layer_device(x, lengths, rnn, ...)`` takes the lengths as an int32 device tensor and never reads them on the host,
+so that a whole training step can be captured in a CUDA graph; it runs the native path or raises, never the stock layer.
+
 ``lstm_stack(x, hx, rnn, dropout_p, training)`` runs a multi-layer ``nn.LSTM`` from a carried state (the PTB language
 model) under bf16 / fp16 autocast on a second pair of kernels, whose step product runs on the tensor cores, and with
 ``fp32=True`` in fp32 on the fp32 forms of the same kernels; see its docstring.
@@ -108,6 +111,18 @@ def stock_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module) -> torch
 def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, autocast: bool,
                bidirectional: bool) -> Optional[Tuple[LstmGeometry, torch.dtype]]:
     """The geometry (of one direction) and the kernels' storage type when the native path applies, else None."""
+    ok = _native_layer_ok(x, rnn, autocast, bidirectional)
+    if ok is None or lengths.dim() != 1 or lengths.numel() != x.size(1):
+        return None
+    host = lengths.cpu()
+    if int(host.min()) < 1 or int(host.max()) > x.size(0):        # stock raises on these; let it
+        return None
+    return ok
+
+
+def _native_layer_ok(x: torch.Tensor, rnn: nn.Module, autocast: bool,
+                     bidirectional: bool) -> Optional[Tuple[LstmGeometry, torch.dtype]]:
+    """``_native_ok`` without the lengths: nothing here reads device memory."""
     if not (isinstance(rnn, nn.LSTM) and rnn.num_layers == 1 and (bidirectional or not rnn.bidirectional) and rnn.bias
             and rnn.proj_size == 0 and not rnn.batch_first):
         return None
@@ -123,10 +138,7 @@ def _native_ok(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, autocast:
     if any(p.dtype != torch.float32 or p.device != x.device for p in _params(rnn)):
         return None
     T, N = x.size(0), x.size(1)
-    if lengths.dim() != 1 or lengths.numel() != N or T == 0:
-        return None
-    host = lengths.cpu()
-    if int(host.min()) < 1 or int(host.max()) > T:          # stock raises on these; let it
+    if T == 0:
         return None
     geom = _device_geometry(rnn.hidden_size, N, x.device, dt.itemsize, 2 if rnn.bidirectional else 1)
     return None if geom is None else (geom, dt)
@@ -223,6 +235,11 @@ def lstm_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, dev_lengt
     geom, dt = ok
     if dev_lengths is None or dev_lengths.device != x.device or dev_lengths.dtype != torch.int32:
         dev_lengths = lengths.to(device=x.device, dtype=torch.int32)
+    return _native_layer(x, dev_lengths, geom, dt, rnn)
+
+
+def _native_layer(x: torch.Tensor, dev_lengths: torch.Tensor, geom: LstmGeometry, dt: torch.dtype,
+                  rnn: nn.Module) -> torch.Tensor:
     ps = list(_params(rnn))
     for i in range(1, len(ps), 4):
         w_hh = ps[i].contiguous()
@@ -230,6 +247,27 @@ def lstm_layer(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, dev_lengt
             w_hh = w_hh.clone()
         ps[i] = w_hh
     return _LstmLayer.apply(x.contiguous(), dev_lengths.contiguous(), geom, dt, *ps)
+
+
+def lstm_layer_device(x: torch.Tensor, lengths: torch.Tensor, rnn: nn.Module, autocast: bool = False,
+                      bidirectional: bool = False) -> torch.Tensor:
+    """``lstm_layer`` with the lengths on the device only: ``lengths`` is an int32 tensor of N lengths on ``x``'s device,
+    each in [1, T], and nothing is read back to the host, so the layer can be captured in a CUDA graph.  It always runs
+    the native path and raises ``RuntimeError`` where ``lstm_layer`` would take the stock one (which packs with host
+    lengths).  The kernels stop at the longest length (``csrc/lstm.cu``), so frames padded past it cost the recurrence
+    nothing; y there is exactly 0, as at every t >= len_b.  A length outside [1, T] is not checked: the longest one is
+    capped at T, and the rows' results are undefined."""
+    if not (isinstance(lengths, torch.Tensor) and lengths.dtype == torch.int32 and lengths.dim() == 1
+            and lengths.device == x.device and lengths.numel() == (x.size(1) if x.dim() == 3 else -1)):
+        raise RuntimeError("lstm_layer_device needs int32 lengths, one per batch row, on the input's device")
+    ok = _native_layer_ok(x, rnn, autocast, bidirectional)
+    if ok is None:
+        raise RuntimeError("the fused LSTM kernels do not apply to this layer and input (a single-layer nn.LSTM with "
+                           "bias on CUDA, fp32 or, with autocast=True, under bf16 / fp16 autocast; bidirectional only "
+                           "with bidirectional=True; H %% 4 == 0 and N <= %d), and the stock layer needs host lengths"
+                           % MAX_BATCH)
+    geom, dt = ok
+    return _native_layer(x, lengths, geom, dt, rnn)
 
 
 # ---- stacked layers from a carried state (the PTB language model) -----------------------------------------------------

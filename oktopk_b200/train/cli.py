@@ -106,6 +106,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fused-ctc", action="store_true",
                    help="lstman4: the CTC loss runs on the fused softmax + CTC kernels, the lengths read on the device "
                         "and the backward deterministic (default: stock log_softmax + nn.CTCLoss)")
+    p.add_argument("--an4-pad-multiple", type=int, default=0, metavar="M",
+                   help="lstman4: pad every training batch's frames up to a multiple of M and keep its lengths on the "
+                        "device; with --cuda-graph, --fused-lstm and --fused-ctc the steps are captured in CUDA graphs, "
+                        "one set per padded length.  The batch-norm statistics count the padded frames (default: 0, off)")
     p.add_argument("--bidirectional", action="store_true",
                    help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
                         "(default: uni-directional)")
@@ -203,7 +207,7 @@ def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namesp
     ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
     needs ``--fused-lstm`` and ``--bidirectional``.  ``--fused-lstm-lm`` is for the PTB model (``--dnn lstm``) and
     needs ``--bf16`` or ``--fp16``; ``--fused-lstm-lm-fp32`` is for the PTB model too, in fp32 only.  ``--fused-ctc`` is
-    for ``lstman4`` only."""
+    for ``lstman4`` only, as is ``--an4-pad-multiple`` (>= 0)."""
     if args.fused_lstm and model_args(args)[0] != "lstman4":
         parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
     if args.fused_lstm_lm and model_args(args)[0] != "lstm":
@@ -226,6 +230,10 @@ def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namesp
         parser.error("--fused-lstm-bidirectional needs --bidirectional")
     if args.fused_ctc and model_args(args)[0] != "lstman4":
         parser.error("--fused-ctc applies to lstman4, not %s" % model_args(args)[0])
+    if args.an4_pad_multiple and model_args(args)[0] != "lstman4":
+        parser.error("--an4-pad-multiple applies to lstman4, not %s" % model_args(args)[0])
+    if args.an4_pad_multiple < 0:
+        parser.error("--an4-pad-multiple must be >= 1 (or 0, off), got %d" % args.an4_pad_multiple)
 
 
 def main(argv=None) -> int:
@@ -269,7 +277,8 @@ def main(argv=None) -> int:
                      density=args.density, max_iters=args.max_iters, checkpoint_dir=args.checkpoint_dir, cfg=cfg,
                      log_dir=args.log_dir, seq_len=args.max_seq_length, seed=args.seed, backend=args.backend,
                      cuda_graph=args.cuda_graph, model_kwargs=model_kwargs or None, norm_clip=args.norm_clip,
-                     autocast="bf16" if args.bf16 else ("fp16" if args.fp16 else None), loss_scale=args.loss_scale)
+                     autocast="bf16" if args.bf16 else ("fp16" if args.fp16 else None), loss_scale=args.loss_scale,
+                     an4_pad_multiple=args.an4_pad_multiple)
     if args.trace:
         import json
         os.makedirs(args.trace, exist_ok=True)

@@ -14,7 +14,7 @@ Batches are produced in pinned host memory; ``Prefetcher`` moves them to the dev
 from __future__ import annotations
 
 import math
-from typing import Dict, Iterator, List, Optional, Tuple
+from typing import Dict, Iterator, List, NamedTuple, Optional, Tuple
 
 import torch
 from torch.utils.data import DataLoader, Dataset, DistributedSampler
@@ -105,6 +105,48 @@ def an4_collate(batch):
         tsizes[i] = tg.numel()
         targets.append(tg)
     return inputs, torch.cat(targets).int(), in_pct, tsizes
+
+
+AN4_MAX_TARGETS = 2047          # ops/fused_ctc's fast-path limit on a batch's targets (csrc/ctc.cu kCtcMaxTargets)
+
+
+class PaddedAN4Batch(NamedTuple):
+    """An AN4 training batch staged for a fixed-shape step (``pad_an4_batch``): every tensor's shape depends on the batch
+    size and the padded frame count ``T_b`` only, and no field needs a host read of device memory."""
+    inputs: torch.Tensor        # [B, 1, 161, T_b]: the batch, then zero frames
+    lengths: torch.Tensor       # int32 [B] on the device: (in_pct * T).int() clamped to [1, T], T the unpadded length
+    targets: torch.Tensor       # int32 [capacity]: the concatenated targets, then zeros ([ntargets] if over capacity)
+    tsizes: torch.Tensor        # int32 [B]: target sizes
+    ntargets: int               # the batch's number of targets (a host value: targets.numel() before padding)
+    over_capacity: bool         # ntargets > capacity: the targets are not padded, and the shape is the batch's own
+
+
+def an4_padded_frames(T: int, multiple: int) -> int:
+    """``T`` rounded up to a multiple of ``multiple`` (>= 1)."""
+    return -(-T // multiple) * multiple
+
+
+def an4_target_capacity(B: int, out_frames: int) -> int:
+    """The targets a padded batch holds: one per output frame of every utterance, at most ``AN4_MAX_TARGETS``."""
+    return min(B * out_frames, AN4_MAX_TARGETS)
+
+
+def pad_an4_batch(batch, multiple: int, out_frames) -> PaddedAN4Batch:
+    """Stage the trainer's AN4 batch ``(inputs [B, 1, 161, T], targets, in_pct, tsizes)`` (device tensors) into a
+    ``PaddedAN4Batch`` with ``T_b = an4_padded_frames(T, multiple)`` frames.  ``out_frames(T_b)``: the model's output
+    frames for ``T_b`` input frames, which sets the target capacity.  A few tensor ops on the current stream; every size
+    comes from the shapes, so nothing is read back to the host."""
+    inputs, targets, in_pct, tsizes = batch
+    B, T = inputs.size(0), inputs.size(3)
+    Tb = an4_padded_frames(T, multiple)
+    padded = torch.nn.functional.pad(inputs, (0, Tb - T)) if Tb > T else inputs
+    lengths = (in_pct * T).int().clamp_(1, T)           # the eager formula, kept inside the tensor
+    n = targets.numel()
+    cap = an4_target_capacity(B, out_frames(Tb))
+    tg = targets.to(torch.int32)
+    if n <= cap:
+        tg = torch.cat([tg, tg.new_zeros(cap - n)])
+    return PaddedAN4Batch(padded, lengths, tg, tsizes.to(torch.int32), n, n > cap)
 
 
 class SyntheticPTB(Dataset):

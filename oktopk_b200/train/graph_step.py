@@ -8,6 +8,14 @@ and the learning rate live in device memory, and the persistent cooperative kern
 node.  The only host-side variation is *which* flavour of the kernel a step needs (exact threshold
 re-computation / region re-partition iterations, SURVEY 3.3): each engine's ``plan_call``.  One graph
 is captured per flavour the first time it occurs and the host picks the graph from the iteration counter.
+
+AN4 batches vary in length.  With the trainer's ``an4_pad_multiple`` they arrive staged (``data.PaddedAN4Batch``):
+frames padded to a multiple of m, lengths on the device, targets in a fixed-capacity buffer, so that a batch's shapes
+depend on its padded length T_b only.  Graphs and static inputs are then keyed by (padded input shape, flavour), and
+every flavour of a new T_b is captured the first time it appears.  At most ``MAX_AN4_SHAPES`` padded shapes get graphs;
+a batch of another shape after that, or one whose targets exceed the capacity, runs that step eagerly on the same
+padded form (counted in ``fallbacks``).  The step needs every LSTM layer fused and the fused CTC loss, the two parts that
+read the lengths on the device; otherwise the graph step disables itself and the padded batches run eagerly.
 """
 from __future__ import annotations
 
@@ -17,6 +25,16 @@ import torch
 
 from ..ops import ext
 from ..parallel.state import plan_call, schedule_period
+from .data import PaddedAN4Batch
+
+# Padded AN4 input shapes (one per T_b at a fixed batch size) that get graphs; batches of further shapes run eagerly.
+# Each shape holds a graph per flavour; at m = 32 the synthetic AN4 utterances (96-396 frames) pad to 11 lengths.
+MAX_AN4_SHAPES = 16
+
+
+def _clone(batch):
+    vals = [t.clone() if torch.is_tensor(t) else t for t in batch]
+    return type(batch)(*vals) if isinstance(batch, PaddedAN4Batch) else tuple(vals)
 
 
 class GraphedTrainStep:
@@ -31,13 +49,30 @@ class GraphedTrainStep:
         self.enabled = True
         self.pool = None
         self.why_disabled = ""
-        self._precaptured = False
         self._cap_counters, self._cap_opt_counter = [], None
         self._loss_of: Dict[Tuple, torch.Tensor] = {}
+        # AN4 (padded batches): static inputs per padded shape, the shapes whose sparse flavours are all captured, and
+        # the steps that ran eagerly because their shape was past MAX_AN4_SHAPES or their targets past the capacity
+        self.an4 = getattr(trainer, "dataset", None) == "an4"
+        self._static_of: Dict[Tuple, tuple] = {}
+        self._precaptured_shapes = set()
+        self._shape: Optional[Tuple] = None
+        self.fallbacks = {"shapes": 0, "targets": 0}
+        if self.an4:
+            net = trainer.net
+            why = net.device_lengths_error(True, trainer.autocast is not None)
+            if why is None and not getattr(net, "fuse_ctc", False):
+                why = "fuse_ctc is off: the stock CTC loss copies the lengths to the host"
+            if why is not None:
+                self.enabled, self.why_disabled = False, why
 
     # ------------------------------------------------------------------ iteration flavour
     def _engines(self):
         return [self.opt._allreducer._engines.get(b.name) for b in self.opt._buckets]
+
+    def _full_key(self, flavour: Tuple) -> Tuple:
+        """The graph key: the flavour, and for AN4 the padded input shape before it."""
+        return (self._shape, flavour) if self.an4 else flavour
 
     def _key(self, counters=None) -> Tuple:
         """The flavour of the step the engines are about to run (or would run at the given iteration counters): the
@@ -76,8 +111,9 @@ class GraphedTrainStep:
         real = [e.host.counter for e in engines]
         real_opt = getattr(self.opt, "counter", None)
         made = 0
-        for key, it in self._sparse_flavours().items():
-            if key in self.graphs or key == ("nograph",):
+        for flavour, it in self._sparse_flavours().items():
+            key = self._full_key(flavour)
+            if key in self.graphs or flavour == ("nograph",):
                 continue
             for e in engines:
                 e.host.counter = cfg.warmup_iters + it
@@ -89,13 +125,17 @@ class GraphedTrainStep:
             if not ok:
                 break
             made += 1
-        self._precaptured = True
-        # every long-lived object of the training process exists now (model, optimizer state, engines, graphs): move them
-        # to the permanent generation so that the cyclic collector's full passes stop walking them -- a generation-2
-        # collection otherwise stalls a 1.2 ms step loop for tens of milliseconds
-        import gc
-        gc.collect()
-        gc.freeze()
+        first = not self._precaptured_shapes
+        self._precaptured_shapes.add(self._shape)
+        if first:
+            # every long-lived object of the training process exists now (model, optimizer state, engines, graphs): move
+            # them to the permanent generation so that the cyclic collector's full passes stop walking them -- a
+            # generation-2 collection otherwise stalls a 1.2 ms step loop for tens of milliseconds.  Once only: a later
+            # padded AN4 length adds a few graphs and static inputs, not worth a pause of that size each, and freezing
+            # again would also pin whatever garbage exists at that moment
+            import gc
+            gc.collect()
+            gc.freeze()
         return made
 
     # ------------------------------------------------------------------ one step
@@ -112,24 +152,39 @@ class GraphedTrainStep:
         (self.opt.scale_loss(loss) if getattr(self.opt, "_ls", None) is not None else loss).backward()
 
     def step(self, batch) -> torch.Tensor:
-        """Run one optimizer step on ``batch`` (device tensors); returns the (device) loss."""
+        """Run one optimizer step on ``batch`` (device tensors; an AN4 batch is staged by the trainer first); returns the
+        (device) loss."""
+        if self.an4:
+            batch = self.tr.stage_batch(batch)
         if not self.enabled or self.eager_left > 0:
             self.eager_left -= 1
             return self._eager(batch)
-        key = self._key()
-        if key == ("nograph",):
+        flavour = self._key()
+        if flavour == ("nograph",):
             return self._eager(batch)
-        if self.static_in is None:
-            self.static_in = tuple(t.clone() if torch.is_tensor(t) else t for t in batch)
-        for s, t in zip(self.static_in, batch):
+        shape = None
+        if self.an4:
+            if batch.over_capacity:
+                self.fallbacks["targets"] += 1
+                return self._eager(batch)
+            shape = tuple(batch.inputs.shape)
+            if shape not in self._static_of and len(self._static_of) >= MAX_AN4_SHAPES:
+                self.fallbacks["shapes"] += 1
+                return self._eager(batch)
+        static = self._static_of.get(shape)
+        if static is None:
+            static = self._static_of[shape] = _clone(batch)
+        for s, t in zip(static, batch):
             if torch.is_tensor(t):
                 if s.shape != t.shape:
                     self.enabled, self.why_disabled = False, "batch shape changed"
                     return self._eager(batch)
                 s.copy_(t, non_blocking=True)
+        self.static_in, self._shape = static, shape
+        key = self._full_key(flavour)
         self.opt.refresh_lr()
-        if not self._precaptured and all(plan.kind != "dense" for plan in key[1:]):
-            self.precapture_sparse()             # first sparse step: capture every flavour of the schedule at once
+        if shape not in self._precaptured_shapes and all(plan.kind != "dense" for plan in flavour[1:]):
+            self.precapture_sparse()             # first sparse step (of this shape): capture every flavour at once
         g = self.graphs.get(key)
         if g is None:
             g = self._capture(key)

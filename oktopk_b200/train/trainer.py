@@ -52,7 +52,12 @@ class Trainer:
                  seed: int = 0, prefix: str = "run", log_dir: Optional[str] = None, num_workers: int = 0,
                  seq_len: int = 128, t_total: int = -1, warmup: float = -1, pretrain: Optional[str] = None,
                  norm_clip: Optional[float] = None, backend: Optional[str] = None, cuda_graph: bool = False,
-                 model_kwargs: Optional[dict] = None, autocast: Optional[str] = None, loss_scale=None):
+                 model_kwargs: Optional[dict] = None, autocast: Optional[str] = None, loss_scale=None,
+                 an4_pad_multiple: int = 0):
+        """``an4_pad_multiple=m >= 1`` (AN4 only; 0, the default, is off): every training batch is staged into a
+        ``data.PaddedAN4Batch`` with its frames padded up to a multiple of m and its lengths on the device, and with
+        ``cuda_graph`` the steps are captured per padded length (``GraphedTrainStep``).  The padded frames change one
+        thing: the batch-norm layers count them in their statistics, as they count the padding inside a batch."""
         self.world = world or _world()
         self.rank, self.nworkers = self.world.rank, self.world.size
         # The host side of a step is tiny tensor ops (collate 16 images, one pinned copy): on a many-core box an
@@ -67,6 +72,11 @@ class Trainer:
                 torch.set_num_threads(want)
         self.dnn = dnn
         self.dataset = (dataset or _DATASET_OF.get(dnn, "cifar10")).lower()
+        if an4_pad_multiple < 0 or (an4_pad_multiple and self.dataset != "an4"):
+            raise ValueError("an4_pad_multiple must be 0 (off) or, for the AN4 dataset, >= 1; got %r for %s"
+                             % (an4_pad_multiple, self.dataset))
+        self.an4_pad_multiple = int(an4_pad_multiple)
+        self._an4_out_frames: Dict[int, int] = {}
         self.batch_size, self.lr, self.nsteps_update, self.max_epochs = batch_size, lr, nsteps_update, max_epochs
         self.device = device or (torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available()
                                  else torch.device("cpu"))
@@ -144,9 +154,11 @@ class Trainer:
         self.host_us = {"next": 0.0, "launch": 0.0, "stage_next": 0.0, "steps": 0}
         self.sparsities: List[float] = []
         self._iter_times: List[float] = []
-        # whole-step CUDA graphs (fixed-shape workloads only; AN4 batches vary in length, PTB carries hidden state)
+        # whole-step CUDA graphs: fixed-shape workloads, and AN4 when its batches are padded to a few lengths (one set of
+        # graphs per padded length); unpadded AN4 batches vary in length, and PTB carries hidden state
         self.graphed = None
-        if cuda_graph and self.device.type == "cuda" and self.dataset not in ("an4", "ptb") and nsteps_update == 1:
+        graph_ok = self.dataset != "ptb" and (self.dataset != "an4" or self.an4_pad_multiple >= 1)
+        if cuda_graph and self.device.type == "cuda" and graph_ok and nsteps_update == 1:
             from .graph_step import GraphedTrainStep
             self.graphed = GraphedTrainStep(self)
 
@@ -181,6 +193,20 @@ class Trainer:
         return lr
 
     # ------------------------------------------------------------------ one micro-step: forward + backward
+    def stage_batch(self, batch):
+        """The batch as a step takes it: with ``an4_pad_multiple`` an AN4 batch becomes a ``data.PaddedAN4Batch``
+        (device ops only); anything else, or a batch already staged, is returned as it is."""
+        if not self.an4_pad_multiple or isinstance(batch, D.PaddedAN4Batch):
+            return batch
+        return D.pad_an4_batch(batch, self.an4_pad_multiple, self.an4_out_frames)
+
+    def an4_out_frames(self, frames: int) -> int:
+        """The AN4 model's output frames for ``frames`` input frames (a host computation, cached)."""
+        n = self._an4_out_frames.get(frames)
+        if n is None:
+            n = self._an4_out_frames[frames] = int(self.net.get_seq_lens(torch.tensor([frames]))[0])
+        return n
+
     def _forward_loss(self, batch):
         if self.autocast is not None:
             with torch.autocast(self.device.type, dtype=self.autocast):
@@ -192,9 +218,17 @@ class Trainer:
             ids, seg, mask, labels, nxt = batch
             return self.net(ids, seg, mask, labels, nxt), None
         if self.dataset == "an4":
-            inputs, targets, in_pct, tsizes = batch
-            lengths = (in_pct * inputs.size(3)).int()
-            out, out_lens = self.net(inputs, lengths)
+            if isinstance(batch, D.PaddedAN4Batch):
+                inputs, targets, tsizes = batch.inputs, batch.targets, batch.tsizes
+                # device lengths wherever every layer is fused; the stock layers read them on the host
+                dev = self.net.device_lengths_error(inputs.is_cuda, torch.is_autocast_enabled("cuda")) is None
+                out, out_lens = self.net(inputs, batch.lengths, device_lengths=dev)
+                if not (getattr(self.net, "fuse_ctc", False) and targets.is_cuda):
+                    targets = targets[:batch.ntargets]     # the stock loss wants exactly the batch's targets
+            else:
+                inputs, targets, in_pct, tsizes = batch
+                lengths = (in_pct * inputs.size(3)).int()
+                out, out_lens = self.net(inputs, lengths)
             if getattr(self.net, "fuse_ctc", False):
                 return ctc_loss(out.transpose(0, 1), targets, out_lens, tsizes) / inputs.size(0), None
             logp = F.log_softmax(out.transpose(0, 1), dim=-1)          # T x N x C
@@ -234,7 +268,7 @@ class Trainer:
         for _ in range(num_of_iters):
             self.adjust_learning_rate()
             t0 = time.perf_counter()
-            batch = self.prefetch.next(defer=True)
+            batch = self.stage_batch(self.prefetch.next(defer=True))
             self.timers.add("io", time.perf_counter() - t0)
             loss, aux = self._forward_loss(batch)
             self.backward(loss)
