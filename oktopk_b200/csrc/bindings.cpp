@@ -739,6 +739,37 @@ static void ctc_backward(uint64_t x, uint64_t t, int t64, uint64_t tn, uint64_t 
                            P_<const float>(ws), P_<float>(ab), P_<const float>(g), P_<void>(dx), T, N, C, nt, dtype_arg(dtype, "ctc_backward"), S_(stream)),
        "ctc_backward");
 }
+// Batch-norm over the frames of the longest utterance (csrc/frame_bn.cu): conv = 1, x [N, C, F, Tb] with the conv
+// blocks' masked Hardtanh; conv = 0, x [Tb, N, C].  x / y / dy / dx of type dtype (codes as dtype_arg); len [N] int32;
+// gamma ... dbeta [C] fp32; nbt one int64 or 0.
+static void frame_bn_check(const char* what, int conv, int N, int C, int F, int Tb, int dtype,
+                           std::initializer_list<uint64_t> elems, std::initializer_list<uint64_t> ptrs) {
+    if (!frame_bn_supported(conv, N, C, F, Tb))
+        throw std::runtime_error(std::string(what) + ": needs N, C, F, Tb > 0 and fewer than 2^24 elements per channel");
+    for (uint64_t p : ptrs)
+        if (p == 0 || (p & 3)) throw std::runtime_error(std::string(what) + ": null or misaligned pointer");
+    for (uint64_t p : elems)
+        if (p == 0 || (p & (dtype == 0 ? 3 : 1))) throw std::runtime_error(std::string(what) + ": null or misaligned tensor");
+}
+static void frame_bn_forward(int conv, uint64_t x, uint64_t len, uint64_t gamma, uint64_t beta, uint64_t y, uint64_t mean,
+                             uint64_t rstd, uint64_t rmean, uint64_t rvar, uint64_t nbt, int N, int C, int F, int Tb,
+                             double eps, double momentum, int dtype, uint64_t stream) {
+    frame_bn_check("frame_bn_forward", conv, N, C, F, Tb, dtype, {x, y}, {len, gamma, beta, mean, rstd, rmean, rvar});
+    if (nbt & 7) throw std::runtime_error("frame_bn_forward: misaligned num_batches_tracked");
+    ck(launch_frame_bn_forward(conv, P_<const void>(x), P_<const int>(len), P_<const float>(gamma), P_<const float>(beta),
+                               P_<void>(y), P_<float>(mean), P_<float>(rstd), P_<float>(rmean), P_<float>(rvar),
+                               P_<long long>(nbt), N, C, F, Tb, (float)eps, (float)momentum,
+                               dtype_arg(dtype, "frame_bn_forward"), S_(stream)), "frame_bn_forward");
+}
+static void frame_bn_backward(int conv, uint64_t x, uint64_t dy, uint64_t len, uint64_t gamma, uint64_t beta, uint64_t mean,
+                              uint64_t rstd, uint64_t dx, uint64_t dgamma, uint64_t dbeta, int N, int C, int F, int Tb,
+                              int dtype, uint64_t stream) {
+    frame_bn_check("frame_bn_backward", conv, N, C, F, Tb, dtype, {x, dy, dx}, {len, gamma, beta, mean, rstd, dgamma, dbeta});
+    ck(launch_frame_bn_backward(conv, P_<const void>(x), P_<const void>(dy), P_<const int>(len), P_<const float>(gamma),
+                                P_<const float>(beta), P_<const float>(mean), P_<const float>(rstd), P_<void>(dx),
+                                P_<float>(dgamma), P_<float>(dbeta), N, C, F, Tb, dtype_arg(dtype, "frame_bn_backward"),
+                                S_(stream)), "frame_bn_backward");
+}
 // Fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels [R] int64, rows [M] int32, tgt [M]
 // int64, slot [R] int32, count one int64, overflow one int64 or 0; x / dx [R, H] and out / dout [M, H] of type dtype.
 static void mlm_select(uint64_t labels, uint64_t rows, uint64_t tgt, uint64_t slot, uint64_t count, uint64_t overflow,
@@ -999,6 +1030,14 @@ PYBIND11_MODULE(_C, m) {
           py::arg("ws"), py::arg("ab"), py::arg("g"), py::arg("dx"), py::arg("T"), py::arg("N"), py::arg("C"), py::arg("nt"),
           py::arg("dtype"), py::arg("stream"));
     m.def("ctc_supported", &ctc_supported);
+    m.def("frame_bn_forward", &frame_bn_forward, py::arg("conv"), py::arg("x"), py::arg("len"), py::arg("gamma"),
+          py::arg("beta"), py::arg("y"), py::arg("mean"), py::arg("rstd"), py::arg("rmean"), py::arg("rvar"),
+          py::arg("nbt"), py::arg("N"), py::arg("C"), py::arg("F"), py::arg("Tb"), py::arg("eps"), py::arg("momentum"),
+          py::arg("dtype"), py::arg("stream"));
+    m.def("frame_bn_backward", &frame_bn_backward, py::arg("conv"), py::arg("x"), py::arg("dy"), py::arg("len"),
+          py::arg("gamma"), py::arg("beta"), py::arg("mean"), py::arg("rstd"), py::arg("dx"), py::arg("dgamma"),
+          py::arg("dbeta"), py::arg("N"), py::arg("C"), py::arg("F"), py::arg("Tb"), py::arg("dtype"), py::arg("stream"));
+    m.def("frame_bn_supported", &frame_bn_supported);
     m.def("ctc_workspace_floats", &ctc_workspace_floats);
     m.def("ctc_ab_floats", &ctc_ab_floats);
     m.def("mlm_select", &mlm_select, py::arg("labels"), py::arg("rows"), py::arg("tgt"), py::arg("slot"), py::arg("count"),

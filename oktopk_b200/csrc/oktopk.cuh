@@ -446,6 +446,18 @@ cudaError_t launch_ctc_forward(const void* x, const void* targets, int targets64
 cudaError_t launch_ctc_backward(const void* x, const void* targets, int targets64, const int* tn, const int* ln,
                                 const float* ws, float* ab, const float* g, void* dx, int T, int N, int C, long long nt,
                                 Dtype dtype, cudaStream_t stream);
+// batch-norm over the frames of the longest utterance, training mode (csrc/frame_bn.cu): conv = 1 takes x [N, C, F, Tb]
+// and applies the masked Hardtanh(0, 20) of DeepSpeech's conv blocks; conv = 0 takes x [Tb, N, C] (F ignored).  x, y,
+// dy and dx of type `dtype` (a Dtype); len [N] int32 on the device; gamma, beta, mean, rstd, rmean, rvar, dgamma and
+// dbeta [C] fp32; nbt one int64 (num_batches_tracked) or null.  Needs frame_bn_supported.  One launch each.
+bool frame_bn_supported(int conv, int N, int C, int F, int Tb);
+cudaError_t launch_frame_bn_forward(int conv, const void* x, const int* len, const float* gamma, const float* beta,
+                                    void* y, float* mean, float* rstd, float* rmean, float* rvar, long long* nbt,
+                                    int N, int C, int F, int Tb, float eps, float momentum, Dtype dtype,
+                                    cudaStream_t stream);
+cudaError_t launch_frame_bn_backward(int conv, const void* x, const void* dy, const int* len, const float* gamma,
+                                     const float* beta, const float* mean, const float* rstd, void* dx, float* dgamma,
+                                     float* dbeta, int N, int C, int F, int Tb, Dtype dtype, cudaStream_t stream);
 // fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels and tgt int64, rows [M] and slot
 // [R] int32, count one int64, overflow one int64 that accumulates max(count - M, 0) (or null); x [R, H] and out [M, H],
 // dout [M, H] and dx [R, H] of type `dtype` (a Dtype).  One launch each.

@@ -28,8 +28,8 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     ``fuse_emb=True`` ``net.fuse_emb``; for
     ``lstman4``,
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
-    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``) and ``fuse_ctc=True``
-    ``net.fuse_ctc``; for ``lstm`` (PTB),
+    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``), ``fuse_ctc=True``
+    ``net.fuse_ctc`` and ``fuse_bn=True`` ``net.fuse_bn``; for ``lstm`` (PTB),
     ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_fp32=True`` ``net.fuse_lstm_fp32`` and ``fuse_xent=True``
     ``net.fuse_xent``."""
     ext = None

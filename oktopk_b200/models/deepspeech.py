@@ -15,6 +15,12 @@ The bidirectional network (``bidirectional=True``) keeps stock layers under ``fu
 ``fuse_lstm_bidirectional=True`` (``net.fuse_lstm_bidirectional``) is set as well, which runs both directions of each
 layer in one launch of the kernels.  ``fuse_ctc=True`` (``net.fuse_ctc``, a plain attribute) asks the trainer to compute
 the CTC loss with the fused softmax + CTC kernels (``ops/fused_ctc``); it does not change the network.
+``fuse_bn=True`` (or ``net.fuse_bn = True`` at any time) runs the seven batch-norm sites on the kernels of
+``ops/fused_frame_bn.py``: each conv block's mask -> BatchNorm2d -> mask -> Hardtanh -> mask in one kernel per pass, and
+the BatchNorm1d in front of LSTM layers 1-4 and of ``fc`` likewise, with the lengths copied to the device once per
+forward pass and shared with the LSTM layers.  Their statistics stop at the longest utterance, so a batch padded past it
+(``Trainer(an4_pad_multiple=m)``) gives the unpadded batch's loss and gradients to rounding.  Off the kernels' domain (CPU, eval mode, ...)
+those sites are the stock modules.
 """
 from __future__ import annotations
 
@@ -25,6 +31,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.fused_frame_bn import conv_block_bn, seq_bn
 from ..ops.fused_lstm import lstm_layer, lstm_layer_device, lstm_stack, stock_layer
 
 AN4_LABELS = "_'ABCDEFGHIJKLMNOPQRSTUVWXYZ "     # 29 symbols, index 0 = CTC blank
@@ -37,7 +44,15 @@ class _TimeMaskedConv(nn.Module):
         super().__init__()
         self.seq_module = seq
 
-    def forward(self, x: torch.Tensor, lengths: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, lengths: torch.Tensor,
+                bn_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``bn_lengths`` (the lengths on ``x``'s device): each Conv2d is followed by ``conv_block_bn`` on the
+        BatchNorm2d in place of the mask / batch-norm / Hardtanh modules."""
+        if bn_lengths is not None:
+            mods = list(self.seq_module)
+            for conv, bn in zip(mods[0::3], mods[1::3]):
+                x = conv_block_bn(conv(x), bn, bn_lengths)
+            return x
         t = torch.arange(x.size(3), device=x.device).view(1, 1, 1, -1)
         for m in self.seq_module:
             x = m(x)
@@ -54,9 +69,16 @@ class _SeqBN(nn.Module):
         super().__init__()
         self.module = module
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, bn_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``bn_lengths`` (the lengths on ``x``'s device): the batch-norm (the module, or the first of a Sequential)
+        runs as ``seq_bn``."""
         t, n = x.size(0), x.size(1)
-        return self.module(x.reshape(t * n, -1)).view(t, n, -1)
+        if bn_lengths is None:
+            return self.module(x.reshape(t * n, -1)).view(t, n, -1)
+        if isinstance(self.module, nn.Sequential):
+            x = seq_bn(x, self.module[0], bn_lengths)
+            return self.module[1:](x.reshape(t * n, -1)).view(t, n, -1)
+        return seq_bn(x, self.module, bn_lengths)
 
 
 class BatchRNN(nn.Module):
@@ -77,14 +99,15 @@ class BatchRNN(nn.Module):
         self.rnn = rnn_type(input_size=input_size, hidden_size=hidden_size, bidirectional=bidirectional, bias=True)
 
     def forward(self, x: torch.Tensor, lengths: Optional[torch.Tensor],
-                dev_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """``lengths``: host int tensor; ``dev_lengths``: optionally the same as int32 on the device (fused path).
+                dev_lengths: Optional[torch.Tensor] = None, bn_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``lengths``: host int tensor; ``dev_lengths``: optionally the same as int32 on the device (fused path);
+        ``bn_lengths``: the same on ``x``'s device, to run the batch-norm as ``seq_bn``.
         ``lengths=None``: the lengths are ``dev_lengths`` only and are never read on the host (``lstm_layer_device``);
         the layer must then take the fused kernels, else ``RuntimeError``."""
         if lengths is None and not self.fuse:
             raise RuntimeError("device-only lengths need the fused LSTM layer (fuse_lstm)")
         if self.batch_norm is not None:
-            x = self.batch_norm(x)
+            x = self.batch_norm(x, bn_lengths)
         if lengths is None:
             return lstm_layer_device(x, dev_lengths, self.rnn, autocast=self.fuse_autocast,
                                      bidirectional=self.fuse_bidirectional)
@@ -116,7 +139,7 @@ class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
                  window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-                 fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False):
+                 fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -142,6 +165,17 @@ class DeepSpeech(nn.Module):
         self.fuse_lstm_autocast = fuse_lstm_autocast
         self.fuse_lstm_bidirectional = fuse_lstm_bidirectional
         self.fuse_ctc = fuse_ctc
+        self.fuse_bn = fuse_bn
+
+    @property
+    def fuse_bn(self) -> bool:
+        """Whether the batch-norm sites take the fused kernels of ``ops/fused_frame_bn.py``, with statistics over the
+        frames of the longest utterance."""
+        return self._fuse_bn
+
+    @fuse_bn.setter
+    def fuse_bn(self, on: bool) -> None:
+        self._fuse_bn = bool(on)
 
     @property
     def fuse_lstm(self) -> bool:
@@ -214,16 +248,19 @@ class DeepSpeech(nn.Module):
     def _forward(self, x: torch.Tensor, out_lens: torch.Tensor,
                  host_lens: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
         """``out_lens`` on the host (``host_lens`` the same tensor) or on the device only (``host_lens`` None)."""
-        x = self.conv(x, out_lens)
+        # the fused batch-norm and LSTM layers read the lengths on the device: one copy for all of them
+        bn_lens = out_lens.to(x.device) if self.fuse_bn else None
+        x = self.conv(x, out_lens, bn_lens)
         b, c, d, t = x.size()
         x = x.view(b, c * d, t).permute(2, 0, 1).contiguous()        # T x N x H
-        # the fused layers read the lengths on the device: one copy for all of them
-        dev_lens = out_lens.to(x.device) if x.is_cuda and any(m.fuse for m in self.rnns) else None
+        dev_lens = None
+        if x.is_cuda and any(m.fuse for m in self.rnns):
+            dev_lens = bn_lens if bn_lens is not None else out_lens.to(x.device)
         for rnn in self.rnns:
-            x = rnn(x, host_lens, dev_lens)
+            x = rnn(x, host_lens, dev_lens, bn_lens)
         if self.lookahead is not None:
             x = self.lookahead(x)
-        x = self.fc(x).transpose(0, 1)                                # N x T x classes
+        x = self.fc(x, bn_lens).transpose(0, 1)                       # N x T x classes
         if not self.training:
             x = F.softmax(x, dim=-1)
         return x, out_lens
@@ -231,11 +268,11 @@ class DeepSpeech(nn.Module):
 
 def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
             fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-            fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False) -> DeepSpeech:
+            fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
     return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
                       fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast,
-                      fuse_lstm_bidirectional=fuse_lstm_bidirectional, fuse_ctc=fuse_ctc)
+                      fuse_lstm_bidirectional=fuse_lstm_bidirectional, fuse_ctc=fuse_ctc, fuse_bn=fuse_bn)
 
 
 class PTBLSTM(nn.Module):

@@ -69,7 +69,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "(default: stock modules under fp16; a ResNet also needs --fused-bn)")
     p.add_argument("--fused-bn", action="store_true",
                    help="CIFAR ResNets (resnet20 ... resnet110): every conv -> BN [+ shortcut] -> ReLU takes the fused "
-                        "batch-norm kernels (default: stock modules; VGG always fuses)")
+                        "batch-norm kernels (default: stock modules; VGG always fuses).  lstman4: the seven batch-norm "
+                        "sites take the fused kernels, their statistics over the frames of the longest utterance, so "
+                        "--an4-pad-multiple no longer changes them (default: stock modules)")
     p.add_argument("--fused-ln", action="store_true",
                    help="BERT: both LayerNorm(x + dropout(a)) sites of every encoder layer take the fused dropout + "
                         "residual + LayerNorm kernels (default: stock ops)")
@@ -109,7 +111,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--an4-pad-multiple", type=int, default=0, metavar="M",
                    help="lstman4: pad every training batch's frames up to a multiple of M and keep its lengths on the "
                         "device; with --cuda-graph, --fused-lstm and --fused-ctc the steps are captured in CUDA graphs, "
-                        "one set per padded length.  The batch-norm statistics count the padded frames (default: 0, off)")
+                        "one set per padded length.  The batch-norm statistics count the padded frames unless --fused-bn is "
+                        "on (default: 0, off)")
     p.add_argument("--bidirectional", action="store_true",
                    help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
                         "(default: uni-directional)")
@@ -175,10 +178,11 @@ def model_args(args: argparse.Namespace):
 
 
 def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-bn`` is for the CIFAR ResNets only; on one of them, ``--fused-bn-fp16`` needs it."""
+    """``--fused-bn`` is for the CIFAR ResNets and lstman4 only; on one of the ResNets, ``--fused-bn-fp16`` needs it."""
     from ..models import FUSED_BN_RESNETS
-    if args.fused_bn and args.dnn not in FUSED_BN_RESNETS:
-        parser.error("--fused-bn applies to %s (VGG fuses by default), not %s" % (", ".join(FUSED_BN_RESNETS), args.dnn))
+    if args.fused_bn and args.dnn not in FUSED_BN_RESNETS + ("lstman4",):
+        parser.error("--fused-bn applies to %s and lstman4 (VGG fuses by default), not %s"
+                     % (", ".join(FUSED_BN_RESNETS), args.dnn))
     if args.fused_bn_fp16 and args.dnn in FUSED_BN_RESNETS and not args.fused_bn:
         parser.error("--fused-bn-fp16 on %s needs --fused-bn" % args.dnn)
 

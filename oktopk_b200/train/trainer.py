@@ -56,8 +56,10 @@ class Trainer:
                  an4_pad_multiple: int = 0):
         """``an4_pad_multiple=m >= 1`` (AN4 only; 0, the default, is off): every training batch is staged into a
         ``data.PaddedAN4Batch`` with its frames padded up to a multiple of m and its lengths on the device, and with
-        ``cuda_graph`` the steps are captured per padded length (``GraphedTrainStep``).  The padded frames change one
-        thing: the batch-norm layers count them in their statistics, as they count the padding inside a batch."""
+        ``cuda_graph`` the steps are captured per padded length (``GraphedTrainStep``).  With the stock batch-norm the
+        padded frames change one thing: those layers count them in their statistics, as they count the padding inside a
+        batch.  With ``fuse_bn`` (``model_kwargs``) the statistics stop at the longest utterance and the padded batch
+        gives the unpadded batch's loss and gradients to rounding."""
         self.world = world or _world()
         self.rank, self.nworkers = self.world.rank, self.world.size
         # The host side of a step is tiny tensor ops (collate 16 images, one pinned copy): on a many-core box an
