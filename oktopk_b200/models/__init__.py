@@ -9,35 +9,27 @@ from .deepspeech import DeepSpeech, lstman4, PTBLSTM, AN4_LABELS      # noqa: F4
 from .bert import (BertConfig, BertForPreTraining, bert_base, build_stages, synthetic_batch as bert_synthetic_batch,  # noqa: F401
                    StartingStage, IntermediateStage, EndingStage, PretrainingCriterion)
 from . import zoo
+from .switches import FUSED_BN_RESNETS, SWITCH_MODELS                 # noqa: F401
 
 DNNS = ["vgg16", "vgg19", "vgg11", "vgg13", "resnet20", "resnet32", "resnet44", "resnet56", "resnet110",
         "preresnet110", "resnext29", "densenet100", "caffe_cifar", "alexnet", "resnet18", "resnet34", "resnet50",
         "resnet101", "resnet152", "mnistnet", "lstman4", "lstm", "bert_base", "bert"]
 
 
-# the ResNets whose batch-norms take the fused kernels with ``fuse_bn=True`` (VGG fuses by default; the ImageNet
-# ResNets keep the stock modules, see ROADMAP)
-FUSED_BN_RESNETS = ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110")
-
-
 def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
-    """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  For the ResNets of
-    ``FUSED_BN_RESNETS``, ``fuse_bn=True`` turns on ``net.fuse`` (and ``fuse_fp16=True`` ``net.fuse_fp16``); for BERT,
-    ``fuse_ln=True`` turns on ``net.fuse_ln``, ``fuse_xent=True`` ``net.fuse_xent`` and ``sparse_mlm=True``
-    ``net.sparse_mlm`` (``mlm_capacity=F`` sets ``net.mlm_capacity``), ``fuse_attn=True`` ``net.fuse_attn`` and
-    ``fuse_emb=True`` ``net.fuse_emb``; for
-    ``lstman4``,
-    ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_autocast=True`` ``net.fuse_lstm_autocast`` and
-    ``fuse_lstm_bidirectional=True`` ``net.fuse_lstm_bidirectional`` (with ``bidirectional=True``), ``fuse_ctc=True``
-    ``net.fuse_ctc`` and ``fuse_bn=True`` ``net.fuse_bn``; for ``lstm`` (PTB),
-    ``fuse_lstm=True`` turns on ``net.fuse_lstm``, ``fuse_lstm_fp32=True`` ``net.fuse_lstm_fp32`` and ``fuse_xent=True``
-    ``net.fuse_xent``."""
+    """Returns ``(net, ext)`` like the reference (``ext`` carries e.g. the AN4 label set).  The opt-in switches, such as
+    ``fuse_bn=True``, and the models that take each are listed in ``switches.py``; a switch the model does not take
+    raises ``ValueError``."""
     ext = None
     d = dnn.lower()
+    switches = {k: kwargs.pop(k) for k in list(kwargs) if k in SWITCH_MODELS}
+    for k in switches:
+        if d not in SWITCH_MODELS[k]:
+            raise ValueError("%s applies to %s, not %s" % (k, ", ".join(SWITCH_MODELS[k]), dnn))
     if d.startswith("vgg"):
-        net = VGG(d, num_classes, fuse_fp16=bool(kwargs.get("fuse_fp16", False)))
+        net = VGG(d, num_classes, **switches)
     elif d in ("resnet20", "resnet32", "resnet44", "resnet56", "resnet110"):
-        net = zoo.CifarResNet(int(d[6:]), num_classes)
+        net = zoo.CifarResNet(int(d[6:]), num_classes, **switches)
     elif d.startswith("preresnet"):
         net = zoo.PreResNet(int(d[9:]), num_classes)
     elif d == "resnext29":
@@ -53,17 +45,10 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
     elif d == "mnistnet":
         net = zoo.MnistNet()
     elif d == "lstman4":
-        kw = dict(kwargs)
-        fuse_lstm = bool(kw.pop("fuse_lstm", False))
-        fuse_ctc = bool(kw.pop("fuse_ctc", False))
-        net = lstman4(**kw)
-        net.fuse_lstm = fuse_lstm
-        net.fuse_ctc = fuse_ctc
+        net = lstman4(**kwargs, **switches)
         ext = {"labels": AN4_LABELS}
     elif d == "lstm":
-        net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20),
-                      fuse_lstm=bool(kwargs.get("fuse_lstm", False)), fuse_xent=bool(kwargs.get("fuse_xent", False)),
-                      fuse_lstm_fp32=bool(kwargs.get("fuse_lstm_fp32", False)))
+        net = PTBLSTM(vocab_size=kwargs.get("vocab_size", 10000), batch_size=kwargs.get("batch_size", 20), **switches)
     elif d in ("bert", "bert_base"):
         cfg = kwargs.get("config")
         if isinstance(cfg, str):
@@ -73,15 +58,7 @@ def create_net(num_classes: int, dnn: str = "resnet20", **kwargs):
             import dataclasses
             cfg = dataclasses.replace(cfg, num_hidden_layers=int(kwargs["num_hidden_layers"]))
         net = BertForPreTraining(cfg, kwargs.get("depth", 4), recompute=bool(kwargs.get("recompute", False)),
-                                 fuse_ln=bool(kwargs.get("fuse_ln", False)),
-                                 fuse_xent=bool(kwargs.get("fuse_xent", False)),
-                                 sparse_mlm=bool(kwargs.get("sparse_mlm", False)),
-                                 mlm_capacity=float(kwargs.get("mlm_capacity", 0.25)),
-                                 fuse_attn=bool(kwargs.get("fuse_attn", False)),
-                                 fuse_emb=bool(kwargs.get("fuse_emb", False)))
+                                 **switches)
     else:
         raise ValueError("unknown dnn %r (have %s)" % (dnn, DNNS))
-    if d in FUSED_BN_RESNETS:
-        net.fuse = bool(kwargs.get("fuse_bn", False))
-        net.fuse_fp16 = bool(kwargs.get("fuse_fp16", False))
     return net, ext

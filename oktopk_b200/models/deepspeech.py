@@ -164,7 +164,7 @@ class DeepSpeech(nn.Module):
         self.fuse_lstm = fuse_lstm
         self.fuse_lstm_autocast = fuse_lstm_autocast
         self.fuse_lstm_bidirectional = fuse_lstm_bidirectional
-        self.fuse_ctc = fuse_ctc
+        self.fuse_ctc = bool(fuse_ctc)
         self.fuse_bn = fuse_bn
 
     @property
@@ -289,9 +289,9 @@ class PTBLSTM(nn.Module):
                  num_layers: int = 2, dp_keep_prob: float = 0.35, fuse_lstm: bool = False, fuse_xent: bool = False,
                  fuse_lstm_fp32: bool = False):
         super().__init__()
-        self.fuse_lstm = fuse_lstm
-        self.fuse_lstm_fp32 = fuse_lstm_fp32
-        self.fuse_xent = fuse_xent
+        self.fuse_lstm = bool(fuse_lstm)
+        self.fuse_lstm_fp32 = bool(fuse_lstm_fp32)
+        self.fuse_xent = bool(fuse_xent)
         self.embedding_dim, self.num_layers = embedding_dim, num_layers
         self.dropout = nn.Dropout(1 - dp_keep_prob)
         self.word_embeddings = nn.Embedding(vocab_size, embedding_dim)

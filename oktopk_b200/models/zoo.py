@@ -46,9 +46,9 @@ class CifarResNet(nn.Module):
     the fused batch-norm kernels in training on the GPU, ``net.fuse_fp16`` adds fp16 activations to that path (as for
     VGG).  The option-A shortcut (stride slice + channel zero-pad) stays stock torch ops."""
 
-    def __init__(self, depth: int = 20, num_classes: int = 10):
+    def __init__(self, depth: int = 20, num_classes: int = 10, fuse_bn: bool = False, fuse_fp16: bool = False):
         super().__init__()
-        self.fuse, self.fuse_fp16 = False, False
+        self.fuse, self.fuse_fp16 = bool(fuse_bn), bool(fuse_fp16)
         assert (depth - 2) % 6 == 0
         n = (depth - 2) // 6
         self.stem = nn.Sequential(nn.Conv2d(3, 16, 3, 1, 1, bias=False), nn.BatchNorm2d(16), nn.ReLU(inplace=True))

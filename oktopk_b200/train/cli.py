@@ -19,6 +19,8 @@ import sys
 
 import torch
 
+from ..models.switches import FP16, FP32, FUSED_BN_RESNETS, HALF, SWITCHES
+
 
 def build_parser() -> argparse.ArgumentParser:
     from ..compression import compressors
@@ -64,61 +66,11 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--cuda-graph", action="store_true", help="capture forward+backward+allreduce+update into CUDA graphs")
     p.add_argument("--fp16", action="store_true", help="fp16 autocast (reference: apex amp O3, main_bert.py:1009-1023)")
     p.add_argument("--bf16", action="store_true", help="bf16 autocast")
-    p.add_argument("--fused-bn-fp16", action="store_true",
-                   help="with --fp16: VGG's Conv -> BN -> ReLU [-> pool] blocks take the fused fp16 batch-norm kernels "
-                        "(default: stock modules under fp16; a ResNet also needs --fused-bn)")
-    p.add_argument("--fused-bn", action="store_true",
-                   help="CIFAR ResNets (resnet20 ... resnet110): every conv -> BN [+ shortcut] -> ReLU takes the fused "
-                        "batch-norm kernels (default: stock modules; VGG always fuses).  lstman4: the seven batch-norm "
-                        "sites take the fused kernels, their statistics over the frames of the longest utterance, so "
-                        "--an4-pad-multiple no longer changes them (default: stock modules)")
-    p.add_argument("--fused-ln", action="store_true",
-                   help="BERT: both LayerNorm(x + dropout(a)) sites of every encoder layer take the fused dropout + "
-                        "residual + LayerNorm kernels (default: stock ops)")
-    p.add_argument("--fused-xent", action="store_true",
-                   help="BERT: the masked-LM loss takes the fused softmax cross-entropy kernels, which read only the "
-                        "labelled rows (default: stock cross_entropy)")
-    p.add_argument("--sparse-mlm", action="store_true",
-                   help="BERT: the masked-LM head (transform, LayerNorm, decoder GEMM) runs on the labelled rows only, "
-                        "gathered into a fixed number of rows (default: every token row)")
-    p.add_argument("--mlm-capacity", type=float, default=None,
-                   help="with --sparse-mlm: the gathered rows as a fraction of the batch's tokens, rounded up to a "
-                        "multiple of 8 (default 0.25; labelled rows past it stop training with an error; 1.0 never "
-                        "overflows)")
-    p.add_argument("--fused-attn", action="store_true",
-                   help="BERT: the self-attention of every encoder layer takes the fused attention kernels, which read "
-                        "the packed QKV projection and regenerate the dropout mask (default: stock "
-                        "scaled_dot_product_attention)")
-    p.add_argument("--fused-emb", action="store_true",
-                   help="BERT: the embedding sum + LayerNorm + dropout runs on the fused embedding kernels, one kernel "
-                        "forward and the table gradients without a sort (default: stock ops)")
-    p.add_argument("--fused-lstm", action="store_true",
-                   help="lstman4: the LSTM layers run on the persistent fused recurrence kernels, one launch per layer "
-                        "and pass, instead of packed sequences through cuDNN (default: stock)")
-    p.add_argument("--fused-lstm-lm", action="store_true",
-                   help="lstm (PTB), with --bf16 or --fp16: the stacked LSTM runs on the 16-bit stacked-layer fused "
-                        "recurrence kernels, the hidden state carried in and out (default: stock cuDNN layer)")
-    p.add_argument("--fused-lstm-lm-fp32", action="store_true",
-                   help="lstm (PTB), in fp32 (no --bf16 / --fp16): the stacked LSTM runs on the fp32 stacked-layer fused "
-                        "recurrence kernels, W_hh partly read from L2 every step, the step product in 3xTF32 "
-                        "(default: stock cuDNN layer)")
-    p.add_argument("--fused-lstm-autocast", action="store_true",
-                   help="with --fused-lstm and --bf16 or --fp16: the LSTM layers take the 16-bit fused recurrence kernels "
-                        "(default: stock layers under autocast)")
-    p.add_argument("--fused-ctc", action="store_true",
-                   help="lstman4: the CTC loss runs on the fused softmax + CTC kernels, the lengths read on the device "
-                        "and the backward deterministic (default: stock log_softmax + nn.CTCLoss)")
-    p.add_argument("--an4-pad-multiple", type=int, default=0, metavar="M",
-                   help="lstman4: pad every training batch's frames up to a multiple of M and keep its lengths on the "
-                        "device; with --cuda-graph, --fused-lstm and --fused-ctc the steps are captured in CUDA graphs, "
-                        "one set per padded length.  The batch-norm statistics count the padded frames unless --fused-bn is "
-                        "on (default: 0, off)")
-    p.add_argument("--bidirectional", action="store_true",
-                   help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
-                        "(default: uni-directional)")
-    p.add_argument("--fused-lstm-bidirectional", action="store_true",
-                   help="with --fused-lstm and --bidirectional: both directions of each LSTM layer run on the fused "
-                        "recurrence kernels in one launch (default: stock bidirectional layers)")
+    for sw in SWITCHES:
+        if sw.type is None:
+            p.add_argument(sw.flag, action="store_true", help=sw.help)
+        else:
+            p.add_argument(sw.flag, type=sw.type, default=sw.default, metavar=sw.metavar, help=sw.help)
     p.add_argument("--loss-scale", type=str, default=None,
                    help="loss scaling: 'dynamic' (torch GradScaler's rule, checked on the device) or a fixed scale; off by default")
     p.add_argument("--recompute_step", action="store_true", help="activation recomputation in the BERT encoder")
@@ -146,108 +98,48 @@ def model_args(args: argparse.Namespace):
         model_kwargs["config"] = cfg_path
     if args.recompute_step:
         model_kwargs["recompute"] = True
-    if args.fused_bn_fp16:
-        model_kwargs["fuse_fp16"] = True
-    if args.fused_bn:
-        model_kwargs["fuse_bn"] = True
-    if args.fused_ln:
-        model_kwargs["fuse_ln"] = True
-    if args.fused_xent:
-        model_kwargs["fuse_xent"] = True
-    if args.sparse_mlm:
-        model_kwargs["sparse_mlm"] = True
-    if args.mlm_capacity is not None:
-        model_kwargs["mlm_capacity"] = args.mlm_capacity
-    if args.fused_attn:
-        model_kwargs["fuse_attn"] = True
-    if args.fused_emb:
-        model_kwargs["fuse_emb"] = True
-    if args.fused_lstm or args.fused_lstm_lm or args.fused_lstm_lm_fp32:
-        model_kwargs["fuse_lstm"] = True
-    if args.fused_lstm_lm_fp32:
-        model_kwargs["fuse_lstm_fp32"] = True
-    if args.fused_lstm_autocast:
-        model_kwargs["fuse_lstm_autocast"] = True
-    if args.bidirectional:
-        model_kwargs["bidirectional"] = True
-    if args.fused_lstm_bidirectional:
-        model_kwargs["fuse_lstm_bidirectional"] = True
-    if args.fused_ctc:
-        model_kwargs["fuse_ctc"] = True
+    for sw in SWITCHES:
+        value = getattr(args, sw.dest)
+        if value != sw.default:
+            model_kwargs.update(dict.fromkeys(sw.keywords, value))
     return dnn, model_kwargs
 
 
-def check_fused_bn_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-bn`` is for the CIFAR ResNets and lstman4 only; on one of the ResNets, ``--fused-bn-fp16`` needs it."""
-    from ..models import FUSED_BN_RESNETS
-    if args.fused_bn and args.dnn not in FUSED_BN_RESNETS + ("lstman4",):
-        parser.error("--fused-bn applies to %s and lstman4 (VGG fuses by default), not %s"
-                     % (", ".join(FUSED_BN_RESNETS), args.dnn))
-    if args.fused_bn_fp16 and args.dnn in FUSED_BN_RESNETS and not args.fused_bn:
-        parser.error("--fused-bn-fp16 on %s needs --fused-bn" % args.dnn)
-
-
-def check_fused_ln_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-ln``, ``--sparse-mlm``, ``--mlm-capacity``, ``--fused-attn`` and ``--fused-emb`` are for BERT only (``--dnn bert_base``
-    / ``bert``, or a ``--module models.bertN.depth=M``), ``--fused-xent`` for BERT and the PTB model (``--dnn lstm``);
-    ``--mlm-capacity`` needs ``--sparse-mlm`` and a value in (0, 1]."""
+def check_switch_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
+    """Each switch flag of ``models/switches.py`` that is given must apply to the model that ``model_args`` resolves
+    (``--dnn``, or ``--module``), and come with the flags and the precision it needs."""
     dnn = model_args(args)[0]
-    if args.fused_xent and dnn not in ("bert", "bert_base", "lstm"):
-        parser.error("--fused-xent applies to BERT (bert_base, bert) and lstm, not %s" % dnn)
-    for flag, on in (("--fused-ln", args.fused_ln), ("--sparse-mlm", args.sparse_mlm),
-                     ("--mlm-capacity", args.mlm_capacity is not None), ("--fused-attn", args.fused_attn),
-                     ("--fused-emb", args.fused_emb)):
-        if on and dnn not in ("bert", "bert_base"):
-            parser.error("%s applies to BERT (bert_base, bert), not %s" % (flag, dnn))
-    if args.mlm_capacity is not None:
-        if not args.sparse_mlm:
-            parser.error("--mlm-capacity needs --sparse-mlm")
-        if not 0.0 < args.mlm_capacity <= 1.0:
-            parser.error("--mlm-capacity must be in (0, 1], got %r" % args.mlm_capacity)
-
-
-def check_fused_lstm_args(parser: argparse.ArgumentParser, args: argparse.Namespace) -> None:
-    """``--fused-lstm`` and ``--bidirectional`` are for the AN4 DeepSpeech model (``--dnn lstman4``) only;
-    ``--fused-lstm-autocast`` needs ``--fused-lstm`` and one of ``--bf16`` / ``--fp16``; ``--fused-lstm-bidirectional``
-    needs ``--fused-lstm`` and ``--bidirectional``.  ``--fused-lstm-lm`` is for the PTB model (``--dnn lstm``) and
-    needs ``--bf16`` or ``--fp16``; ``--fused-lstm-lm-fp32`` is for the PTB model too, in fp32 only.  ``--fused-ctc`` is
-    for ``lstman4`` only, as is ``--an4-pad-multiple`` (>= 0)."""
-    if args.fused_lstm and model_args(args)[0] != "lstman4":
-        parser.error("--fused-lstm applies to lstman4, not %s" % model_args(args)[0])
-    if args.fused_lstm_lm and model_args(args)[0] != "lstm":
-        parser.error("--fused-lstm-lm applies to lstm, not %s" % model_args(args)[0])
-    if args.fused_lstm_lm and not (args.bf16 or args.fp16):
-        parser.error("--fused-lstm-lm needs --bf16 or --fp16")
-    if args.fused_lstm_lm_fp32 and model_args(args)[0] != "lstm":
-        parser.error("--fused-lstm-lm-fp32 applies to lstm, not %s" % model_args(args)[0])
-    if args.fused_lstm_lm_fp32 and (args.bf16 or args.fp16):
-        parser.error("--fused-lstm-lm-fp32 runs fp32: with --bf16 or --fp16 use --fused-lstm-lm")
-    if args.fused_lstm_autocast and not args.fused_lstm:
-        parser.error("--fused-lstm-autocast needs --fused-lstm")
-    if args.fused_lstm_autocast and not (args.bf16 or args.fp16):
-        parser.error("--fused-lstm-autocast needs --bf16 or --fp16")
-    if args.bidirectional and model_args(args)[0] != "lstman4":
-        parser.error("--bidirectional applies to lstman4, not %s" % model_args(args)[0])
-    if args.fused_lstm_bidirectional and not args.fused_lstm:
-        parser.error("--fused-lstm-bidirectional needs --fused-lstm")
-    if args.fused_lstm_bidirectional and not args.bidirectional:
-        parser.error("--fused-lstm-bidirectional needs --bidirectional")
-    if args.fused_ctc and model_args(args)[0] != "lstman4":
-        parser.error("--fused-ctc applies to lstman4, not %s" % model_args(args)[0])
-    if args.an4_pad_multiple and model_args(args)[0] != "lstman4":
-        parser.error("--an4-pad-multiple applies to lstman4, not %s" % model_args(args)[0])
+    given = {sw.flag for sw in SWITCHES if getattr(args, sw.dest) != sw.default}
+    half = args.bf16 or args.fp16
+    for sw in SWITCHES:
+        if sw.flag not in given:
+            continue
+        if dnn not in sw.models:
+            parser.error("%s applies to %s, not %s" % (sw.flag, ", ".join(sw.models), dnn))
+        for need in sw.needs:
+            if need not in given:
+                parser.error("%s needs %s" % (sw.flag, need))
+        if (sw.precision == FP16 and not args.fp16) or (sw.precision == HALF and not half):
+            parser.error("%s needs %s" % (sw.flag, sw.precision))
+        if sw.precision == FP32 and half:
+            alt = next(o.flag for o in SWITCHES if o.precision == HALF and o.models == sw.models)
+            parser.error("%s runs fp32: with --bf16 or --fp16 use %s" % (sw.flag, alt))
+    if args.fused_bn_fp16 and dnn in FUSED_BN_RESNETS and not args.fused_bn:
+        parser.error("--fused-bn-fp16 on %s needs --fused-bn" % dnn)
+    if args.mlm_capacity is not None and not 0.0 < args.mlm_capacity <= 1.0:
+        parser.error("--mlm-capacity must be in (0, 1], got %r" % args.mlm_capacity)
     if args.an4_pad_multiple < 0:
         parser.error("--an4-pad-multiple must be >= 1 (or 0, off), got %d" % args.an4_pad_multiple)
+
+
+# the names of the per-family checks that check_switch_args replaced, kept for their callers: each checks every switch
+check_fused_bn_args = check_fused_ln_args = check_fused_lstm_args = check_switch_args
 
 
 def main(argv=None) -> int:
     parser = build_parser()
     args = parser.parse_args(argv)
-    if args.fused_bn_fp16 and not args.fp16:
-        parser.error("--fused-bn-fp16 needs --fp16")
-    check_fused_bn_args(parser, args)
-    check_fused_ln_args(parser, args)
-    check_fused_lstm_args(parser, args)
+    check_switch_args(parser, args)
     import oktopk_b200 as okt
     from .trainer import preset_for, robust_ssgd
     okt.init()

@@ -81,11 +81,10 @@ def test_create_net_and_the_cli_flag():
     assert create_net(29, "lstman4", fuse_bn=True, fuse_lstm=True)[0].fuse_bn is True
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "lstman4", "--fused-bn"])
-    cli.check_fused_bn_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"fuse_bn": True})
     args = p.parse_args(["--dnn", "lstman4", "--fused-bn", "--fused-lstm", "--fused-ctc", "--an4-pad-multiple", "32"])
-    cli.check_fused_bn_args(p, args)
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"fuse_bn": True, "fuse_lstm": True, "fuse_ctc": True})
     for bad in (["--dnn", "vgg16", "--fused-bn"], ["--dnn", "lstm", "--fused-bn"], ["--dnn", "bert_base", "--fused-bn"],
                 ["--dnn", "resnet50", "--fused-bn"], ["--dnn", "resnet20", "--fp16", "--fused-bn-fp16"]):

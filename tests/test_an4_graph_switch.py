@@ -124,13 +124,13 @@ def test_trainer_rejects_the_option_off_an4():
 def test_cli_flag():
     parser = cli.build_parser()
     args = parser.parse_args(["--dnn", "lstman4", "--an4-pad-multiple", "32"])
-    cli.check_fused_lstm_args(parser, args)
+    cli.check_switch_args(parser, args)
     assert args.an4_pad_multiple == 32
     assert parser.parse_args(["--dnn", "lstman4"]).an4_pad_multiple == 0
     for argv in (["--dnn", "vgg16", "--an4-pad-multiple", "32"], ["--dnn", "lstman4", "--an4-pad-multiple", "-1"]):
         args = parser.parse_args(argv)
         with pytest.raises(SystemExit):
-            cli.check_fused_lstm_args(parser, args)
+            cli.check_switch_args(parser, args)
 
 
 def _padded_against_unpadded(device, model_kwargs, frozen_bn):

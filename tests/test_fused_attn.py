@@ -340,16 +340,23 @@ def test_fallbacks_run_the_stock_ops(case):
     dout = torch.randn(B, S, H * dh, device="cuda", dtype=dtype)
     n0 = _counts()
     res = []
-    for fused in (True, False):
-        torch.manual_seed(3)
-        if fused:
-            res.append(_run(lambda x: self_attention(x, H, mask, p), qkv, dout))
-        else:
-            def stock(x):
-                q, k, v = x.view(B, S, 3, H, dh).permute(2, 0, 3, 1, 4)
-                o = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)
-                return o.transpose(1, 2).reshape(B, S, H * dh)
-            res.append(_run(stock, qkv, dout))
+    # stock SDPA's memory-efficient backward sums over key blocks in a varying order unless deterministic algorithms
+    # are on, so without them two stock runs can differ in the last bit
+    old = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(True)
+    try:
+        for fused in (True, False):
+            torch.manual_seed(3)
+            if fused:
+                res.append(_run(lambda x: self_attention(x, H, mask, p), qkv, dout))
+            else:
+                def stock(x):
+                    q, k, v = x.view(B, S, 3, H, dh).permute(2, 0, 3, 1, 4)
+                    o = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)
+                    return o.transpose(1, 2).reshape(B, S, H * dh)
+                res.append(_run(stock, qkv, dout))
+    finally:
+        torch.use_deterministic_algorithms(old)
     assert _delta(n0) == {"attn_forward": 0, "attn_backward": 0}
     for u, v in zip(*res):                              # p = 1: stock returns NaN (0 / 0), and so must the fallback
         torch.testing.assert_close(u, v, rtol=0, atol=0, equal_nan=True)

@@ -75,10 +75,10 @@ def test_fuse_attn_is_a_run_time_switch():
 def test_cli_fused_attn_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "bert_base", "--fused-attn"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"fuse_attn": True})
     args = p.parse_args(["--module", "models.bert12.depth=4", "--fused-attn", "--fused-ln", "--recompute_step"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"num_hidden_layers": 12, "depth": 4, "recompute": True,
                                                   "fuse_ln": True, "fuse_attn": True})
     assert cli.model_args(p.parse_args(["--dnn", "bert"])) == ("bert", {})

@@ -37,10 +37,10 @@ def test_fuse_bn_is_a_run_time_switch_and_carries_fuse_fp16():
 def test_cli_fused_bn_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "resnet20", "--fused-bn"])
-    cli.check_fused_bn_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("resnet20", {"fuse_bn": True})
     args = p.parse_args(["--dnn", "resnet56", "--fp16", "--fused-bn", "--fused-bn-fp16"])
-    cli.check_fused_bn_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("resnet56", {"fuse_fp16": True, "fuse_bn": True})
     assert cli.model_args(p.parse_args(["--dnn", "resnet20"])) == ("resnet20", {})
     for bad in (["--dnn", "vgg16", "--fused-bn"], ["--dnn", "preresnet110", "--fused-bn"],

@@ -119,7 +119,7 @@ def test_fallbacks_call_the_stock_expression(case):
 def test_cli_fused_ctc_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "lstman4", "--fused-ctc"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"fuse_ctc": True})
     args = p.parse_args(["--dnn", "lstman4", "--fused-ctc", "--fused-lstm"])
     assert cli.model_args(args) == ("lstman4", {"fuse_lstm": True, "fuse_ctc": True})

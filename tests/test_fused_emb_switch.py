@@ -89,10 +89,10 @@ def test_glue_models_take_the_switch():
 def test_cli_fused_emb_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "bert_base", "--fused-emb"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"fuse_emb": True})
     args = p.parse_args(["--module", "models.bert12.depth=4", "--fused-emb", "--fused-ln"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"num_hidden_layers": 12, "depth": 4, "fuse_ln": True,
                                                   "fuse_emb": True})
     assert cli.model_args(p.parse_args(["--dnn", "bert"])) == ("bert", {})

@@ -90,7 +90,7 @@ def test_cli_fused_lstm_autocast_flag(capsys):
     p = cli.build_parser()
     for prec in ("--bf16", "--fp16"):
         args = p.parse_args(["--dnn", "lstman4", "--fused-lstm", "--fused-lstm-autocast", prec])
-        cli.check_fused_lstm_args(p, args)
+        cli.check_switch_args(p, args)
         assert cli.model_args(args) == ("lstman4", {"fuse_lstm": True, "fuse_lstm_autocast": True})
     for bad, word in ((["--dnn", "lstman4", "--fused-lstm-autocast", "--bf16"], "needs --fused-lstm"),
                       (["--dnn", "lstman4", "--fused-lstm", "--fused-lstm-autocast"], "needs --bf16 or --fp16")):

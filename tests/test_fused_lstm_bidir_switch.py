@@ -88,15 +88,15 @@ def test_create_net_and_factory_carry_the_keyword():
 def test_cli_bidirectional_flags(capsys):
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "lstman4", "--bidirectional"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"bidirectional": True})
     args = p.parse_args(["--dnn", "lstman4", "--fused-lstm", "--bidirectional", "--fused-lstm-bidirectional"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"fuse_lstm": True, "bidirectional": True,
                                                 "fuse_lstm_bidirectional": True})
     args = p.parse_args(["--dnn", "lstman4", "--fused-lstm", "--bidirectional", "--fused-lstm-bidirectional",
                          "--fused-lstm-autocast", "--bf16"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args)[1] == {"fuse_lstm": True, "fuse_lstm_autocast": True, "bidirectional": True,
                                        "fuse_lstm_bidirectional": True}
     for bad, word in ((["--dnn", "vgg16", "--bidirectional"], "--bidirectional applies to lstman4"),

@@ -124,11 +124,10 @@ def test_cpu_is_exactly_the_stock_model(flags):
 def test_cli_fused_lstm_lm_fp32_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "lstm", "--fused-lstm-lm-fp32"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstm", {"fuse_lstm": True, "fuse_lstm_fp32": True})
     args = p.parse_args(["--dnn", "lstm", "--fused-lstm-lm-fp32", "--fused-xent"])
-    cli.check_fused_ln_args(p, args)
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstm", {"fuse_xent": True, "fuse_lstm": True, "fuse_lstm_fp32": True})
     args = p.parse_args(["--dnn", "lstm", "--bf16", "--fused-lstm-lm"])
     assert "fuse_lstm_fp32" not in cli.model_args(args)[1]
@@ -139,5 +138,5 @@ def test_cli_fused_lstm_lm_fp32_flag():
                      (["--dnn", "lstm", "--fused-lstm-lm"], "needs --bf16 or --fp16")):
         args = p.parse_args(bad)
         with mock.patch.object(p, "error", side_effect=SystemExit) as err, pytest.raises(SystemExit):
-            cli.check_fused_lstm_args(p, args)
+            cli.check_switch_args(p, args)
         assert msg in err.call_args[0][0], (bad, err.call_args)

@@ -125,14 +125,13 @@ def test_cli_fused_lstm_lm_and_fused_xent_flags():
     p = cli.build_parser()
     for argv in (["--dnn", "lstm", "--bf16", "--fused-lstm-lm"], ["--dnn", "lstm", "--fp16", "--fused-lstm-lm"]):
         args = p.parse_args(argv)
-        cli.check_fused_lstm_args(p, args)
+        cli.check_switch_args(p, args)
         assert cli.model_args(args) == ("lstm", {"fuse_lstm": True})
     args = p.parse_args(["--dnn", "lstm", "--bf16", "--fused-lstm-lm", "--fused-xent"])
-    cli.check_fused_ln_args(p, args)
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstm", {"fuse_xent": True, "fuse_lstm": True})
     args = p.parse_args(["--dnn", "lstm", "--fused-xent"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstm", {"fuse_xent": True})
     for bad in (["--dnn", "lstm", "--fused-lstm-lm"],                              # no 16-bit autocast
                 ["--dnn", "lstman4", "--bf16", "--fused-lstm-lm"],

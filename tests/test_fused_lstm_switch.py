@@ -98,7 +98,7 @@ def test_geometry_accepts_deepspeech_and_rejects_ptb():
 def test_cli_fused_lstm_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "lstman4", "--fused-lstm"])
-    cli.check_fused_lstm_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("lstman4", {"fuse_lstm": True})
     args = p.parse_args(["--dnn", "lstman4"])
     assert cli.model_args(args) == ("lstman4", {})

@@ -123,10 +123,10 @@ def test_fallbacks_call_stock_cross_entropy(case):
 def test_cli_fused_xent_flag():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "bert_base", "--fused-xent"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"fuse_xent": True})
     args = p.parse_args(["--module", "models.bert12.depth=4", "--fused-xent", "--fused-ln"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"num_hidden_layers": 12, "depth": 4, "fuse_ln": True,
                                                   "fuse_xent": True})
     for bad in (["--dnn", "vgg16", "--fused-xent"], ["--dnn", "resnet20", "--fused-xent"]):

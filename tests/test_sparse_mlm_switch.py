@@ -186,10 +186,10 @@ def test_masked_lm_model_switch():
 def test_cli_sparse_mlm_flags():
     p = cli.build_parser()
     args = p.parse_args(["--dnn", "bert_base", "--sparse-mlm"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"sparse_mlm": True})
     args = p.parse_args(["--module", "models.bert12.depth=4", "--sparse-mlm", "--mlm-capacity", "0.5", "--fused-xent"])
-    cli.check_fused_ln_args(p, args)
+    cli.check_switch_args(p, args)
     assert cli.model_args(args) == ("bert_base", {"num_hidden_layers": 12, "depth": 4, "fuse_xent": True,
                                                   "sparse_mlm": True, "mlm_capacity": 0.5})
     for bad in (["--dnn", "vgg16", "--sparse-mlm"], ["--dnn", "lstman4", "--sparse-mlm", "--mlm-capacity", "0.5"],
