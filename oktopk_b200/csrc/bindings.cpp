@@ -498,11 +498,11 @@ static void kth_abs(uint64_t x, int n, int k, uint64_t st, uint64_t out, int gri
 
 static void fused_sgd(uint64_t p, uint64_t g, uint64_t mom, int n, double momentum, double dampening, double wd,
                       int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
-                      uint64_t skip_ptr) {
+                      uint64_t skip_ptr, uint64_t coef_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_sgd: scal_ptr must point at the group's device scalars");
     ck(launch_fused_sgd(P_<float>(p), P_<float>(g), P_<float>(mom), n, (float)momentum, (float)dampening, (float)wd,
                         nesterov, first, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
-                        S_(stream)),
+                        P_<const float>(coef_ptr), S_(stream)),
        "fused_sgd");
 }
 // [(lo, hi), ...] element ranges of an n-element (bucket, param group) slice, at multiples of 4 and inside its whole
@@ -537,30 +537,34 @@ static void fused_sgd_tail(uint64_t p, uint64_t g, uint64_t mom, uint64_t sp, ui
                            const std::vector<std::pair<long long, long long>>& ahead,
                            const std::vector<std::pair<long long, long long>>& dense, double momentum, double dampening,
                            double wd, int nesterov, int first, int zero_grad, uint64_t stream, uint64_t scal_ptr,
-                           uint64_t fault_ptr, uint64_t skip_ptr) {
+                           uint64_t fault_ptr, uint64_t skip_ptr, uint64_t coef_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_sgd_tail: scal_ptr must point at the group's device scalars");
     if (momentum != 0.0 && (mom == 0 || sm == 0)) throw std::runtime_error("fused_sgd_tail: momentum needs mom and sm");
     const SgdHyper h{(float)momentum, (float)dampening, (float)wd, nesterov, first};
     ck(launch_fused_sgd_tail(P_<float>(p), P_<float>(g), P_<float>(mom), P_<const float>(sp), P_<const float>(sm), n,
                              sgd_ranges(ahead, n, "fused_sgd_tail"), sgd_ranges(dense, n, "fused_sgd_tail"), h,
-                             zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
+                             zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
+                             P_<const float>(coef_ptr), S_(stream)),
        "fused_sgd_tail");
 }
 static void fused_bert_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double b1, double b2, double eps,
                             double wd, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
-                            uint64_t skip_ptr) {
+                            uint64_t skip_ptr, uint64_t coef_ptr, uint64_t ends_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_bert_adam: scal_ptr must point at the group's device scalars");
+    if (ends_ptr != 0 && coef_ptr == 0) throw std::runtime_error("fused_bert_adam: segment ends need the factors");
+    const ClipRef clip{P_<const float>(coef_ptr), P_<const int>(ends_ptr)};
     ck(launch_fused_bert_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, (float)b1, (float)b2,
                               (float)eps, (float)wd, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
-                              S_(stream)),
+                              clip, S_(stream)),
        "fused_bert_adam");
 }
 static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double beta1, double beta2, double eps,
                        double wd, int decoupled, int zero_grad, uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr,
-                       uint64_t skip_ptr) {
+                       uint64_t skip_ptr, uint64_t coef_ptr) {
     if (scal_ptr == 0) throw std::runtime_error("fused_adam: scal_ptr must point at the group's device scalars");
     ck(launch_fused_adam(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, beta1, beta2, (float)eps, (float)wd,
-                         decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr), S_(stream)),
+                         decoupled, zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
+                         P_<const float>(coef_ptr), S_(stream)),
        "fused_adam");
 }
 // dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case).
@@ -870,9 +874,41 @@ static void maxpool2_bwd(uint64_t dy, uint64_t arg, uint64_t dx, int N, int H, i
 static void momentum_correct(uint64_t g, uint64_t buf, int n, double momentum, uint64_t stream) {
     ck(launch_momentum_correct(P_<float>(g), P_<float>(buf), n, (float)momentum, S_(stream)), "momentum_correct");
 }
-static void clip_by_norm(uint64_t x, int n, uint64_t scratch, double max_norm, uint64_t stream) {
-    ck(launch_l2norm_sq(P_<float>(x), n, P_<float>(scratch), S_(stream)), "l2norm");
-    ck(launch_scale(P_<float>(x), n, P_<float>(scratch), (float)max_norm, S_(stream)), "clip scale");
+// Sum of squares of the segments (offsets, lengths) of the flat fp32 bucket g into partial[0, P), P = the sum over
+// segments of max(1, ceil(len / SUMSQ_CHUNK)), in segment order.  More than kSrcSegMax segments take one launch per
+// kSrcSegMax of them, each writing the next partials.
+static void grad_sumsq(uint64_t g, const std::vector<long long>& offs, const std::vector<long long>& lens,
+                       uint64_t partial, uint64_t stream) {
+    const size_t T = offs.size();
+    if (lens.size() != T || T == 0) throw std::runtime_error("grad_sumsq: bad segment table");
+    if (g % 16 || partial % 8) throw std::runtime_error("grad_sumsq: misaligned bucket or partials");
+    double* out = P_<double>(partial);
+    for (size_t b = 0; b < T; b += kSrcSegMax) {
+        SumsqSegs t;
+        std::memset(&t, 0, sizeof(t));
+        t.nseg = (int)std::min<size_t>(kSrcSegMax, T - b);
+        long long blk = 0;
+        for (int i = 0; i < t.nseg; ++i) {
+            const long long o = offs[b + i], l = lens[b + i];
+            if (o < 0 || o % 4 || l < 0 || o + l > (1LL << 31) - 1)
+                throw std::runtime_error("grad_sumsq: segments must lie at multiples of 4 inside an int32 range");
+            t.off[i] = (int)o;
+            t.len[i] = (int)l;
+            t.blk_begin[i] = (int)blk;
+            blk += std::max(1LL, (l + kSumsqChunk - 1) / kSumsqChunk);
+        }
+        t.blk_begin[t.nseg] = (int)blk;
+        ck(launch_grad_sumsq(P_<const float>(g), t, out, S_(stream)), "grad_sumsq");
+        out += blk;
+    }
+}
+static void clip_coef(uint64_t partial, int np, uint64_t seg_blk, uint64_t seg_scal, int nseg, uint64_t scal,
+                      double max_norm, uint64_t norm, uint64_t coef, uint64_t stream) {
+    if (seg_blk != 0 && (seg_scal == 0 || scal == 0 || nseg <= 0))
+        throw std::runtime_error("clip_coef: per-segment factors need seg_scal, scal and nseg");
+    ck(launch_clip_coef(P_<const double>(partial), np, P_<const int>(seg_blk), P_<const int>(seg_scal), nseg,
+                        P_<const float>(scal), (float)max_norm, P_<float>(norm), P_<float>(coef), S_(stream)),
+       "clip_coef");
 }
 
 // ------------------------------------------------------------------------------------------- loss scaling
@@ -953,21 +989,28 @@ PYBIND11_MODULE(_C, m) {
     m.def("kth_abs", &kth_abs);
     m.def("fused_sgd", &fused_sgd, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("n"), py::arg("momentum"),
           py::arg("dampening"), py::arg("wd"), py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"),
-          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0,
+          py::arg("coef_ptr") = 0);
     m.def("sgd_ahead", &sgd_ahead, py::arg("p"), py::arg("mom"), py::arg("sp"), py::arg("sm"), py::arg("n"),
           py::arg("ranges"), py::arg("momentum"), py::arg("dampening"), py::arg("wd"), py::arg("nesterov"),
           py::arg("max_ctas"), py::arg("stream"), py::arg("scal_ptr"));
     m.def("fused_sgd_tail", &fused_sgd_tail, py::arg("p"), py::arg("g"), py::arg("mom"), py::arg("sp"), py::arg("sm"),
           py::arg("n"), py::arg("ahead"), py::arg("dense"), py::arg("momentum"), py::arg("dampening"), py::arg("wd"),
           py::arg("nesterov"), py::arg("first"), py::arg("zero_grad"), py::arg("stream"), py::arg("scal_ptr"),
-          py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
+          py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0, py::arg("coef_ptr") = 0);
     m.def("fused_bert_adam", &fused_bert_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("zero_grad"), py::arg("stream"),
-          py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
+          py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0, py::arg("coef_ptr") = 0,
+          py::arg("ends_ptr") = 0);
     m.def("fused_adam", &fused_adam, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
           py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("decoupled"), py::arg("zero_grad"),
-          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0);
+          py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0,
+          py::arg("coef_ptr") = 0);
     m.def("momentum_correct", &momentum_correct);
+    m.def("grad_sumsq", &grad_sumsq, py::arg("g"), py::arg("offs"), py::arg("lens"), py::arg("partial"),
+          py::arg("stream"));
+    m.def("clip_coef", &clip_coef, py::arg("partial"), py::arg("np"), py::arg("seg_blk"), py::arg("seg_scal"),
+          py::arg("nseg"), py::arg("scal"), py::arg("max_norm"), py::arg("norm"), py::arg("coef"), py::arg("stream"));
     m.def("unscale_check", &unscale_check);
     m.def("scale_update", [](uint64_t ls, double growth, double backoff, int interval, uint64_t stream) {
         ck(launch_scale_update(P_<LossScaleDev>(ls), growth, backoff, interval, S_(stream)), "scale_update");
@@ -1059,11 +1102,11 @@ PYBIND11_MODULE(_C, m) {
           py::arg("c0"), py::arg("dhn"), py::arg("dcn"), py::arg("dg"), py::arg("dc0"), py::arg("bar"), py::arg("T"),
           py::arg("N"), py::arg("H"), py::arg("u"), py::arg("rows"), py::arg("stream"), py::arg("dtype"),
           py::arg("r_on") = 0, py::arg("kc") = 0);
-    m.def("clip_by_norm", &clip_by_norm);
     m.attr("MAXP") = OKT_MAXP;
     m.attr("TRACE_LEN") = kTraceLen;
     m.attr("LAND_MAX") = kLandMax;
     m.attr("SRC_SEG_MAX") = kSrcSegMax;
     m.attr("PACK_RANGE_MAX") = kPackRangeMax;
     m.attr("CHUNK") = kChunk;
+    m.attr("SUMSQ_CHUNK") = kSumsqChunk;
 }

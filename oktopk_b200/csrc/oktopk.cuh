@@ -290,11 +290,39 @@ int gtopk_max_coop_grid(int device);
 int gather_max_coop_grid(int device);
 cudaError_t launch_dense_allreduce(const DenseParams& p, int grid, cudaStream_t stream);
 cudaError_t launch_kth_abs(const float* x, int n, int k, OktState* st, float* out_thr, int grid, cudaStream_t stream);
-// fused optimizer updates: scal -> the step's scalars in device memory ({lr} for SGD and BertAdam); skip -> the step
-// verdict of loss scaling (null = off): when set, p / m / v are left alone and only the gradient is cleared
+// Gradient clipping (optim.cu).  grad_sumsq: the sum of squares of each segment [off, off + len) of a flat fp32 bucket,
+// in fp64, one partial per kSumsqChunk elements of a segment (CTA blk_begin[s] + j covers chunk j of segment s): the
+// partials depend on the lengths alone, and no atomics order them.  A segment is the whole bucket (one norm over every
+// gradient) or one parameter (a norm per parameter).  Offsets are multiples of 4 elements.  Passed by value, like
+// OktParams's source table.
+constexpr int kSumsqChunk = 16384;
+struct SumsqSegs {
+    int nseg;
+    int off[kSrcSegMax];
+    int len[kSrcSegMax];
+    int blk_begin[kSrcSegMax + 1];
+};
+static_assert(sizeof(SumsqSegs) <= 4096, "SumsqSegs must fit the 4 KB kernel-parameter limit");
+cudaError_t launch_grad_sumsq(const float* g, const SumsqSegs& t, double* partial, cudaStream_t stream);
+// One CTA: the norm and the clip factor from the partials, summed in a fixed order.  seg_blk null: one norm over
+// partial[0, np), factor min(max_norm / (norm + 1e-6), 1) as torch.nn.utils.clip_grad_norm_ computes it.  Else nseg
+// norms, segment s over partial[seg_blk[s], seg_blk[s + 1]), factor max / (norm + 1e-6) where norm > max > 0 (else 1)
+// with max = scal[seg_scal[s]] (BertAdam's clip_reduced).  norm and coef: one float, or one per segment.
+cudaError_t launch_clip_coef(const double* partial, int np, const int* seg_blk, const int* seg_scal, int nseg,
+                             const float* scal, float max_norm, float* norm, float* coef, cudaStream_t stream);
+// The clip factor an update kernel multiplies the gradient by before its update.  coef null: no clip.  ends null: one
+// factor coef[0].  Else the slice's float4 vectors before ends[t] (and after ends[t - 1]) take coef[t]; the last
+// segment's end is INT_MAX.
+struct ClipRef {
+    const float* coef;
+    const int* ends;
+};
+// fused optimizer updates: scal -> the step's scalars in device memory ({lr} for SGD, {lr, max_grad_norm} for BertAdam);
+// skip -> the step verdict of loss scaling (null = off): when set, p / m / v are left alone and only the gradient is
+// cleared; coef / clip -> the clip factor (null = no clip)
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
-                             const int* skip, cudaStream_t stream);
+                             const int* skip, const float* coef, cudaStream_t stream);
 // Early SGD update (sgd_ahead_kernel / fused_sgd_tail_kernel in optim.cu).  SgdRanges: float4 vector ranges [lo, hi) of a
 // (bucket, param group) slice, in slice order, at most kPackRangeMax of them; SgdHyper: torch.optim.SGD's group options.
 struct SgdRanges {
@@ -315,14 +343,15 @@ cudaError_t launch_sgd_ahead(float* p, float* mom, float* sp, float* sm, const S
 // n-element slice take fused_sgd's update
 cudaError_t launch_fused_sgd_tail(float* p, float* g, float* mom, const float* sp, const float* sm, int n,
                                   const SgdRanges& ahead, const SgdRanges& dense, const SgdHyper& h, int zero_grad,
-                                  const float* scal, const int* fault, const int* skip, cudaStream_t stream);
+                                  const float* scal, const int* fault, const int* skip, const float* coef,
+                                  cudaStream_t stream);
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
                                    float weight_decay, int zero_grad, const float* scal, const int* fault,
-                                   const int* skip, cudaStream_t stream);
+                                   const int* skip, const ClipRef& clip, cudaStream_t stream);
 // torch.optim.Adam / AdamW update; scal -> {1 - lr*wd, -lr / (1 - beta1^t), sqrt(1 - beta2^t)} of this step
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
-                              const int* skip, cudaStream_t stream);
+                              const int* skip, const float* coef, cudaStream_t stream);
 
 // ---- dynamic loss scaling (csrc/scale.cu) ------------------------------------------------------------
 // One per optimizer, in device memory.  found_inf is the step verdict: the OR of the bucket verdicts of the step.
@@ -504,7 +533,5 @@ cudaError_t launch_attn_backward(const void* qkv, const void* out, const void* d
                                  const unsigned long long* seed, const float* lse, float* delta, void* dqkv, int B, int S,
                                  int H, long long keep_thr, float scale, Dtype dtype, cudaStream_t stream);
 cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum, cudaStream_t stream);
-cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream);
-cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream);
 
 }  // namespace okt

@@ -11,17 +11,42 @@ namespace okt {
 
 constexpr int kOptThreads = 256;
 
+// The clip factor of an update, read where update_pass reads the gradient (see ClipRef in oktopk.cuh).  A thread's vector
+// index only grows, so the per-segment lookup is a cursor that steps over the segment ends it passes: no search, no
+// extra pass.
+struct ClipCursor {
+    const float* coef;
+    const int* ends;
+    int t;
+    float f;
+    __device__ __forceinline__ explicit ClipCursor(const ClipRef& c)
+        : coef(c.coef), ends(c.ends), t(0), f(c.coef != nullptr ? c.coef[0] : 1.f) {}
+    __device__ __forceinline__ float at(int vec) {
+        if (ends != nullptr && vec >= __ldg(ends + t)) {
+            do ++t; while (vec >= __ldg(ends + t));
+            f = coef[t];
+        }
+        return f;
+    }
+};
+
+__device__ __forceinline__ void scale4(float4& gw, float c) {
+    gw.x = __fmul_rn(gw.x, c); gw.y = __fmul_rn(gw.y, c); gw.z = __fmul_rn(gw.z, c); gw.w = __fmul_rn(gw.w, c);
+}
+
 // The pass all three update kernels share.  A bounded cross-GPU wait timed out inside the reduction of this bucket: the
 // gradient is partial, do NOT apply it (the host sees the mirrored fault flag at its next step() and re-synchronises the
 // replicas).  Otherwise the kScal per-step scalars are read from device memory (the launch is CUDA-graph replayable)
 // and upd(s, p, g, m, v) updates every element; m and v are its first and, with kState == 2, second state element,
 // loaded when `load` (else 0) and written back when `store`.  Only the non-zero gradient lines are zeroed: the
-// reduced gradient is sparse, ~k/n of the lines are dirty.
+// reduced gradient is sparse, ~k/n of the lines are dirty.  With a clip factor (clip.coef set) upd sees the gradient
+// times the factor, one fp32 multiply as torch's _foreach_mul_ does it; the bucket keeps the unscaled value until it
+// is zeroed.  A skipped step never reads the factor.
 template <int kScal, int kState, typename Upd>
 __device__ __forceinline__ void update_pass(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                                             float* __restrict__ v, int n, bool load, bool store, int zero_grad,
                                             const float* __restrict__ scal, const int* __restrict__ fault,
-                                            const int* __restrict__ skip, Upd upd) {
+                                            const int* __restrict__ skip, const ClipRef clip, Upd upd) {
     if (fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0) return;
     const int n4 = n >> 2;
     float4* p4 = reinterpret_cast<float4*>(p);
@@ -42,8 +67,11 @@ __device__ __forceinline__ void update_pass(float* __restrict__ p, float* __rest
     float s[kScal];
 #pragma unroll
     for (int j = 0; j < kScal; ++j) s[j] = scal[j];
+    ClipCursor cc(clip);
     for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
         float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = zero, vw = zero;
+        const bool dirty = gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f;
+        if (clip.coef != nullptr) scale4(gw, cc.at(i));
         if (load) {
             mw = m4[i];
             if (kState == 2) vw = v4[i];
@@ -55,11 +83,12 @@ __device__ __forceinline__ void update_pass(float* __restrict__ p, float* __rest
             m4[i] = mw;
             if (kState == 2) v4[i] = vw;
         }
-        if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
+        if (zero_grad && dirty) g4[i] = zero;
     }
     if (blockIdx.x == 0)
         for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
             float pw = p[i], gw = g[i], mw = 0.f, vw = 0.f;
+            if (clip.coef != nullptr) gw = __fmul_rn(gw, cc.at(i >> 2));
             if (load) {
                 mw = m[i];
                 if (kState == 2) vw = v[i];
@@ -91,14 +120,16 @@ __device__ __forceinline__ void sgd_update4(const SgdHyper& h, float lr, float4&
     sgd_update(h, lr, pw.z, gw.z, mw.z); sgd_update(h, lr, pw.w, gw.w, mw.w);
 }
 
-// scal -> {lr}
+// scal -> {lr}; coef: the clip factor or null
 __global__ void __launch_bounds__(kOptThreads) fused_sgd_kernel(float* __restrict__ p, float* __restrict__ g,
                                                                  float* __restrict__ mom, int n, const SgdHyper h,
                                                                  int zero_grad, const float* __restrict__ scal,
                                                                  const int* __restrict__ fault,
-                                                                 const int* __restrict__ skip) {
+                                                                 const int* __restrict__ skip,
+                                                                 const float* __restrict__ coef) {
     update_pass<1, 1>(p, g, mom, nullptr, n, h.momentum != 0.f && !h.first, h.momentum != 0.f, zero_grad, scal, fault,
-                      skip, [=](const float* s, float& pw, float gw, float& mw, float&) { sgd_update(h, s[0], pw, gw, mw); });
+                      skip, ClipRef{coef, nullptr},
+                      [=](const float* s, float& pw, float gw, float& mw, float&) { sgd_update(h, s[0], pw, gw, mw); });
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -161,6 +192,8 @@ __device__ __forceinline__ bool any_bits(const float4& v) {
 }
 
 // scal -> {lr}.  A vector is zeroed in g under fused_sgd_kernel's rule (a lane != 0), so the bucket ends up the same too.
+// coef: the clip factor or null.  The ahead pass's zero-gradient update holds for any finite factor (0 * c == 0); a NaN
+// factor reaches every element under torch's multiply, so then every vector of the ahead ranges is recomputed.
 __global__ void __launch_bounds__(kOptThreads) fused_sgd_tail_kernel(float* __restrict__ p, float* __restrict__ g,
                                                                       float* __restrict__ mom,
                                                                       const float* __restrict__ sp,
@@ -169,7 +202,8 @@ __global__ void __launch_bounds__(kOptThreads) fused_sgd_tail_kernel(float* __re
                                                                       const SgdHyper h, int zero_grad,
                                                                       const float* __restrict__ scal,
                                                                       const int* __restrict__ fault,
-                                                                      const int* __restrict__ skip) {
+                                                                      const int* __restrict__ skip,
+                                                                      const float* __restrict__ coef) {
     const bool use_m = h.momentum != 0.f;
     float4* p4 = reinterpret_cast<float4*>(p);
     float4* g4 = reinterpret_cast<float4*>(g);
@@ -188,34 +222,41 @@ __global__ void __launch_bounds__(kOptThreads) fused_sgd_tail_kernel(float* __re
                 if (use_m) m4[i] = sm4[i];
             }
         if (faulted) return;
-        update_pass<1, 1>(p, g, mom, nullptr, n, false, false, zero_grad, scal, nullptr, skip,
+        update_pass<1, 1>(p, g, mom, nullptr, n, false, false, zero_grad, scal, nullptr, skip, ClipRef{nullptr, nullptr},
                           [](const float*, float&, float, float&, float&) {});
         return;
     }
     const float lr = scal[0];
+    const float c = coef != nullptr ? *coef : 1.f;
+    const bool every = c != c;                          // NaN factor
     for (int q = 0; q < ahead.nr; ++q)
         for (int i = ahead.lo[q] + first; i < ahead.hi[q]; i += stride) {
-            const float4 gw = ld_stream_f4(g4 + i);
-            if (!any_bits(gw)) continue;                // the ahead pass's result stands
+            float4 gw = ld_stream_f4(g4 + i);
+            if (!any_bits(gw) && !every) continue;      // the ahead pass's result stands
+            const bool dirty = gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f;
+            if (coef != nullptr) scale4(gw, c);
             float4 pw = sp4[i], mw = zero;
             if (use_m) mw = sm4[i];
             sgd_update4(h, lr, pw, gw, mw);
             p4[i] = pw;
             if (use_m) m4[i] = mw;
-            if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
+            if (zero_grad && dirty) g4[i] = zero;
         }
     for (int q = 0; q < dense.nr; ++q)
         for (int i = dense.lo[q] + first; i < dense.hi[q]; i += stride) {
             float4 pw = p4[i], gw = ld_stream_f4(g4 + i), mw = zero;
+            const bool dirty = gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f;
+            if (coef != nullptr) scale4(gw, c);
             if (use_m && !h.first) mw = m4[i];
             sgd_update4(h, lr, pw, gw, mw);
             p4[i] = pw;
             if (use_m) m4[i] = mw;
-            if (zero_grad && (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f)) g4[i] = zero;
+            if (zero_grad && dirty) g4[i] = zero;
         }
     if (blockIdx.x == 0)
         for (int i = (n >> 2) * 4 + threadIdx.x; i < n; i += kOptThreads) {
             float pw = p[i], gw = g[i], mw = 0.f;
+            if (coef != nullptr) gw = __fmul_rn(gw, c);
             if (use_m && !h.first) mw = mom[i];
             sgd_update(h, lr, pw, gw, mw);
             p[i] = pw;
@@ -224,14 +265,14 @@ __global__ void __launch_bounds__(kOptThreads) fused_sgd_tail_kernel(float* __re
         }
 }
 
-// scal -> {scheduled lr}
+// scal -> {scheduled lr, max_grad_norm}; clip: none, or one factor per parameter (clip_reduced)
 __global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __restrict__ p, float* __restrict__ g,
                                                                        float* __restrict__ m, float* __restrict__ v,
                                                                        int n, float b1, float b2, float eps, float wd,
                                                                        int zero_grad, const float* __restrict__ scal,
                                                                        const int* __restrict__ fault,
-                                                                       const int* __restrict__ skip) {
-    update_pass<1, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip,
+                                                                       const int* __restrict__ skip, const ClipRef clip) {
+    update_pass<1, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip, clip,
                       [=](const float* s, float& pw, float gw, float& mw, float& vw) {
                           mw = b1 * mw + (1.f - b1) * gw;
                           vw = b2 * vw + (1.f - b2) * gw * gw;
@@ -245,7 +286,7 @@ __global__ void __launch_bounds__(kOptThreads) fused_bert_adam_kernel(float* __r
 // step_size = -lr / (1 - beta1^t), bc2_sqrt = sqrt(1 - beta2^t)) are computed on the host in double, so that a captured
 // CUDA graph picks up the schedule and the bias correction of every replay.
 // decoupled: AdamW (p *= 1 - lr*wd) instead of L2 (g += wd*p).  w = 1 - beta1 is the weight of torch's lerp, whose
-// formula depends on whether the weight is below 0.5.  (48 registers, 5 CTAs per SM: capping at 32 for 8 CTAs spills
+// formula depends on whether the weight is below 0.5.  (44 registers, 5 CTAs per SM: capping at 32 for 8 CTAs spills
 // around the IEEE division's slow path.)
 __global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restrict__ p, float* __restrict__ g,
                                                                   float* __restrict__ m, float* __restrict__ v, int n,
@@ -253,10 +294,11 @@ __global__ void __launch_bounds__(kOptThreads) fused_adam_kernel(float* __restri
                                                                   int decoupled, int zero_grad,
                                                                   const float* __restrict__ scal,
                                                                   const int* __restrict__ fault,
-                                                                  const int* __restrict__ skip) {
+                                                                  const int* __restrict__ skip,
+                                                                  const float* __restrict__ coef) {
     const bool small_w = fabsf(w) < 0.5f;
     const float lw = small_w ? w : 1.f - w;
-    update_pass<3, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip,
+    update_pass<3, 2>(p, g, m, v, n, true, true, zero_grad, scal, fault, skip, ClipRef{coef, nullptr},
                       [=](const float* s, float& pw, float gw, float& mw, float& vw) {
                           const float decay = s[0], step_size = s[1], bc2_sqrt = s[2];
                           if (decoupled) pw = pw * decay;                  // decay == 1 exactly when wd == 0
@@ -279,30 +321,84 @@ __global__ void __launch_bounds__(kOptThreads) momentum_correct_kernel(float* __
     }
 }
 
-__global__ void __launch_bounds__(kOptThreads) l2norm_sq_kernel(const float* __restrict__ x, int n, float* out) {
-    double acc = 0.0;
-    for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n; i += gridDim.x * kOptThreads) {
-        double v = (double)x[i];
-        acc += v * v;
-    }
-    acc = warp_sum_d(acc);
-    __shared__ double s[kOptThreads / 32];
-    if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = acc;
+// ------------------------------------------------------------------------------------------------------------
+// Gradient clipping on the device.  grad_sumsq_kernel: one CTA per kSumsqChunk elements of a segment (a fixed function
+// of the segment lengths, not of the device), each writing its sum of squares in fp64 to its own partial: no atomics.
+// Within a CTA thread j sums the float4 vectors j, j + 256, ... and the scalar tail in order, then the warps and the
+// eight warp sums are combined in a fixed tree.  clip_coef_kernel (one CTA) combines the partials in a fixed order too,
+// so the norm and the factor are a function of the gradient's bits alone: bitwise equal buckets give bitwise equal
+// factors on every rank.
+// ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double block_sum_d(double v) {
+    __shared__ double ws[kOptThreads / 32];
+    v = warp_sum_d(v);
+    if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = v;
     __syncthreads();
-    if (threadIdx.x < 32) {
-        double v = (threadIdx.x < kOptThreads / 32) ? s[threadIdx.x] : 0.0;
-        v = warp_sum_d(v);
-        if (threadIdx.x == 0) atomicAdd(out, (float)v);
-    }
+    double t = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < kOptThreads / 32; ++w) t += ws[w];
+    __syncthreads();
+    return t;                                           // thread 0's value
 }
 
-// x *= max_norm / norm  when norm > max_norm (norm^2 is on the device: no host sync)
-__global__ void __launch_bounds__(kOptThreads) clip_scale_kernel(float* __restrict__ x, int n, const float* norm_sq,
-                                                                  float max_norm) {
-    const float nrm = sqrtf(*norm_sq);
-    if (!(nrm > max_norm) || nrm == 0.f) return;
-    const float s = max_norm / nrm;
-    for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n; i += gridDim.x * kOptThreads) x[i] *= s;
+__global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const float* __restrict__ g, const SumsqSegs t,
+                                                                  double* __restrict__ partial) {
+    int lo = 0, hi = t.nseg - 1;                        // this CTA's segment (binary search over the CTA prefix table)
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if ((int)blockIdx.x >= t.blk_begin[mid]) lo = mid; else hi = mid - 1;
+    }
+    const int begin = (blockIdx.x - t.blk_begin[lo]) * kSumsqChunk;
+    const int len = min(t.len[lo] - begin, kSumsqChunk);
+    const float* x = g + t.off[lo] + begin;             // 16-byte aligned: offsets and kSumsqChunk are multiples of 4
+    const float4* x4 = reinterpret_cast<const float4*>(x);
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < (len >> 2); i += kOptThreads) {
+        const float4 w = ld_stream_f4(x4 + i);
+        acc += (double)w.x * w.x;
+        acc += (double)w.y * w.y;
+        acc += (double)w.z * w.z;
+        acc += (double)w.w * w.w;
+    }
+    const int i = (len & ~3) + threadIdx.x;
+    if (i < len) acc += (double)x[i] * x[i];
+    acc = block_sum_d(acc);
+    if (threadIdx.x == 0) partial[blockIdx.x] = acc;
+}
+
+// seg_blk null: one norm over the np partials, torch.nn.utils.clip_grad_norm_'s factor min(max_norm / (norm + 1e-6), 1)
+// with its fp32 operations (reciprocal, then multiply: torch's scalar / tensor), NaN propagated by the clamp as
+// torch.clamp does.  Else nseg segments, segment s over partials [seg_blk[s], seg_blk[s + 1]) with the bound
+// scal[seg_scal[s]]: BertAdam's rule, max / (norm + 1e-6) only where norm > max > 0, in double as the host computed it.
+__global__ void __launch_bounds__(kOptThreads) clip_coef_kernel(const double* __restrict__ partial, int np,
+                                                                 const int* __restrict__ seg_blk,
+                                                                 const int* __restrict__ seg_scal, int nseg,
+                                                                 const float* __restrict__ scal, float max_norm,
+                                                                 float* __restrict__ norm, float* __restrict__ coef) {
+    if (seg_blk == nullptr) {
+        double acc = 0.0;
+        for (int i = threadIdx.x; i < np; i += kOptThreads) acc += partial[i];
+        acc = block_sum_d(acc);
+        if (threadIdx.x == 0) {
+            const float nrm = (float)sqrt(acc);
+            const float c = __fmul_rn(__frcp_rn(__fadd_rn(nrm, 1e-6f)), max_norm);
+            *norm = nrm;
+            *coef = c > 1.f ? 1.f : c;
+        }
+        return;
+    }
+    const int lane = threadIdx.x & 31;
+    for (int s = threadIdx.x >> 5; s < nseg; s += kOptThreads / 32) {
+        double acc = 0.0;
+        for (int i = seg_blk[s] + lane; i < seg_blk[s + 1]; i += 32) acc += partial[i];
+        acc = warp_sum_d(acc);
+        if (lane == 0) {
+            const float nrm = (float)sqrt(acc);
+            const float mx = scal[seg_scal[s]];
+            norm[s] = nrm;
+            coef[s] = (mx > 0.f && nrm > mx) ? (float)((double)mx / ((double)nrm + 1e-6)) : 1.f;
+        }
+    }
 }
 
 static inline int opt_grid(int n) {
@@ -314,9 +410,9 @@ static inline int opt_grid(int n) {
 
 cudaError_t launch_fused_sgd(float* p, float* g, float* mom, int n, float momentum, float dampening, float weight_decay,
                              int nesterov, int first_step, int zero_grad, const float* scal, const int* fault,
-                             const int* skip, cudaStream_t stream) {
+                             const int* skip, const float* coef, cudaStream_t stream) {
     const SgdHyper h{momentum, dampening, weight_decay, nesterov, first_step};
-    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, h, zero_grad, scal, fault, skip);
+    fused_sgd_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, n, h, zero_grad, scal, fault, skip, coef);
     return cudaGetLastError();
 }
 
@@ -334,27 +430,28 @@ cudaError_t launch_sgd_ahead(float* p, float* mom, float* sp, float* sm, const S
 
 cudaError_t launch_fused_sgd_tail(float* p, float* g, float* mom, const float* sp, const float* sm, int n,
                                   const SgdRanges& ahead, const SgdRanges& dense, const SgdHyper& h, int zero_grad,
-                                  const float* scal, const int* fault, const int* skip, cudaStream_t stream) {
+                                  const float* scal, const int* fault, const int* skip, const float* coef,
+                                  cudaStream_t stream) {
     fused_sgd_tail_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, mom, sp, sm, n, ahead, dense, h, zero_grad,
-                                                                  scal, fault, skip);
+                                                                  scal, fault, skip, coef);
     return cudaGetLastError();
 }
 
 cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n, float b1, float b2, float eps,
                                    float weight_decay, int zero_grad, const float* scal, const int* fault,
-                                   const int* skip, cudaStream_t stream) {
+                                   const int* skip, const ClipRef& clip, cudaStream_t stream) {
     fused_bert_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, b1, b2, eps, weight_decay, zero_grad,
-                                                                   scal, fault, skip);
+                                                                   scal, fault, skip, clip);
     return cudaGetLastError();
 }
 
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
-                              const int* skip, cudaStream_t stream) {
+                              const int* skip, const float* coef, cudaStream_t stream) {
     // 1 - beta in double, rounded once: torch passes these factors as Python floats
     fused_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, (float)(1.0 - beta1), (float)beta2,
                                                               (float)(1.0 - beta2), eps, weight_decay, decoupled,
-                                                              zero_grad, scal, fault, skip);
+                                                              zero_grad, scal, fault, skip, coef);
     return cudaGetLastError();
 }
 
@@ -409,14 +506,15 @@ cudaError_t launch_momentum_correct(float* g, float* buf, int n, float momentum,
     return cudaGetLastError();
 }
 
-cudaError_t launch_l2norm_sq(const float* x, int n, float* out, cudaStream_t stream) {
-    cudaMemsetAsync(out, 0, sizeof(float), stream);
-    l2norm_sq_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(x, n, out);
+cudaError_t launch_grad_sumsq(const float* g, const SumsqSegs& t, double* partial, cudaStream_t stream) {
+    if (t.nseg <= 0) return cudaSuccess;
+    grad_sumsq_kernel<<<t.blk_begin[t.nseg], kOptThreads, 0, stream>>>(g, t, partial);
     return cudaGetLastError();
 }
 
-cudaError_t launch_scale(float* x, int n, const float* norm_sq, float max_norm, cudaStream_t stream) {
-    clip_scale_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(x, n, norm_sq, max_norm);
+cudaError_t launch_clip_coef(const double* partial, int np, const int* seg_blk, const int* seg_scal, int nseg,
+                             const float* scal, float max_norm, float* norm, float* coef, cudaStream_t stream) {
+    clip_coef_kernel<<<1, kOptThreads, 0, stream>>>(partial, np, seg_blk, seg_scal, nseg, scal, max_norm, norm, coef);
     return cudaGetLastError();
 }
 

@@ -84,6 +84,11 @@ SWITCHES = (
                 "device; with --cuda-graph, --fused-lstm and --fused-ctc the steps are captured in CUDA graphs, "
                 "one set per padded length.  The batch-norm statistics count the padded frames unless --fused-bn is "
                 "on (default: 0, off)"),
+    # a Trainer argument, not a create_net keyword
+    Switch("--fused-clip", (), ("lstman4", "lstm"),
+           help="lstman4 and lstm (PTB): clip the reduced gradient on the device inside the optimizer step, one "
+                "deterministic norm pass with the factor applied by the fused update, instead of torch's "
+                "clip_grad_norm_ before it (default: clip_grad_norm_)"),
     Switch("--bidirectional", ("bidirectional",), ("lstman4",),
            help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
                 "(default: uni-directional)"),

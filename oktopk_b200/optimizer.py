@@ -122,7 +122,8 @@ class _BucketedComm:
     """Bucket bookkeeping, autograd hooks, stream choreography.  Mixed into optimizer classes."""
 
     def _okt_setup(self, named_parameters, allreducer: AllReducer, flatten_params: bool = True,
-                   loss_scale: Optional[LossScale] = None) -> None:
+                   loss_scale: Optional[LossScale] = None, max_grad_norm: Optional[float] = None,
+                   clip_per_param: bool = False) -> None:
         if named_parameters is not None:
             named_parameters = list(named_parameters)
             if any(not isinstance(p, tuple) for p in named_parameters):
@@ -230,6 +231,13 @@ class _BucketedComm:
                 stage = self._hyper_dev = torch.zeros(groups * 4, dtype=torch.float64, device=dev0)
             self._lr_pin = [torch.zeros_like(stage, device="cpu").pin_memory() for _ in range(8)]
             self._lr_ev = [None] * len(self._lr_pin)
+        # gradient clipping: on the device when every bucket takes a fused kernel (_GradClip), else torch's
+        # clip_grad_norm_ over the bucket views before the update
+        self._max_grad_norm = max_grad_norm
+        self._grad_norm: Optional[torch.Tensor] = None
+        self._clip: Optional[_GradClip] = None
+        if (max_grad_norm is not None or clip_per_param) and self._device_update():
+            self._clip = _GradClip(self, clip_per_param, max_grad_norm or 0.0)
 
     def _resync_replicas(self) -> None:
         """After a handled fault: every replica takes rank 0's parameters (and momentum) again."""
@@ -550,6 +558,12 @@ class _BucketedComm:
     def comm_stats(self) -> Dict:
         return self._allreducer.stats()
 
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """The gradient norm the last ``step()`` clipped with, as ``clip_grad_norm_`` returns it: a 0-dim tensor on the
+        parameters' device, written by the step without a host synchronisation (BertAdam with ``clip_reduced`` on the
+        device: one norm per parameter, in bucket order).  None before the first clipped step."""
+        return self._grad_norm
+
     def check_faults(self) -> None:
         """Raise / call ``err_handler`` if a peer timed out inside a communication kernel (synchronous read)."""
         self._allreducer.check_faults()
@@ -569,6 +583,9 @@ class _BucketedComm:
                 loss = closure()
         if not self.local:
             self.synchronize()
+        if self._clip is None and self._max_grad_norm is not None:
+            self._grad_norm = torch.nn.utils.clip_grad_norm_([p for g in self.param_groups for p in g["params"]],
+                                                             self._max_grad_norm)
         # the fused kernels read the step verdict themselves; the torch update paths need it on the host
         host_skip = self._ls is not None and not self._device_update() and self._ls.found_host()
         if self._update is None:
@@ -581,6 +598,8 @@ class _BucketedComm:
             if self._hyper_dev is not None and self._update is _AdamUpdate:
                 ext.require().adam_scalars(self._ls.ptr, self._hyper_dev.data_ptr(), self._lr_dev.data_ptr(),
                                            len(self.param_groups), torch.cuda.current_stream().cuda_stream)
+            if self._clip is not None:
+                self._grad_norm = self._clip.run(self)
             with torch.no_grad():
                 for b in self._buckets:
                     self._fused_update(b, host_skip)
@@ -619,10 +638,11 @@ class _BucketedComm:
             return
         for gi, s, e in b.group_slices:
             def launch(fn, *hyper):
+                clip = self._clip.ref(b, s) if self._clip is not None else {}
                 fn(b.flat_param.data_ptr() + 4 * s, b.grad.data_ptr() + 4 * s,
                    *(fs[k].data_ptr() + 4 * s for k in self._update.keys), e - s, *hyper, zero_grad,
                    torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi), self._allreducer.fault_ptr(b.name),
-                   skip_ptr)
+                   skip_ptr, **clip)
             if on_gpu or not host_skip:
                 self._update.update(self, b, self.param_groups[gi], s, e, fs, first, launch if on_gpu else None)
             if not on_gpu:
@@ -644,7 +664,8 @@ class _BucketedComm:
                              sm.data_ptr() + 4 * s if sm is not None else 0, e - s, _clip_ranges(ahead, s, e),
                              _clip_ranges(rest, s, e), m, damp, wd, int(nest), 0, zero_grad,
                              torch.cuda.current_stream().cuda_stream, self._lr_ptr(gi),
-                             self._allreducer.fault_ptr(b.name), skip_ptr)
+                             self._allreducer.fault_ptr(b.name), skip_ptr,
+                             **(self._clip.ref(b, s) if self._clip is not None else {}))
 
     def _adopt_state(self, counter: Optional[int] = None) -> None:
         """Move per-parameter state (from ``load_state_dict`` or the wrapped optimizer) into the flat buffers.  A bucket
@@ -660,6 +681,7 @@ class _BucketedComm:
                 warnings.warn("DistributedOptimizer: the loaded Adam state has unequal step counts per parameter %s; "
                               "using torch's Adam step from now on" % sorted(steps))
                 self._update = None
+                self._clip = None                 # torch's step: the clip runs before it, in torch
                 self._clear_buckets()
                 self._direct = False              # torch's step reads the gradients from the landed bucket
                 for b in self._buckets:
@@ -697,6 +719,70 @@ def _clip_ranges(ranges, s: int, e: int):
         if lo < hi:
             out.append((lo, hi))
     return out
+
+
+class _GradClip:
+    """Gradient clipping on the device, between ``synchronize()`` and the fused update: one ``grad_sumsq`` per bucket
+    (fp64 partial sums of squares, a fixed number per bucket, no atomics), one ``clip_coef`` that combines them in a
+    fixed order into the norm and the factor, and the update kernels multiply the gradient by the factor as they read
+    it.  Two launches per step more than an unclipped one-bucket step, no host synchronisation: a CUDA graph captures
+    it.  After the reduction every rank holds the same bucket bits, so every rank computes the same factor.
+
+    Global (``DistributedOptimizer(max_grad_norm=c)``): one norm over every bucket, each bucket one segment (its padding
+    between parameters is zero), torch's ``clip_grad_norm_`` factor.  Per parameter (``BertAdam(clip_reduced=True)``):
+    one segment, norm and factor per parameter, the bound ``max_grad_norm`` of its group read from the device scalars
+    (``_BertAdamUpdate.scalars``); the update kernel finds a vector's factor from the segment ends of its group slice."""
+
+    def __init__(self, opt, per_param: bool, max_norm: float):
+        C = ext.require()
+        dev = opt._buckets[0].grad.device
+        self.per_param, self.max_norm = per_param, float(max_norm)
+        self.tables = []                          # (bucket, offsets, lengths, first partial)
+        self.first_seg: Dict[tuple, int] = {}     # (bucket index, group slice start) -> its first segment
+        seg_blk, seg_scal, ends, npart = [0], [], [], 0
+        for b in opt._buckets:
+            if per_param:
+                offs, lens = list(b.offsets), [p.numel() for p in b.params]
+                for gi, s, e in b.group_slices:
+                    ts = [t for t, o in enumerate(offs) if s <= o < e]
+                    self.first_seg[b.index, s] = len(seg_scal)
+                    for j, t in enumerate(ts):
+                        seg_scal.append(gi * opt._update.n_scalars + 1)
+                        ends.append((offs[ts[j + 1]] - s) // 4 if j + 1 < len(ts) else 2 ** 31 - 1)
+            else:
+                offs, lens = [0], [b.numel]
+            self.tables.append((b, offs, lens, npart))
+            for n in lens:
+                npart += max(1, -(-n // C.SUMSQ_CHUNK))
+                seg_blk.append(npart)
+        self.nseg = len(seg_scal) if per_param else 1
+        self.partial = torch.zeros(npart, dtype=torch.float64, device=dev)
+        self.norm = torch.zeros(self.nseg, dtype=torch.float32, device=dev)
+        self.coef = torch.ones(self.nseg, dtype=torch.float32, device=dev)
+        as_dev = lambda v: torch.tensor(v, dtype=torch.int32).to(dev)      # noqa: E731
+        self.seg_blk = as_dev(seg_blk) if per_param else None
+        self.seg_scal = as_dev(seg_scal) if per_param else None
+        self.ends = as_dev(ends) if per_param else None
+
+    def run(self, opt) -> torch.Tensor:
+        """Enqueue the norm and the factor on the current stream; returns the norm (0-dim, or one per parameter)."""
+        C, stream = ext.require(), torch.cuda.current_stream().cuda_stream
+        for b, offs, lens, p0 in self.tables:
+            C.grad_sumsq(b.grad.data_ptr(), offs, lens, self.partial.data_ptr() + 8 * p0, stream)
+        if self.per_param:
+            C.clip_coef(self.partial.data_ptr(), self.partial.numel(), self.seg_blk.data_ptr(), self.seg_scal.data_ptr(),
+                        self.nseg, opt._lr_dev.data_ptr(), 0.0, self.norm.data_ptr(), self.coef.data_ptr(), stream)
+            return self.norm
+        C.clip_coef(self.partial.data_ptr(), self.partial.numel(), 0, 0, 0, 0, self.max_norm, self.norm.data_ptr(),
+                    self.coef.data_ptr(), stream)
+        return self.norm[0]
+
+    def ref(self, b: Bucket, s: int) -> Dict[str, int]:
+        """The factor arguments of the update of bucket ``b``'s group slice starting at element ``s``."""
+        if not self.per_param:
+            return {"coef_ptr": self.coef.data_ptr()}
+        t = self.first_seg[b.index, s]
+        return {"coef_ptr": self.coef.data_ptr() + 4 * t, "ends_ptr": self.ends.data_ptr() + 4 * t}
 
 
 # ====================================================================================== fused update families
@@ -767,17 +853,18 @@ class _AdamUpdate:
 
 
 class _BertAdamUpdate:
-    """``BertAdam``: no bias correction, decoupled weight decay, the learning rate of its schedule."""
+    """``BertAdam``: no bias correction, decoupled weight decay, the learning rate of its schedule.  Device scalars: the
+    scheduled lr and the group's ``max_grad_norm`` (the bound of the per-parameter clip on the device)."""
     keys = ("next_m", "next_v")
-    n_scalars = 1
+    n_scalars = 2
 
     @staticmethod
     def scalars(opt, g):
-        return (float(opt._scheduled_lr(g, opt.counter)),)
+        return (float(opt._scheduled_lr(g, opt.counter)), float(g["max_grad_norm"]))
 
     @staticmethod
     def update(opt, b, g, s, e, fs, first, launch):
-        if opt.clip_reduced and g["max_grad_norm"] > 0:
+        if opt.clip_reduced and g["max_grad_norm"] > 0 and opt._clip is None:     # the reference of the device clip
             for p, o in zip(b.params, b.offsets):
                 if s <= o < e:
                     gv = b.grad[o:o + p.numel()]
@@ -839,7 +926,7 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
                          density: float = 0.1, norm_clip: Optional[float] = None, writer=None,
                          cfg: Optional[OkTopkConfig] = None, world: Optional[World] = None,
                          backend: Optional[str] = None, flatten_params: bool = True,
-                         loss_scale: Optional[LossScale] = None):
+                         loss_scale: Optional[LossScale] = None, max_grad_norm: Optional[float] = None):
     """Wrap ``optimizer`` so that ``step()`` first allreduces the gradients with the chosen scheme.
 
     Horovod-style dynamic subclass of the user's optimizer class, as in the reference
@@ -847,7 +934,13 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
     class (``compressors['oktopk']``) or an instance; ``cfg`` overrides the scalar arguments.
     ``loss_scale``: dynamic loss scaling for fp16 training (see ``LossScale``); back-propagate
     ``opt.scale_loss(loss)``.
+    ``max_grad_norm``: clip the reduced gradient as ``synchronize(); clip_grad_norm_(params, max_grad_norm); step()``
+    does, the norm over every parameter of the optimizer (``grad_norm()`` returns it).  With SGD or the fused Adam /
+    AdamW on flat CUDA buckets the clip runs on the device inside ``step()`` (the update kernels apply the factor; the
+    bucket is not rescaled in place); otherwise ``step()`` calls ``clip_grad_norm_`` over the bucket views.
     """
+    if max_grad_norm is not None and not float(max_grad_norm) > 0:
+        raise ValueError("max_grad_norm must be a positive number, got %r" % (max_grad_norm,))
     base_cls = optimizer.__class__
     cls = type(base_cls.__name__, (_DistributedOptimizerMixin, base_cls), {})
     obj = cls.__new__(cls)
@@ -864,7 +957,8 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
         obj._update = None                        # torch's own step()
     if obj._update is not None:
         obj.counter = 0                           # steps taken: Adam's bias correction (GraphedTrainStep keeps it too)
-    obj._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale)
+    obj._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale,
+                   max_grad_norm=None if max_grad_norm is None else float(max_grad_norm))
     if obj._update is not None and obj.state:
         obj._adopt_state()
         obj._load_scale_state(None, obj.counter)
@@ -950,7 +1044,8 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
     ``max_grad_norm``: the reference calls ``clip_grad_norm_(p, ...)`` on the *local* ``p.grad`` and
     then applies the *reduced* gradient, so its clipping never affects the update (A.4-6).  Here
     ``clip_reduced=True`` clips the reduced per-parameter gradient for real; the default reproduces the
-    reference's effective behaviour (no clipping).
+    reference's effective behaviour (no clipping).  On flat CUDA buckets that clip runs on the device (``_GradClip``:
+    no host synchronisation, so the step can be captured in a CUDA graph), elsewhere in torch per parameter.
     """
 
     def __init__(self, params, lr=1e-3, warmup=-1, t_total=-1, schedule="warmup_linear", b1=0.9, b2=0.999, e=1e-6,
@@ -979,7 +1074,8 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
             global_adapt_high=5 / 4, global_adapt_inc=1.036, global_adapt_dec=1.025, balanced_allgather=True)
         ar = AllReducer(compression=compressor, sparse=(compressor != "none"), density=density,
                         cfg=base.replace(density=density), world=world, backend=backend)
-        self._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale)
+        self._okt_setup(named_parameters, ar, flatten_params=flatten_params, loss_scale=loss_scale,
+                        clip_per_param=clip_reduced)
 
     def get_lr(self) -> List[float]:
         out = []

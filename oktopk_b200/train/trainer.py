@@ -53,13 +53,18 @@ class Trainer:
                  seq_len: int = 128, t_total: int = -1, warmup: float = -1, pretrain: Optional[str] = None,
                  norm_clip: Optional[float] = None, backend: Optional[str] = None, cuda_graph: bool = False,
                  model_kwargs: Optional[dict] = None, autocast: Optional[str] = None, loss_scale=None,
-                 an4_pad_multiple: int = 0):
+                 an4_pad_multiple: int = 0, fused_clip: bool = False):
         """``an4_pad_multiple=m >= 1`` (AN4 only; 0, the default, is off): every training batch is staged into a
         ``data.PaddedAN4Batch`` with its frames padded up to a multiple of m and its lengths on the device, and with
         ``cuda_graph`` the steps are captured per padded length (``GraphedTrainStep``).  With the stock batch-norm the
         padded frames change one thing: those layers count them in their statistics, as they count the padding inside a
         batch.  With ``fuse_bn`` (``model_kwargs``) the statistics stop at the longest utterance and the padded batch
-        gives the unpadded batch's loss and gradients to rounding."""
+        gives the unpadded batch's loss and gradients to rounding.
+
+        ``fused_clip`` (AN4 and PTB, the two workloads that clip the reduced gradient every step; off by default): the
+        clip runs on the device inside the optimizer's step (``DistributedOptimizer(max_grad_norm=...)``): one norm pass
+        and a factor that the fused update applies, instead of ``clip_grad_norm_`` between ``synchronize()`` and
+        ``step()``.  The same factor as torch's up to the norm's rounding, no host synchronisation."""
         self.world = world or _world()
         self.rank, self.nworkers = self.world.rank, self.world.size
         # The host side of a step is tiny tensor ops (collate 16 images, one pinned copy): on a many-core box an
@@ -73,6 +78,11 @@ class Trainer:
             if torch.get_num_threads() > want:
                 torch.set_num_threads(want)
         self.dnn = dnn
+        # the bound LSTM/main_trainer.py:94-99 clips the reduced gradient to, per model
+        self.clip_norm = {"lstman4": 400.0, "lstm": 0.25}.get(dnn)
+        if fused_clip and self.clip_norm is None:
+            raise ValueError("fused_clip applies to lstman4 and lstm, the models that clip their gradient; not %s" % dnn)
+        self.fused_clip = bool(fused_clip)
         self.dataset = (dataset or _DATASET_OF.get(dnn, "cifar10")).lower()
         if an4_pad_multiple < 0 or (an4_pad_multiple and self.dataset != "an4"):
             raise ValueError("an4_pad_multiple must be 0 (off) or, for the AN4 dataset, >= 1; got %r for %s"
@@ -141,7 +151,8 @@ class Trainer:
             self.optimizer = DistributedOptimizer(base, named_parameters=self.net.named_parameters(),
                                                   compression=_comp.compressors[self.cfg.compressor],
                                                   is_sparse=self.cfg.sparse, cfg=self.cfg, world=self.world,
-                                                  err_handler=self._err_handler, loss_scale=self.loss_scale)
+                                                  err_handler=self._err_handler, loss_scale=self.loss_scale,
+                                                  max_grad_norm=self.clip_norm if self.fused_clip else None)
         # ---- data -----------------------------------------------------------------------------
         self.trainset = D.build_dataset(self.dataset, data_dir, train=True, seed=seed, seq=seq_len, batch_size=batch_size)
         self.loader, self.sampler = D.build_loader(self.trainset, self.dataset, batch_size, self.rank, self.nworkers,
@@ -343,12 +354,9 @@ class Trainer:
                                        "--mlm-capacity (mlm_capacity; 1.0 never overflows)" % (n, h.mlm_capacity))
 
     def update_model(self) -> None:
-        if self.dnn == "lstman4":                # LSTM/main_trainer.py:94-99: clip the *reduced* gradient
+        if self.clip_norm is not None and not self.fused_clip:     # clip the *reduced* gradient (fused_clip: in step())
             self.optimizer.synchronize()
-            torch.nn.utils.clip_grad_norm_(self.net.parameters(), 400)
-        elif self.dnn == "lstm":
-            self.optimizer.synchronize()
-            torch.nn.utils.clip_grad_norm_(self.net.parameters(), 0.25)
+            torch.nn.utils.clip_grad_norm_(self.net.parameters(), self.clip_norm)
         self.optimizer.step()
 
     def _bookkeep_iter(self) -> None:

@@ -29,7 +29,7 @@ FAMILIES = [
     ("bn+relu+pool (bnrelu.cu)", r"okt::(bn_|maxpool2_)"),
     ("ok-topk allreduce", r"okt::(oktopk|gather|gtopk|dense_allreduce|kth_abs)"),
     ("gradient landing", r"okt::land"),
-    ("fused update", r"okt::(fused_sgd|fused_bert_adam|fused_adam|momentum_correct|clip|l2norm)"),
+    ("fused update", r"okt::(fused_sgd|fused_bert_adam|fused_adam|momentum_correct|grad_sumsq|clip_coef)"),
     ("other okt::", r"okt::"),
     ("convolution (cuDNN)", r"(?i)conv|cudnn|xmma|implicit|wgrad|dgrad|fprop|winograd|fft"),
     ("gemm (cuBLAS)", r"(?i)gemm|cutlass|sm90_|ampere_|gemv"),
