@@ -63,7 +63,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--trace", type=str, default=None, help="directory: dump the device-side per-call trace ring of every bucket at the end")
     p.add_argument("--deterministic", action="store_true")
     p.add_argument("--seed", type=int, default=0)
-    p.add_argument("--cuda-graph", action="store_true", help="capture forward+backward+allreduce+update into CUDA graphs")
+    p.add_argument("--cuda-graph", action="store_true", help="capture forward+backward+allreduce+update into CUDA graphs (PTB --dnn lstm: with "
+                   "--fused-lstm-lm under --bf16 / --fp16, --fused-lstm-lm-fp32, or the stock layer in fp32)")
     p.add_argument("--fp16", action="store_true", help="fp16 autocast (reference: apex amp O3, main_bert.py:1009-1023)")
     p.add_argument("--bf16", action="store_true", help="bf16 autocast")
     for sw in SWITCHES:

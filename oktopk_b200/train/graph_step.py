@@ -16,6 +16,14 @@ every flavour of a new T_b is captured the first time it appears.  At most ``MAX
 a batch of another shape after that, or one whose targets exceed the capacity, runs that step eagerly on the same
 padded form (counted in ``fallbacks``).  The step needs every LSTM layer fused and the fused CTC loss, the two parts that
 read the lengths on the device; otherwise the graph step disables itself and the padded batches run eagerly.
+
+The PTB language model carries (h, c) from one batch to the next.  Its graphs read the state from one static pair
+[L, N, H] (h in the autocast type on the 16-bit fused path, c fp32; both fp32 in fp32) and, as their last node, after
+backward and the update, copy the step's (h_n, c_n) into it; the trainer's ``hidden`` *is* that pair between replays.
+Before a replay the eager step's rule is applied to whatever ``hidden`` is then (a reset, ``Trainer.test()``, an eager
+step): None or another batch size zeroes the pair, anything else is copied in.  A batch of another shape (the short last
+batch of an epoch), or a state whose dtypes differ from the pair's, runs that step eagerly (counted in ``fallbacks``)
+and the graphs stay.  Graphed PTB needs the fused LSTM layers or the stock layer in fp32 (``ptb_graph_error``).
 """
 from __future__ import annotations
 
@@ -30,6 +38,18 @@ from .data import PaddedAN4Batch
 # Padded AN4 input shapes (one per T_b at a fixed batch size) that get graphs; batches of further shapes run eagerly.
 # Each shape holds a graph per flavour; at m = 32 the synthetic AN4 utterances (96-396 frames) pad to 11 lengths.
 MAX_AN4_SHAPES = 16
+
+
+def ptb_graph_error(net, autocast: Optional[torch.dtype]) -> Optional[str]:
+    """Why the PTB language model ``net`` (a ``PTBLSTM``) does not get graphed steps under ``autocast`` (None: fp32), or
+    None when it does: the fused stacked-layer LSTM in bf16, fp16 and fp32, and the stock cuDNN layer in fp32, are the
+    configurations whose graphed steps are checked against eager ones bit for bit."""
+    if net.fuse_lstm and (autocast is not None or net.fuse_lstm_fp32):
+        return None
+    if autocast is not None:
+        return ("the stock nn.LSTM under %s autocast has no graphed step: set fuse_lstm (--fused-lstm-lm) for the "
+                "fused 16-bit layers" % str(autocast).replace("torch.", ""))
+    return None
 
 
 def _clone(batch):
@@ -58,6 +78,15 @@ class GraphedTrainStep:
         self._precaptured_shapes = set()
         self._shape: Optional[Tuple] = None
         self.fallbacks = {"shapes": 0, "targets": 0}
+        # PTB: the static (h, c) every graph reads and writes back (allocated at the first graphed step); the steps that
+        # ran eagerly because their batch had another shape or their carried state another dtype
+        self.ptb = getattr(trainer, "dataset", None) == "ptb"
+        self._state: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
+        if self.ptb:
+            self.fallbacks = {"shapes": 0, "state": 0}
+            why = ptb_graph_error(trainer.net, trainer.autocast)
+            if why is not None:
+                self.enabled, self.why_disabled = False, why
         if self.an4:
             net = trainer.net
             why = net.device_lengths_error(True, trainer.autocast is not None)
@@ -177,9 +206,15 @@ class GraphedTrainStep:
         for s, t in zip(static, batch):
             if torch.is_tensor(t):
                 if s.shape != t.shape:
+                    if self.ptb:                 # a short batch: this step eagerly, the graphs stay
+                        self.fallbacks["shapes"] += 1
+                        return self._eager(batch)
                     self.enabled, self.why_disabled = False, "batch shape changed"
                     return self._eager(batch)
                 s.copy_(t, non_blocking=True)
+        if self.ptb and not self._load_state(batch[0].size(0)):
+            self.fallbacks["state"] += 1
+            return self._eager(batch)
         self.static_in, self._shape = static, shape
         key = self._full_key(flavour)
         self.opt.refresh_lr()
@@ -204,8 +239,47 @@ class GraphedTrainStep:
         self.static_loss = self._loss_of[key]
         return self.static_loss
 
+    # ------------------------------------------------------------------ PTB: the carried state
+    def _load_state(self, n: int) -> bool:
+        """Make the trainer's ``hidden`` the static pair for a batch of ``n`` sequences, by the eager step's rule
+        (``Trainer._forward_loss_impl``): None or another batch size starts from zeros, anything else is carried in
+        exactly.  False (nothing changed) when the state cannot be copied exactly: its dtypes are not the pair's."""
+        tr = self.tr
+        st = self._state
+        if st is None:
+            shape = (tr.net.num_layers, n, tr.net.embedding_dim)
+            h_dt = tr.autocast if tr.net.fuse_lstm and tr.autocast is not None else torch.float32
+            st = self._state = (torch.empty(shape, dtype=h_dt, device=tr.device),
+                                torch.empty(shape, dtype=torch.float32, device=tr.device))
+        hid = tr.hidden
+        if hid is not None and hid[0] is st[0] and hid[1] is st[1]:
+            return True
+        if hid is None or hid[0].size(1) != st[0].size(1):
+            for s in st:
+                s.zero_()
+        elif all(h.dtype == s.dtype and h.shape == s.shape for h, s in zip(hid, st)):
+            # detached: a copy from a tensor with autograd history would attach that history to the pair and keep the
+            # eager step's graph (its AccumulateGrad nodes, bound to the stream they were made on) alive into a capture
+            for h, s in zip(hid, st):
+                s.copy_(h.detach())
+        else:
+            return False
+        tr.hidden = st
+        return True
+
+    def _store_state(self) -> None:
+        """Inside a capture, after the update: copy the step's (h_n, c_n) into the static pair.  Last, because the
+        backward pass reads (h0, c0) from it."""
+        for s, h in zip(self._state, self.tr.hidden):
+            if h.dtype != s.dtype or h.shape != s.shape:
+                raise RuntimeError("the carried state comes back as %s %s, the static buffer is %s %s"
+                                   % (h.dtype, tuple(h.shape), s.dtype, tuple(s.shape)))
+            s.copy_(h.detach())
+
     def _capture(self, key) -> Optional[torch.cuda.CUDAGraph]:
         tr = self.tr
+        if self.ptb:
+            tr.hidden = self._state
         counters = [eng.host.counter for eng in self._engines()]
         opt_counter = getattr(self.opt, "counter", None)
         self._cap_counters, self._cap_opt_counter = counters, opt_counter
@@ -219,6 +293,10 @@ class GraphedTrainStep:
                 self._backward(loss)
                 tr.update_model()
                 out = loss.detach()
+                if self.ptb:
+                    self._store_state()
+            if self.ptb:
+                tr.hidden = self._state
             if self.static_loss is None:
                 self.static_loss = out
             else:
@@ -230,6 +308,8 @@ class GraphedTrainStep:
                 self.pool = g.pool()
         except Exception as e:  # noqa: BLE001 - fall back to eager for good
             self.enabled, self.why_disabled = False, "capture failed: %r" % (e,)
+            if self.ptb:
+                tr.hidden = self._state          # nothing ran: the pair still holds the state this step starts from
             # capture executed the Python side effects (counters) but no kernels: undo them
             for eng, c in zip(self._engines(), counters):
                 eng.host.counter = c

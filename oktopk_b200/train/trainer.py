@@ -167,10 +167,10 @@ class Trainer:
         self.host_us = {"next": 0.0, "launch": 0.0, "stage_next": 0.0, "steps": 0}
         self.sparsities: List[float] = []
         self._iter_times: List[float] = []
-        # whole-step CUDA graphs: fixed-shape workloads, and AN4 when its batches are padded to a few lengths (one set of
-        # graphs per padded length); unpadded AN4 batches vary in length, and PTB carries hidden state
+        # whole-step CUDA graphs: fixed-shape workloads, PTB with its carried state in static buffers, and AN4 when its
+        # batches are padded to a few lengths (one set of graphs per padded length); unpadded AN4 batches vary in length
         self.graphed = None
-        graph_ok = self.dataset != "ptb" and (self.dataset != "an4" or self.an4_pad_multiple >= 1)
+        graph_ok = self.dataset != "an4" or self.an4_pad_multiple >= 1
         if cuda_graph and self.device.type == "cuda" and graph_ok and nsteps_update == 1:
             from .graph_step import GraphedTrainStep
             self.graphed = GraphedTrainStep(self)
