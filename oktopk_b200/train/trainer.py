@@ -167,8 +167,7 @@ class Trainer:
         self.host_us = {"next": 0.0, "launch": 0.0, "stage_next": 0.0, "steps": 0}
         self.sparsities: List[float] = []
         self._iter_times: List[float] = []
-        # whole-step CUDA graphs: fixed-shape workloads, PTB with its carried state in static buffers, and AN4 when its
-        # batches are padded to a few lengths (one set of graphs per padded length); unpadded AN4 batches vary in length
+        # whole-step CUDA graphs (graph_step: one input rule per kind of batch); unpadded AN4 batches vary in length
         self.graphed = None
         graph_ok = self.dataset != "an4" or self.an4_pad_multiple >= 1
         if cuda_graph and self.device.type == "cuda" and graph_ok and nsteps_update == 1:
@@ -267,11 +266,14 @@ class Trainer:
         return self.criterion(out, y), (out, y)
 
     def backward(self, loss: torch.Tensor) -> None:
-        """Back-propagate ``loss``, multiplied by the optimizer's loss scale when loss scaling is on (the recorded loss
-        stays unscaled)."""
-        if self.loss_scale is not None:
-            loss = self.optimizer.scale_loss(loss)
-        loss.backward()
+        """Back-propagate ``loss`` times the optimizer's loss scale when scaling is on (read on the device: capturable)."""
+        self.optimizer.scale_loss(loss).backward()
+
+    def _forward_backward(self, batch) -> torch.Tensor:
+        """Every eager step's and captured graph's body; it reads only ``_forward_loss`` and ``optimizer``."""
+        loss, _ = self._forward_loss(batch)
+        self.optimizer.scale_loss(loss).backward()
+        return loss
 
     def train(self, num_of_iters: int = 1) -> float:
         """``DLTrainer.train`` (``VGG/dl_trainer.py:597-707``): forward+backward micro-steps; the
@@ -283,15 +285,10 @@ class Trainer:
             t0 = time.perf_counter()
             batch = self.stage_batch(self.prefetch.next(defer=True))
             self.timers.add("io", time.perf_counter() - t0)
-            loss, aux = self._forward_loss(batch)
-            self.backward(loss)
+            loss = self._forward_backward(batch)
             self.prefetch.advance()              # stage the next batch while the GPU works through this one
             self._last_loss = loss.detach()
-            self.loss_n += 1
-            if self.train_iter % self.iters_per_epoch == self.iters_per_epoch - 1:
-                self.train_epoch += 1
-                self.optimizer.add_train_epoch()
-            self.train_iter += 1
+            self._bookkeep_iter()
         return loss_val
 
     def last_loss(self) -> float:
@@ -365,6 +362,23 @@ class Trainer:
             self.train_epoch += 1
             self.optimizer.add_train_epoch()
         self.train_iter += 1
+
+    def step(self, batch) -> torch.Tensor:
+        """One optimizer step on ``batch`` (device tensors), graphed when ``cuda_graph`` left the graph step enabled.
+        Returns the device loss: the graph's static loss buffer, which the next replay overwrites, or the eager loss."""
+        if self.nsteps_update > 1:
+            raise ValueError("step() runs one micro-step per update: use train_step() with nsteps_update > 1")
+        self.net.train()
+        self.adjust_learning_rate()
+        if self.graphed is not None and self.graphed.enabled:
+            loss = self.graphed.step(batch)
+        else:
+            self.optimizer.zero_grad()
+            loss = self._forward_backward(self.stage_batch(batch)).detach()
+            self.update_model()
+        self._bookkeep_iter()
+        self._last_loss = loss
+        return loss
 
     def train_step(self) -> None:
         """One optimizer update = ``nsteps_update`` micro-steps (``VGG/main_trainer.py:83-100``)."""

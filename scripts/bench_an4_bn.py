@@ -113,17 +113,7 @@ class _Arm:
     def steps(self, pool, n):
         tr, loss = self.tr, None
         for _ in range(n):
-            b = pool[self.it % len(pool)]
-            tr.net.train()
-            tr.adjust_learning_rate()
-            if tr.graphed is not None and tr.graphed.enabled:
-                loss = tr.graphed.step(b)
-            else:
-                tr.optimizer.zero_grad()
-                loss, _ = tr._forward_loss(tr.stage_batch(b))
-                tr.backward(loss)
-                tr.update_model()
-            tr._bookkeep_iter()
+            loss = tr.step(pool[self.it % len(pool)])
             self.it += 1
         return loss
 

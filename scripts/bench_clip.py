@@ -64,10 +64,7 @@ class _Arm:
             if self.pool is None:
                 tr.train_step()
                 continue
-            tr.net.train()
-            tr.adjust_learning_rate()
-            tr.graphed.step(self.pool[self.it % len(self.pool)])
-            tr._bookkeep_iter()
+            tr.step(self.pool[self.it % len(self.pool)])
             self.it += 1
 
 

@@ -73,11 +73,7 @@ def main(argv=None) -> int:
         arms[name] = {"tr": tr, "pool": pool, "it": 0, "ms": []}
 
     def step(arm):
-        tr = arm["tr"]
-        tr.net.train()
-        tr.adjust_learning_rate()
-        loss = tr.graphed.step(arm["pool"][arm["it"] % 4])
-        tr._bookkeep_iter()
+        loss = arm["tr"].step(arm["pool"][arm["it"] % 4])
         arm["it"] += 1
         return loss
 

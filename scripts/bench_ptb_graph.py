@@ -77,20 +77,8 @@ class _Arm:
             gs._capture = timed
 
     def steps(self, n):
-        tr = self.tr
         for _ in range(n):
-            batch = self.pool[self.it % len(self.pool)]
-            tr.net.train()
-            tr.adjust_learning_rate()
-            if self.graph:
-                tr._last_loss = tr.graphed.step(batch)
-            else:
-                tr.optimizer.zero_grad()
-                loss, _ = tr._forward_loss(batch)
-                tr.backward(loss)
-                tr.update_model()
-                tr._last_loss = loss.detach()
-            tr._bookkeep_iter()
+            self.tr.step(self.pool[self.it % len(self.pool)])
             self.it += 1
 
 

@@ -27,17 +27,7 @@ for _ in range(N):
     t0 = time.perf_counter()
     batch = tr.prefetch.next()
     t1 = time.perf_counter()
-    tr.net.train()
-    tr.adjust_learning_rate()
-    if tr.graphed is not None and tr.graphed.enabled:
-        tr._last_loss = tr.graphed.step(batch)
-    else:
-        tr.optimizer.zero_grad()
-        loss, _ = tr._forward_loss(batch)
-        loss.backward()
-        tr._last_loss = loss.detach()
-        tr.update_model()
-    tr._bookkeep_iter()
+    tr.step(batch)
     t2 = time.perf_counter()
     tr.last_loss()
     t3 = time.perf_counter()

@@ -97,21 +97,14 @@ def main(argv=None) -> int:
         g["lr"] = lr
     pool = [tuple(t.to(tr.device) for t in bench.make_batch("vgg16", i, w.rank, bs, 128)) for i in range(4)]
 
-    def step(i):
-        tr.net.train()
-        tr.adjust_learning_rate()
-        loss = tr.graphed.step(pool[i % len(pool)])
-        tr._bookkeep_iter()
-        return loss
-
     it = 0
     for _ in range(int(cfg.warmup_iters) + a.warmup):
-        step(it)
+        tr.step(pool[it % len(pool)])
         it += 1
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(a.steps):
-            step(it)
+            tr.step(pool[it % len(pool)])
             it += 1
         torch.cuda.synchronize()
     fd, path = tempfile.mkstemp(suffix=".json")

@@ -350,25 +350,6 @@ def _trainer(m, graph, autocast=None, loss_scale=None, model_kwargs=KW, dense=Fa
                    autocast=autocast, loss_scale=loss_scale, model_kwargs=dict(model_kwargs), **comp)
 
 
-def _eager_step(tr, batch):
-    tr.net.train()
-    tr.adjust_learning_rate()
-    tr.optimizer.zero_grad()
-    loss, _ = tr._forward_loss(tr.stage_batch(batch))
-    tr.backward(loss)
-    tr.update_model()
-    tr._bookkeep_iter()
-    return loss.detach()
-
-
-def _graph_step(tr, batch):
-    tr.net.train()
-    tr.adjust_learning_rate()
-    loss = tr.graphed.step(batch)
-    tr._bookkeep_iter()
-    return loss
-
-
 def _mixed_batches(n, bs=2):
     from oktopk_b200.train.data import SyntheticAN4, an4_collate
     ds = SyntheticAN4(n=n * bs, seed=3)
@@ -387,19 +368,19 @@ def test_graphed_padded_follows_eager_padded(mode):
     assert gs.enabled, gs.why_disabled
     for it in range(16):
         b = pool[it % len(pool)]
-        la = _eager_step(eager, b)
-        lb = _graph_step(graphed, b)
+        la = eager.step(b)
+        lb = graphed.step(b)
         assert torch.equal(_bits(la), _bits(lb)), (mode, it)
     torch.cuda.synchronize()
     n_graphs = len(gs.graphs)
     torch.cuda.set_sync_debug_mode("error")
     try:
         for b in pool:
-            _graph_step(graphed, b)
+            graphed.step(b)
     finally:
         torch.cuda.set_sync_debug_mode(0)
     for b in pool:
-        _eager_step(eager, b)
+        eager.step(b)
     torch.cuda.synchronize()
     assert len(gs.graphs) == n_graphs
     for pa, pb in zip(eager.net.parameters(), graphed.net.parameters()):
@@ -447,11 +428,11 @@ def test_every_step_of_an_unpadded_run_gets_the_padded_batch_gradients(_fp32_exa
     tr.close()
 
 
-def _divergence(a, b, steps_a, steps_b, batches):
+def _divergence(a, b, batches):
     start = [p.detach().clone() for p in a.net.parameters()]
     rel = []
     for batch in batches:
-        la, lb = steps_a(a, batch).item(), steps_b(b, batch).item()
+        la, lb = a.step(batch).item(), b.step(batch).item()
         rel.append(abs(la - lb) / abs(la))
     drift = [((pa.double() - pb.double()).norm() / (pa.double() - p0.double()).norm().clamp_min(1e-30)).item()
              for p0, pa, pb in zip(start, a.net.parameters(), b.net.parameters())]
@@ -471,14 +452,14 @@ def test_ten_graphed_padded_steps_follow_ten_eager_unpadded_steps(_fp32_exact):
     assert len({b[0].size(3) for b in batches}) > 1 and any(b[2].min() < 1 for b in batches)
     ref, padded = _trainer(0, False, dense=True), _trainer(32, True, dense=True)
     assert padded.graphed is not None and padded.graphed.enabled, padded.graphed.why_disabled
-    loss_pad, drift_pad = _divergence(ref, padded, _eager_step, _graph_step, batches)
+    loss_pad, drift_pad = _divergence(ref, padded, batches)
     ref.close()
     ref, ctl = _trainer(0, False, dense=True), _trainer(0, False, dense=True)
     g = torch.Generator(device="cuda").manual_seed(1)
     with torch.no_grad():
         for p in ctl.net.parameters():
             p.mul_(1 + 2.0 ** -23 * torch.randn(p.shape, device="cuda", generator=g).sign())
-    loss_ctl, drift_ctl = _divergence(ref, ctl, _eager_step, _eager_step, batches)
+    loss_ctl, drift_ctl = _divergence(ref, ctl, batches)
     assert 0 < loss_ctl and loss_pad <= 4 * loss_ctl, (loss_pad, loss_ctl)
     assert drift_pad <= 4 * drift_ctl, (drift_pad, drift_ctl)
     for tr in (ref, padded, ctl):

@@ -182,25 +182,6 @@ def _pool(idx):
     return [tuple(t.cuda() for t in bench.make_batch("lstman4", i, 0, 2, 128)) for i in idx]
 
 
-def _eager_step(tr, batch):
-    tr.net.train()
-    tr.adjust_learning_rate()
-    tr.optimizer.zero_grad()
-    loss, _ = tr._forward_loss(tr.stage_batch(batch))
-    tr.backward(loss)
-    tr.update_model()
-    tr._bookkeep_iter()
-    return loss.detach()
-
-
-def _graph_step(tr, batch):
-    tr.net.train()
-    tr.adjust_learning_rate()
-    loss = tr.graphed.step(batch)
-    tr._bookkeep_iter()
-    return loss
-
-
 def _same_state(a, b):
     for pa, pb in zip(a.net.parameters(), b.net.parameters()):
         assert torch.equal(_bits(pa), _bits(pb))
@@ -278,8 +259,8 @@ def test_graphed_at_multiple_one_follows_todays_eager_trainer():
         b = pool[it % len(pool)]
         if it >= 3:
             flavours.append(graphed.graphed._key())
-        la = _eager_step(eager, b)
-        lb = _graph_step(graphed, b)
+        la = eager.step(b)
+        lb = graphed.step(b)
         assert torch.equal(_bits(la), _bits(lb)), it
     torch.cuda.synchronize()
     _same_state(eager, graphed)
@@ -308,8 +289,8 @@ def test_graphed_padded_follows_eager_padded(mode):
         b = pool[it % len(pool)]
         if it >= 3 and gs._key()[1].kind == "dense":
             dense.add(((2, 1, 161, -(-b[0].size(3) // 32) * 32), gs._key()))
-        la = _eager_step(eager, b)
-        lb = _graph_step(graphed, b)
+        la = eager.step(b)
+        lb = graphed.step(b)
         assert torch.equal(_bits(la), _bits(lb)), (mode, it)
     # every shape is captured now: one more pass replays without a single synchronisation
     torch.cuda.synchronize()
@@ -317,11 +298,11 @@ def test_graphed_padded_follows_eager_padded(mode):
     torch.cuda.set_sync_debug_mode("error")
     try:
         for b in pool:
-            _graph_step(graphed, b)
+            graphed.step(b)
     finally:
         torch.cuda.set_sync_debug_mode(0)
     for b in pool:
-        _eager_step(eager, b)
+        eager.step(b)
     torch.cuda.synchronize()
     assert len(gs.graphs) == n_graphs
     _same_state(eager, graphed)
@@ -344,8 +325,8 @@ def test_fallbacks_run_eagerly_counted_and_equal_eager(monkeypatch):
     seq = [pool[0]] * 6 + [pool[1], over, pool[0], pool[1]]
     eager, graphed = _trainer(32, False, warmup_iters=3), _trainer(32, True, warmup_iters=3)
     for it, b in enumerate(seq):
-        la = _eager_step(eager, b)
-        lb = _graph_step(graphed, b)
+        la = eager.step(b)
+        lb = graphed.step(b)
         assert torch.equal(_bits(la), _bits(lb)), it
     torch.cuda.synchronize()
     _same_state(eager, graphed)

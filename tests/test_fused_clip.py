@@ -492,10 +492,7 @@ def test_an4_graphed_padded_fused_clip_follows_stock_clip():
         assert (tr.optimizer._clip is not None) is (arm == "fused")
         seq = []
         for it in range(10):
-            tr.net.train()
-            tr.adjust_learning_rate()
-            seq.append(tr.graphed.step(pool[it % len(pool)]).clone())
-            tr._bookkeep_iter()
+            seq.append(tr.step(pool[it % len(pool)]).clone())
         assert len(tr.graphed.graphs) > 0
         losses[arm] = [float(x) for x in seq]
         tr.close()

@@ -51,20 +51,6 @@ def _bits(t):
     return t.view({8: torch.int64, 4: torch.int32, 2: torch.int16}[t.element_size()])
 
 
-def _step(tr, batch, graph):
-    tr.net.train()
-    tr.adjust_learning_rate()
-    if graph:
-        loss = tr.graphed.step(batch)
-    else:
-        tr.optimizer.zero_grad()
-        loss, _ = tr._forward_loss(batch)
-        tr.backward(loss)
-        tr.update_model()
-    tr._bookkeep_iter()
-    return loss.detach()
-
-
 def _leaves(o, out):
     if torch.is_tensor(o):
         out.append(o.detach().clone())
@@ -89,7 +75,7 @@ def _run(mode, graph, seq, hooks=None, **kw):
     for i, b in enumerate(seq):
         if hooks and i in hooks:
             hooks[i](tr)
-        loss = _step(tr, b, graph).clone()
+        loss = tr.step(b).clone()
         per_step.append((loss, tuple(h.detach().clone() for h in tr.hidden), tr.optimizer.loss_scale_state()))
     torch.cuda.synchronize()
     final = [p.detach().clone() for p in tr.net.parameters()] + _leaves(tr.optimizer.state_dict(), [])
@@ -215,14 +201,14 @@ def test_replay_loop_has_no_synchronisation(mode):
     tr = _trainer(mode, True)
     seq = _batches(8)
     for b in seq:
-        _step(tr, b, True)
+        tr.step(b)
     torch.cuda.synchronize()
     gs = tr.graphed
     n = len(gs.graphs)
     torch.cuda.set_sync_debug_mode("error")
     try:
         for b in seq:
-            _step(tr, b, True)
+            tr.step(b)
     finally:
         torch.cuda.set_sync_debug_mode(0)
     torch.cuda.synchronize()

@@ -156,10 +156,7 @@ def test_vgg_trainer_with_and_without_sgd_ahead_agree():
     pool = [tuple(t.to(trs[0].device) for t in bench.make_batch("vgg16", i, 0, bs, 128)) for i in range(4)]
     for it in range(3 + 40):
         for tr in trs:
-            tr.net.train()
-            tr.adjust_learning_rate()
-            tr.graphed.step(pool[it % 4])
-            tr._bookkeep_iter()
+            tr.step(pool[it % 4])
     torch.cuda.synchronize()
     assert calls, "the early SGD update never ran"
     a, b = (tr.optimizer for tr in trs)
