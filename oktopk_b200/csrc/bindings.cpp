@@ -774,6 +774,31 @@ static void frame_bn_backward(int conv, uint64_t x, uint64_t dy, uint64_t len, u
                                 P_<float>(dgamma), P_<float>(dbeta), N, C, F, Tb, dtype_arg(dtype, "frame_bn_backward"),
                                 S_(stream)), "frame_bn_backward");
 }
+// Look-ahead convolution + Hardtanh (csrc/lookahead.cu): x / y / dy / dx [Tb, N, H] of type dtype (codes as
+// dtype_arg); w / dw [H, K] fp32; len [N] int32.
+static void lookahead_check(const char* what, int N, int H, int Tb, int K, int dtype,
+                            std::initializer_list<uint64_t> elems, std::initializer_list<uint64_t> ptrs) {
+    if (!lookahead_supported(N, H, Tb, K))
+        throw std::runtime_error(std::string(what) + ": needs N, H, Tb > 0 and 1 <= K <= " +
+                                 std::to_string(lookahead_max_taps()) + " taps");
+    for (uint64_t p : ptrs)
+        if (p == 0 || (p & 3)) throw std::runtime_error(std::string(what) + ": null or misaligned pointer");
+    for (uint64_t p : elems)
+        if (p == 0 || (p & (dtype == 0 ? 3 : 1))) throw std::runtime_error(std::string(what) + ": null or misaligned tensor");
+}
+static void lookahead_forward(uint64_t x, uint64_t w, uint64_t len, uint64_t y, int N, int H, int Tb, int K, int dtype,
+                              uint64_t stream) {
+    lookahead_check("lookahead_forward", N, H, Tb, K, dtype, {x, y}, {w, len});
+    ck(launch_lookahead_forward(P_<const void>(x), P_<const float>(w), P_<const int>(len), P_<void>(y), N, H, Tb, K,
+                                dtype_arg(dtype, "lookahead_forward"), S_(stream)), "lookahead_forward");
+}
+static void lookahead_backward(uint64_t x, uint64_t y, uint64_t dy, uint64_t w, uint64_t len, uint64_t dx, uint64_t dw,
+                               int N, int H, int Tb, int K, int dtype, uint64_t stream) {
+    lookahead_check("lookahead_backward", N, H, Tb, K, dtype, {x, y, dy, dx}, {w, len, dw});
+    ck(launch_lookahead_backward(P_<const void>(x), P_<const void>(y), P_<const void>(dy), P_<const float>(w),
+                                 P_<const int>(len), P_<void>(dx), P_<float>(dw), N, H, Tb, K,
+                                 dtype_arg(dtype, "lookahead_backward"), S_(stream)), "lookahead_backward");
+}
 // Fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels [R] int64, rows [M] int32, tgt [M]
 // int64, slot [R] int32, count one int64, overflow one int64 or 0; x / dx [R, H] and out / dout [M, H] of type dtype.
 static void mlm_select(uint64_t labels, uint64_t rows, uint64_t tgt, uint64_t slot, uint64_t count, uint64_t overflow,
@@ -1081,6 +1106,13 @@ PYBIND11_MODULE(_C, m) {
           py::arg("gamma"), py::arg("beta"), py::arg("mean"), py::arg("rstd"), py::arg("dx"), py::arg("dgamma"),
           py::arg("dbeta"), py::arg("N"), py::arg("C"), py::arg("F"), py::arg("Tb"), py::arg("dtype"), py::arg("stream"));
     m.def("frame_bn_supported", &frame_bn_supported);
+    m.def("lookahead_forward", &lookahead_forward, py::arg("x"), py::arg("w"), py::arg("len"), py::arg("y"), py::arg("N"),
+          py::arg("H"), py::arg("Tb"), py::arg("K"), py::arg("dtype"), py::arg("stream"));
+    m.def("lookahead_backward", &lookahead_backward, py::arg("x"), py::arg("y"), py::arg("dy"), py::arg("w"),
+          py::arg("len"), py::arg("dx"), py::arg("dw"), py::arg("N"), py::arg("H"), py::arg("Tb"), py::arg("K"),
+          py::arg("dtype"), py::arg("stream"));
+    m.def("lookahead_supported", &lookahead_supported);
+    m.def("lookahead_max_taps", &lookahead_max_taps);
     m.def("ctc_workspace_floats", &ctc_workspace_floats);
     m.def("ctc_ab_floats", &ctc_ab_floats);
     m.def("mlm_select", &mlm_select, py::arg("labels"), py::arg("rows"), py::arg("tgt"), py::arg("slot"), py::arg("count"),

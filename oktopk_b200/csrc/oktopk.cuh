@@ -487,6 +487,16 @@ cudaError_t launch_frame_bn_forward(int conv, const void* x, const int* len, con
 cudaError_t launch_frame_bn_backward(int conv, const void* x, const void* dy, const int* len, const float* gamma,
                                      const float* beta, const float* mean, const float* rstd, void* dx, float* dgamma,
                                      float* dbeta, int N, int C, int F, int Tb, Dtype dtype, cudaStream_t stream);
+// look-ahead convolution + Hardtanh(0, 20) of DeepSpeech (csrc/lookahead.cu): x, y, dy and dx [Tb, N, H] of type
+// `dtype` (a Dtype); w and dw [H, K] fp32, K = context + 1 taps; len [N] int32 on the device.  Needs
+// lookahead_supported (K <= lookahead_max_taps()).  One launch each.
+bool lookahead_supported(int N, int H, int Tb, int K);
+int lookahead_max_taps();
+cudaError_t launch_lookahead_forward(const void* x, const float* w, const int* len, void* y, int N, int H, int Tb,
+                                     int K, Dtype dtype, cudaStream_t stream);
+cudaError_t launch_lookahead_backward(const void* x, const void* y, const void* dy, const float* w, const int* len,
+                                      void* dx, float* dw, int N, int H, int Tb, int K, Dtype dtype,
+                                      cudaStream_t stream);
 // fixed-capacity gather of the labelled masked-LM rows (csrc/mlm_gather.cu): labels and tgt int64, rows [M] and slot
 // [R] int32, count one int64, overflow one int64 that accumulates max(count - M, 0) (or null); x [R, H] and out [M, H],
 // dout [M, H] and dx [R, H] of type `dtype` (a Dtype).  One launch each.

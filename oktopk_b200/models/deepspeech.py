@@ -21,6 +21,9 @@ the BatchNorm1d in front of LSTM layers 1-4 and of ``fc`` likewise, with the len
 forward pass and shared with the LSTM layers.  Their statistics stop at the longest utterance, so a batch padded past it
 (``Trainer(an4_pad_multiple=m)``) gives the unpadded batch's loss and gradients to rounding.  Off the kernels' domain (CPU, eval mode, ...)
 those sites are the stock modules.
+``fuse_lookahead=True`` (or ``net.fuse_lookahead = True`` at any time) runs the look-ahead convolution and its Hardtanh
+on the kernels of ``ops/fused_lookahead.py``, one kernel per pass, the frames past each length read as 0 and written +0,
+with the same device copy of the lengths; the bidirectional network has no look-ahead and refuses it (``ValueError``).
 """
 from __future__ import annotations
 
@@ -32,6 +35,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.fused_frame_bn import conv_block_bn, seq_bn
+from ..ops.fused_lookahead import lookahead_hardtanh
 from ..ops.fused_lstm import lstm_layer, lstm_layer_device, lstm_stack, stock_layer
 
 AN4_LABELS = "_'ABCDEFGHIJKLMNOPQRSTUVWXYZ "     # 29 symbols, index 0 = CTC blank
@@ -139,7 +143,8 @@ class DeepSpeech(nn.Module):
     def __init__(self, rnn_hidden_size: int = 800, nb_layers: int = 5, labels: str = AN4_LABELS,
                  rnn_type=nn.LSTM, bidirectional: bool = False, context: int = 20, sample_rate: int = 16000,
                  window_size: float = 0.02, fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-                 fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False):
+                 fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False,
+                 fuse_lookahead: bool = False):
         super().__init__()
         self._labels = labels
         self._bidirectional = bidirectional
@@ -166,6 +171,19 @@ class DeepSpeech(nn.Module):
         self.fuse_lstm_bidirectional = fuse_lstm_bidirectional
         self.fuse_ctc = bool(fuse_ctc)
         self.fuse_bn = fuse_bn
+        self.fuse_lookahead = fuse_lookahead
+
+    @property
+    def fuse_lookahead(self) -> bool:
+        """Whether the look-ahead convolution and its Hardtanh take the fused kernels of ``ops/fused_lookahead.py``.
+        Setting it on the bidirectional network, which has no look-ahead, raises ``ValueError``."""
+        return self._fuse_lookahead
+
+    @fuse_lookahead.setter
+    def fuse_lookahead(self, on: bool) -> None:
+        if on and self.lookahead is None:
+            raise ValueError("fuse_lookahead needs the look-ahead convolution: the bidirectional network has none")
+        self._fuse_lookahead = bool(on)
 
     @property
     def fuse_bn(self) -> bool:
@@ -248,7 +266,7 @@ class DeepSpeech(nn.Module):
     def _forward(self, x: torch.Tensor, out_lens: torch.Tensor,
                  host_lens: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
         """``out_lens`` on the host (``host_lens`` the same tensor) or on the device only (``host_lens`` None)."""
-        # the fused batch-norm and LSTM layers read the lengths on the device: one copy for all of them
+        # the fused batch-norm, LSTM layers and look-ahead read the lengths on the device: one copy for all of them
         bn_lens = out_lens.to(x.device) if self.fuse_bn else None
         x = self.conv(x, out_lens, bn_lens)
         b, c, d, t = x.size()
@@ -259,7 +277,11 @@ class DeepSpeech(nn.Module):
         for rnn in self.rnns:
             x = rnn(x, host_lens, dev_lens, bn_lens)
         if self.lookahead is not None:
-            x = self.lookahead(x)
+            if self.fuse_lookahead:
+                la_lens = dev_lens if dev_lens is not None else bn_lens if bn_lens is not None else out_lens.to(x.device)
+                x = lookahead_hardtanh(x, self.lookahead[0].weight, la_lens)
+            else:
+                x = self.lookahead(x)
         x = self.fc(x, bn_lens).transpose(0, 1)                       # N x T x classes
         if not self.training:
             x = F.softmax(x, dim=-1)
@@ -268,11 +290,13 @@ class DeepSpeech(nn.Module):
 
 def lstman4(hidden_size: int = 800, hidden_layers: int = 5, bidirectional: bool = False,
             fuse_lstm: bool = False, fuse_lstm_autocast: bool = False,
-            fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False) -> DeepSpeech:
+            fuse_lstm_bidirectional: bool = False, fuse_ctc: bool = False, fuse_bn: bool = False,
+            fuse_lookahead: bool = False) -> DeepSpeech:
     """``VGG/models/lstman4.py:8`` defaults."""
     return DeepSpeech(rnn_hidden_size=hidden_size, nb_layers=hidden_layers, bidirectional=bidirectional,
                       fuse_lstm=fuse_lstm, fuse_lstm_autocast=fuse_lstm_autocast,
-                      fuse_lstm_bidirectional=fuse_lstm_bidirectional, fuse_ctc=fuse_ctc, fuse_bn=fuse_bn)
+                      fuse_lstm_bidirectional=fuse_lstm_bidirectional, fuse_ctc=fuse_ctc, fuse_bn=fuse_bn,
+                      fuse_lookahead=fuse_lookahead)
 
 
 class PTBLSTM(nn.Module):

@@ -78,6 +78,10 @@ SWITCHES = (
     Switch("--fused-ctc", ("fuse_ctc",), ("lstman4",),
            help="lstman4: the CTC loss runs on the fused softmax + CTC kernels, the lengths read on the device "
                 "and the backward deterministic (default: stock log_softmax + nn.CTCLoss)"),
+    Switch("--fused-lookahead", ("fuse_lookahead",), ("lstman4",),
+           help="lstman4: the look-ahead convolution and its Hardtanh run on one fused kernel per pass, the lengths "
+                "read on the device, the weight gradient deterministic and the weight kept in fp32 under autocast "
+                "(default: stock pad -> depthwise conv1d -> Hardtanh; not with --bidirectional)"),
     # a Trainer argument, not a create_net keyword
     Switch("--an4-pad-multiple", (), ("lstman4",), type=int, default=0, metavar="M",
            help="lstman4: pad every training batch's frames up to a multiple of M and keep its lengths on the "

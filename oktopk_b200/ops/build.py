@@ -18,7 +18,7 @@ CSRC = PKG / "csrc"
 BUILD = CSRC / "build"
 CU_SOURCES = ["oktopk.cu", "gather.cu", "gtopk.cu", "dense.cu", "optim.cu", "bnrelu.cu", "scale.cu", "layernorm.cu",
               "xent.cu", "lstm.cu", "mlm_gather.cu", "attention.cu", "ctc.cu", "embedding.cu",
-              "frame_bn.cu"]
+              "frame_bn.cu", "lookahead.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 HEADERS = ["common.cuh", "oktopk.cuh", "devlib.cuh", "elem.cuh"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

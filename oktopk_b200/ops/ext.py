@@ -20,7 +20,7 @@ _LAUNCHERS = {"oktopk_run": 1, "gather_run": 1, "gtopk_run": 1, "dense_run": 1, 
               "xent_forward": 2, "xent_backward": 1, "lstm_forward": 1, "lstm_backward": 1, "mlm_select": 1,
               "mlm_gather": 1, "mlm_scatter": 1, "attn_forward": 1, "attn_backward": 2, "lstm_seq_forward": 1,
               "lstm_seq_backward": 1, "ctc_forward": 2, "ctc_backward": 1, "emb_forward": 1, "emb_backward": 3,
-              "frame_bn_forward": 1, "frame_bn_backward": 1}
+              "frame_bn_forward": 1, "frame_bn_backward": 1, "lookahead_forward": 1, "lookahead_backward": 1}
 
 
 class _CountingModule:
