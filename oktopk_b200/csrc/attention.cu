@@ -8,9 +8,11 @@
 //
 // Tiling (FlashAttention-2): a CTA of 4 warps owns 64 rows of one (sequence, head); each warp owns 16 of them and every
 // product is a warp-level mma.sync over 64-wide tiles staged in shared memory.  The forward pass (one CTA per query
-// block) keeps a running row max, sum and fp32 accumulator over the key blocks and writes O and each row's log-sum-exp
-// (base 2, lse2 = log2 sum_j 2^(s_ij log2 e)); no S x S tensor is stored.  The backward pass recomputes
-// P = 2^(s log2 e - lse2) in two kernels, each writing every element it owns exactly once, with no atomics:
+// block) keeps a running row max, sum and fp32 accumulator over the key blocks and writes O and each row's final max m
+// and log2 l of its sum (base 2: m + log2 l = log2 sum_j 2^(s_ij log2 e)); no S x S tensor is stored.  The two are kept
+// apart because a row's max can be as large as the mask makes it, and m + log2 l in fp32 would then lose log2 l.  The
+// backward pass recomputes P = 2^((s log2 e - m) - log2 l) in two kernels, each writing every element it owns exactly
+// once, with no atomics:
 //   attn_bwd_dq_kernel  (one CTA per query block): Delta_i = dO_i . O_i (written out), then over the key blocks
 //                        dS = P o (dP o M - Delta) with dP = dO V^T, and dQ = sum dS K / sqrt(D);
 //   attn_bwd_dkv_kernel (one CTA per key block, after it): over the query blocks, with S^T and dP^T,
@@ -33,9 +35,15 @@
 // (p = 0) reads no seed and runs no generator.
 //
 // Ragged tiles: S need not be a multiple of 64.  Rows past S are staged as zeros; keys past S get the bias -inf, queries
-// past S the log-sum-exp +inf, so their P is exactly 0, and nothing past S is stored.  16-bit stores round to nearest
-// even without saturating, so an overflow arrives as inf.  A sequence whose mask is -inf at every key has l = 0 and
-// lse2 = -inf in every row: its O and d(qkv) are NaN, as softmax over an all -inf row is.
+// past S the row max +inf, so their P is exactly 0, and nothing past S is stored.  16-bit stores round to nearest
+// even without saturating, so an overflow arrives as inf.
+//
+// Masks: a finite mask entry gives a finite bias.  Where m log2 e overflows fp32 (torch.finfo(torch.float32).min, or
+// bf16's minimum widened) the bias saturates at -FLT_MAX, so a sequence masked at every key with such a minimum has
+// every score at -FLT_MAX and averages V uniformly, as the float64 formula does.  A sequence whose mask is -inf at every
+// key has m = -inf and l = 0 in every row: its O and d(qkv) are NaN, as softmax over an all -inf row is.
+#include <cfloat>
+
 #include "common.cuh"
 #include "devlib.cuh"
 #include "elem.cuh"
@@ -213,15 +221,19 @@ __device__ __forceinline__ float att_mult(const AttDrop& d, unsigned long long i
     return w < d.thr ? d.s : 0.f;
 }
 
-// the key bias of key j in log2 units: the mask's entry (0 without one), -inf past S
+// the key bias of key j in log2 units: the mask's entry (0 without one), -inf past S.  A finite entry saturates at
+// +-FLT_MAX instead of overflowing to +-inf; +-inf and NaN entries pass through.
 __device__ __forceinline__ float att_bias(const float* mask, int b, int S, int j) {
-    return j < S ? (mask != nullptr ? mask[(size_t)b * S + j] * kAttLog2e : 0.f) : -INFINITY;
+    if (j >= S) return -INFINITY;
+    if (mask == nullptr) return 0.f;
+    const float x = mask[(size_t)b * S + j];
+    return isfinite(x) ? fminf(fmaxf(x * kAttLog2e, -FLT_MAX), FLT_MAX) : x;
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const T* __restrict__ qkv, const float* __restrict__ mask,
                                                                const unsigned long long* seed, T* __restrict__ out,
-                                                               float* __restrict__ lse, int S, int H, long long keep_thr,
+                                                               float2* __restrict__ lse, int S, int H, long long keep_thr,
                                                                float dscale) {
     extern __shared__ __align__(16) unsigned char att_smem[];
     T* sq = reinterpret_cast<T*>(att_smem);
@@ -294,14 +306,14 @@ __global__ void __launch_bounds__(kAttThreads) attn_fwd_kernel(const T* __restri
         T* orow = out + ((long long)b * S + i) * HD + h * kAttD + 2 * t;
 #pragma unroll
         for (int nt = 0; nt < kAttNt; ++nt) Elem<T>::st2(orow + nt * 8, o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
-        if (t == 0) lse[bh * S + i] = mx[r] + log2f(l[r]);
+        if (t == 0) lse[bh * S + i] = make_float2(mx[r], log2f(l[r]));
     }
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __restrict__ qkv, const T* __restrict__ out,
                                                                   const T* __restrict__ dout, const float* __restrict__ mask,
-                                                                  const unsigned long long* seed, const float* __restrict__ lse,
+                                                                  const unsigned long long* seed, const float2* __restrict__ lse,
                                                                   float* __restrict__ delta, T* __restrict__ dqkv, int S,
                                                                   int H, long long keep_thr, float dscale) {
     extern __shared__ __align__(16) unsigned char att_smem[];
@@ -322,7 +334,8 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __res
     att_stage(sdo, dout + ((long long)b * S + q0) * HD + h * kAttD, HD, min(kAttBlk, S - q0));
     __syncthreads();
     // Delta of rows g, g + 8: lane t adds columns 16t .. 16t + 15, then the four lanes in lane order
-    float dl[2], ls[2];
+    float dl[2];
+    float2 ls[2];                                       // the row's max and log2 of its sum
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int i = q0 + row0 + g + 8 * r;
@@ -336,7 +349,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __res
         acc += __shfl_xor_sync(0xffffffffu, acc, 1);
         acc += __shfl_xor_sync(0xffffffffu, acc, 2);
         dl[r] = acc;
-        ls[r] = i < S ? lse[bh * S + i] : INFINITY;
+        ls[r] = i < S ? lse[bh * S + i] : make_float2(INFINITY, 0.f);
         if (t == 0 && i < S) delta[bh * S + i] = acc;
     }
     float dq[kAttNt][4];
@@ -357,7 +370,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dq_kernel(const T* __res
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int r = e >> 1, col = nt * 8 + 2 * t + (e & 1);
-                const float p = exp2f(fmaf(s[nt][e], c, sbias[col]) - ls[r]);
+                const float p = exp2f(fmaf(s[nt][e], c, sbias[col]) - ls[r].x - ls[r].y);
                 const long long i = q0 + row0 + g + 8 * r, j = k0 + col;
                 s[nt][e] = p * (dp[nt][e] * att_mult(d, (unsigned long long)((bh * S + i) * S + j)) - dl[r]);
             }
@@ -377,7 +390,7 @@ template <typename T>
 __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __restrict__ qkv, const T* __restrict__ dout,
                                                                    const float* __restrict__ mask,
                                                                    const unsigned long long* seed,
-                                                                   const float* __restrict__ lse,
+                                                                   const float2* __restrict__ lse,
                                                                    const float* __restrict__ delta, T* __restrict__ dqkv,
                                                                    int S, int H, long long keep_thr, float dscale) {
     extern __shared__ __align__(16) unsigned char att_smem[];
@@ -385,8 +398,9 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __re
     T* sv = sk + kAttBlk * kAttLd;
     T* sq = sv + kAttBlk * kAttLd;
     T* sdo = sq + kAttBlk * kAttLd;
-    float* slse = reinterpret_cast<float*>(sdo + kAttBlk * kAttLd);
-    float* sdl = slse + kAttBlk;
+    float* smx = reinterpret_cast<float*>(sdo + kAttBlk * kAttLd);      // the query rows' max, log2 sum and Delta
+    float* sll = smx + kAttBlk;
+    float* sdl = sll + kAttBlk;
     const int b = blockIdx.z, h = blockIdx.y, j0 = blockIdx.x * kAttBlk;
     const int lane = lane_id(), g = lane >> 2, t = lane & 3, row0 = (threadIdx.x >> 5) * 16;
     const int HD = H * kAttD;
@@ -407,7 +421,9 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __re
         att_stage(sdo, dout + ((long long)b * S + i0) * HD + h * kAttD, HD, min(kAttBlk, S - i0));
         for (int i = threadIdx.x; i < kAttBlk; i += kAttThreads) {
             const bool in = i0 + i < S;
-            slse[i] = in ? lse[bh * S + i0 + i] : INFINITY;
+            const float2 st = in ? lse[bh * S + i0 + i] : make_float2(INFINITY, 0.f);
+            smx[i] = st.x;
+            sll[i] = st.y;
             sdl[i] = in ? delta[bh * S + i0 + i] : 0.f;
         }
         __syncthreads();
@@ -426,7 +442,7 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __re
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int r = e >> 1, col = c0 + nt * 8 + 2 * t + (e & 1);
-                    const float p = exp2f(fmaf(s[nt][e], c, kb[r]) - slse[col]);
+                    const float p = exp2f(fmaf(s[nt][e], c, kb[r]) - smx[col] - sll[col]);
                     const long long i = i0 + col, j = j0 + row0 + g + 8 * r;
                     const float m = att_mult(d, (unsigned long long)((bh * S + i) * S + j));
                     s[nt][e] = p * m;
@@ -451,10 +467,10 @@ __global__ void __launch_bounds__(kAttThreads) attn_bwd_dkv_kernel(const T* __re
 
 bool attn_supported(int B, int S, int H) { return B >= 1 && B <= 65535 && H >= 1 && H <= 65535 && S >= 1 && S <= kAttMaxS; }
 
-// Dynamic shared memory: 3 (forward) or 4 (backward) padded tiles and 64 or 128 floats.  fp32 needs more than the
+// Dynamic shared memory: 3 (forward) or 4 (backward) padded tiles and 64 or 192 floats.  fp32 needs more than the
 // default 48 KB, so each kernel's limit is raised once per device and the launches after that query nothing.
 template <typename T> constexpr size_t att_smem_fwd() { return 3 * kAttBlk * kAttLd * sizeof(T) + kAttBlk * sizeof(float); }
-template <typename T> constexpr size_t att_smem_bwd() { return 4 * kAttBlk * kAttLd * sizeof(T) + 2 * kAttBlk * sizeof(float); }
+template <typename T> constexpr size_t att_smem_bwd() { return 4 * kAttBlk * kAttLd * sizeof(T) + 3 * kAttBlk * sizeof(float); }
 
 template <typename T, int Kernel>
 static cudaError_t att_prepare(const void* kernel, size_t smem) {
@@ -482,7 +498,8 @@ static cudaError_t attn_forward_t(const void* qkv, const float* mask, const unsi
     cudaError_t e = att_prepare<T, 0>((const void*)attn_fwd_kernel<T>, smem);
     if (e != cudaSuccess) return e;
     attn_fwd_kernel<T><<<att_grid(B, S, H), kAttThreads, smem, stream>>>(static_cast<const T*>(qkv), mask, seed,
-                                                                        static_cast<T*>(out), lse, S, H, keep_thr, scale);
+                                                                        static_cast<T*>(out), reinterpret_cast<float2*>(lse),
+                                                                        S, H, keep_thr, scale);
     return cudaGetLastError();
 }
 
@@ -497,11 +514,12 @@ static cudaError_t attn_backward_t(const void* qkv, const void* out, const void*
     const T* q = static_cast<const T*>(qkv);
     const T* dt = static_cast<const T*>(dout);
     T* dq = static_cast<T*>(dqkv);
+    const float2* st = reinterpret_cast<const float2*>(lse);
     attn_bwd_dq_kernel<T><<<att_grid(B, S, H), kAttThreads, smem, stream>>>(q, static_cast<const T*>(out), dt, mask, seed,
-                                                                           lse, delta, dq, S, H, keep_thr, scale);
+                                                                           st, delta, dq, S, H, keep_thr, scale);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    attn_bwd_dkv_kernel<T><<<att_grid(B, S, H), kAttThreads, smem, stream>>>(q, dt, mask, seed, lse, delta, dq, S, H,
+    attn_bwd_dkv_kernel<T><<<att_grid(B, S, H), kAttThreads, smem, stream>>>(q, dt, mask, seed, st, delta, dq, S, H,
                                                                             keep_thr, scale);
     return cudaGetLastError();
 }

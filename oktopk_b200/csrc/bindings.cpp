@@ -664,8 +664,8 @@ static void emb_backward(uint64_t ids, uint64_t tt, uint64_t word, uint64_t pos,
                            nv, np, nt, p_keep_thr, (float)scale, S_(stream)), "emb_backward");
 }
 // Fused self-attention, head dim 64 (csrc/attention.cu): qkv / dqkv [B, S, 3 H 64] and out / dout [B, S, H 64] of type
-// dtype (codes as dtype_arg), 16-byte aligned; mask [B, S] fp32 or 0; lse / delta [B, H, S] fp32.  p_keep_thr and seed as
-// for ln_forward; scale = 1 / (1 - p).
+// dtype (codes as dtype_arg), 16-byte aligned; mask [B, S] fp32 or 0; lse [B, H, S, 2] and delta [B, H, S] fp32, 8-byte
+// aligned.  p_keep_thr and seed as for ln_forward; scale = 1 / (1 - p).
 static void attn_check(const char* what, int B, int S, int H, long long p_keep_thr, uint64_t seed,
                        std::initializer_list<uint64_t> vec_ptrs, std::initializer_list<uint64_t> f32_ptrs) {
     if (!attn_supported(B, S, H)) throw std::runtime_error(std::string(what) + ": needs B, H >= 1 and 1 <= S <= 512");
@@ -674,7 +674,7 @@ static void attn_check(const char* what, int B, int S, int H, long long p_keep_t
     for (uint64_t p : vec_ptrs)
         if (p == 0 || (p & 15)) throw std::runtime_error(std::string(what) + ": tensors must be non-null and 16-byte aligned");
     for (uint64_t p : f32_ptrs)
-        if (p == 0 || (p & 3)) throw std::runtime_error(std::string(what) + ": lse / delta must be non-null fp32");
+        if (p == 0 || (p & 7)) throw std::runtime_error(std::string(what) + ": lse / delta must be non-null, 8-byte aligned");
 }
 static void attn_forward(uint64_t qkv, uint64_t mask, uint64_t seed, uint64_t out, uint64_t lse, int B, int S, int H,
                          long long p_keep_thr, double scale, int dtype, uint64_t stream) {

@@ -533,8 +533,9 @@ cudaError_t launch_lstm_seq_backward(const void* dy, const float* gates, const f
                                      unsigned long long* bar, int T, int N, int H, int u, int rows, int r_on, int kc,
                                      cudaStream_t stream, Dtype dtype);
 // fused self-attention, head dim 64 (csrc/attention.cu): qkv and dqkv [B, S, 3 H 64], out and dout [B, S, H 64], all of
-// type `dtype` (a Dtype), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse and delta [B, H, S]
-// fp32 (lse written by the forward pass, delta scratch of the backward pass).  keep_thr >= 2^32 turns the dropout off
+// type `dtype` (a Dtype), 16-byte aligned; mask [B, S] fp32 additive key bias or null; lse [B, H, S, 2] fp32, 8-byte
+// aligned (each row's max and log2 of its sum, base 2, written by the forward pass); delta [B, H, S] fp32 (scratch of
+// the backward pass).  keep_thr >= 2^32 turns the dropout off
 // (seed may then be null); `scale` is the kept elements' 1 / (1 - p).  One launch forward, two backward.
 bool attn_supported(int B, int S, int H);
 cudaError_t launch_attn_forward(const void* qkv, const float* mask, const unsigned long long* seed, void* out, float* lse,

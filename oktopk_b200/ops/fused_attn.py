@@ -8,7 +8,8 @@ returns ``[B, S, H·D]``: per sequence b, head h and query i, with D = 64,
 which is what ``F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)`` computes with the additive
 ``[B, 1, 1, S]`` key-padding mask (dropout on the normalised probabilities).  On CUDA it is one kernel forward and two
 backward, reading Q, K and V straight out of ``qkv`` and writing the output and d(qkv) in their final layouts, with no
-S x S tensor stored: the backward pass recomputes P from the saved per-row log-sum-exp.  d(qkv) is the only gradient.
+S x S tensor stored: the backward pass recomputes P from each row's saved max and log-sum, kept apart so that the sum
+survives beside a max of any magnitude.  d(qkv) is the only gradient.
 
 Dropout (``ops/fused_ln.py``'s convention): each call draws one int64 seed on the device from torch's default CUDA
 generator, and element (b, h, i, j), flat index ``((b·H + h)·S + i)·S + j`` over [B, H, S, S], is kept iff word
@@ -23,9 +24,12 @@ over a 16-bit tensor and the mask stays fp32: the kernels read the fp32 mask as 
 rounds the mask to the 16-bit type (BERT's -10000 becomes -9984 in bf16; either way a padded key's weight is 0 in fp32).
 The backward pass is deterministic: no atomics, a fixed order of every sum.
 
-A sequence whose mask is -inf at every key has no finite score in any row: its output and its rows of d(qkv) are NaN,
-as ``torch.softmax`` over an all -inf row is.  BERT's ``(1 - m) · -10000`` mask never does this (a padded key's weight
-underflows to 0 instead), and neither does any mask with at least one finite entry per sequence.
+A finite mask entry always gives a finite score, even where the kernels' conversion to base 2 (``mask · log2 e``) would
+overflow fp32: it saturates at the largest finite float.  So a sequence masked at every key with a finite value, BERT's
+``(1 - m) · -10000`` or ``torch.finfo(torch.float32).min`` alike, gets a softmax over its scores as float64 computes
+it; with ``finfo.min``, whose scores all round to the same value, that is the uniform average of V.  A sequence whose
+mask is -inf at every key has no finite score in any row: its output and its rows of d(qkv) are NaN, as
+``torch.softmax`` over an all -inf row is.
 
 Falls back to exactly today's expression (view, permute, ``F.scaled_dot_product_attention``, transpose, reshape)
 wherever the fast path does not apply: CPU tensors or no native extension, ``qkv`` not a 3-d fp32 / bf16 / fp16 tensor,
@@ -64,7 +68,7 @@ class _FusedAttention(torch.autograd.Function):
         B, S, _ = qkv.shape
         seed = torch.empty(1, dtype=torch.int64, device=qkv.device).random_() if p > 0 else None
         out = torch.empty((B, S, heads * HEAD_DIM), dtype=qkv.dtype, device=qkv.device)
-        lse = torch.empty((B, heads, S), dtype=torch.float32, device=qkv.device)
+        lse = torch.empty((B, heads, S, 2), dtype=torch.float32, device=qkv.device)    # each row's max, log2 of its sum
         thr, scale = keep_threshold(p), 1.0 / (1.0 - p)
         C.attn_forward(qkv.data_ptr(), 0 if mask is None else mask.data_ptr(), 0 if seed is None else seed.data_ptr(),
                        out.data_ptr(), lse.data_ptr(), B, S, heads, thr, scale, DTYPE_CODE[qkv.dtype],
@@ -80,7 +84,7 @@ class _FusedAttention(torch.autograd.Function):
         B, S, _ = qkv.shape
         dout = dense16(dout.to(qkv.dtype))
         dqkv = torch.empty_like(qkv)
-        delta = torch.empty_like(lse)
+        delta = torch.empty((B, ctx.heads, S), dtype=torch.float32, device=qkv.device)
         C.attn_backward(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), 0 if mask is None else mask.data_ptr(),
                         0 if seed is None else seed.data_ptr(), lse.data_ptr(), delta.data_ptr(), dqkv.data_ptr(), B, S,
                         ctx.heads, ctx.thr, ctx.scale, DTYPE_CODE[qkv.dtype], torch.cuda.current_stream().cuda_stream)

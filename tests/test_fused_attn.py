@@ -1,6 +1,8 @@
 """Fused self-attention (``ops/fused_attn.py``, ``csrc/attention.cu``) on the GPU: O and d(qkv) against a float64
-reference of the formula (within twice stock SDPA's error plus a few ulps), the Philox dropout mask against a NumPy
-Philox4x32-10, determinism, checkpoint recompute and CUDA-graph replays, fp16 overflow, the whole BERT model, a graphed
+reference of the formula (within twice stock SDPA's error plus a few ulps) at every 64-row tile edge, on skewed score
+rows and at the masks' extremes, fully masked sequences, per-slice independence, the largest grid and unaligned
+inputs; the Philox dropout mask against a NumPy Philox4x32-10, read off element by element at rates up to 0.99 and past
+counter 2^32; determinism, checkpoint recompute and CUDA-graph replays, fp16 overflow, the whole BERT model, a graphed
 Trainer step with every fused BERT op, and the fallbacks."""
 import copy
 
@@ -42,18 +44,17 @@ def seed_of(s):
     return int(torch.empty(1, dtype=torch.int64, device="cuda").random_().item())
 
 
-def keep_mask(seed, B, H, S, p):
-    """[B, H, S, S] bool: element idx = ((b H + h) S + i) S + j is kept iff word idx % 4 at counter idx // 4 is below
-    floor((1-p) 2^32)."""
+def keep_mask(seed, B, H, S, p, b0=0):
+    """[B, H, S, S] bool for the sequences b0 .. b0 + B - 1: element idx = ((b H + h) S + i) S + j is kept iff word
+    idx % 4 at counter idx // 4 is below floor((1-p) 2^32)."""
     from oktopk_b200.ops.fused_ln import keep_threshold
-    n = B * H * S * S
-    nq = (n + 3) // 4
-    q = np.arange(nq, dtype=np.uint64)
-    ctr = np.zeros((nq, 4), np.uint32)
+    n, lo = B * H * S * S, b0 * H * S * S
+    q = np.arange(lo // 4, (lo + n + 3) // 4, dtype=np.uint64)
+    ctr = np.zeros((len(q), 4), np.uint32)
     ctr[:, 0] = (q & np.uint64(0xFFFFFFFF)).astype(np.uint32)
     ctr[:, 1] = (q >> np.uint64(32)).astype(np.uint32)
     u = seed & ((1 << 64) - 1)
-    words = philox4x32_10(ctr, (u & 0xFFFFFFFF, u >> 32)).reshape(-1)[:n]
+    words = philox4x32_10(ctr, (u & 0xFFFFFFFF, u >> 32)).reshape(-1)[lo % 4:lo % 4 + n]
     return torch.from_numpy(words.astype(np.int64) < keep_threshold(p)).view(B, H, S, S).cuda()
 
 
@@ -126,12 +127,30 @@ def _within(got, base, want, dtype, what):
     assert e <= tol, (what, e, eb, tol)
 
 
+def _reference(qkv, dout, H, mask):
+    """(O, d(qkv)) of the float64 formula and of stock SDPA in qkv's dtype."""
+    ref = _run(lambda x: _formula(x, H, mask.double() if mask is not None else None, None, 0.0), qkv.double(),
+               dout.double())
+    return ref, _stock(qkv, dout, H, mask)
+
+
+def _check(o, g, qkv, dout, H, mask, what=""):
+    """The fused (o, g) of (qkv, dout, mask) at p = 0 within the criterion of _within, O and d(qkv)."""
+    (od, gd), (os_, gs) = _reference(qkv, dout, H, mask)
+    _within(o, os_, od, qkv.dtype, what + "O")
+    _within(g, gs, gd, qkv.dtype, what + "dqkv")
+
+
 DTYPES = [torch.float32, torch.bfloat16, torch.float16]
-SHAPES = [(8, 128, 12), (2, 512, 16), (3, 1, 2), (3, 7, 2), (2, 100, 3), (2, 129, 2), (2, 200, 2)]
+# 64-row tiles: S = 64 k - 1, 64 k, 64 k + 1 around every boundary up to 512 (64 k + 1 leaves a final query and key
+# tile with one valid row), one and three heads
+TILE_EDGES = [63, 64, 65, 127, 191, 192, 193, 255, 256, 257, 383, 384, 385, 447, 448, 449, 511]
+SHAPES = ([(8, 128, 12), (2, 512, 16), (3, 1, 2), (3, 7, 2), (2, 100, 3), (2, 129, 2), (2, 200, 2)]
+          + [(2, S, H) for S in TILE_EDGES for H in (1, 3)] + [(4, 256, 2)])
 
 
 # ------------------------------------------------------------------------------------------ 1. accuracy at p = 0
-@pytest.mark.parametrize("masking", ["none", "padding", "single_key"])
+@pytest.mark.parametrize("masking", ["none", "padding", "single_key", "tiles"])
 @pytest.mark.parametrize("B,S,H", SHAPES)
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_matches_float64_reference(dtype, B, S, H, masking):
@@ -141,16 +160,185 @@ def test_matches_float64_reference(dtype, B, S, H, masking):
     elif masking == "single_key":
         lengths = [S] * B
         lengths[-1] = 1
+    elif masking == "tiles":                            # whole key tiles padded: lengths 1, 63, 64, 65
+        lengths = [min(S, (1, 63, 64, 65)[b % 4]) for b in range(B)]
     qkv, dout, mask = _inputs(B, S, H, dtype, B * 1000 + S + H, lengths)
     n0 = _counts()
     o, g = _fused(qkv, dout, H, mask, 0.0)
     assert _delta(n0) == {"attn_forward": 1, "attn_backward": 2}
     assert o.dtype == g.dtype == dtype and o.shape == (B, S, H * D) and g.shape == qkv.shape
-    od, gd = _run(lambda x: _formula(x, H, mask.double() if mask is not None else None, None, 0.0), qkv.double(),
-                  dout.double())
-    os_, gs = _stock(qkv, dout, H, mask)
-    _within(o, os_, od, dtype, "O")
-    _within(g, gs, gd, dtype, "dqkv")
+    _check(o, g, qkv, dout, H, mask)
+
+
+def _skewed(case, B, S, H, dtype, seed):
+    """Inputs whose score rows are far from N(0, 1): see test_skewed_score_rows_match_float64_reference."""
+    gen = torch.Generator("cuda").manual_seed(seed)
+    x = torch.randn(B, S, 3, H, D, device="cuda", generator=gen)
+    mask = None
+    if case in ("rising", "falling"):
+        ramp = torch.linspace(-1.0, 1.0, S, device="cuda")
+        x[:, :, :2] *= 0.1
+        x[:, :, 0, :, 0] = 16.0                         # s_ij ~ 16 * 20 / 8 * ramp_j: -40 .. 40 along the keys
+        x[:, :, 1, :, 0] = 20.0 * (ramp if case == "rising" else ramp.flip(0))[None, :, None]
+    elif case == "wide":                                # score std ~ 12: P underflows for most keys of a row
+        x[:, :, :2] *= 3.5
+    elif case == "off_centre":                          # scores ~ 128 +- 6: the split and lse precision in fp32
+        x[:, :, :2] += 4.0
+    elif case == "constant":                            # q = 0: P uniform
+        x[:, :, 0] = 0.0
+    elif case == "first_tile_masked":                   # the row max jumps from ~ -14427 to ~ 0 in key block 1
+        mask = torch.zeros(B, 1, 1, S, device="cuda")
+        mask[..., :64] = -10000.0
+    dout = torch.randn(B, S, H * D, device="cuda", generator=gen).to(dtype)
+    return x.reshape(B, S, 3 * H * D).to(dtype), dout, mask
+
+
+@pytest.mark.parametrize("case", ["rising", "falling", "wide", "off_centre", "constant", "first_tile_masked"])
+@pytest.mark.parametrize("S", [65, 256, 512])
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_skewed_score_rows_match_float64_reference(dtype, S, case):
+    """Rows whose max arrives in a late key block (rising), sits in the first one (falling), or jumps out of a masked
+    first tile, so that the running max's rescale factor is far from 1; rows where most of P underflows; scores far
+    from 0; and uniform rows."""
+    B, H = 2, 2
+    qkv, dout, mask = _skewed(case, B, S, H, dtype, 300 + S)
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    _check(o, g, qkv, dout, H, mask)
+
+
+def _fill(name, dtype):
+    return {"-inf": float("-inf"), "-1e9": -1e9, "bert": -10000.0, "f32_min": torch.finfo(torch.float32).min,
+            "dtype_min": torch.finfo(dtype).min}[name]
+
+
+@pytest.mark.parametrize("fill", ["-inf", "-1e9", "f32_min", "dtype_min"])
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_extreme_partial_masks_match_float64_reference(dtype, fill):
+    """Sequence 0 masks its whole first key tile, 1 every third key, 2 its two middle tiles, all with `fill`; every row
+    keeps finite keys.  Stock SDPA takes the mask in qkv's type, where f32_min and -1e9 (fp16) round to -inf."""
+    B, S, H = 3, 200, 2
+    qkv, dout, _ = _inputs(B, S, H, dtype, 70)
+    j = torch.arange(S, device="cuda")
+    masked = torch.stack([j < 64, j % 3 == 0, (j >= 64) & (j < 192)])
+    mask = torch.where(masked, _fill(fill, dtype), 0.0)[:, None, None, :].float()
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    _check(o, g, qkv, dout, H, mask)
+
+
+FULL = [(d, f) for d in DTYPES for f in ("bert", "f32_min", "dtype_min") if (d, f) != (torch.float32, "dtype_min")]
+
+
+@pytest.mark.parametrize("dtype,fill", FULL, ids=["%s-%s" % (str(d)[6:], f) for d, f in FULL])
+def test_fully_masked_sequence_matches_float64_reference(dtype, fill):
+    """Sequence 1 masked at every key with a finite `fill`, between a full and a padded one.  Where fill * log2 e
+    overflows fp32 (f32_min, bf16's minimum), float64 absorbs every score into the fill, so its softmax is uniform and
+    O the plain average of V: the fused result must be that within ULPS ulps.  Stock SDPA is no yardstick there (it may
+    give NaN).  Below that (-10000, fp16's -65504) fp32 holds a biased score only to 2^-24 of its magnitude, 2^-11 at
+    -10000 log2 e, which float64's exact scores are beyond; the criterion is stock's, which is finite there."""
+    B, S, H = 3, 200, 2
+    qkv, dout, mask = _inputs(B, S, H, dtype, 80, [S, S, 150])
+    v = _fill(fill, dtype)
+    mask[1] = v
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    for b in (0, 2):
+        _check(o[b:b + 1], g[b:b + 1], qkv[b:b + 1], dout[b:b + 1], H, mask[b:b + 1], "seq %d " % b)
+    x, dy, m = qkv[1:2], dout[1:2], mask[1:2]
+    if abs(v) * np.log2(np.e) > torch.finfo(torch.float32).max:
+        (od, gd), _ = _reference(x, dy, H, m)
+        mean_v = x.double().view(S, 3, H, D)[:, 2].mean(0).reshape(1, 1, H * D).expand(1, S, H * D)
+        torch.testing.assert_close(od, mean_v, rtol=1e-12, atol=1e-12)
+        for got, want, what in ((o[1:2], od, "O"), (g[1:2], gd, "dqkv")):
+            tol = ULPS * EPS[dtype] * float(want.abs().max())
+            assert _err(got, want) <= tol, (what, _err(got, want), tol)
+    else:
+        _check(o[1:2], g[1:2], x, dy, H, m, "seq 1 ")
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_all_inf_sequence_is_nan_and_leaves_the_others_alone(dtype):
+    B, S, H = 3, 200, 2
+    qkv, dout, mask = _inputs(B, S, H, dtype, 90, [S, 150, 77])
+    o0, g0 = _fused(qkv, dout, H, mask, 0.0)
+    mask[1] = float("-inf")
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    assert torch.isnan(o[1]).all() and torch.isnan(g[1]).all()
+    rest = [0, 2]
+    assert torch.isfinite(o[rest]).all() and torch.isfinite(g[rest]).all()
+    assert torch.equal(o[rest], o0[rest]) and torch.equal(g[rest], g0[rest])
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_16bit_mask_is_the_fp32_mask_of_its_values(dtype):
+    B, S, H = 3, 130, 2
+    qkv, dout, _ = _inputs(B, S, H, dtype, 95)
+    gen = torch.Generator("cuda").manual_seed(96)
+    mask = torch.randn(B, 1, 1, S, device="cuda", generator=gen) * 3
+    mask[0, ..., 100:] = -10000.0                       # -9984 in bf16
+    mask[2, ..., :70] = torch.finfo(dtype).min
+    mask = mask.to(dtype)
+    n0 = _counts()
+    a = _fused(qkv, dout, H, mask, 0.0)
+    b = _fused(qkv, dout, H, mask.float(), 0.0)
+    assert _delta(n0) == {"attn_forward": 2, "attn_backward": 4}
+    for u, v in zip(a, b):
+        assert torch.equal(u, v)
+
+
+@pytest.mark.parametrize("S", [65, 200, 512])
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_every_sequence_and_head_is_its_own_launch(dtype, S):
+    """Every sum's order depends on S alone, so each (b, h) slice of a batched launch is bit for bit a launch on that
+    slice by itself: anything else is an indexing bug."""
+    B, H = 3, 5
+    qkv, dout, mask = _inputs(B, S, H, dtype, 600 + S, [S, S - 13, 1])
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    q5, d5, o5, g5 = qkv.view(B, S, 3, H, D), dout.view(B, S, H, D), o.view(B, S, H, D), g.view(B, S, 3, H, D)
+    for b in range(B):
+        for h in range(H):
+            x = q5[b:b + 1, :, :, h].reshape(1, S, 3 * D)
+            ob, gb = _fused(x, d5[b:b + 1, :, h].contiguous(), 1, mask[b:b + 1], 0.0)
+            assert torch.equal(ob.view(1, S, D), o5[b:b + 1, :, h]), (b, h)
+            assert torch.equal(gb.view(1, S, 3, D), g5[b:b + 1, :, :, h]), (b, h)
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_largest_grid_matches_float64_reference(dtype):
+    """65535 sequences, the most grid.z takes; by the test above a sample of sequences stands for all of them."""
+    B, S, H = 65535, 64, 1
+    qkv, dout, mask = _inputs(B, S, H, dtype, 65, [1 + (37 * b) % S for b in range(B)])
+    n0 = _counts()
+    o, g = _fused(qkv, dout, H, mask, 0.0)
+    assert _delta(n0) == {"attn_forward": 1, "attn_backward": 2}
+    for b in (0, 1, 40000, B - 2, B - 1):
+        s = slice(b, b + 1)
+        _check(o[s], g[s], qkv[s], dout[s], H, mask[s], "seq %d " % b)
+    del qkv, dout, o, g
+    torch.cuda.empty_cache()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_misaligned_qkv_strided_dout_and_mask_match_the_dense_result(dtype):
+    """qkv 2 or 4 bytes past a 16-byte boundary, dout and the mask every other element of a wider tensor: the op copies
+    them dense and aligned, and the result is bit for bit that of the dense inputs."""
+    from oktopk_b200.ops.fused_attn import self_attention
+    B, S, H = 2, 100, 3
+    qkv, dout, mask = _inputs(B, S, H, dtype, 45, [S, 61])
+    o0, g0 = _fused(qkv, dout, H, mask, 0.0)
+    buf = torch.zeros(qkv.numel() + 1, dtype=dtype, device="cuda")
+    buf[1:] = qkv.reshape(-1)
+    buf.requires_grad_(True)
+    x = buf[1:].view(qkv.shape)
+    wide = torch.zeros(B, S, 2 * H * D, dtype=dtype, device="cuda")
+    wide[..., ::2] = dout
+    wmask = torch.zeros(B, 1, 1, 2 * S, device="cuda")
+    wmask[..., ::2] = mask
+    dy, m = wide[..., ::2], wmask[..., ::2]
+    assert x.data_ptr() % 16 != 0 and not dy.is_contiguous() and not m.is_contiguous()
+    n0 = _counts()
+    o = self_attention(x, H, m, 0.0)
+    o.backward(dy)
+    assert _delta(n0) == {"attn_forward": 1, "attn_backward": 2}
+    assert torch.equal(o.detach(), o0) and torch.equal(buf.grad[1:].view(qkv.shape), g0)
 
 
 # ------------------------------------------------------------------------------------------ 2. dropout
@@ -179,6 +367,63 @@ def test_kept_fraction_of_the_kernel():
     frac = float(o.mean()) * (1 - p)
     sigma = (p * (1 - p) / (B * H * S * S)) ** 0.5
     assert abs(frac - (1 - p)) < 6 * sigma
+
+
+@pytest.mark.parametrize("p", [1e-3, 0.5, 0.9, 0.99])
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_dropout_mask_and_scale_are_exact_at_every_rate(dtype, p):
+    """With q = 0 every P_ij is 1/S, and with S = D = 64, v_j = e_j and dO_i = e_i, O[b, i, h, j] and dV[b, j, h, i]
+    are both keep(b,h,i,j) / (1-p) / S: the forward and the backward mask read off element by element.  Then O and
+    d(qkv) of random inputs against the formula with keep_mask."""
+    B, S, H = 2, 64, 3
+    eye = torch.eye(S, device="cuda")
+    x = torch.zeros(B, S, 3, H, D, device="cuda")
+    x[:, :, 1] = torch.randn(B, S, H, D, device="cuda", generator=torch.Generator("cuda").manual_seed(1))
+    x[:, :, 2] = eye[None, :, None, :]
+    qkv = x.view(B, S, -1).to(dtype)
+    dout = eye[None, :, None, :].expand(B, S, H, D).reshape(B, S, H * D).to(dtype)
+    o, g = _fused(qkv, dout, H, None, p, cuda_seed=31)
+    keep = keep_mask(seed_of(31), B, H, S, p)
+    fo = o.view(B, S, H, D).permute(0, 2, 1, 3)                     # [b, h, i, j]
+    dv = g.view(B, S, 3, H, D)[:, :, 2].permute(0, 2, 3, 1)         # [b, h, i, j]
+    value = (1.0 / (1.0 - p)) / S
+    for got, what in ((fo, "forward"), (dv, "backward")):
+        assert torch.equal(got != 0, keep), what
+        err = float((got[keep].double() - value).abs().max())
+        assert err <= 2 * EPS[dtype] * value, (what, err, value)
+
+    B, S, H = 2, 77, 3
+    qkv, dout, mask = _inputs(B, S, H, dtype, 7 + S, [S, 40])
+    o, g = _fused(qkv, dout, H, mask, p, cuda_seed=32)
+    keep = keep_mask(seed_of(32), B, H, S, p)
+    od, gd = _run(lambda x: _formula(x, H, mask.double(), keep, p), qkv.double(), dout.double())
+    of, gf = _run(lambda x: _formula(x, H, mask.to(dtype), keep, p), qkv, dout)
+    _within(o, of, od, dtype, "O")
+    _within(g, gf, gd, dtype, "dqkv")
+
+
+def test_dropout_counter_past_2_32():
+    """B H S^2 > 2^34, so the Philox counter idx // 4 passes 2^32: (b, h) = (4095, 15) holds the counters just below
+    it, (4096, 0) those from 2^32 on, whose high word is 1.  A forward-only launch of about 17 GB."""
+    from oktopk_b200.ops.fused_attn import self_attention
+    B, S, H, p, dtype = 4100, 512, 16, 0.1, torch.bfloat16
+    if torch.cuda.mem_get_info()[0] < 24 * 2 ** 30:
+        pytest.skip("needs about 24 GB of free device memory")
+    assert ((4095 * H + 15) * S * S + S * S) // 4 == 2 ** 32 == (4096 * H * S * S) // 4
+    qkv = torch.zeros(B, S, 3 * H * D, dtype=dtype, device="cuda")
+    gen = torch.Generator("cuda").manual_seed(4)
+    qkv[4095:4097] = torch.randn(2, S, 3 * H * D, device="cuda", generator=gen).to(dtype)
+    torch.cuda.manual_seed(41)
+    with torch.no_grad():
+        o = self_attention(qkv, H, None, p)
+    x, o = qkv[4095:4097].clone(), o[4095:4097].clone()
+    del qkv
+    torch.cuda.empty_cache()
+    keep = keep_mask(seed_of(41), 2, H, S, p, b0=4095)
+    od, of = _formula(x.double(), H, None, keep, p), _formula(x, H, None, keep, p)
+    for b, h in ((0, 15), (1, 0)):
+        c = (slice(b, b + 1), slice(None), slice(h * D, (h + 1) * D))
+        _within(o[c], of[c], od[c], dtype, (4095 + b, h))
 
 
 # ------------------------------------------------------------------------------------------ 3. determinism
