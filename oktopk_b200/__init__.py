@@ -20,7 +20,7 @@ __version__ = "0.1.0"
 
 def __getattr__(name):
     # heavier modules are imported lazily so that `import oktopk_b200` stays cheap
-    if name in ("DistributedOptimizer", "BertAdam", "broadcast_parameters"):
+    if name in ("DistributedOptimizer", "BertAdam", "Lamb", "broadcast_parameters"):
         from . import optimizer as _o
         return getattr(_o, name)
     if name in ("optimizer", "models", "train", "utils", "ops", "parallel", "compression", "config"):

@@ -567,6 +567,26 @@ static void fused_adam(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, do
                          P_<const float>(coef_ptr), S_(stream)),
        "fused_adam");
 }
+// LAMB on one (bucket, param group) slice, three launches (launch_fused_lamb).  off / len / blk / ends: device int32
+// tables of the slice's nseg segments (blk: nseg + 1 entries); nblk = blk[nseg] - blk[0], which the host knows from the
+// same table.
+static void fused_lamb(uint64_t p, uint64_t g, uint64_t m, uint64_t v, int n, double beta1, double beta2, double eps,
+                       int nseg, uint64_t off, uint64_t len, uint64_t blk, uint64_t ends, int nblk, uint64_t part_w,
+                       uint64_t part_u, uint64_t norm_w, uint64_t norm_u, uint64_t ratio, int zero_grad,
+                       uint64_t stream, uint64_t scal_ptr, uint64_t fault_ptr, uint64_t skip_ptr, uint64_t coef_ptr) {
+    if (scal_ptr == 0) throw std::runtime_error("fused_lamb: scal_ptr must point at the group's device scalars");
+    if (nseg <= 0 || nblk < nseg || n < 0 || !off || !len || !blk || !ends || !part_w || !part_u || !norm_w || !norm_u ||
+        !ratio)
+        throw std::runtime_error("fused_lamb: bad segment table or buffers");
+    if ((p | g | m | v) % 16 || (part_w | part_u) % 8)
+        throw std::runtime_error("fused_lamb: p, g, m and v must be 16-byte aligned");
+    const LambSegs t{P_<const int>(off), P_<const int>(len), P_<const int>(blk), P_<const int>(ends), nseg};
+    ck(launch_fused_lamb(P_<float>(p), P_<float>(g), P_<float>(m), P_<float>(v), n, beta1, beta2, (float)eps, t, nblk,
+                         P_<double>(part_w), P_<double>(part_u), P_<float>(norm_w), P_<float>(norm_u), P_<float>(ratio),
+                         zero_grad, P_<float>(scal_ptr), P_<int>(fault_ptr), P_<int>(skip_ptr),
+                         P_<const float>(coef_ptr), S_(stream)),
+       "fused_lamb");
+}
 // dtype of x, y, dy, dx: 0 = fp32, 1 = bf16, 2 = fp16 (parameters, statistics and dgamma / dbeta are fp32 in every case).
 // res (forward and backward) and dres (backward), 0 = absent: y = relu(bn(x) + res) and dres = the residual's gradient,
 // [M, C] in x's dtype, with relu = 1 and W = 0.
@@ -1031,6 +1051,11 @@ PYBIND11_MODULE(_C, m) {
           py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("decoupled"), py::arg("zero_grad"),
           py::arg("stream"), py::arg("scal_ptr"), py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0,
           py::arg("coef_ptr") = 0);
+    m.def("fused_lamb", &fused_lamb, py::arg("p"), py::arg("g"), py::arg("m"), py::arg("v"), py::arg("n"),
+          py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("nseg"), py::arg("off"), py::arg("len"),
+          py::arg("blk"), py::arg("ends"), py::arg("nblk"), py::arg("part_w"), py::arg("part_u"), py::arg("norm_w"),
+          py::arg("norm_u"), py::arg("ratio"), py::arg("zero_grad"), py::arg("stream"), py::arg("scal_ptr"),
+          py::arg("fault_ptr") = 0, py::arg("skip_ptr") = 0, py::arg("coef_ptr") = 0);
     m.def("momentum_correct", &momentum_correct);
     m.def("grad_sumsq", &grad_sumsq, py::arg("g"), py::arg("offs"), py::arg("lens"), py::arg("partial"),
           py::arg("stream"));
@@ -1040,10 +1065,11 @@ PYBIND11_MODULE(_C, m) {
     m.def("scale_update", [](uint64_t ls, double growth, double backoff, int interval, uint64_t stream) {
         ck(launch_scale_update(P_<LossScaleDev>(ls), growth, backoff, interval, S_(stream)), "scale_update");
     });
-    m.def("adam_scalars", [](uint64_t ls, uint64_t hyper, uint64_t scal, int groups, uint64_t stream) {
-        ck(launch_adam_scalars(P_<const LossScaleDev>(ls), P_<const double>(hyper), P_<float>(scal), groups, S_(stream)),
+    m.def("adam_scalars", [](uint64_t ls, uint64_t hyper, uint64_t scal, int groups, uint64_t stream, int lamb) {
+        ck(launch_adam_scalars(P_<const LossScaleDev>(ls), P_<const double>(hyper), P_<float>(scal), groups, lamb,
+                               S_(stream)),
            "adam_scalars");
-    });
+    }, py::arg("ls"), py::arg("hyper"), py::arg("scal"), py::arg("groups"), py::arg("stream"), py::arg("lamb") = 0);
     m.def("carry_residual", [](uint64_t g, uint64_t res, int n, uint64_t skip, uint64_t stream) {
         ck(launch_carry_residual(P_<float>(g), P_<float>(res), n, P_<const int>(skip), S_(stream)), "carry_residual");
     });

@@ -352,6 +352,27 @@ cudaError_t launch_fused_bert_adam(float* p, float* g, float* m, float* v, int n
 cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
                               float weight_decay, int decoupled, int zero_grad, const float* scal, const int* fault,
                               const int* skip, const float* coef, cudaStream_t stream);
+// LAMB on one (bucket, param group) slice [p, p + n) of nseg parameters (segments), in three launches (optim.cu).  All
+// four tables are device arrays: segment j starts at element off[j] of the slice (a multiple of 4) and has len[j]
+// elements; its chunk partials are [blk[j], blk[j + 1]) of the bucket-wide arrays part_w / part_u (one per kSumsqChunk
+// elements, at least one), so blk has nseg + 1 entries; ends[j] is the float4 vector of the slice where segment j + 1
+// starts (INT_MAX for the last).  nblk = blk[nseg] - blk[0] CTAs run the first pass.
+struct LambSegs {
+    const int* off;
+    const int* len;
+    const int* blk;
+    const int* ends;
+    int nseg;
+};
+struct LambHyper {
+    float b1, omb1, b2, omb2, eps;
+};
+// scal -> {lr, weight_decay, 1 - beta1^t, 1 - beta2^t}; norm_w / norm_u / ratio: ||w||, ||u|| and r per segment;
+// coef: the global clip factor or null
+cudaError_t launch_fused_lamb(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
+                              const LambSegs& t, int nblk, double* part_w, double* part_u, float* norm_w,
+                              float* norm_u, float* ratio, int zero_grad, const float* scal, const int* fault,
+                              const int* skip, const float* coef, cudaStream_t stream);
 
 // ---- dynamic loss scaling (csrc/scale.cu) ------------------------------------------------------------
 // One per optimizer, in device memory.  found_inf is the step verdict: the OR of the bucket verdicts of the step.
@@ -390,10 +411,12 @@ static_assert(sizeof(ScaleParams) <= 4096, "ScaleParams must fit the 4 KB kernel
 cudaError_t launch_unscale_check(const ScaleParams& p, cudaStream_t stream);
 // end of step: growth / backoff of torch._amp_update_scale_, new inv_scale, skipped-step and Adam step counts, verdict
 // cleared.  adam_scalars (start of step): the wrapped Adam's per-group scalars for step adam_step + 1, in double, from
-// hyper = {lr, weight_decay, beta1, beta2} per group into scal (3 floats per group).
+// hyper = {lr, weight_decay, beta1, beta2} per group into scal (3 floats per group); lamb: LAMB's instead (4 per group,
+// see launch_fused_lamb; betas of 0 give its scalars without bias correction).
 cudaError_t launch_scale_update(LossScaleDev* ls, double growth_factor, double backoff_factor, int growth_interval,
                                 cudaStream_t stream);
-cudaError_t launch_adam_scalars(const LossScaleDev* ls, const double* hyper, float* scal, int groups, cudaStream_t stream);
+cudaError_t launch_adam_scalars(const LossScaleDev* ls, const double* hyper, float* scal, int groups, int lamb,
+                                cudaStream_t stream);
 // dense switch carry-over under loss scaling: g += res; res = 0 -- unless the bucket verdict is set
 cudaError_t launch_carry_residual(float* g, float* res, int n, const int* skip, cudaStream_t stream);
 // multi-tensor gradient landing: copy up to kLandMax autograd-produced gradient tensors into the flat bucket in ONE launch

@@ -401,6 +401,169 @@ __global__ void __launch_bounds__(kOptThreads) clip_coef_kernel(const double* __
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// LAMB, as apex's FusedLAMB computes it by default (adam_w_mode, grad_averaging, no nvlamb).  Per parameter tensor w:
+// u = m_hat / (sqrt(v_hat) + eps) + wd*w and w -= lr * r * u with the trust ratio r = ||w|| / ||u|| (1 where wd == 0
+// or either norm is 0).  r needs the whole tensor's ||u|| before any element of w may change, so a (bucket, param
+// group) slice takes three streaming passes:
+//   lamb_moments_kernel  p, g, m, v in; m, v out; one CTA per kSumsqChunk elements of a segment (a parameter), as
+//                        grad_sumsq_kernel lays them out, each writing its fp64 sums of w^2 and u^2 to its own
+//                        partials; the dirty gradient lines cleared as update_pass clears them.  p is not written.
+//   lamb_ratio_kernel    one CTA: each segment's partials summed in a fixed order into ||w||, ||u|| and r
+//   lamb_apply_kernel    p, m, v in; u recomputed by lamb_u, the function pass 1 used, so bit for bit the same;
+//                        p -= lr*r*u, r found per float4 vector by ClipCursor over the segment ends
+// Storing u instead of recomputing it moves as many bytes (it has to be written and read back) and would need a
+// scratch buffer, or the gradient bucket, which would then have to be cleared densely.  The partials depend on the
+// segment lengths alone and nothing orders them but the code, so the step is a function of its inputs' bits.
+// scal -> {lr, weight_decay, 1 - beta1^t, 1 - beta2^t} of the group: the step's scalars (1, 1 without bias correction).
+// ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float lamb_u(const float* s, float pw, float mw, float vw, float eps) {
+    const float mh = __fdiv_rn(mw, s[2]), vh = __fdiv_rn(vw, s[3]);
+    return __fmaf_rn(s[1], pw, __fdiv_rn(mh, __fadd_rn(__fsqrt_rn(vh), eps)));
+}
+
+// new m and v of one element, its w^2 and u^2 added to the CTA's sums
+__device__ __forceinline__ void lamb_moments(const LambHyper& h, const float* s, float pw, float gw, float& mw,
+                                             float& vw, double& aw, double& au) {
+    mw = __fmaf_rn(h.omb1, gw, __fmul_rn(h.b1, mw));
+    vw = __fmaf_rn(h.omb2, __fmul_rn(gw, gw), __fmul_rn(h.b2, vw));
+    const float u = lamb_u(s, pw, mw, vw, h.eps);
+    aw += (double)pw * pw;
+    au += (double)u * u;
+}
+
+__device__ __forceinline__ bool stopped(const int* fault) {
+    return fault != nullptr && *reinterpret_cast<const volatile int*>(fault) != 0;
+}
+
+// coef: the global clip factor or null
+__global__ void __launch_bounds__(kOptThreads) lamb_moments_kernel(const float* __restrict__ p, float* __restrict__ g,
+                                                                    float* __restrict__ m, float* __restrict__ v,
+                                                                    const LambSegs t, const LambHyper h, int zero_grad,
+                                                                    const float* __restrict__ scal,
+                                                                    const int* __restrict__ fault,
+                                                                    const int* __restrict__ skip,
+                                                                    const float* __restrict__ coef,
+                                                                    double* __restrict__ part_w,
+                                                                    double* __restrict__ part_u) {
+    if (stopped(fault)) return;
+    const int q = __ldg(t.blk) + blockIdx.x;            // this CTA's partial; its segment by binary search
+    int lo = 0, hi = t.nseg - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (q >= __ldg(t.blk + mid)) lo = mid; else hi = mid - 1;
+    }
+    const int begin = (q - __ldg(t.blk + lo)) * kSumsqChunk;
+    const int len = min(__ldg(t.len + lo) - begin, kSumsqChunk);
+    const int base = __ldg(t.off + lo) + begin;          // a multiple of 4
+    const float4* p4 = reinterpret_cast<const float4*>(p + base);
+    float4* g4 = reinterpret_cast<float4*>(g + base);
+    float4* m4 = reinterpret_cast<float4*>(m + base);
+    float4* v4 = reinterpret_cast<float4*>(v + base);
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int n4 = len >> 2, tail = (len & ~3) + threadIdx.x;
+    if (verdict_set(skip)) {              // loss scaling skips this step: parameters and state stay, the gradient is cleared
+        if (!zero_grad) return;
+        for (int i = threadIdx.x; i < n4; i += kOptThreads) {
+            const float4 gw = ld_stream_f4(g4 + i);
+            if (gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f) g4[i] = zero;
+        }
+        if (tail < len) g[base + tail] = 0.f;
+        return;
+    }
+    float s[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s[j] = scal[j];
+    const float c = coef != nullptr ? *coef : 1.f;
+    double aw = 0.0, au = 0.0;
+    for (int i = threadIdx.x; i < n4; i += kOptThreads) {
+        const float4 pw = p4[i];
+        float4 gw = ld_stream_f4(g4 + i), mw = m4[i], vw = v4[i];
+        const bool dirty = gw.x != 0.f || gw.y != 0.f || gw.z != 0.f || gw.w != 0.f;
+        if (coef != nullptr) scale4(gw, c);
+        lamb_moments(h, s, pw.x, gw.x, mw.x, vw.x, aw, au); lamb_moments(h, s, pw.y, gw.y, mw.y, vw.y, aw, au);
+        lamb_moments(h, s, pw.z, gw.z, mw.z, vw.z, aw, au); lamb_moments(h, s, pw.w, gw.w, mw.w, vw.w, aw, au);
+        m4[i] = mw;
+        v4[i] = vw;
+        if (zero_grad && dirty) g4[i] = zero;
+    }
+    if (tail < len) {                     // the segment's last len % 4 elements, one per thread
+        const int i = base + tail;
+        float gw = g[i], mw = m[i], vw = v[i];
+        if (coef != nullptr) gw = __fmul_rn(gw, c);
+        lamb_moments(h, s, p[i], gw, mw, vw, aw, au);
+        m[i] = mw;
+        v[i] = vw;
+        if (zero_grad) g[i] = 0.f;
+    }
+    aw = block_sum_d(aw);
+    au = block_sum_d(au);
+    if (threadIdx.x == 0) {
+        part_w[q] = aw;
+        part_u[q] = au;
+    }
+}
+
+// One CTA, a warp per segment as in clip_coef_kernel.  r in double from the fp64 norms, rounded once.
+__global__ void __launch_bounds__(kOptThreads) lamb_ratio_kernel(const LambSegs t, const double* __restrict__ part_w,
+                                                                  const double* __restrict__ part_u,
+                                                                  const float* __restrict__ scal,
+                                                                  const int* __restrict__ fault,
+                                                                  const int* __restrict__ skip,
+                                                                  float* __restrict__ norm_w,
+                                                                  float* __restrict__ norm_u, float* __restrict__ ratio) {
+    if (stopped(fault) || verdict_set(skip)) return;
+    const bool decay = scal[1] != 0.f;
+    const int lane = threadIdx.x & 31;
+    for (int j = threadIdx.x >> 5; j < t.nseg; j += kOptThreads / 32) {
+        double aw = 0.0, au = 0.0;
+        for (int i = t.blk[j] + lane; i < t.blk[j + 1]; i += 32) {
+            aw += part_w[i];
+            au += part_u[i];
+        }
+        aw = warp_sum_d(aw);
+        au = warp_sum_d(au);
+        if (lane == 0) {
+            const double wn = sqrt(aw), un = sqrt(au);
+            norm_w[j] = (float)wn;
+            norm_u[j] = (float)un;
+            ratio[j] = (decay && wn > 0.0 && un > 0.0) ? (float)(wn / un) : 1.f;
+        }
+    }
+}
+
+// r: the trust ratios of the slice's segments and their ends (float4 vectors)
+__global__ void __launch_bounds__(kOptThreads) lamb_apply_kernel(float* __restrict__ p, const float* __restrict__ m,
+                                                                  const float* __restrict__ v, int n, float eps,
+                                                                  const float* __restrict__ scal,
+                                                                  const int* __restrict__ fault,
+                                                                  const int* __restrict__ skip, const ClipRef r) {
+    if (stopped(fault) || verdict_set(skip)) return;
+    float s[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s[j] = scal[j];
+    ClipCursor rc(r);
+    const int n4 = n >> 2;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    const float4* m4 = reinterpret_cast<const float4*>(m);
+    const float4* v4 = reinterpret_cast<const float4*>(v);
+    for (int i = blockIdx.x * kOptThreads + threadIdx.x; i < n4; i += gridDim.x * kOptThreads) {
+        float4 pw = p4[i];
+        const float4 mw = ld_stream_f4(m4 + i), vw = ld_stream_f4(v4 + i);
+        const float step = __fmul_rn(s[0], rc.at(i));
+        pw.x = __fmaf_rn(-step, lamb_u(s, pw.x, mw.x, vw.x, eps), pw.x);
+        pw.y = __fmaf_rn(-step, lamb_u(s, pw.y, mw.y, vw.y, eps), pw.y);
+        pw.z = __fmaf_rn(-step, lamb_u(s, pw.z, mw.z, vw.z, eps), pw.z);
+        pw.w = __fmaf_rn(-step, lamb_u(s, pw.w, mw.w, vw.w, eps), pw.w);
+        p4[i] = pw;
+    }
+    if (blockIdx.x == 0)
+        for (int i = n4 * 4 + threadIdx.x; i < n; i += kOptThreads) {
+            const float step = __fmul_rn(s[0], rc.at(i >> 2));
+            p[i] = __fmaf_rn(-step, lamb_u(s, p[i], m[i], v[i], eps), p[i]);
+        }
+}
+
 static inline int opt_grid(int n) {
     int g = (n / 4 + kOptThreads - 1) / kOptThreads;
     if (g < 1) g = 1;
@@ -452,6 +615,20 @@ cudaError_t launch_fused_adam(float* p, float* g, float* m, float* v, int n, dou
     fused_adam_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, g, m, v, n, (float)(1.0 - beta1), (float)beta2,
                                                               (float)(1.0 - beta2), eps, weight_decay, decoupled,
                                                               zero_grad, scal, fault, skip, coef);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fused_lamb(float* p, float* g, float* m, float* v, int n, double beta1, double beta2, float eps,
+                              const LambSegs& t, int nblk, double* part_w, double* part_u, float* norm_w,
+                              float* norm_u, float* ratio, int zero_grad, const float* scal, const int* fault,
+                              const int* skip, const float* coef, cudaStream_t stream) {
+    // 1 - beta in double, rounded once, as for Adam
+    const LambHyper h{(float)beta1, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), eps};
+    lamb_moments_kernel<<<nblk, kOptThreads, 0, stream>>>(p, g, m, v, t, h, zero_grad, scal, fault, skip, coef, part_w,
+                                                          part_u);
+    lamb_ratio_kernel<<<1, kOptThreads, 0, stream>>>(t, part_w, part_u, scal, fault, skip, norm_w, norm_u, ratio);
+    lamb_apply_kernel<<<opt_grid(n), kOptThreads, 0, stream>>>(p, m, v, n, eps, scal, fault, skip,
+                                                               ClipRef{ratio, t.ends});
     return cudaGetLastError();
 }
 

@@ -87,11 +87,18 @@ __global__ void scale_update_kernel(LossScaleDev* ls, double growth_factor, doub
     ls->found_inf = 0;
 }
 
-__global__ void adam_scalars_kernel(const LossScaleDev* ls, const double* hyper, float* scal, int groups) {
+__global__ void adam_scalars_kernel(const LossScaleDev* ls, const double* hyper, float* scal, int groups, int lamb) {
     // torch's non-capturable Adam, in double: t = the step about to run (skipped steps do not count)
     const double t = (double)(ls->adam_step + 1);
     for (int gi = threadIdx.x; gi < groups; gi += blockDim.x) {
         const double lr = hyper[4 * gi], wd = hyper[4 * gi + 1], b1 = hyper[4 * gi + 2], b2 = hyper[4 * gi + 3];
+        if (lamb) {                                     // _LambUpdate.scalars, in the same double arithmetic
+            scal[4 * gi] = (float)lr;
+            scal[4 * gi + 1] = (float)wd;
+            scal[4 * gi + 2] = (float)(1.0 - pow(b1, t));
+            scal[4 * gi + 3] = (float)(1.0 - pow(b2, t));
+            continue;
+        }
         scal[3 * gi] = (float)(1.0 - lr * wd);
         scal[3 * gi + 1] = (float)((lr / (1.0 - pow(b1, t))) * -1.0);
         scal[3 * gi + 2] = (float)sqrt(1.0 - pow(b2, t));
@@ -119,8 +126,9 @@ cudaError_t launch_scale_update(LossScaleDev* ls, double growth_factor, double b
     return cudaGetLastError();
 }
 
-cudaError_t launch_adam_scalars(const LossScaleDev* ls, const double* hyper, float* scal, int groups, cudaStream_t stream) {
-    adam_scalars_kernel<<<1, 32, 0, stream>>>(ls, hyper, scal, groups);
+cudaError_t launch_adam_scalars(const LossScaleDev* ls, const double* hyper, float* scal, int groups, int lamb,
+                                cudaStream_t stream) {
+    adam_scalars_kernel<<<1, 32, 0, stream>>>(ls, hyper, scal, groups, lamb);
     return cudaGetLastError();
 }
 

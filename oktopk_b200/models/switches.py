@@ -93,6 +93,12 @@ SWITCHES = (
            help="lstman4 and lstm (PTB): clip the reduced gradient on the device inside the optimizer step, one "
                 "deterministic norm pass with the factor applied by the fused update, instead of torch's "
                 "clip_grad_norm_ before it (default: clip_grad_norm_)"),
+    # a Trainer argument, not a create_net keyword
+    Switch("--lamb", (), BERTS,
+           help="BERT: train with LAMB (okt.Lamb: per-parameter trust ratios ||w|| / ||u||, bias correction, weight "
+                "decay 0.01 except biases and LayerNorm) on the fused LAMB kernels, the reduced gradient clipped to "
+                "a global norm of 1.0 on the device and the learning rate on BertAdam's warmup_linear schedule "
+                "(default: BertAdam)"),
     Switch("--bidirectional", ("bidirectional",), ("lstman4",),
            help="lstman4: bidirectional LSTM layers, the two directions summed, and no look-ahead convolution "
                 "(default: uni-directional)"),

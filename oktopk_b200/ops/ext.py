@@ -15,7 +15,7 @@ _ERR: Optional[BaseException] = None
 # kernels launched by this package since import (the bench reports the delta over its timed region)
 LAUNCH_COUNT = {"total": 0}
 _LAUNCHERS = {"oktopk_run": 1, "gather_run": 1, "gtopk_run": 1, "dense_run": 1, "kth_abs": 1, "fused_sgd": 1,
-              "sgd_ahead": 1, "fused_sgd_tail": 1, "fused_bert_adam": 1, "fused_adam": 1, "momentum_correct": 1, "grad_sumsq": 1, "clip_coef": 1, "land_grads": 1, "bn_forward": 1, "bn_backward": 1,
+              "sgd_ahead": 1, "fused_sgd_tail": 1, "fused_bert_adam": 1, "fused_adam": 1, "fused_lamb": 3, "momentum_correct": 1, "grad_sumsq": 1, "clip_coef": 1, "land_grads": 1, "bn_forward": 1, "bn_backward": 1,
               "maxpool2_fwd": 1, "maxpool2_bwd": 1, "unscale_check": 1, "ln_forward": 1, "ln_backward": 2,
               "xent_forward": 2, "xent_backward": 1, "lstm_forward": 1, "lstm_backward": 1, "mlm_select": 1,
               "mlm_gather": 1, "mlm_scatter": 1, "attn_forward": 1, "attn_backward": 2, "lstm_seq_forward": 1,

@@ -16,8 +16,8 @@ What is different by design (GPU-first):
     per (bucket, param group) that also zeroes the gradient bucket (``zero_grad()`` is then free);
   * any torch optimizer can be wrapped (the reference re-implements SGD only, A.4-7): SGD, BertAdam and
     ``torch.optim.Adam`` / ``AdamW`` built with ``fused=True`` take the fused kernels (Adam: fp32 CUDA parameters,
-    no amsgrad / maximize / differentiable, Python-number lr and betas); everything else falls through to its own
-    ``step()``;
+    no amsgrad / maximize / differentiable, Python-number lr and betas) and ``Lamb`` (LAMB, three kernels per bucket and
+    param group) take the fused kernels; everything else falls through to its own ``step()``;
   * ``state_dict()`` carries residuals, thresholds, region boundaries and counters (SURVEY 5.4).
 """
 from __future__ import annotations
@@ -218,8 +218,9 @@ class _BucketedComm:
         # device-resident per-group scalars (the learning rate; for wrapped Adam the step's decay, step size and bias
         # correction): the fused update kernels read them from memory so that a captured CUDA graph of the whole step
         # stays valid when the schedule moves
-        # With loss scaling the wrapped Adam's step count is on the device (a skipped step does not advance it): the host
-        # stages {lr, weight_decay, beta1, beta2} per group in double (_hyper_dev) and a kernel derives the scalars.
+        # With loss scaling the wrapped Adam's or Lamb's step count is on the device (a skipped step does not advance it):
+        # the host stages {lr, weight_decay, beta1, beta2} per group in double (_hyper_dev) and a kernel derives the
+        # scalars.
         self._lr_dev = self._hyper_dev = None
         self._lr_pin, self._lr_ev, self._lr_ring, self._lr_last = [], [], 0, None
         dev0 = self._buckets[0].params[0].device if self._buckets else torch.device("cpu")
@@ -227,7 +228,7 @@ class _BucketedComm:
             groups = max(len(self.param_groups), 1)
             self._lr_dev = torch.zeros(groups * self._update.n_scalars, dtype=torch.float32, device=dev0)
             stage = self._lr_dev
-            if self._ls is not None and self._update is _AdamUpdate:
+            if self._ls is not None and (self._update is _AdamUpdate or self._update is _LambUpdate):
                 stage = self._hyper_dev = torch.zeros(groups * 4, dtype=torch.float64, device=dev0)
             self._lr_pin = [torch.zeros_like(stage, device="cpu").pin_memory() for _ in range(8)]
             self._lr_ev = [None] * len(self._lr_pin)
@@ -238,6 +239,7 @@ class _BucketedComm:
         self._clip: Optional[_GradClip] = None
         if (max_grad_norm is not None or clip_per_param) and self._device_update():
             self._clip = _GradClip(self, clip_per_param, max_grad_norm or 0.0)
+        self._lamb = _LambNorms(self) if self._update is _LambUpdate and self._device_update() else None
 
     def _resync_replicas(self) -> None:
         """After a handled fault: every replica takes rank 0's parameters (and momentum) again."""
@@ -595,9 +597,10 @@ class _BucketedComm:
                 b.dirty = True
         else:
             self._maybe_refresh_lr()
-            if self._hyper_dev is not None and self._update is _AdamUpdate:
+            if self._hyper_dev is not None:
                 ext.require().adam_scalars(self._ls.ptr, self._hyper_dev.data_ptr(), self._lr_dev.data_ptr(),
-                                           len(self.param_groups), torch.cuda.current_stream().cuda_stream)
+                                           len(self.param_groups), torch.cuda.current_stream().cuda_stream,
+                                           lamb=int(self._update is _LambUpdate))
             if self._clip is not None:
                 self._grad_norm = self._clip.run(self)
             with torch.no_grad():
@@ -678,8 +681,8 @@ class _BucketedComm:
         if counter is None:
             steps = {float(self.state[p]["step"]) for p in have if "step" in self.state[p]}
             if len(steps) > 1:
-                warnings.warn("DistributedOptimizer: the loaded Adam state has unequal step counts per parameter %s; "
-                              "using torch's Adam step from now on" % sorted(steps))
+                warnings.warn("DistributedOptimizer: the loaded %s state has unequal step counts per parameter %s; "
+                              "using its own step() from now on" % (type(self).__name__, sorted(steps)))
                 self._update = None
                 self._clip = None                 # torch's step: the clip runs before it, in torch
                 self._clear_buckets()
@@ -734,35 +737,26 @@ class _GradClip:
     (``_BertAdamUpdate.scalars``); the update kernel finds a vector's factor from the segment ends of its group slice."""
 
     def __init__(self, opt, per_param: bool, max_norm: float):
-        C = ext.require()
         dev = opt._buckets[0].grad.device
         self.per_param, self.max_norm = per_param, float(max_norm)
-        self.tables = []                          # (bucket, offsets, lengths, first partial)
-        self.first_seg: Dict[tuple, int] = {}     # (bucket index, group slice start) -> its first segment
-        seg_blk, seg_scal, ends, npart = [0], [], [], 0
-        for b in opt._buckets:
-            if per_param:
-                offs, lens = list(b.offsets), [p.numel() for p in b.params]
-                for gi, s, e in b.group_slices:
-                    ts = [t for t, o in enumerate(offs) if s <= o < e]
-                    self.first_seg[b.index, s] = len(seg_scal)
-                    for j, t in enumerate(ts):
-                        seg_scal.append(gi * opt._update.n_scalars + 1)
-                        ends.append((offs[ts[j + 1]] - s) // 4 if j + 1 < len(ts) else 2 ** 31 - 1)
-            else:
-                offs, lens = [0], [b.numel]
-            self.tables.append((b, offs, lens, npart))
-            for n in lens:
-                npart += max(1, -(-n // C.SUMSQ_CHUNK))
-                seg_blk.append(npart)
-        self.nseg = len(seg_scal) if per_param else 1
+        self.segs = None
+        if per_param:
+            self.segs = _SegTable(opt._buckets, dev)
+            self.tables = self.segs.tables
+            self.nseg, npart = self.segs.nseg, self.segs.npart
+            self.seg_blk, self.ends = self.segs.blk, self.segs.ends
+            self.seg_scal = _as_dev([gi * opt._update.n_scalars + 1 for gi in self.segs.group], dev)
+        else:
+            self.tables = []                      # (bucket, offsets, lengths, first partial)
+            npart = 0
+            for b in opt._buckets:
+                self.tables.append((b, [0], [b.numel], npart))
+                npart += max(1, -(-b.numel // ext.require().SUMSQ_CHUNK))
+            self.nseg = 1
+            self.seg_blk = self.seg_scal = self.ends = None
         self.partial = torch.zeros(npart, dtype=torch.float64, device=dev)
         self.norm = torch.zeros(self.nseg, dtype=torch.float32, device=dev)
         self.coef = torch.ones(self.nseg, dtype=torch.float32, device=dev)
-        as_dev = lambda v: torch.tensor(v, dtype=torch.int32).to(dev)      # noqa: E731
-        self.seg_blk = as_dev(seg_blk) if per_param else None
-        self.seg_scal = as_dev(seg_scal) if per_param else None
-        self.ends = as_dev(ends) if per_param else None
 
     def run(self, opt) -> torch.Tensor:
         """Enqueue the norm and the factor on the current stream; returns the norm (0-dim, or one per parameter)."""
@@ -781,8 +775,46 @@ class _GradClip:
         """The factor arguments of the update of bucket ``b``'s group slice starting at element ``s``."""
         if not self.per_param:
             return {"coef_ptr": self.coef.data_ptr()}
-        t = self.first_seg[b.index, s]
+        t = self.segs.slices[b.index, s][0]
         return {"coef_ptr": self.coef.data_ptr() + 4 * t, "ends_ptr": self.ends.data_ptr() + 4 * t}
+
+
+def _as_dev(values, dev) -> torch.Tensor:
+    return torch.tensor(values, dtype=torch.int32).to(dev)
+
+
+class _SegTable:
+    """One segment per parameter tensor of every bucket, for the kernels that reduce over each parameter (the
+    per-parameter clip, LAMB's norms).  Segments are numbered in bucket order, which is also group-slice order, and
+    each gets the chunk partials [blk[t], blk[t + 1]) that a per-segment pass writes, one per SUMSQ_CHUNK elements
+    (at least one).  On the device, int32: ``off`` (the segment's offset in its group slice), ``len``, ``blk`` and
+    ``ends`` (the float4 vector of the group slice where the next segment starts, INT_MAX for a slice's last: the
+    cursor the update kernels find a vector's segment with).  Host side: ``tables`` (bucket, offsets, lengths, first
+    partial) for ``grad_sumsq``, ``group`` and ``params`` per segment, and ``slices``: (bucket index, group slice
+    start) -> (first segment, segments, partials)."""
+
+    def __init__(self, buckets: List[Bucket], dev: torch.device):
+        chunk = ext.require().SUMSQ_CHUNK
+        off, lens, blk, ends = [], [], [0], []
+        self.group, self.params, self.tables = [], [], []
+        self.slices: Dict[tuple, tuple] = {}
+        for b in buckets:
+            self.tables.append((b, list(b.offsets), [p.numel() for p in b.params], blk[-1]))
+            for gi, s, e in b.group_slices:
+                ts = [t for t, o in enumerate(b.offsets) if s <= o < e]
+                self.slices[b.index, s] = (len(lens), len(ts), blk[-1])
+                for j, t in enumerate(ts):
+                    n = b.params[t].numel()
+                    off.append(b.offsets[t] - s)
+                    lens.append(n)
+                    blk.append(blk[-1] + max(1, -(-n // chunk)))
+                    ends.append((b.offsets[ts[j + 1]] - s) // 4 if j + 1 < len(ts) else 2 ** 31 - 1)
+                    self.group.append(gi)
+                    self.params.append(b.params[t])
+                t0, nseg, p0 = self.slices[b.index, s]
+                self.slices[b.index, s] = (t0, nseg, blk[-1] - p0)
+        self.nseg, self.npart = len(lens), blk[-1]
+        self.off, self.len, self.blk, self.ends = (_as_dev(v, dev) for v in (off, lens, blk, ends))
 
 
 # ====================================================================================== fused update families
@@ -893,16 +925,64 @@ class _BertAdamUpdate:
                     p.data.add_(u, alpha=-lr)
 
 
+class _LambUpdate:
+    """``Lamb``: ``fused_lamb``'s three kernels per slice, or ``_lamb_param`` per parameter on the bucket's views.  Device
+    scalars: {lr, weight_decay, 1 - beta1^t, 1 - beta2^t}; under loss scaling the device derives them from its step count
+    (``adam_scalars`` with lamb=1) out of {lr, weight_decay, beta1, beta2}.  Betas of 0 stand for no bias correction:
+    1 - 0^t = 1."""
+    keys = ("exp_avg", "exp_avg_sq")
+    n_scalars = 4
+
+    @staticmethod
+    def scalars(opt, g):
+        b1, b2 = g["betas"] if g["bias_correction"] else (0.0, 0.0)
+        if opt._hyper_dev is not None:
+            return (float(g["lr"]), float(g["weight_decay"]), float(b1), float(b2))
+        t = float(opt.counter + 1)
+        return (float(g["lr"]), float(g["weight_decay"]), 1 - b1 ** t, 1 - b2 ** t)
+
+    @staticmethod
+    def update(opt, b, g, s, e, fs, first, launch):
+        if launch is not None:
+            n = opt._lamb
+            t0, nseg, nblk = n.segs.slices[b.index, s]
+            tab = [x.data_ptr() + 4 * t0 for x in (n.segs.off, n.segs.len, n.segs.blk, n.segs.ends)]
+            launch(ext.require().fused_lamb, g["betas"][0], g["betas"][1], g["eps"], nseg, *tab, nblk,
+                   n.partial[0].data_ptr(), n.partial[1].data_ptr(), n.norm[0].data_ptr() + 4 * t0,
+                   n.norm[1].data_ptr() + 4 * t0, n.ratio.data_ptr() + 4 * t0)
+            return
+        t = opt.counter + 1
+        for p, o, gv in zip(b.params, b.offsets, b.grad_views):
+            if s <= o < e:
+                _lamb_param(p.data, gv, opt.state[p]["exp_avg"], opt.state[p]["exp_avg_sq"], g, t)
+
+
+class _LambNorms:
+    """What ``fused_lamb`` keeps between its passes, allocated with the optimizer (never inside a captured step): the
+    per-parameter segment table, the fp64 partial sums of w^2 and u^2 (``partial[0]`` / ``partial[1]``), and per
+    parameter ||w||, ||u|| (``norm[0]`` / ``norm[1]``) and the trust ratio, in the table's segment order
+    (``segs.params``) as of the last applied step."""
+
+    def __init__(self, opt):
+        dev = opt._buckets[0].grad.device
+        self.segs = _SegTable(opt._buckets, dev)
+        self.partial = torch.zeros(2, self.segs.npart, dtype=torch.float64, device=dev)
+        self.norm = torch.zeros(2, self.segs.nseg, dtype=torch.float32, device=dev)
+        self.ratio = torch.ones(self.segs.nseg, dtype=torch.float32, device=dev)
+
+
 # ====================================================================================== DistributedOptimizer
 class _DistributedOptimizerMixin(_BucketedComm):
     def state_dict(self):
         sd = super().state_dict()
         scale = self._scale_state_dict()
-        if self._update is _AdamUpdate:           # torch's fused Adam format: a float32 0-dim step on the param's device
+        if self._update is _AdamUpdate or self._update is _LambUpdate:
+            # torch's Adam format: a float32 0-dim step, on the param's device for fused Adam, on the host for Lamb
             params = [p for g in self.param_groups for p in g["params"]]
             steps = scale["adam_step"] if scale is not None else self.counter     # skipped steps do not count
             for i, st in list(sd["state"].items()):
-                sd["state"][i] = dict(st, step=torch.tensor(float(steps), dtype=torch.float32, device=params[i].device))
+                dev = params[i].device if self._update is _AdamUpdate else "cpu"
+                sd["state"][i] = dict(st, step=torch.tensor(float(steps), dtype=torch.float32, device=dev))
         sd["oktopk"] = self._allreducer.state_dict()
         if scale is not None:
             sd["loss_scale"] = scale
@@ -936,8 +1016,9 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
     ``opt.scale_loss(loss)``.
     ``max_grad_norm``: clip the reduced gradient as ``synchronize(); clip_grad_norm_(params, max_grad_norm); step()``
     does, the norm over every parameter of the optimizer (``grad_norm()`` returns it).  With SGD or the fused Adam /
-    AdamW on flat CUDA buckets the clip runs on the device inside ``step()`` (the update kernels apply the factor; the
-    bucket is not rescaled in place); otherwise ``step()`` calls ``clip_grad_norm_`` over the bucket views.
+    AdamW or ``Lamb`` on flat CUDA buckets the clip runs on the device inside ``step()`` (the update kernels apply the
+    factor; the bucket is not rescaled in place); otherwise ``step()`` calls ``clip_grad_norm_`` over the bucket views.
+    A wrapped ``Lamb`` takes the fused LAMB kernels on flat CUDA buckets, its own per-parameter math elsewhere.
     """
     if max_grad_norm is not None and not float(max_grad_norm) > 0:
         raise ValueError("max_grad_norm must be a positive number, got %r" % (max_grad_norm,))
@@ -953,6 +1034,8 @@ def DistributedOptimizer(optimizer: torch.optim.Optimizer, named_parameters=None
         obj._update = _SGDUpdate
     elif _fused_adam_applies(optimizer):
         obj._update = _AdamUpdate
+    elif isinstance(optimizer, Lamb):
+        obj._update = _LambUpdate
     else:
         obj._update = None                        # torch's own step()
     if obj._update is not None:
@@ -1037,6 +1120,14 @@ SCHEDULES = {
 }
 
 
+def scheduled_lr(lr: float, step: int, t_total: int, warmup: float, schedule: str = "warmup_linear") -> float:
+    """BertAdam's learning rate after ``step`` steps: ``lr`` times ``schedule`` at step / t_total, or ``lr`` itself
+    when ``t_total`` is -1."""
+    if t_total != -1:
+        return lr * SCHEDULES[schedule](step / t_total, warmup)
+    return lr
+
+
 class BertAdam(_BucketedComm, torch.optim.Optimizer):
     """BERT's Adam (no bias correction, decoupled weight decay, warm-up schedules) with the sparse
     allreducer embedded -- ``BERT/bert/transformers/optimization.py:68-227``.
@@ -1085,9 +1176,7 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
 
     @staticmethod
     def _scheduled_lr(g: dict, step: int) -> float:
-        if g["t_total"] != -1:
-            return g["lr"] * SCHEDULES[g["schedule"]](step / g["t_total"], g["warmup"])
-        return g["lr"]
+        return scheduled_lr(g["lr"], step, g["t_total"], g["warmup"], g["schedule"])
 
     def state_dict(self):
         sd = torch.optim.Optimizer.state_dict(self)
@@ -1111,3 +1200,67 @@ class BertAdam(_BucketedComm, torch.optim.Optimizer):
         if okt is not None:
             self._allreducer.load_state_dict(okt)
         self._clear_buckets()
+
+
+# ====================================================================================== LAMB
+def _lamb_param(w: torch.Tensor, g: torch.Tensor, m: torch.Tensor, v: torch.Tensor, group: dict, t: int) -> None:
+    """One LAMB step of parameter tensor ``w`` (in place, with its moments ``m`` and ``v``) at step ``t`` (1-based)."""
+    b1, b2 = group["betas"]
+    m.mul_(b1).add_(g, alpha=1 - b1)
+    v.mul_(b2).addcmul_(g, g, value=1 - b2)
+    bc1, bc2 = (1 - b1 ** t, 1 - b2 ** t) if group["bias_correction"] else (1.0, 1.0)
+    u = (m / bc1).div_((v / bc2).sqrt_().add_(group["eps"]))
+    wd = group["weight_decay"]
+    if wd == 0:
+        w.add_(u, alpha=-group["lr"])
+        return
+    u.add_(w, alpha=wd)
+    wn, un = w.norm(), u.norm()
+    r = torch.where((wn > 0) & (un > 0), wn / un, torch.ones_like(wn))       # the trust ratio, 1 for a zero norm
+    w.sub_(u.mul_(r * group["lr"]))
+
+
+class Lamb(torch.optim.Optimizer):
+    """LAMB (You et al., "Large Batch Optimization for Deep Learning: Training BERT in 76 minutes"), as apex's
+    ``FusedLAMB`` computes it with its defaults (``adam_w_mode=True``, ``grad_averaging=True``, ``use_nvlamb=False``)
+    but without its global gradient clip.  For each parameter tensor w with gradient g at step t (1-based)::
+
+        m = b1*m + (1-b1)*g;   v = b2*v + (1-b2)*g*g
+        m_hat = m / (1 - b1^t);   v_hat = v / (1 - b2^t)          (bias_correction=False: m_hat = m, v_hat = v)
+        u = m_hat / (sqrt(v_hat) + eps) + wd*w
+        r = ||w|| / ||u||  if wd != 0 and both norms are > 0, else 1      (norms over the one tensor)
+        w = w - lr * r * u
+
+    This class runs that in torch ops, one parameter at a time (state ``exp_avg``, ``exp_avg_sq`` and ``step`` as in
+    torch's Adam).  Wrapped in ``DistributedOptimizer`` on flat CUDA buckets it runs on the fused LAMB kernels, and
+    ``DistributedOptimizer(..., max_grad_norm=c)`` adds the global clip of ``clip_grad_norm_`` before the step."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6, weight_decay: float = 0.01,
+                 bias_correction: bool = True):
+        if torch.is_tensor(lr) or not lr >= 0.0:
+            raise ValueError("Invalid learning rate: %r (a number >= 0)" % (lr,))
+        if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
+            raise ValueError("Invalid betas: %r" % (betas,))
+        if not eps >= 0.0 or not weight_decay >= 0.0:
+            raise ValueError("Invalid eps or weight_decay: %r, %r" % (eps, weight_decay))
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
+                                      bias_correction=bool(bias_correction)))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                st = self.state[p]
+                if not st:
+                    st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["step"] += 1
+                _lamb_param(p, p.grad, st["exp_avg"], st["exp_avg_sq"], group, int(st["step"]))
+        return loss

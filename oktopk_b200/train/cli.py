@@ -175,7 +175,7 @@ def main(argv=None) -> int:
                      log_dir=args.log_dir, seq_len=args.max_seq_length, seed=args.seed, backend=args.backend,
                      cuda_graph=args.cuda_graph, model_kwargs=model_kwargs or None, norm_clip=args.norm_clip,
                      autocast="bf16" if args.bf16 else ("fp16" if args.fp16 else None), loss_scale=args.loss_scale,
-                     an4_pad_multiple=args.an4_pad_multiple, fused_clip=args.fused_clip)
+                     an4_pad_multiple=args.an4_pad_multiple, fused_clip=args.fused_clip, lamb=args.lamb)
     if args.trace:
         import json
         os.makedirs(args.trace, exist_ok=True)

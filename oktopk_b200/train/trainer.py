@@ -25,7 +25,7 @@ from ..models import create_net
 from ..models.bert import BertPreTrainingHeads
 from ..ops.fused_ctc import ctc_loss
 from ..ops.fused_xent import softmax_cross_entropy
-from ..optimizer import BertAdam, DistributedOptimizer, broadcast_parameters
+from ..optimizer import BertAdam, DistributedOptimizer, Lamb, broadcast_parameters, scheduled_lr
 from ..parallel.world import World, world as _world
 from ..utils.logging import get_logger
 from ..utils.metrics import MetricsWriter, PhaseTimers
@@ -53,7 +53,7 @@ class Trainer:
                  seq_len: int = 128, t_total: int = -1, warmup: float = -1, pretrain: Optional[str] = None,
                  norm_clip: Optional[float] = None, backend: Optional[str] = None, cuda_graph: bool = False,
                  model_kwargs: Optional[dict] = None, autocast: Optional[str] = None, loss_scale=None,
-                 an4_pad_multiple: int = 0, fused_clip: bool = False):
+                 an4_pad_multiple: int = 0, fused_clip: bool = False, lamb: bool = False):
         """``an4_pad_multiple=m >= 1`` (AN4 only; 0, the default, is off): every training batch is staged into a
         ``data.PaddedAN4Batch`` with its frames padded up to a multiple of m and its lengths on the device, and with
         ``cuda_graph`` the steps are captured per padded length (``GraphedTrainStep``).  With the stock batch-norm the
@@ -64,7 +64,12 @@ class Trainer:
         ``fused_clip`` (AN4 and PTB, the two workloads that clip the reduced gradient every step; off by default): the
         clip runs on the device inside the optimizer's step (``DistributedOptimizer(max_grad_norm=...)``): one norm pass
         and a factor that the fused update applies, instead of ``clip_grad_norm_`` between ``synchronize()`` and
-        ``step()``.  The same factor as torch's up to the norm's rounding, no host synchronisation."""
+        ``step()``.  The same factor as torch's up to the norm's rounding, no host synchronisation.
+
+        ``lamb`` (BERT only; off by default): the optimizer is ``Lamb`` wrapped in ``DistributedOptimizer`` with the
+        global clip ``max_grad_norm=1.0`` on the device, over BertAdam's two param groups (weight decay 0.01, none for
+        biases and LayerNorm), its learning rate following BertAdam's warmup_linear schedule over ``t_total`` /
+        ``warmup``, instead of ``BertAdam``."""
         self.world = world or _world()
         self.rank, self.nworkers = self.world.rank, self.world.size
         # The host side of a step is tiny tensor ops (collate 16 images, one pinned copy): on a many-core box an
@@ -83,6 +88,10 @@ class Trainer:
         if fused_clip and self.clip_norm is None:
             raise ValueError("fused_clip applies to lstman4 and lstm, the models that clip their gradient; not %s" % dnn)
         self.fused_clip = bool(fused_clip)
+        if lamb and not dnn.startswith("bert"):
+            raise ValueError("lamb applies to the BERT models; not %s" % dnn)
+        self.lamb = bool(lamb)
+        self.t_total, self.warmup = t_total, warmup
         self.dataset = (dataset or _DATASET_OF.get(dnn, "cifar10")).lower()
         if an4_pad_multiple < 0 or (an4_pad_multiple and self.dataset != "an4"):
             raise ValueError("an4_pad_multiple must be 0 (off) or, for the AN4 dataset, >= 1; got %r for %s"
@@ -138,9 +147,16 @@ class Trainer:
             named = list(self.net.named_parameters())
             groups = [{"params": [p for n, p in named if not any(nd in n for nd in no_decay)], "weight_decay": 0.01},
                       {"params": [p for n, p in named if any(nd in n for nd in no_decay)], "weight_decay": 0.0}]
-            self.optimizer = BertAdam(groups, lr=lr, warmup=warmup, t_total=t_total, density=self.cfg.density,
-                                      compressor=self.cfg.compressor, rank=self.rank, named_parameters=named,
-                                      cfg=self.cfg, world=self.world, loss_scale=self.loss_scale)
+            if self.lamb:
+                self.optimizer = DistributedOptimizer(Lamb(groups, lr=lr), named_parameters=named,
+                                                      compression=_comp.compressors[self.cfg.compressor],
+                                                      is_sparse=self.cfg.sparse, density=self.cfg.density,
+                                                      cfg=self.cfg, world=self.world, err_handler=self._err_handler,
+                                                      loss_scale=self.loss_scale, max_grad_norm=1.0)
+            else:
+                self.optimizer = BertAdam(groups, lr=lr, warmup=warmup, t_total=t_total, density=self.cfg.density,
+                                          compressor=self.cfg.compressor, rank=self.rank, named_parameters=named,
+                                          cfg=self.cfg, world=self.world, loss_scale=self.loss_scale)
         else:
             if self.dataset == "ptb":
                 base = torch.optim.SGD(self.net.parameters(), lr=lr, momentum=0.0, weight_decay=0.0)
@@ -178,9 +194,11 @@ class Trainer:
     def adjust_learning_rate(self) -> float:
         """``VGG/dl_trainer.py:507-563``."""
         e = self.train_epoch + (self.train_iter % self.iters_per_epoch) / float(self.iters_per_epoch)
-        if self.is_bert:
+        if self.is_bert and not self.lamb:
             return self.lr                                     # BertAdam schedules internally
-        if self.dnn == "lstman4":
+        if self.is_bert:                                       # BertAdam's schedule at the optimizer's step count
+            lr = scheduled_lr(self.lr, self.optimizer.counter, self.t_total, self.warmup)
+        elif self.dnn == "lstman4":
             lr = self.lr / (1.01 ** self.train_epoch)           # /1.01 per epoch (:507-512)
         elif self.dnn == "lstm":
             # PTB step schedule (:514-529; the first boundary is 23+40 = 63 there, *after* the second one at 60, so the
